@@ -137,7 +137,7 @@ __device__ __forceinline__ float gms_rcp(float x) {
     return y;
 }
 
-struct GmsSlab3 {              // pair-duplicated per-splat data
+struct GmsSlab3 {              // pair-duplicated per-splat data of the float2-pair forward (k_composite_fwd3)
     float4 q0[GMS_WB];         // x, x, y, y
     float4 q1[GMS_WB];         // conx, conx, -cony, -cony
     float4 q2[GMS_WB];         // conz, conz, op, op

@@ -24,15 +24,14 @@
 static thread_local char g_err[512] = "";
 static int64_t g_launches = 0;
 // Defaults chosen on an H100 SXM (400 W) at 1M mesh-Gaussians / 1080p: step time with each alternative, default = 2.61-2.66 ms
-// over five interleaved runs (DESIGN.md 3.7).
+// over five interleaved runs, measured with the earlier float2-pair composite backward; 2.45 ms with the scalar one (DESIGN.md 3.7).
 static int g_opt_warp_emit = 1;    // (emit + sort path) warp-cooperative duplicate emission for large rects (0: 2.65 ms)
 static int g_opt_fwd = 2;          // composite forward: 2 scalar (default; writes the survivor lists), 3 float2 pairs (bit-identical; 2.81 ms)
 static int g_opt_bwd = 5;          // composite backward: 5 survivor-list driven (default), 3 predecessor (streams the whole tile list; 2.73 ms)
 static int g_opt_adam_sh_ieee = 0;  // k_adam_sh: 1 = nvcc's sqrtf / division with slow-path branches (A/B arm of the branch-free sequences)
 static int g_opt_key16 = 1;        // tile sort on 16-bit keys when T <= 65535 (0: always 32-bit keys; 2.66 ms)
-static int g_opt_bwd_minb = 6;     // __launch_bounds__ min CTAs/SM of the backward kernels (4: 128 regs, 2.63 ms; 6: 80; 5: 2.65; 8: 64, 2.69)
-static int g_opt_bwd_group = 1;    // k_composite_bwd5: 3 = a panel group's three alpha evaluations issued ahead of the recurrence (2.66 ms),
-                                   // 1 = one splat at a time
+static int g_opt_bwd_minb = 6;     // __launch_bounds__ min CTAs/SM of the backward kernels (6: 75 regs, 2.445-2.458 ms; 4: 76, 2.449;
+                                   // 8: 64, 2.449; 5: 76)
 static int g_opt_tile_order = 1;   // launch tiles longest list first (0: 2.79 ms)
 static int g_opt_sh_staged = 1;     // preprocess fwd/bwd: SH rows through a per-warp shared-memory tile (coalesced 128-bit accesses);
                                     // 0: direct (2.66 ms), 1: tile + register rows, 2: bwd in place in the tile (2.63 ms)
@@ -1097,7 +1096,6 @@ int gms_set_option(const char* key, int value) {
     else if (!strcmp(key, "composite_fwd")) p = &g_opt_fwd;
     else if (!strcmp(key, "composite_bwd")) p = &g_opt_bwd;
     else if (!strcmp(key, "bwd_minblocks")) p = &g_opt_bwd_minb;
-    else if (!strcmp(key, "bwd_group")) p = &g_opt_bwd_group;
     else if (!strcmp(key, "key16")) p = &g_opt_key16;
     else if (!strcmp(key, "adam_sh_ieee")) p = &g_opt_adam_sh_ieee;
     else if (!strcmp(key, "tile_order")) p = &g_opt_tile_order;
@@ -1440,10 +1438,8 @@ static int raster_backward_impl(const gms_raster_settings* s, const gms_raster_i
 #define GMS_BWD_ARGS IL.ranges, to, BL.vals_out, GL.rec, W, H, gx, s->bg, IL.final_T, IL.n_contrib, dL_dout_color, dL_dout_invdepth, GL.dgeom
 #define GMS_BWD_LAUNCH(MB)                                                                                                        \
             do {                                                                                                                  \
-                if (lists && g_opt_bwd_group == 3) { if (depth) k_composite_bwd5<MB, true, 3><<<T, GMS_CB, 0, st>>>(GMS_BWD_ARGS, surv, IL.nsurv); \
-                             else k_composite_bwd5<MB, false, 3><<<T, GMS_CB, 0, st>>>(GMS_BWD_ARGS, surv, IL.nsurv); }           \
-                else if (lists) { if (depth) k_composite_bwd5<MB, true, 1><<<T, GMS_CB, 0, st>>>(GMS_BWD_ARGS, surv, IL.nsurv);   \
-                             else k_composite_bwd5<MB, false, 1><<<T, GMS_CB, 0, st>>>(GMS_BWD_ARGS, surv, IL.nsurv); }           \
+                if (lists) { if (depth) k_composite_bwd5<MB, true><<<T, GMS_CB, 0, st>>>(GMS_BWD_ARGS, surv, IL.nsurv);           \
+                             else k_composite_bwd5<MB, false><<<T, GMS_CB, 0, st>>>(GMS_BWD_ARGS, surv, IL.nsurv); }              \
                 else { if (depth) k_composite_bwd3<MB, true><<<T, GMS_CB, 0, st>>>(GMS_BWD_ARGS);                                 \
                        else k_composite_bwd3<MB, false><<<T, GMS_CB, 0, st>>>(GMS_BWD_ARGS); }                                    \
             } while (0)
