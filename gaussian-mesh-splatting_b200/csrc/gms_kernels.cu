@@ -257,14 +257,15 @@ constexpr int GMS_SH_STRIDE_V = 52;    // floats per tile row, 128-bit per-lane 
 constexpr int GMS_SH_STRIDE_S = 49;    // floats per tile row, scalar per-lane accesses (odd: conflict-free)
 constexpr int GMS_SH_TILE = 32 * GMS_SH_STRIDE_V;      // floats of shared memory per warp (either layout fits)
 
-template <int STRIDE>
-__device__ __forceinline__ void sh_tile_load(const float* __restrict__ shs, int i0, unsigned rows, int lane, float* t) {
+// NC: through the read-only data cache.  Not when the same kernel later writes the rows (the fused SH Adam update).
+template <int STRIDE, bool NC = true>
+__device__ __forceinline__ void sh_tile_load(const float* shs, int i0, unsigned rows, int lane, float* t) {
     const float4* src = reinterpret_cast<const float4*>(shs) + (size_t)i0 * GMS_SH_ROW4;
 #pragma unroll
     for (int it = 0; it < GMS_SH_ROW4; it++) {
         const int j = it * 32 + lane, r = j / GMS_SH_ROW4, c = j - r * GMS_SH_ROW4;
         if ((rows >> r) & 1u) {
-            const float4 v = __ldg(src + j);
+            const float4 v = NC ? __ldg(src + j) : src[j];
             float* d = t + r * STRIDE + 4 * c;
             if (STRIDE % 4 == 0) *reinterpret_cast<float4*>(d) = v;
             else { d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w; }
@@ -466,12 +467,115 @@ __global__ void k_fill_background(int W, int H, const float* __restrict__ bg, fl
     out_invdepth[i] = 0.f;
 }
 
+// ---- Adam on the packed SH parameter [P,16,3] with the gradient rebuilt from its factors, dL/dSH[k][c] = basis_k(dir) * dcolor[c]:
+// k_adam_sh (gms_adam_sh_factored) and the fused update of k_preprocess_bwd (gms_train_frame with sh_adam) share these pieces,
+// so the two give bit-identical p, m and v.
+
+// torch.optim.Adam's constants: (1 - beta), lr / (1 - beta1^t), sqrt(1 - beta2^t) are formed in double on the host and rounded
+// once (torch: Python floats).  The DC coefficient uses lr_dc, the other 15 lr_rest.
+struct AdamShConst { float lr_dc, lr_rest, beta1, beta2, omb1, omb2, eps, bc2_sqrt; };
+
+static AdamShConst adam_sh_const(double lr_dc, double lr_rest, double beta1, double beta2, double eps, int step) {
+    AdamShConst c;
+    const double bc1 = 1.0 - pow(beta1, (double)step);
+    c.lr_dc = (float)(lr_dc / bc1); c.lr_rest = (float)(lr_rest / bc1);
+    c.beta1 = (float)beta1; c.beta2 = (float)beta2; c.eps = (float)eps;
+    c.omb1 = (float)(1.0 - beta1); c.omb2 = (float)(1.0 - beta2);
+    c.bc2_sqrt = (float)sqrt(1.0 - pow(beta2, (double)step));
+    return c;
+}
+
+// SH basis at normalize(xyz - campos) (same direction arithmetic as gms_sh_backward), zeros above degree D.
+__device__ __forceinline__ void sh_grad_basis(int D, float mx, float my, float mz, const float* cp, float B[16]) {
+    float dx = mx - __ldg(cp), dy = my - __ldg(cp + 1), dz = mz - __ldg(cp + 2);
+    const float len = GMS_SQRTP(dx * dx + dy * dy + dz * dz);
+    dx = GMS_DIVP(dx, len); dy = GMS_DIVP(dy, len); dz = GMS_DIVP(dz, len);
+#pragma unroll
+    for (int k = 0; k < 16; k++) B[k] = 0.f;
+    gms_sh_basis(D, dx, dy, dz, B);
+}
+
+// One float4 of a packed row (elements 4c .. 4c+3 of the 48) through the update.  The default uses the branch-free correctly-
+// rounded division / square root of gms_common.cuh (GMS_DIVN / GMS_SQRTN): the three slow-path branches per element of
+// `sqrtf(v) / bc + eps` and `m / denom` serialised the twelve MUFU chains of a float4 (stalled on fixed-latency dependencies,
+// not on memory).  Adam's divisors are normal numbers (bias correction; sqrt(v)/bc + eps >= eps); tiny / denormal second
+// moments are handled inside gms_sqrt_rn_normal; a denormal numerator m only loses bits below 1e-38.
+// Every multiply-add is spelled out: left to the compiler, whether `p - step * q` becomes one FFMA or FMUL + FADD depends on
+// the code around it, and the two kernels must round alike.  The explicit forms are the ones k_adam_sh was compiled to.
+template <bool IEEE_CALLS>
+__device__ __forceinline__ void adam_sh_update4(const AdamShConst& a, int c, const float gv[4], float pv[4], float mv[4], float vv[4]) {
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        const float step = (4 * c + k < 3) ? a.lr_dc : a.lr_rest;       // coefficient 0 = the DC term (f_dc), the rest f_rest
+        mv[k] = __fmaf_rn(a.beta1, mv[k], __fmul_rn(a.omb1, gv[k]));
+        vv[k] = __fmaf_rn(a.beta2, vv[k], __fmul_rn(__fmul_rn(a.omb2, gv[k]), gv[k]));
+        if (IEEE_CALLS) {       // A/B arm (option adam_sh_ieee=1): nvcc's own sqrtf and `/` with their slow-path branches
+            const float denom = __fadd_rn(sqrtf(vv[k]) / a.bc2_sqrt, a.eps);
+            pv[k] = __fmaf_rn(-step, mv[k] / denom, pv[k]);
+        } else {
+            const float denom = __fadd_rn(gms_div_rn_normal(gms_sqrt_rn_normal(vv[k]), a.bc2_sqrt), a.eps);
+            pv[k] = __fmaf_rn(-step, gms_div_rn_normal(mv[k], denom), pv[k]);
+        }
+    }
+}
+
+constexpr int GMS_SH_FSTRIDE = 19;     // floats per lane of the factor tile: 16 basis values + 3 colour gradients (odd: conflict-free)
+
+// The fused update of a warp's 32 rows, after the preprocess backward (every lane of the warp takes part).  tile: the rows
+// (p) at row stride GMS_SH_STRIDE_V, loaded for every in-bounds Gaussian.  f: the lane's factors, which k_adam_sh's phase A
+// would have multiplied out with one rank and scale 1 -- the basis and the clamp-masked colour gradient, or zeros when the
+// whole colour gradient is zero (culled / unblended / clamped).  The walk over p / m / v is k_adam_sh's phase B, with p from
+// the tile instead of memory and the gradient formed as the same single product basis_k * dcolor[c].
+template <bool IEEE_CALLS>
+__device__ __forceinline__ void sh_adam_warp(const AdamShConst& ac, float* p, float* m, float* v, int P, int i0, int lane,
+                                             const float* tile, const float* f) {
+    const size_t base4 = (size_t)i0 * GMS_SH_ROW4;
+    const float4* m4 = reinterpret_cast<const float4*>(m) + base4;
+    const float4* v4 = reinterpret_cast<const float4*>(v) + base4;
+    const int nrow = min(32, P - i0), n4 = GMS_SH_ROW4 * nrow;
+    constexpr int AHEAD = 2;
+    float4 Mb[AHEAD + 1], Vb[AHEAD + 1];
+#pragma unroll
+    for (int q = 0; q < AHEAD; q++) {
+        Mb[q] = Vb[q] = make_float4(0, 0, 0, 0);
+        if (q * 32 + lane < n4) { Mb[q] = m4[q * 32 + lane]; Vb[q] = v4[q * 32 + lane]; }
+    }
+    __syncwarp();
+    float4* po = reinterpret_cast<float4*>(p) + base4;
+    float4* mo = reinterpret_cast<float4*>(m) + base4;
+    float4* vo = reinterpret_cast<float4*>(v) + base4;
+#pragma unroll
+    for (int it = 0; it < GMS_SH_ROW4; it++) {
+        const int j = it * 32 + lane;
+        if (it + AHEAD < GMS_SH_ROW4) {
+            const int jn = j + AHEAD * 32, sl = (it + AHEAD) % (AHEAD + 1);
+            Mb[sl] = Vb[sl] = make_float4(0, 0, 0, 0);
+            if (jn < n4) { Mb[sl] = m4[jn]; Vb[sl] = v4[jn]; }
+        }
+        const float4 Mc = Mb[it % (AHEAD + 1)], Vc = Vb[it % (AHEAD + 1)];
+        if (j < n4) {
+            const int r = j / GMS_SH_ROW4, c = j - r * GMS_SH_ROW4;
+            const float4 Pc = *reinterpret_cast<const float4*>(tile + r * GMS_SH_STRIDE_V + 4 * c);
+            const float* fr = f + r * GMS_SH_FSTRIDE;
+            float gv[4];
+#pragma unroll
+            for (int k = 0; k < 4; k++) { const int e = 4 * c + k, kk = e / 3; gv[k] = fr[kk] * fr[16 + e - 3 * kk]; }
+            float pv[4] = {Pc.x, Pc.y, Pc.z, Pc.w}, mv[4] = {Mc.x, Mc.y, Mc.z, Mc.w}, vv[4] = {Vc.x, Vc.y, Vc.z, Vc.w};
+            adam_sh_update4<IEEE_CALLS>(ac, c, gv, pv, mv, vv);
+            po[j] = make_float4(pv[0], pv[1], pv[2], pv[3]);
+            mo[j] = make_float4(mv[0], mv[1], mv[2], mv[3]);
+            vo[j] = make_float4(vv[0], vv[1], vv[2], vv[3]);
+        }
+    }
+}
+
 struct PreBwdArgs {
     PreArgs f;
     const int* radii; const float* cov3D; const uint32_t* clamped; const float4* dgeom;
     float* dmeans3D; float* dmeans2D; float* dopac; float* dshs; float* dcolors_pre; float* dscales; float* drots; float* dcov_pre;
     float* dopac_raw;   // gms_train_frame: dL/d(opacity before the sigmoid) = dL/dopacity * y (1 - y) goes here instead of dopac
     float* dcol_sh;     // [P,3] clamp-masked dL/dcolour of SH-coloured Gaussians (factored SH gradient: dL/dSH[k][c] = basis_k(dir) * this[c]); with it dshs may be NULL
+    float* sh_p; float* sh_m; float* sh_v; AdamShConst sh_adam;    // ADAM: the SH parameter (= f.shs, updated in place) and its moments
 };
 
 // STAGED 0: per-lane global accesses.  1: SH rows and gradient rows through the warp's shared-memory tile, held in
@@ -479,10 +583,17 @@ struct PreBwdArgs {
 // odd row stride): no register copies of the two 48-float rows.
 // FACT: factored SH gradient -- the SH rows are read (their view-direction term feeds dL/dmean) but no gradient rows are
 // written; the clamp-masked colour gradient (12 B instead of 192 B per Gaussian) goes to b.dcol_sh (gms_adam_sh_factored).
-template <int STAGED, int MINB, bool FACT = false>
+// ADAM (with STAGED 1 and FACT; one camera per step): instead of handing the colour gradient to k_adam_sh, the kernel applies
+// the SH Adam step itself to the rows it already holds in its tile (sh_adam_warp), so p is not read twice and the exchange
+// slot is not needed (b.dcol_sh is then optional).  The tile holds every in-bounds row: culled Gaussians get an update with a
+// zero gradient.  p is the SH input itself (b.sh_p == f.shs): each warp reads its rows before it writes them, and no other
+// warp touches them, so the rows are loaded without the read-only cache.  ADAM_IEEE: the adam_sh_ieee arm of the update.
+template <int STAGED, int MINB, bool FACT = false, bool ADAM = false, bool ADAM_IEEE = false>
 __global__ void __launch_bounds__(128, MINB) k_preprocess_bwd(PreBwdArgs b) {
+    static_assert(!ADAM || (STAGED == 1 && FACT), "the fused SH Adam update works on the STAGED 1 tile of the factored path");
     constexpr int STRIDE = STAGED == 2 ? GMS_SH_STRIDE_S : GMS_SH_STRIDE_V;
     __shared__ __align__(16) float s_sh[STAGED ? 4 : 1][STAGED ? GMS_SH_TILE : 4];
+    __shared__ float s_f[ADAM ? 4 : 1][ADAM ? 32 * GMS_SH_FSTRIDE : 1];
     const PreArgs& a = b.f;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -490,8 +601,8 @@ __global__ void __launch_bounds__(128, MINB) k_preprocess_bwd(PreBwdArgs b) {
     const bool inb = i < a.P;
     const bool vis = inb && b.radii[i] > 0;
     if (STAGED) {       // (only launched with shs, dshs != NULL and M == 16)
-        const unsigned rows = __ballot_sync(0xffffffffu, vis);
-        if (rows) sh_tile_load<STRIDE>(a.shs, blockIdx.x * blockDim.x + warp * 32, rows, lane, s_sh[warp]);
+        const unsigned rows = __ballot_sync(0xffffffffu, ADAM ? inb : vis);
+        if (rows) sh_tile_load<STRIDE, !ADAM>(ADAM ? b.sh_p : a.shs, blockIdx.x * blockDim.x + warp * 32, rows, lane, s_sh[warp]);
     }
     GmsPreGradOut go;
     go.dmean3D[0] = go.dmean3D[1] = go.dmean3D[2] = 0.f;
@@ -570,7 +681,21 @@ __global__ void __launch_bounds__(128, MINB) k_preprocess_bwd(PreBwdArgs b) {
         }
     }
     if (FACT) {
-        if (inb) { b.dcol_sh[3 * i] = dcol[0]; b.dcol_sh[3 * i + 1] = dcol[1]; b.dcol_sh[3 * i + 2] = dcol[2]; }
+        if (inb && (!ADAM || b.dcol_sh)) { b.dcol_sh[3 * i] = dcol[0]; b.dcol_sh[3 * i + 1] = dcol[1]; b.dcol_sh[3 * i + 2] = dcol[2]; }
+    }
+    if (ADAM) {
+        float* f = s_f[warp] + lane * GMS_SH_FSTRIDE;
+        if (inb && !(dcol[0] == 0.f && dcol[1] == 0.f && dcol[2] == 0.f)) {
+            float B[16];
+            sh_grad_basis(a.D, a.means[3 * i], a.means[3 * i + 1], a.means[3 * i + 2], a.campos, B);
+#pragma unroll
+            for (int k = 0; k < 16; k++) f[k] = B[k];
+            f[16] = dcol[0]; f[17] = dcol[1]; f[18] = dcol[2];
+        } else {
+#pragma unroll
+            for (int k = 0; k < GMS_SH_FSTRIDE; k++) f[k] = 0.f;
+        }
+        sh_adam_warp<ADAM_IEEE>(b.sh_adam, b.sh_p, b.sh_m, b.sh_v, a.P, blockIdx.x * blockDim.x + warp * 32, lane, s_sh[warp], s_f[warp]);
     }
     if (STAGED && FACT) { if (!inb) return; }
     else if (STAGED) {       // gradient rows -> the warp's tile (zeros for culled Gaussians) -> coalesced 128-bit stores
@@ -839,14 +964,10 @@ struct AdamShArgs {
     int P, D, R; long long slot;     // slot = floats between the ranks' exchange slots ([3P colour gradients | 3 campos | pad])
     const float* xyz; const float* xbuf;
     float* p; float* m; float* v;
-    float scale, lr_dc, lr_rest, beta1, beta2, omb1, omb2, eps, bc2_sqrt;
+    float scale;
+    AdamShConst c;
 };
 
-// k_adam_sh's update uses the branch-free correctly-rounded division / square root of gms_common.cuh (GMS_DIVN / GMS_SQRTN): the
-// three slow-path branches per element of `sqrtf(v) / bc + eps` and `m / denom` serialised the twelve MUFU chains of a float4
-// (stalled on fixed-latency dependencies, not on memory).  Adam's divisors are normal numbers (bias correction;
-// sqrt(v)/bc + eps >= eps); tiny / denormal second moments are handled inside gms_sqrt_rn_normal; a denormal numerator m only
-// loses bits below 1e-38.
 template <bool IEEE_CALLS>
 __global__ void __launch_bounds__(128, 6) k_adam_sh(AdamShArgs a) {
     // A warp handles 32 Gaussians.  Phase A: lane i rebuilds Gaussian i's 48 gradient values from the R colour gradients
@@ -883,14 +1004,8 @@ __global__ void __launch_bounds__(128, 6) k_adam_sh(AdamShArgs a) {
                 const float g0 = n0 * a.scale, g1 = n1 * a.scale, g2 = n2 * a.scale;
                 if (r + 1 < a.R) { const float* nx = a.xbuf + (size_t)(r + 1) * a.slot + 3 * i; n0 = nx[0]; n1 = nx[1]; n2 = nx[2]; }
                 if (g0 == 0.f && g1 == 0.f && g2 == 0.f) continue;      // culled / unblended / clamped at that camera
-                const float* cp = a.xbuf + (size_t)r * a.slot + 3 * (size_t)a.P;
-                float dx = mx - __ldg(cp), dy = my - __ldg(cp + 1), dz = mz - __ldg(cp + 2);
-                const float len = GMS_SQRTP(dx * dx + dy * dy + dz * dz);     // same direction arithmetic as gms_sh_backward
-                dx = GMS_DIVP(dx, len); dy = GMS_DIVP(dy, len); dz = GMS_DIVP(dz, len);
                 float B[16];
-#pragma unroll
-                for (int k = 0; k < 16; k++) B[k] = 0.f;
-                gms_sh_basis(a.D, dx, dy, dz, B);
+                sh_grad_basis(a.D, mx, my, mz, a.xbuf + (size_t)r * a.slot + 3 * (size_t)a.P, B);
                 if (first) {
 #pragma unroll
                     for (int k = 0; k < 16; k++) { row[3 * k] = B[k] * g0; row[3 * k + 1] = B[k] * g1; row[3 * k + 2] = B[k] * g2; }
@@ -924,19 +1039,7 @@ __global__ void __launch_bounds__(128, 6) k_adam_sh(AdamShArgs a) {
             const float* gq = tile + r * STRIDE + 4 * c;
             const float gv[4] = {gq[0], gq[1], gq[2], gq[3]};
             float pv[4] = {Pc.x, Pc.y, Pc.z, Pc.w}, mv[4] = {Mc.x, Mc.y, Mc.z, Mc.w}, vv[4] = {Vc.x, Vc.y, Vc.z, Vc.w};
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                const float step = (4 * c + k < 3) ? a.lr_dc : a.lr_rest;       // coefficient 0 = the DC term (f_dc), the rest f_rest
-                mv[k] = a.beta1 * mv[k] + a.omb1 * gv[k];
-                vv[k] = a.beta2 * vv[k] + a.omb2 * gv[k] * gv[k];
-                if (IEEE_CALLS) {       // A/B arm (option adam_sh_ieee=1): nvcc's own sqrtf and `/` with their slow-path branches
-                    const float denom = sqrtf(vv[k]) / a.bc2_sqrt + a.eps;
-                    pv[k] = pv[k] - step * (mv[k] / denom);
-                } else {
-                    const float denom = gms_div_rn_normal(gms_sqrt_rn_normal(vv[k]), a.bc2_sqrt) + a.eps;
-                    pv[k] = pv[k] - step * gms_div_rn_normal(mv[k], denom);
-                }
-            }
+            adam_sh_update4<IEEE_CALLS>(a.c, c, gv, pv, mv, vv);
             po[j] = make_float4(pv[0], pv[1], pv[2], pv[3]);
             mo[j] = make_float4(mv[0], mv[1], mv[2], mv[3]);
             vo[j] = make_float4(vv[0], vv[1], vv[2], vv[3]);
@@ -1064,11 +1167,7 @@ int gms_adam_sh_factored(const gms_adam_sh_args* a, void* cuda_stream) {
     AdamShArgs k;
     k.P = a->P; k.D = a->sh_degree; k.R = a->R; k.slot = a->slot_floats; k.xyz = a->xyz; k.xbuf = a->exchange;
     k.p = a->p; k.m = a->m; k.v = a->v; k.scale = a->grad_scale;
-    const double bc1 = 1.0 - pow(a->beta1, (double)a->step);
-    k.lr_dc = (float)(a->lr_dc / bc1); k.lr_rest = (float)(a->lr_rest / bc1);
-    k.beta1 = (float)a->beta1; k.beta2 = (float)a->beta2; k.eps = (float)a->eps;
-    k.omb1 = (float)(1.0 - a->beta1); k.omb2 = (float)(1.0 - a->beta2);
-    k.bc2_sqrt = (float)sqrt(1.0 - pow(a->beta2, (double)a->step));
+    k.c = adam_sh_const(a->lr_dc, a->lr_rest, a->beta1, a->beta2, a->eps, a->step);
     span_begin(K_ADAM, st);
     if (g_opt_adam_sh_ieee) k_adam_sh<true><<<(a->P + 127) / 128, 128, 0, st>>>(k);
     else k_adam_sh<false><<<(a->P + 127) / 128, 128, 0, st>>>(k);
@@ -1409,7 +1508,7 @@ int gms_rasterize_forward_nosync(const gms_raster_settings* s, const gms_raster_
 
 static int raster_backward_impl(const gms_raster_settings* s, const gms_raster_inputs* in, const int32_t* radii,
                                 const gms_raster_saved* saved, const float* dL_dout_color, const float* dL_dout_invdepth,
-                                const gms_raster_grads* gr, void* cuda_stream, float* dopac_raw) {
+                                const gms_raster_grads* gr, void* cuda_stream, float* dopac_raw, const gms_sh_adam* sh_adam) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (!s || !saved || !gr || !dL_dout_color || !in) return set_err(GMS_E_ARG, "null argument%s%s");
     if (in->P == 0) return GMS_OK;
@@ -1465,7 +1564,20 @@ static int raster_backward_impl(const gms_raster_settings* s, const gms_raster_i
     b.dcol_sh = in->shs ? gr->dL_dcolors_sh : nullptr;
     b.dopac_raw = dopac_raw;
     span_begin(K_PRE_BWD, st);
-    if (b.dcol_sh) {        // factored SH gradient
+    if (sh_adam) {          // factored SH gradient applied in place: the SH Adam step of the frame (gms_sh_adam)
+        if (b.f.M != 16 || !b.f.shs) return set_err(GMS_E_ARG, "sh_adam needs shs with 16 coefficients%s%s");
+        b.dshs = nullptr;
+        b.sh_p = const_cast<float*>(b.f.shs); b.sh_m = sh_adam->m; b.sh_v = sh_adam->v;
+        b.sh_adam = adam_sh_const(sh_adam->lr_dc, sh_adam->lr_rest, sh_adam->beta1, sh_adam->beta2, sh_adam->eps, sh_adam->step);
+        const int grid = (P + 127) / 128;
+        if (g_opt_pre_bwd_minb >= 4) {
+            if (g_opt_adam_sh_ieee) k_preprocess_bwd<1, 4, true, true, true><<<grid, 128, 0, st>>>(b);
+            else k_preprocess_bwd<1, 4, true, true><<<grid, 128, 0, st>>>(b);
+        } else {
+            if (g_opt_adam_sh_ieee) k_preprocess_bwd<1, 1, true, true, true><<<grid, 128, 0, st>>>(b);
+            else k_preprocess_bwd<1, 1, true, true><<<grid, 128, 0, st>>>(b);
+        }
+    } else if (b.dcol_sh) {        // factored SH gradient
         if (b.f.M != 16 || !b.f.shs) return set_err(GMS_E_ARG, "dL_dcolors_sh needs shs with 16 coefficients%s%s");
         b.dshs = nullptr;
         if (g_opt_pre_bwd_minb >= 4) k_preprocess_bwd<1, 4, true><<<(P + 127) / 128, 128, 0, st>>>(b);
@@ -1488,7 +1600,7 @@ static int raster_backward_impl(const gms_raster_settings* s, const gms_raster_i
 int gms_rasterize_backward(const gms_raster_settings* s, const gms_raster_inputs* in, const int32_t* radii,
                            const gms_raster_saved* saved, const float* dL_dout_color, const float* dL_dout_invdepth,
                            const gms_raster_grads* gr, void* cuda_stream) {
-    return raster_backward_impl(s, in, radii, saved, dL_dout_color, dL_dout_invdepth, gr, cuda_stream, nullptr);
+    return raster_backward_impl(s, in, radii, saved, dL_dout_color, dL_dout_invdepth, gr, cuda_stream, nullptr, nullptr);
 }
 
 int gms_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present, void* cuda_stream) {
@@ -1601,8 +1713,10 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     if (!a || !alloc || !a->workspace || !a->loss || !a->gt) return set_err(GMS_E_ARG, "gms_train_frame: null argument%s%s");
     if (!a->vertices || !a->faces || !a->alpha_raw || !a->scale_raw || !a->features || !a->opacity_raw)
         return set_err(GMS_E_ARG, "gms_train_frame: model tensors required%s%s");
-    if (!a->d_vertices || !a->d_alpha_raw || !a->d_scale_raw || (!a->d_features && !a->d_color_sh) || !a->d_opacity_raw)
+    if (!a->d_vertices || !a->d_alpha_raw || !a->d_scale_raw || (!a->d_features && !a->d_color_sh && !a->sh_adam) || !a->d_opacity_raw)
         return set_err(GMS_E_ARG, "gms_train_frame: gradient tensors required%s%s");
+    if (a->sh_adam && (!a->sh_adam->m || !a->sh_adam->v || a->sh_adam->step < 1 || a->settings.sh_degree < 0 || a->settings.sh_degree > 3))
+        return set_err(GMS_E_ARG, "gms_train_frame: bad sh_adam%s%s");
     const int P = a->F * a->K, W = a->settings.image_width, H = a->settings.image_height;
     if (a->workspace_bytes < gms_frame_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_train_frame: workspace too small%s%s");
     FrameLayout FL = frame_layout(aligned_base_c(a->workspace), P, W, H);
@@ -1637,9 +1751,12 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     if (a->d_color_sh) {    // factored SH gradient: colour gradient + this camera's centre (right behind it) for gms_adam_sh_factored
         gr.dL_dcolors_sh = a->d_color_sh;
         GMS_CUDA(cudaMemcpyAsync(a->d_color_sh + 3 * (size_t)P, a->settings.campos, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    } else gr.dL_dshs = a->d_features;
+    } else if (!a->sh_adam) gr.dL_dshs = a->d_features;
     gr.dL_dscales = FL.d_scales; gr.dL_drotations = FL.d_rots;
-    if ((rc = raster_backward_impl(&a->settings, &in, FL.radii, &saved, FL.dimage, nullptr, &gr, cuda_stream, a->d_opacity_raw))) return rc;
+    // sh_adam: the preprocess backward updates `features` in place; it is the frame's last reader of them (the expansion
+    // backward below does not read them)
+    if ((rc = raster_backward_impl(&a->settings, &in, FL.radii, &saved, FL.dimage, nullptr, &gr, cuda_stream, a->d_opacity_raw, a->sh_adam)))
+        return rc;
     if (a->event_sh_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_sh_ready), st));
     // expansion backward (vertex gradients are accumulated with atomics: the caller keeps d_vertices zeroed)
     gms_expand_grads eg;

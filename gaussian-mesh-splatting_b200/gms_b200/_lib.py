@@ -100,6 +100,12 @@ class AdamArgs(C.Structure):
                 ("eps", C.c_double), ("step", C.c_int32), ("zero_grad", C.c_int32), ("zero_end", C.c_int64)]
 
 
+class ShAdam(C.Structure):
+    """struct gms_sh_adam"""
+    _fields_ = [("m", C.c_void_p), ("v", C.c_void_p), ("lr_dc", C.c_double), ("lr_rest", C.c_double), ("beta1", C.c_double),
+                ("beta2", C.c_double), ("eps", C.c_double), ("step", C.c_int32)]
+
+
 class FrameArgs(C.Structure):
     _fields_ = [("V", C.c_int32), ("F", C.c_int32), ("K", C.c_int32), ("M", C.c_int32),
                 ("vertices", C.c_void_p), ("faces", C.c_void_p), ("alpha_raw", C.c_void_p), ("scale_raw", C.c_void_p),
@@ -109,7 +115,7 @@ class FrameArgs(C.Structure):
                 ("settings", RasterSettings), ("gt", C.c_void_p), ("lambda_dssim", C.c_float), ("loss", C.c_void_p),
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)),
                 ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p), ("d_color_sh", C.c_void_p),
-                ("event_sh_ready", C.c_void_p), ("event_loss_ready", C.c_void_p)]
+                ("event_sh_ready", C.c_void_p), ("event_loss_ready", C.c_void_p), ("sh_adam", C.POINTER(ShAdam))]
 
 
 class FrameView(C.Structure):

@@ -154,10 +154,29 @@ class FlatAdam:
         self._adam_sh(sh)
         if reduced is not None:
             torch.cuda.current_stream(self.p.device).wait_event(reduced)
-        d = self._adam_desc(prefix, 0, self.p, self.g, 1 if zero_end is None else 2, 0 if zero_end is None else zero_end)
+        self.step_rest(zero_end)
+
+    def step_rest(self, zero_end=None):
+        """Adam on every group but the SH group (one launch, gradient zeroed as in step())."""
+        d = self._adam_desc(self.ends[-2], 0, self.p, self.g, 1 if zero_end is None else 2, 0 if zero_end is None else zero_end)
         for k in ("seg_end", "lr0", "lr1", "inner", "period"):
             d[k] = d[k][:-1]
         self._kernel(d)
+
+    def begin_fused_sh_step(self) -> "_lib.ShAdam":
+        """Single-GPU factored optimizer: the next frame applies the SH group's Adam step itself, inside its preprocess backward
+        (gms_train_frame with this gms_sh_adam descriptor: the parameter rows are read once and no colour gradient goes
+        through memory).  Advances the step count; step_rest() then updates the other groups."""
+        if not self.sh_factored or self.world != 1:
+            raise ValueError("the fused SH step needs a single-GPU FlatAdam built with sh_factored=True")
+        self.t += 1
+        gsh = self.groups[-1]
+        off = self.ends[-2]
+        a = _lib.ShAdam()
+        a.m, a.v = self.m[off:].data_ptr(), self.v[off:].data_ptr()
+        a.lr_dc, a.lr_rest = float(gsh["lr0"]), float(gsh["lr1"])
+        a.beta1, a.beta2, a.eps, a.step = self.betas[0], self.betas[1], self.eps, self.t
+        return a
 
     def _adam_sh(self, sh):
         ex = sh["exchange"]

@@ -183,7 +183,9 @@ class NativeFrame:
         _lib.check(_lib.lib().gms_frame_views(self.ws.data_ptr(), self.model._scale.shape[0], self.W, self.H, C.byref(v)), "gms_frame_views")
         return dict(xyz=v.xyz, exchange=self.exchange, degree=self.model.active_sh_degree, event=self.ev_sh)
 
-    def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, factored: bool = False) -> torch.Tensor:
+    def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, factored: bool = False, sh_adam=None) -> torch.Tensor:
+        """sh_adam (FlatAdam.begin_fused_sh_step()): the frame also applies the SH parameters' Adam step, and writes no SH
+        gradient (unless `factored` asks for the colour gradient as well)."""
         import ctypes as C
         from . import _lib
         for t, what in ((gt, "gt"), (bg, "bg"), (cam.world_view_transform, "camera matrices"), (cam.full_proj_transform, "camera matrices"),
@@ -210,6 +212,9 @@ class NativeFrame:
                     self.ev_sh = torch.cuda.Event()
                     self.ev_sh.record(torch.cuda.current_stream(self.dev))      # (creates the underlying cudaEvent_t)
                 a.event_sh_ready = self.ev_sh.cuda_event
+        if sh_adam is not None:
+            a.d_features = None
+            a.sh_adam = C.pointer(sh_adam)
         if self.ev_loss is None:
             self.ev_loss = torch.cuda.Event()
             self.ev_loss.record(torch.cuda.current_stream(self.dev))            # (creates the underlying cudaEvent_t)
@@ -304,14 +309,20 @@ class MeshTrainer:
                 self._frame = NativeFrame(self.model, cam.image_width, cam.image_height, self.lambda_dssim, sync_free=self.sync_free,
                                           world=self.world, rank=self.rank)
             factored = self.sh_factored and self.optimizer_step      # without an optimizer step the full gradient is materialised
-            loss = self._frame.run(cam, gt, self.bg, factored=factored)
+            # one GPU: the frame applies the SH Adam step itself (no colour-gradient slot, no second read of the SH rows);
+            # data parallel: the colour gradients are exchanged first and k_adam_sh consumes them
+            fused = factored and self.world == 1
+            sh_adam = self.opt.begin_fused_sh_step() if fused else None
+            loss = self._frame.run(cam, gt, self.bg, factored=factored and not fused, sh_adam=sh_adam)
             from . import rasterizer as _r
             _r.last_num_rendered = self._frame.last_num_rendered
             if loss_host is not None:
                 self._frame.read_loss_async(loss_host, loss_ready)
             self._all_reduce()
             # gms_train_frame overwrites every gradient except the atomically accumulated vertex segment (group 0)
-            if self.optimizer_step:
+            if fused:
+                self.opt.step_rest(zero_end=self.opt.ends[0])
+            elif self.optimizer_step:
                 self.opt.step(zero_end=self.opt.ends[0], sh=self._frame.sh_factors() if factored else None)
             else:
                 self.opt.zero_grad_partial(self.opt.ends[0])

@@ -290,6 +290,16 @@ typedef struct gms_adam_args {
 } gms_adam_args;
 int gms_adam_step(const gms_adam_args* a, void* cuda_stream);
 
+/* The Adam step gms_train_frame can apply to the packed SH parameter inside its preprocess backward (gms_frame_args.sh_adam):
+ * bit for bit what gms_adam_sh_factored does with one slot (R = 1, grad_scale 1) holding this frame's d_color_sh, without
+ * the slot's round trip through memory or a second read of the parameter.  One camera per step only (data parallel: exchange
+ * the colour gradients through d_color_sh instead). */
+typedef struct gms_sh_adam {
+    float* m; float* v;         /* [P,16,3] Adam moments of `features` */
+    double lr_dc, lr_rest, beta1, beta2, eps;
+    int32_t step;               /* 1-based step count (bias correction) */
+} gms_sh_adam;
+
 /* One gs_mesh training frame in ONE call (train.py:100-108 + :154-157 of the reference: render + loss + backward +
  * re-expansion), all launches on `cuda_stream`, no Python / autograd in between:
  *   expansion fwd (activated scales/rotations) -> sigmoid(opacity) -> rasterizer fwd -> L1+SSIM -> rasterizer bwd ->
@@ -321,6 +331,8 @@ typedef struct gms_frame_args {
     void* event_loss_ready;     /* optional cudaEvent_t recorded right after the loss kernels (about 40 % into the frame): a caller that
                                    logs the loss every step copies it to the host from another stream and can queue the next
                                    frame while this one's backward pass still runs */
+    const gms_sh_adam* sh_adam; /* optional: the frame also takes the Adam step of `features` (updated in place, M = 16) with
+                                   this frame's SH gradient; then d_features and d_color_sh may be NULL */
 } gms_frame_args;
 size_t gms_frame_workspace_bytes(int32_t P, int32_t W, int32_t H);
 /* Device pointers into a frame workspace (valid after gms_train_frame): this step's expansion outputs and images. */

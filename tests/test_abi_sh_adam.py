@@ -1,0 +1,23 @@
+"""CPU-only: the ctypes mirror of gms_sh_adam (the descriptor of the SH Adam step gms_train_frame applies in place) has the
+size and field offsets the C compiler gives the header's struct."""
+import ctypes
+import os
+import subprocess
+
+from gms_b200 import _lib
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def test_sh_adam_layout_matches_the_ctypes_mirror(tmp_path):
+    cls = _lib.ShAdam
+    body = '    printf("size %zu\\n", sizeof(gms_sh_adam));\n'
+    body += "".join(f'    printf("{f[0]} %zu\\n", offsetof(gms_sh_adam, {f[0]}));\n' for f in cls._fields_)
+    src = tmp_path / "sh_adam.c"
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "gms_b200.h"\nint main(void) {\n' + body + "    return 0;\n}\n")
+    exe = tmp_path / "sh_adam"
+    subprocess.check_call(["gcc", "-std=c99", "-Wall", "-Wextra", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
+    out = dict(l.split() for l in subprocess.check_output([str(exe)], text=True).strip().split("\n"))
+    assert int(out["size"]) == ctypes.sizeof(cls)
+    for f in cls._fields_:
+        assert int(out[f[0]]) == getattr(cls, f[0]).offset, f[0]
