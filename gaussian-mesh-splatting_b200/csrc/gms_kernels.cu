@@ -39,8 +39,9 @@ static int g_opt_pre_bwd_minb = 4;  // k_preprocess_bwd min CTAs/SM (1: 2.67 ms,
 static int g_opt_expand_staged = 1; // expansion kernels, per-Gaussian streams staged through shared memory (coalesced): bit 0 forward
                                     // (0: 2.74 ms), bit 1 backward (3: 2.67 ms, off)
 static int g_opt_sort = 0;         // depth sort (and the emit + sort path's tile sort): 0 cub::DeviceRadixSort, 1 hand-written radix sort
-                                   //    with device-side N (gms_sort.cuh; bit-identical order through the synchronising entry points; renders
-                                   //    empty tile lists in the sync-free native frame -- open defect, DESIGN.md 3.7)
+                                   //    with device-side N clamped to the capacity (gms_sort.cuh; bit-identical order through the
+                                   //    synchronising entry points and the sync-free frame; 2.67-2.70 ms against 2.40-2.42 ms
+                                   //    for the default with the current build, DESIGN.md 3.7)
 static int g_opt_bin = 0;          // tile binning: 0 emit in depth order + ONE stable radix sort on the tile bits (default),
                                    //               1 cooperative counting kernel without any sort over the duplicates (gms_binning.cuh;
                                    //                 2.92 ms -- kept selectable, parity-tested)
@@ -218,9 +219,11 @@ static BinLayout bin_layout(void* base, int64_t N) {
     L.vals_in = carve<uint32_t>(p, Nn);
     L.keys_out = carve<uint32_t>(p, Nn);
     L.vals_out = carve<uint32_t>(p, Nn);
+    // cub's temporary storage grows with the number of digit passes: the 32-bit-key sort is sized for all 32 key bits, since
+    // grids above 65535 tiles sort on 17 or more (sized for 16, the sort rejected its storage at 4096x4096)
     size_t a = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, a, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr,
-                                    (uint32_t*)nullptr, (int)Nn, 0, 16);
+                                    (uint32_t*)nullptr, (int)Nn, 0, 32);
     size_t a16 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, a16, (uint16_t*)nullptr, (uint16_t*)nullptr, (uint32_t*)nullptr,
                                     (uint32_t*)nullptr, (int)Nn, 0, 16);
@@ -1441,7 +1444,11 @@ static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_in
         const bool k16 = !g_opt_sort && g_opt_key16 && T <= 65535;
         if (k16) saved->flags |= 4;
         const uint32_t cap32 = (uint32_t)(cap > 0xFFFFFFFFll ? 0xFFFFFFFFll : cap);
-        if (N < 0 && !g_opt_sort) GMS_CUDA(cudaMemsetAsync(ek, 0xFF, (k16 ? sizeof(uint16_t) : sizeof(uint32_t)) * (size_t)cap, st));     // sentinel keys
+        // Sync-free call: sentinel keys behind the N emitted ones, written BEFORE the emit.  cub sorts the whole capacity, so
+        // they go into its input (ek).  The hand-written sort moves only the N device-side items and leaves the tail of every
+        // buffer as it was, so they go into its final output, keys_out -- which is also the emit target when the sort takes
+        // an even number of passes, so nothing may write keys_out between the emit and the sort.
+        if (N < 0) GMS_CUDA(cudaMemsetAsync(g_opt_sort ? BL.keys_out : ek, 0xFF, (k16 ? sizeof(uint16_t) : sizeof(uint32_t)) * (size_t)cap, st));
         span_begin(K_EMIT, st);
         if (k16) k_emit_dups<uint16_t><<<(P + 255) / 256, 256, 0, st>>>(P, gx, order, GL.offs, GL.rect, reinterpret_cast<uint16_t*>(ek), ev, g_opt_warp_emit, cap32);
         else k_emit_dups<uint32_t><<<(P + 255) / 256, 256, 0, st>>>(P, gx, order, GL.offs, GL.rect, ek, ev, g_opt_warp_emit, cap32);
@@ -1452,7 +1459,6 @@ static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_in
         if (g_opt_sort) {
             uint32_t* k0 = emit_into_out ? BL.keys_in : BL.keys_out; uint32_t* v0 = emit_into_out ? BL.vals_in : BL.vals_out;
             uint32_t* k1 = emit_into_out ? BL.keys_out : BL.keys_in; uint32_t* v1 = emit_into_out ? BL.vals_out : BL.vals_in;
-            if (N < 0) GMS_CUDA(cudaMemsetAsync(BL.keys_out, 0xFF, sizeof(uint32_t) * (size_t)cap, st));   // (device-N sort leaves the tail untouched)
             const int res = gms_radix_sort_pairs(ek, ev, k0, v0, k1, v1, GL.offs + (P - 1), cap, tbits, BL.sort_temp, st, &g_launches);
             if (res < 0 || (res ? k1 : k0) != BL.keys_out) return set_err(GMS_E_CUDA, "radix sort (tiles) failed%s%s");
         } else if (k16) {

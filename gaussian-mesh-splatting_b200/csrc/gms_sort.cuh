@@ -1,7 +1,7 @@
 // gms_sort.cuh -- hand-written stable LSD radix sort of (u32 key, u32 value) pairs for the tile binning, sm_90a.
 //
 // Replaces [upstream rasterizer_impl.cu: cub::DeviceRadixSort::SortPairs] -- and, unlike a library sort, takes the
-// number of items from DEVICE memory (grid sized for a capacity, surplus CTAs exit), which is what a sync-free /
+// number of items from DEVICE memory (grid sized for a capacity, the count clamped to it, surplus CTAs exit), which is what a sync-free /
 // graph-captured frame needs.  Two uses per frame (DESIGN.md section 3.3):
 //   * the P Gaussians by depth bits (4 passes of 8 bits; pass 1 generates value = index on the fly),
 //   * the N duplicates by tile id   (ceil(log2 T) = 13 bits at 1080p: one 8-bit and one 5-bit pass).
@@ -26,11 +26,11 @@
 #define GMS_RS_RADIX 256
 
 __global__ void __launch_bounds__(GMS_RS_THREADS)
-k_rs_hist(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ d_n, int shift, uint32_t mask, int ncta,
+k_rs_hist(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ d_n, uint32_t capacity, int shift, uint32_t mask, int ncta,
           uint32_t* __restrict__ hist /* [RADIX][ncta] */, uint32_t* __restrict__ tickets /* [4], zeroed by the first pass */) {
     __shared__ uint32_t s_h[GMS_RS_RADIX];
     if (blockIdx.x == 0 && threadIdx.x < 4 && shift == 0) tickets[threadIdx.x] = 0;   // one ticket per pass, reset by the first pass
-    const uint32_t n = *d_n;
+    const uint32_t n = min(*d_n, capacity);
     const uint32_t base = blockIdx.x * GMS_RS_TILE;
     const int lane = threadIdx.x & 31;
     s_h[threadIdx.x] = 0;
@@ -107,12 +107,12 @@ __global__ void __launch_bounds__(256) k_rs_scan(uint32_t* __restrict__ hist, in
 
 __global__ void __launch_bounds__(GMS_RS_THREADS, 3)
 k_rs_scatter(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ vals_in /* NULL: value = index */,
-             const uint32_t* __restrict__ d_n, int shift, uint32_t mask, int ncta, const uint32_t* __restrict__ hist,
+             const uint32_t* __restrict__ d_n, uint32_t capacity, int shift, uint32_t mask, int ncta, const uint32_t* __restrict__ hist,
              const uint32_t* __restrict__ bases, uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out,
              uint32_t* __restrict__ hist_next /* NULL on the last pass */, int next_shift, uint32_t next_mask) {
     __shared__ uint32_t s_cnt[8][GMS_RS_RADIX];     // per-warp running digit counts, then CTA-local warp offsets
     __shared__ uint32_t s_gbase[GMS_RS_RADIX];      // global offset of this CTA's first item of each digit
-    const uint32_t n = *d_n;
+    const uint32_t n = min(*d_n, capacity);
     const uint32_t cta_base = blockIdx.x * GMS_RS_TILE;
     if (cta_base >= n) return;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -179,14 +179,17 @@ static inline size_t gms_sort_temp_bytes(int64_t capacity) {
     return (2 * GMS_RS_RADIX * ncta + 2 * GMS_RS_RADIX + 64) * sizeof(uint32_t) + 512;
 }
 
-// Sorts `*d_n` (<= capacity) pairs by key bits [0, nbits).  Ping-pongs between (k0,v0) and (k1,v1); the first pass reads
-// (keys_src, vals_src) where vals_src may be NULL (value = index).  Returns which buffer holds
-// the result (0 or 1), or -1 on launch failure.
+// Sorts min(*d_n, capacity) pairs by key bits [0, nbits).  The clamp keeps an overflowed sync-free frame (device N above
+// the capacity its buffers were sized for) inside those buffers; such a frame renders the background anyway.  Only the
+// first min(*d_n, capacity) entries of any buffer are written.  Ping-pongs between (k0,v0) and (k1,v1); the first pass reads
+// (keys_src, vals_src) where vals_src may be NULL (value = index).  Returns which buffer holds the result (0 or 1), or -1
+// on launch failure.
 static int gms_radix_sort_pairs(const uint32_t* keys_src, const uint32_t* vals_src, uint32_t* k0, uint32_t* v0, uint32_t* k1,
                                 uint32_t* v1, const uint32_t* d_n, int64_t capacity, int nbits, void* temp, cudaStream_t st,
                                 int64_t* launches) {
     const int ncta = (int)((capacity + GMS_RS_TILE - 1) / GMS_RS_TILE);
     if (ncta <= 0) return 0;
+    const uint32_t cap32 = (uint32_t)(capacity > 0xFFFFFFFFll ? 0xFFFFFFFFll : capacity);
     uint32_t* histA = reinterpret_cast<uint32_t*>(temp);
     uint32_t* histB = histA + (size_t)GMS_RS_RADIX * (ncta + 1);
     uint32_t* totals = histB + (size_t)GMS_RS_RADIX * (ncta + 1);
@@ -200,9 +203,9 @@ static int gms_radix_sort_pairs(const uint32_t* keys_src, const uint32_t* vals_s
         uint32_t* ko = dst ? k1 : k0; uint32_t* vo = dst ? v1 : v0;
         // hist_next stays NULL: the digits of each pass are counted by this separate shared-memory histogram pass, not inside
         // the previous pass's scatter with global atomics.
-        k_rs_hist<<<ncta, GMS_RS_THREADS, 0, st>>>(kin, d_n, shift, mask, ncta, histA, tickets);
+        k_rs_hist<<<ncta, GMS_RS_THREADS, 0, st>>>(kin, d_n, cap32, shift, mask, ncta, histA, tickets);
         k_rs_scan<<<GMS_RS_RADIX, 256, 0, st>>>(histA, ncta, totals, bases, tickets + pass, nullptr);
-        k_rs_scatter<<<ncta, GMS_RS_THREADS, 0, st>>>(kin, vin, d_n, shift, mask, ncta, histA, bases, ko, vo, nullptr, 0, 0u);
+        k_rs_scatter<<<ncta, GMS_RS_THREADS, 0, st>>>(kin, vin, d_n, cap32, shift, mask, ncta, histA, bases, ko, vo, nullptr, 0, 0u);
         if (launches) *launches += 3;
         if (cudaGetLastError() != cudaSuccess) return -1;
         kin = ko; vin = vo;

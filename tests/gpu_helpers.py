@@ -4,6 +4,7 @@ import torch
 
 import diff_gaussian_rasterization as dgr
 from gms_b200 import rasterizer
+from oracle import expansion as oexp
 from oracle import raster
 
 
@@ -58,6 +59,37 @@ def run_oracle(S, inputs, dL_dcolor=None, dL_dinv=None):
     return st, g
 
 
+# gradients of the raw mesh-Gaussian parameters (oracle_chain) against the oracle, as max err / max |ref|; 2e-4 for the others
+GRAD_TOL = {"vertices": 5e-3, "_scale": 5e-3, "_alpha": 1e-3}     # through the near-singular 2D covariance (DESIGN.md 2.2)
+
+
+def oracle_chain(p, S, dC, gpu, triangles=None):
+    """Oracle image and gradients of sum(image * dC) w.r.t. the raw mesh-Gaussian parameters.  `gpu` = the (means3D,
+    scales, rotations) the GPU run handed to the rasterizer: they must agree with the oracle's expansion to fp32 rounding
+    and are what the oracle rasterizes (so that integer outputs can be compared bit for bit); the gradient chain runs
+    through the oracle's own expansion graph."""
+    tv, ta, ts = (x.clone().requires_grad_(True) for x in (p.vertices, p._alpha, p._scale))
+    if triangles is None:
+        xyz, sl, rr, _, _ = oexp.expand(tv, p.faces, ta, ts)
+    else:
+        alpha, _, _ = oexp.update_alpha(ta, tv, p.faces)
+        xyz = torch.matmul(alpha, triangles).reshape(-1, 3)
+        sl, rr = oexp.prepare_scaling_rot(triangles, ts, ta.shape[1])
+    top = p._opacity.clone().requires_grad_(True)
+    sc, rot, op, fe = oexp.activate(sl, rr, top, p._features_dc, p._features_rest)
+    gx, gs, gr = (t.detach().cpu() for t in gpu)
+    assert float((gx - xyz.detach()).abs().max()) <= 2e-6 and float((gr - rot.detach()).abs().max()) <= 4e-6
+    assert float(((gs - sc.detach()).abs() / sc.detach()).max()) <= 1e-5
+    st = raster.forward(S, gx, op.detach(), shs=fe.contiguous(), scales=gs, rotations=gr)
+    g = raster.backward(st, dC)
+    outs = [(xyz, g["dL_dmeans3D"]), (sc, g["dL_dscales"]), (rot, g["dL_drotations"]), (op, g["dL_dopacity"])]
+    outs = [(t, torch.tensor(gr).reshape(t.shape)) for t, gr in outs if t.requires_grad]     # animated path: rotation is a constant of the triangles
+    torch.autograd.backward([t for t, _ in outs], [gr for _, gr in outs])
+    grads = dict(vertices=tv.grad, _alpha=ta.grad, _scale=ts.grad, _opacity=top.grad,
+                 _features_dc=torch.tensor(g["dL_dsh"][:, :1]), _features_rest=torch.tensor(g["dL_dsh"][:, 1:]))
+    return st, grads
+
+
 def assert_forward_parity(st, color, radii, invd, state, tol=1e-5):
     """Bit-exact indices, <= tol per pixel (threshold-ambiguous pixels get a bounded looser check)."""
     np.testing.assert_array_equal(radii, st.radii)
@@ -74,10 +106,18 @@ def assert_forward_parity(st, color, radii, invd, state, tol=1e-5):
     np.testing.assert_array_equal(state["point_list"].astype(np.uint32), st.point_list)
     np.testing.assert_array_equal(state["tile_keys"].astype(np.uint64), st.keys_sorted >> np.uint64(32))
     np.testing.assert_array_equal(state["ranges"], st.ranges)
-    # Threshold-ambiguous pixels: the oracle flags a pixel when one of its skip / stop decisions (alpha < 1/255,
-    # T(1-alpha) < 1e-4) lies within the +-1e-6 relative band in which exp() (GPU: ex2.approx.ftz) may fall on the other side.
-    # They are REPORTED (count, worst error) and bounded by the largest change one flipped decision can cause: a splat
-    # blended at alpha = 1/255 with unit transmittance moves a channel by <= |c - behind| / 255 <= max colour / 255.
+    ok = assert_image_parity(st, color, tol)
+    np.testing.assert_array_equal(state["n_contrib"][ok], st.n_contrib[ok])
+    assert np.abs(invd - st.invdepth)[:, ok].max() <= tol
+    assert np.abs(state["final_T"] - st.final_T)[ok].max() <= tol
+
+
+def assert_image_parity(st, color, tol=1e-5):
+    """<= tol per pixel outside the threshold-ambiguous pixels; returns the mask of those other pixels.
+    Threshold-ambiguous pixels: the oracle flags a pixel when one of its skip / stop decisions (alpha < 1/255,
+    T(1-alpha) < 1e-4) lies within the +-1e-6 relative band in which exp() (GPU: ex2.approx.ftz) may fall on the other side.
+    They are REPORTED (count, worst error) and bounded by the largest change one flipped decision can cause: a splat
+    blended at alpha = 1/255 with unit transmittance moves a channel by <= |c - behind| / 255 <= max colour / 255."""
     ok = st.ambiguous == 0
     n_amb = int((~ok).sum())
     err = np.abs(color - st.color)
@@ -87,11 +127,9 @@ def assert_forward_parity(st, color, radii, invd, state, tol=1e-5):
     print(f"[parity] {st.settings.image_width}x{st.settings.image_height} P={st.radii.shape[0]} N={st.N}: max|image-oracle| = {err_ok:.2e}; "
           f"threshold-ambiguous pixels = {n_amb} ({n_amb / ok.size:.1e} of the image), worst there = {err_amb:.2e} (bound {cmax / 255:.1e})")
     assert n_amb <= max(4, 5e-4 * ok.size), f"too many threshold-ambiguous pixels: {n_amb}"
-    np.testing.assert_array_equal(state["n_contrib"][ok], st.n_contrib[ok])
     assert err_ok <= tol, err_ok
-    assert np.abs(invd - st.invdepth)[:, ok].max() <= tol
-    assert np.abs(state["final_T"] - st.final_T)[ok].max() <= tol
     assert err_amb <= 2.0 * cmax / 255.0, err_amb
+    return ok
 
 
 # Gradients w.r.t. scales / rotations / cov3D go through the inverse of a nearly singular 2D covariance (flat mesh

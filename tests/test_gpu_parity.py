@@ -175,62 +175,147 @@ def test_binning_implementations_give_the_stock_order(bin_impl, sort_impl, P, W,
     assert_forward_parity(st, color, radii, invd, state)
 
 
-@pytest.mark.parametrize("bin_impl", [0, 1])
-def test_nosync_forward_matches_and_overflow_degrades_to_background(bin_impl):
-    """gms_rasterize_forward_nosync through the raw C ABI: with enough capacity it equals the synchronising call bit for
-    bit and reports N through the mapped host word; with too little it raises the overflow flag and renders the
-    background (never writes past the region)."""
-    import ctypes as C
-    from gms_b200 import rasterizer as R
-    S, g = _case(20000, 400, 300, seed=9)
-    old_bin = _lib.set_option("bin_impl", bin_impl)
-    try:
-        _nosync_body(S, g, bin_impl)
-    finally:
-        _lib.set_option("bin_impl", old_bin)
+def _expected_flags(bin_impl, sort_impl, key16, T):
+    """saved.flags bits 0 (counting binning ran) and 2 (16-bit tile keys).  The counting kernel needs two 32-bit rows of T
+    counters plus 12 KB within the H100's 227 KB of opt-in shared memory per block; where they do not fit (T > 27518) the
+    call falls back to emit + sort."""
+    counting = bin_impl == 1 and 8 * T + 64 + 12288 <= 227 * 1024
+    return int(counting) | (4 if not counting and sort_impl == 0 and key16 and T <= 65535 else 0)
 
 
-def _nosync_body(S, g, bin_impl):
+def _nosync_call(S, g, cap):
+    """gms_rasterize_forward_nosync through the raw C ABI with binning capacity `cap`; every scratch region carries a canary
+    behind the bytes it asked for.  Returns (color, radii, invdepth, saved, n_host, debug state)."""
     import ctypes as C
+    from types import SimpleNamespace
     from gms_b200 import rasterizer as R
-    color, radii, invd, state, _ = run_gpu(S, g)
-    N = state["num_rendered"]
-    dev = torch.device("cuda")
     from gpu_helpers import gpu_settings
-    rs = gpu_settings(S)
+    dev = torch.device("cuda")
+    W, H = S.image_width, S.image_height
     keep = []
-    s = R._settings_struct(rs, dev, keep)
+    s = R._settings_struct(gpu_settings(S), dev, keep)
     t = {k: v.cuda().float().contiguous() for k, v in g.items()}
     P = t["means3D"].shape[0]
     i = R._inputs_struct(P, 16, t["means3D"], t["opacities"], t["shs"], None, t["scales"], t["rotations"], None)
-    for cap, expect_overflow in ((N + 5, False), (N, False), (N // 2, True)):
-        out_c = torch.full((3, 300, 400), -1.0, device=dev); out_r = torch.zeros(P, dtype=torch.int32, device=dev)
-        out_d = torch.full((1, 300, 400), -1.0, device=dev)
-        o = _lib.RasterOutputs(out_c.data_ptr(), out_r.data_ptr(), out_d.data_ptr())
-        bufs = {}
-        guard = {}
+    out_c = torch.full((3, H, W), -1.0, device=dev); out_r = torch.zeros(P, dtype=torch.int32, device=dev)
+    out_d = torch.full((1, H, W), -1.0, device=dev)
+    o = _lib.RasterOutputs(out_c.data_ptr(), out_r.data_ptr(), out_d.data_ptr())
+    bufs, guard = {}, {}
 
-        def _alloc(user, which, nbytes):
-            b = torch.zeros(int(nbytes) + 4096, dtype=torch.uint8, device=dev)
-            b[int(nbytes):] = 0xAB                              # canary behind the requested region
-            bufs[int(which)] = b; guard[int(which)] = int(nbytes)
-            return b.data_ptr()
+    def _alloc(user, which, nbytes):
+        b = torch.zeros(int(nbytes) + 4096, dtype=torch.uint8, device=dev)
+        b[int(nbytes):] = 0xAB                              # canary behind the requested region
+        bufs[int(which)] = b; guard[int(which)] = int(nbytes)
+        return b.data_ptr()
 
-        cb = _lib.ALLOC_FN(_alloc)
-        saved = _lib.RasterSaved()
-        n_host = torch.zeros(2, dtype=torch.int32).pin_memory()
-        _lib.check(_lib.lib().gms_rasterize_forward_nosync(C.byref(s), C.byref(i), C.byref(o), cb, None, C.byref(saved), cap,
-                                                           n_host.data_ptr(), torch.cuda.current_stream().cuda_stream), "nosync")
-        torch.cuda.synchronize()
-        assert int(saved.num_rendered) == -1 and (int(saved.flags) & 1) == bin_impl and int(saved.binning_capacity) == cap
-        assert int(n_host[0]) == N and int(n_host[1]) == int(expect_overflow)
-        for which, nb in guard.items():
-            assert bool((bufs[which][nb:] == 0xAB).all()), f"scratch region {which} overrun"
+    cb = _lib.ALLOC_FN(_alloc)
+    saved = _lib.RasterSaved()
+    n_host = torch.zeros(2, dtype=torch.int32).pin_memory()
+    _lib.check(_lib.lib().gms_rasterize_forward_nosync(C.byref(s), C.byref(i), C.byref(o), cb, None, C.byref(saved), cap,
+                                                       n_host.data_ptr(), torch.cuda.current_stream().cuda_stream), "nosync")
+    torch.cuda.synchronize()
+    for which, nb in guard.items():
+        assert bool((bufs[which][nb:] == 0xAB).all()), f"scratch region {which} overrun"
+    N = int(n_host[0])
+    state = R.forward_debug_state(SimpleNamespace(bufs=bufs), min(N, cap), P, W, H, out_r,
+                                  bin_state=(int(saved.binning_capacity), int(saved.flags)))
+    return out_c.cpu().numpy(), out_r.cpu().numpy(), out_d.cpu().numpy(), saved, n_host, \
+        {k: v.cpu().numpy() for k, v in state.items()}
+
+
+@pytest.mark.parametrize("bin_impl", [0, 1])
+def test_nosync_forward_matches_and_overflow_degrades_to_background(bin_impl):
+    """gms_rasterize_forward_nosync at the capacity edges: N - 1 (overflow), N, N + 1 and N + 2*4096 + 1 (a sentinel tail
+    longer than one CTA tile of the hand-written sort, and not a multiple of it).  With enough capacity the image and
+    radii equal the synchronising call bit for bit, and the point list and tile ranges equal both the synchronising call and
+    the oracle; N is reported through the mapped host word.  With too little, the overflow flag is raised and the frame
+    renders the background.  No call writes past any scratch region.  Either binning, with the default sort (cub) and
+    16-bit tile keys."""
+    _nosync_with_options(bin_impl, 0, 1)
+
+
+@pytest.mark.parametrize("bin_impl,sort_impl,key16", [(0, 0, 0), (0, 1, 1), (1, 1, 1)])
+def test_nosync_capacity_edges_with_the_other_sorts_and_key_widths(bin_impl, sort_impl, key16):
+    """The capacity edges of test_nosync_forward_matches_and_overflow_degrades_to_background for the remaining
+    implementations: emit + cub sort on 32-bit keys, emit + hand-written sort (32-bit keys, device-side N), and the counting
+    binning behind the hand-written depth sort."""
+    _nosync_with_options(bin_impl, sort_impl, key16)
+
+
+def _nosync_with_options(bin_impl, sort_impl, key16):
+    S, g = _case(20000, 400, 300, seed=9)
+    olds = {k: _lib.set_option(k, v) for k, v in (("bin_impl", bin_impl), ("sort_impl", sort_impl), ("key16", key16))}
+    try:
+        _nosync_body(S, g, _expected_flags(bin_impl, sort_impl, key16, 25 * 19))
+    finally:
+        for k, v in olds.items():
+            _lib.set_option(k, v)
+
+
+def _nosync_body(S, g, flags):
+    color, radii, invd, state, _ = run_gpu(S, g)
+    N = state["num_rendered"]
+    st, _ = run_oracle(S, g)
+    np.testing.assert_array_equal(state["point_list"].astype(np.uint32), st.point_list)
+    np.testing.assert_array_equal(state["ranges"], st.ranges)
+    for cap, expect_overflow in ((N - 1, True), (N, False), (N + 1, False), (N + 2 * 4096 + 1, False)):
+        out_c, out_r, out_d, saved, n_host, ns = _nosync_call(S, g, cap)
+        assert int(saved.num_rendered) == -1 and (int(saved.flags) & 5) == flags and int(saved.binning_capacity) == cap
+        assert int(n_host[0]) == N and int(n_host[1]) == int(expect_overflow), (cap, N, int(n_host[0]), int(n_host[1]))
+        np.testing.assert_array_equal(out_r, radii)
         if expect_overflow:
-            bg = torch.tensor(np.asarray(S.bg, np.float32), device=dev)
-            assert torch.equal(out_c, bg[:, None, None].expand_as(out_c)) and float(out_d.abs().max()) == 0.0
+            bg = np.asarray(S.bg, np.float32)
+            assert np.array_equal(out_c, np.broadcast_to(bg[:, None, None], out_c.shape)) and float(np.abs(out_d).max()) == 0.0
         else:
-            assert torch.equal(out_c.cpu(), torch.tensor(color)) and torch.equal(out_r.cpu(), torch.tensor(radii))
+            np.testing.assert_array_equal(ns["point_list"], state["point_list"], err_msg=f"capacity {cap}")
+            np.testing.assert_array_equal(ns["ranges"], state["ranges"], err_msg=f"capacity {cap}")
+            np.testing.assert_array_equal(out_c, color); np.testing.assert_array_equal(out_d, invd)
+
+
+@pytest.mark.parametrize("bin_impl,sort_impl", [(0, 0), (0, 1), (1, 0), (1, 1)])
+@pytest.mark.parametrize("W,H", [(4080, 4112), (4096, 4096)])
+def test_nosync_binning_at_the_16_32_bit_key_boundary(W, H, bin_impl, sort_impl):
+    """T = 255 x 257 = 65535 tiles, the largest grid on 16-bit tile keys (ids up to 65534, sentinel 0xFFFF; the hand-written
+    sort takes two 8-bit passes), and T = 256 x 256 = 65536 on 32-bit keys (three hand-written passes).  Forward only:
+    the sync-free call gives the synchronising call's image bit for bit and the oracle's point list and tile ranges; the
+    image matches the oracle's composite on every 97th tile."""
+    from oracle import raster
+    S, g = _case(3000, W, H, seed=W, extent=1.1, scale_mu=-3.2)
+    T = (W // 16) * (H // 16)
+    olds = {k: _lib.set_option(k, v) for k, v in (("bin_impl", bin_impl), ("sort_impl", sort_impl))}
+    try:
+        color, radii, invd, state, _ = run_gpu(S, g)
+        N = state["num_rendered"]
+        out_c, out_r, out_d, saved, n_host, ns = _nosync_call(S, g, N + 2 * 4096 + 1)
+    finally:
+        for k, v in olds.items():
+            _lib.set_option(k, v)
+    assert (int(saved.flags) & 5) == _expected_flags(bin_impl, sort_impl, 1, T)
+    assert int(n_host[0]) == N and int(n_host[1]) == 0
+    np.testing.assert_array_equal(out_r, radii)
+    np.testing.assert_array_equal(out_c, color); np.testing.assert_array_equal(out_d, invd)
+    st = raster.preprocess(S, g["means3D"], g["opacities"], shs=g["shs"], scales=g["scales"], rotations=g["rotations"])
+    np.testing.assert_array_equal(radii, st.radii)
+    raster.bin_tiles(st)
+    assert st.N == N and st.ranges.shape[0] == T
+    for what in (state, ns):
+        np.testing.assert_array_equal(what["point_list"].astype(np.uint32), st.point_list)
+        np.testing.assert_array_equal(what["ranges"], st.ranges)
+    raster.set_tile_stride(97)
+    try:
+        raster.composite(st)
+    finally:
+        raster.set_tile_stride(1)
+    gx, worst, amb = W // 16, 0.0, 0
+    for tile in range(0, T, 97):
+        x0, y0 = (tile % gx) * 16, (tile // gx) * 16
+        sl = (slice(None), slice(y0, y0 + 16), slice(x0, x0 + 16))
+        ok = st.ambiguous[sl[1:]] == 0
+        amb += int((~ok).sum())
+        worst = max(worst, float(np.abs(out_c[sl] - st.color[sl])[:, ok].max()) if ok.any() else 0.0)
+    print(f"[key boundary] {W}x{H} T={T} N={N} flags={int(saved.flags)} sampled tiles={len(range(0, T, 97))} "
+          f"ambiguous px={amb} max|image-oracle|={worst:.2e}")
+    assert worst <= 1e-5
 
 
 @pytest.mark.parametrize("P,deg", [(4001, 3), (77, 1), (12345, 0)])

@@ -22,9 +22,9 @@ import pytest
 import torch
 
 from gms_b200 import expansion, scenes
+from gpu_helpers import GRAD_TOL, oracle_chain
 from helpers import settings_from_camera
 from oracle import expansion as oexp
-from oracle import raster
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
@@ -97,33 +97,6 @@ def _assert_sample(got, ref, atol, rtol=0.0, what=""):
     np.testing.assert_allclose(got[sample_rows(got.shape[0])], ref, rtol=rtol, atol=atol, err_msg=what)
 
 
-def _oracle_chain(p, S, dC, gpu, triangles=None):
-    """Oracle image and gradients of sum(image * dC) w.r.t. the raw mesh-Gaussian parameters.  `gpu` = the (means3D,
-    scales, rotations) the GPU run handed to the rasterizer: they must agree with the oracle's expansion to fp32 rounding
-    and are what the oracle rasterizes (so that integer outputs can be compared bit for bit); the gradient chain runs
-    through the oracle's own expansion graph."""
-    tv, ta, ts = (x.clone().requires_grad_(True) for x in (p.vertices, p._alpha, p._scale))
-    if triangles is None:
-        xyz, sl, rr, _, _ = oexp.expand(tv, p.faces, ta, ts)
-    else:
-        alpha, _, _ = oexp.update_alpha(ta, tv, p.faces)
-        xyz = torch.matmul(alpha, triangles).reshape(-1, 3)
-        sl, rr = oexp.prepare_scaling_rot(triangles, ts, ta.shape[1])
-    top = p._opacity.clone().requires_grad_(True)
-    sc, rot, op, fe = oexp.activate(sl, rr, top, p._features_dc, p._features_rest)
-    gx, gs, gr = (t.detach().cpu() for t in gpu)
-    assert float((gx - xyz.detach()).abs().max()) <= 2e-6 and float((gr - rot.detach()).abs().max()) <= 4e-6
-    assert float(((gs - sc.detach()).abs() / sc.detach()).max()) <= 1e-5
-    st = raster.forward(S, gx, op.detach(), shs=fe.contiguous(), scales=gs, rotations=gr)
-    g = raster.backward(st, dC)
-    outs = [(xyz, g["dL_dmeans3D"]), (sc, g["dL_dscales"]), (rot, g["dL_drotations"]), (op, g["dL_dopacity"])]
-    outs = [(t, torch.tensor(gr).reshape(t.shape)) for t, gr in outs if t.requires_grad]     # animated path: rotation is a constant of the triangles
-    torch.autograd.backward([t for t, _ in outs], [gr for _, gr in outs])
-    grads = dict(vertices=tv.grad, _alpha=ta.grad, _scale=ts.grad, _opacity=top.grad,
-                 _features_dc=torch.tensor(g["dL_dsh"][:, :1]), _features_rest=torch.tensor(g["dL_dsh"][:, 1:]))
-    return st, grads
-
-
 def _check_against_oracle(pkg, model, st, ograds, tag, grad_tol):
     img = pkg["render"].detach().cpu().numpy()
     ok = st.ambiguous == 0
@@ -142,9 +115,6 @@ def _check_against_oracle(pkg, model, st, ograds, tag, grad_tol):
         assert e <= grad_tol.get(k, 2e-4), (k, e)
 
 
-GRAD_TOL = {"vertices": 5e-3, "_scale": 5e-3, "_alpha": 1e-3}     # through the near-singular 2D covariance (DESIGN.md 2.2)
-
-
 @pytest.mark.parametrize("patched", [False, True])
 def test_reference_render_on_stock_mesh_model_matches_oracle(patched):
     p = scenes.init_mesh_gaussians(*scenes.icosphere(3), K=3, seed=11, trained_like=True)
@@ -160,7 +130,7 @@ def test_reference_render_on_stock_mesh_model_matches_oracle(patched):
     (pkg["render"] * torch.tensor(dC, device="cuda")).sum().backward()
     assert pkg["viewspace_points"].grad is not None and pkg["visibility_filter"].dtype == torch.bool
     S = settings_from_camera(cam, bg=(1, 1, 1))
-    st, og = _oracle_chain(p, S, dC, (m.get_xyz, m.get_scaling, m.get_rotation))
+    st, og = oracle_chain(p, S, dC, (m.get_xyz, m.get_scaling, m.get_rotation))
     _check_against_oracle(pkg, m, st, og, f"render/{'patched' if patched else 'stock'}-expansion", GRAD_TOL)
 
 
@@ -211,7 +181,7 @@ def test_reference_animated_renderer_matches_oracle(golden, t):
     _assert_sample(means3D, golden[tag + "_means3D"], 2e-6, what="means3D")
     _assert_sample(m.get_scaling, golden[tag + "_scales"], 0.0, 1e-5, what="scales")
     _assert_sample(m.get_rotation, golden[tag + "_rotations"], 4e-6, what="rotations")
-    st, og = _oracle_chain(p, S, dC, (means3D, m.get_scaling, m.get_rotation), triangles=tri)
+    st, og = oracle_chain(p, S, dC, (means3D, m.get_scaling, m.get_rotation), triangles=tri)
     og.pop("vertices")                      # the animated path feeds triangles directly: no gradient reaches pc.vertices
     _check_against_oracle(pkg, m, st, og, f"animated t={t}", GRAD_TOL)
 
