@@ -11,6 +11,15 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+// save_image's byte: mul(255).add(0.5).clamp(0, 255).to(uint8) -- two roundings (mul, add) like ATen's separate passes, then
+// truncation.  NaN -> 0 (fmaxf returns the non-NaN operand).  Shared with the metric kernel's 8-bit round trip.
+__device__ __forceinline__ uint8_t gms_quantize_u8(float x) {
+    const float v = __fadd_rn(__fmul_rn(x, 255.0f), 0.5f);
+    return (uint8_t)fminf(fmaxf(v, 0.0f), 255.0f);
+}
+// ToTensor: byte / 255
+__device__ __forceinline__ float gms_dequantize_u8(uint8_t b) { return __fdiv_rn((float)b, 255.0f); }
+
 // one thread per pixel: reads C coalesced planes, writes C adjacent bytes.  row_prefix: bytes reserved at the start of
 // every output row (1 for PNG: the filter-type byte, written as 0 = "None").
 __global__ void __launch_bounds__(256)
@@ -22,11 +31,7 @@ k_image_quantize(const float* __restrict__ chw, uint8_t* __restrict__ out, int C
     if (row_prefix && x == 0)
         for (int k = 0; k < row_prefix; k++) row[k] = 0;
     uint8_t* px = row + row_prefix + (size_t)x * C;
-    for (int c = 0; c < C; c++) {
-        // mul(255).add(0.5).clamp(0, 255).to(uint8): two roundings (mul, add) like ATen's separate passes, then truncation
-        const float v = __fadd_rn(__fmul_rn(chw[c * HW + pix], 255.0f), 0.5f);
-        px[c] = (uint8_t)fminf(fmaxf(v, 0.0f), 255.0f);     // NaN -> 0 (fmaxf returns the non-NaN operand)
-    }
+    for (int c = 0; c < C; c++) px[c] = gms_quantize_u8(chw[c * HW + pix]);
 }
 
 __global__ void __launch_bounds__(256)
@@ -36,6 +41,6 @@ k_image_dequantize(const uint8_t* __restrict__ src, int src_is_hwc, float* __res
     const size_t HW = (size_t)H * W, pix = (size_t)y * W + x;
     for (int c = 0; c < C; c++) {
         const uint8_t b = src_is_hwc ? src[pix * C + c] : src[c * HW + pix];
-        chw[c * HW + pix] = __fdiv_rn((float)b, 255.0f);     // ToTensor: byte / 255
+        chw[c * HW + pix] = gms_dequantize_u8(b);
     }
 }

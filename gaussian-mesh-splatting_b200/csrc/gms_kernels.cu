@@ -59,10 +59,12 @@ static int sm_count() {
 }
 
 // Optional per-kernel timing with CUDA events recorded on the launching stream (bench.py's roofline numbers).
-enum { K_PRE_FWD = 0, K_SORT_P, K_SCAN, K_EMIT, K_SORT_N, K_RANGES, K_COMP_FWD, K_COMP_BWD, K_PRE_BWD, K_EXP_FWD, K_EXP_BWD, K_LOSS_STATS, K_LOSS_GRAD, K_ADAM, K_MISC, K_COUNT };
+enum { K_PRE_FWD = 0, K_SORT_P, K_SCAN, K_EMIT, K_SORT_N, K_RANGES, K_COMP_FWD, K_COMP_BWD, K_PRE_BWD, K_EXP_FWD, K_EXP_BWD, K_LOSS_STATS, K_LOSS_GRAD, K_ADAM, K_MISC,
+       K_METRICS, K_METRICS_FIN, K_COUNT };
 static const char* const g_kernel_names[K_COUNT] = {"preprocess_fwd", "cub_sort_depth", "cub_scan_tiles", "emit_dups", "cub_sort_tiles",
                                                     "tile_ranges", "composite_fwd", "composite_bwd", "preprocess_bwd", "expand_fwd",
-                                                    "expand_bwd", "ssim_stats", "ssim_grad", "adam", "misc"};
+                                                    "expand_bwd", "ssim_stats", "ssim_grad", "adam", "misc",
+                                                    "image_metrics", "metrics_finalize"};
 static int g_opt_time = 0;
 struct TimedSpan { int id; cudaEvent_t a, b; };
 static TimedSpan g_spans[1 << 15];
@@ -1085,6 +1087,14 @@ int gms_loss_scratch_bytes(int32_t C, int32_t H, int32_t W, size_t* bytes) {
     return GMS_OK;
 }
 
+static GmsGaussWin ssim_window() {
+    GmsGaussWin win;    // utils/loss_utils.py:23-25: exp(-(x-5)^2 / (2*1.5^2)) in fp32, normalised
+    float sum = 0.f;
+    for (int k = 0; k < 11; k++) { win.g[k] = (float)exp(-(double)((k - 5) * (k - 5)) / (2.0 * 1.5 * 1.5)); sum += win.g[k]; }
+    for (int k = 0; k < 11; k++) win.g[k] /= sum;
+    return win;
+}
+
 int gms_l1_ssim_loss(const gms_loss_args* a, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (!a || !a->img || !a->gt || !a->loss || !a->scratch) return set_err(GMS_E_ARG, "gms_l1_ssim_loss: null argument%s%s");
@@ -1095,12 +1105,7 @@ int gms_l1_ssim_loss(const gms_loss_args* a, void* cuda_stream) {
     char* base = reinterpret_cast<char*>(aligned_base_c(a->scratch));
     float* acc = reinterpret_cast<float*>(base);
     float* dmap = reinterpret_cast<float*>(base + 256);
-    GmsGaussWin win;
-    {   // utils/loss_utils.py:23-25: exp(-(x-5)^2 / (2*1.5^2)) in fp32, normalised
-        float sum = 0.f;
-        for (int k = 0; k < 11; k++) { win.g[k] = (float)exp(-(double)((k - 5) * (k - 5)) / (2.0 * 1.5 * 1.5)); sum += win.g[k]; }
-        for (int k = 0; k < 11; k++) win.g[k] /= sum;
-    }
+    const GmsGaussWin win = ssim_window();
     GMS_CUDA(cudaMemsetAsync(acc, 0, 2 * sizeof(float), st));
     dim3 grid((W + GMS_SSIM_T - 1) / GMS_SSIM_T, (H + GMS_SSIM_T - 1) / GMS_SSIM_T, C);
     span_begin(K_LOSS_STATS, st);
@@ -1117,6 +1122,38 @@ int gms_l1_ssim_loss(const gms_loss_args* a, void* cuda_stream) {
         GMS_AFTER_LAUNCH("ssim_grad", 0, st);
         span_end(st);
     }
+    return GMS_OK;
+}
+
+static int metric_tiles(int32_t H, int32_t W) { return ((W + GMS_SSIM_T - 1) / GMS_SSIM_T) * ((H + GMS_SSIM_T - 1) / GMS_SSIM_T); }
+
+int gms_metrics_scratch_bytes(int32_t C, int32_t H, int32_t W, size_t* bytes) {
+    if (C <= 0 || C > GMS_METRIC_MAXC || H <= 0 || W <= 0 || !bytes) return set_err(GMS_E_ARG, "gms_metrics_scratch_bytes: bad sizes%s%s");
+    *bytes = align_up(sizeof(float) * 3 * (size_t)C * metric_tiles(H, W)) + 256;
+    return GMS_OK;
+}
+
+int gms_image_metrics(const gms_metrics_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !a->img || !a->gt || !a->out || !a->scratch) return set_err(GMS_E_ARG, "gms_image_metrics: null argument%s%s");
+    if (a->quantize != 0 && a->quantize != 1) return set_err(GMS_E_ARG, "gms_image_metrics: quantize must be 0 or 1%s%s");
+    const int C = a->C, H = a->H, W = a->W;
+    size_t need = 0;
+    int rc = gms_metrics_scratch_bytes(C, H, W, &need);
+    if (rc) return rc;
+    if (a->scratch_bytes < need) return set_err(GMS_E_ARG, "gms_image_metrics: scratch too small%s%s");
+    float* part = reinterpret_cast<float*>(aligned_base_c(a->scratch));
+    const GmsGaussWin win = ssim_window();
+    dim3 grid((W + GMS_SSIM_T - 1) / GMS_SSIM_T, (H + GMS_SSIM_T - 1) / GMS_SSIM_T, C);
+    span_begin(K_METRICS, st);
+    if (a->quantize) k_image_metrics<1><<<grid, 256, 0, st>>>(C, H, W, a->img, a->gt, win, part);
+    else k_image_metrics<0><<<grid, 256, 0, st>>>(C, H, W, a->img, a->gt, win, part);
+    GMS_AFTER_LAUNCH("image_metrics", 0, st);
+    span_end(st);
+    span_begin(K_METRICS_FIN, st);
+    k_metrics_finalize<<<1, 256, 0, st>>>(C, metric_tiles(H, W), 1.0 / ((double)H * (double)W), part, a->out);
+    GMS_AFTER_LAUNCH("metrics_finalize", 0, st);
+    span_end(st);
     return GMS_OK;
 }
 
@@ -1714,6 +1751,61 @@ int gms_expand_backward(const gms_expand_args* a, const gms_expand_grads* g, voi
 
 size_t gms_frame_workspace_bytes(int32_t P, int32_t W, int32_t H) { return frame_layout(nullptr, P, W, H).total + 512; }
 
+// The forward half of a whole frame, shared by gms_train_frame and gms_render_frame: E1-E4 mesh -> Gaussians (activated
+// scales / rotations) into xyz / scales / rots, then the rasterizer forward.  sigmoid(opacity) is computed inside
+// k_preprocess_fwd (which stores it to `opac` for the backward), its derivative inside k_preprocess_bwd: no separate
+// activation launches.  `ea` and `in` are filled for the training frame's backward passes.
+struct FrameModel {
+    int32_t V, F, K, M;
+    const float* vertices; const int64_t* faces; const float* alpha_raw; const float* scale_raw; const float* features;
+    const float* opacity_raw; float eps;
+};
+
+static int frame_forward(const FrameModel& m, const gms_raster_settings* s, float* xyz, float* scales, float* rots, float* opac,
+                         gms_raster_outputs* out, gms_alloc_fn alloc, void* user, int64_t binning_capacity, uint32_t* n_host,
+                         void* cuda_stream, gms_expand_args* ea, gms_raster_inputs* in, gms_raster_saved* saved) {
+    int rc;
+    memset(ea, 0, sizeof(*ea));
+    ea->V = m.V; ea->F = m.F; ea->K = m.K; ea->vertices = m.vertices; ea->faces = m.faces; ea->alpha_raw = m.alpha_raw;
+    ea->scale_raw = m.scale_raw; ea->eps = m.eps; ea->xyz = xyz; ea->scaling_act = scales; ea->rotation_act = rots;
+    if ((rc = gms_expand_forward(ea, cuda_stream))) return rc;
+    memset(in, 0, sizeof(*in));
+    in->P = m.F * m.K; in->M = m.M; in->means3D = xyz; in->opacities = opac; in->shs = m.features; in->scales = scales; in->rotations = rots;
+    return raster_forward_impl(s, in, out, alloc, user, saved, cuda_stream, binning_capacity, n_host, m.opacity_raw);
+}
+
+struct RenderLayout { float* xyz; float* scales; float* rots; float* opac; size_t total; };
+
+static RenderLayout render_layout(void* base, int P) {
+    RenderLayout L;
+    char* p = reinterpret_cast<char*>(base);
+    const size_t Pn = (size_t)(P > 0 ? P : 1);
+    L.xyz = carve<float>(p, 3 * Pn); L.scales = carve<float>(p, 3 * Pn); L.rots = carve<float>(p, 4 * Pn); L.opac = carve<float>(p, Pn);
+    L.total = (size_t)(p - reinterpret_cast<char*>(base));
+    return L;
+}
+
+size_t gms_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { (void)W; (void)H; return render_layout(nullptr, P).total + 512; }
+
+int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
+    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii) return set_err(GMS_E_ARG, "gms_render_frame: null argument%s%s");
+    if (!a->vertices || !a->faces || !a->alpha_raw || !a->scale_raw || !a->features || !a->opacity_raw)
+        return set_err(GMS_E_ARG, "gms_render_frame: model tensors required%s%s");
+    const int P = a->F * a->K, W = a->settings.image_width, H = a->settings.image_height;
+    if (a->workspace_bytes < gms_render_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_render_frame: workspace too small%s%s");
+    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
+    const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps};
+    gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
+    gms_expand_args ea;
+    gms_raster_inputs in;
+    gms_raster_saved saved;
+    const int rc = frame_forward(m, &a->settings, RL.xyz, RL.scales, RL.rots, RL.opac, &out, alloc, alloc_user, a->binning_capacity,
+                                 a->n_host_mapped, cuda_stream, &ea, &in, &saved);
+    if (rc) return rc;
+    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
+    return GMS_OK;
+}
+
 int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (!a || !alloc || !a->workspace || !a->loss || !a->gt) return set_err(GMS_E_ARG, "gms_train_frame: null argument%s%s");
@@ -1727,22 +1819,13 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     if (a->workspace_bytes < gms_frame_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_train_frame: workspace too small%s%s");
     FrameLayout FL = frame_layout(aligned_base_c(a->workspace), P, W, H);
     int rc;
-    // E1-E4: mesh -> Gaussians (activated scales / rotations), sigmoid(opacity)
+    const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps};
+    gms_raster_outputs out = {FL.image, FL.radii, FL.invdepth, 0};
     gms_expand_args ea;
-    memset(&ea, 0, sizeof(ea));
-    ea.V = a->V; ea.F = a->F; ea.K = a->K; ea.vertices = a->vertices; ea.faces = a->faces; ea.alpha_raw = a->alpha_raw;
-    ea.scale_raw = a->scale_raw; ea.eps = a->eps; ea.xyz = FL.xyz; ea.scaling_act = FL.scales; ea.rotation_act = FL.rots;
-    if ((rc = gms_expand_forward(&ea, cuda_stream))) return rc;
-    // sigmoid(opacity) is computed inside k_preprocess_fwd (which stores it to FL.opac for the backward), its derivative inside
-    // k_preprocess_bwd: no separate activation launches
-    // rasterizer forward
     gms_raster_inputs in;
-    memset(&in, 0, sizeof(in));
-    in.P = P; in.M = a->M; in.means3D = FL.xyz; in.opacities = FL.opac; in.shs = a->features; in.scales = FL.scales; in.rotations = FL.rots;
-    gms_raster_outputs out = {FL.image, FL.radii, FL.invdepth};
     gms_raster_saved saved;
-    if ((rc = raster_forward_impl(&a->settings, &in, &out, alloc, alloc_user, &saved, cuda_stream, a->binning_capacity, a->n_host_mapped,
-                                  a->opacity_raw))) return rc;
+    if ((rc = frame_forward(m, &a->settings, FL.xyz, FL.scales, FL.rots, FL.opac, &out, alloc, alloc_user, a->binning_capacity,
+                            a->n_host_mapped, cuda_stream, &ea, &in, &saved))) return rc;
     // loss + dL/dimage
     gms_loss_args la;
     memset(&la, 0, sizeof(la));

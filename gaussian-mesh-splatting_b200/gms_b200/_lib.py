@@ -123,6 +123,22 @@ class FrameView(C.Structure):
                 ("radii", C.c_void_p), ("image", C.c_void_p), ("invdepth", C.c_void_p)]
 
 
+class RenderArgs(C.Structure):
+    """struct gms_render_args"""
+    _fields_ = [("V", C.c_int32), ("F", C.c_int32), ("K", C.c_int32), ("M", C.c_int32),
+                ("vertices", C.c_void_p), ("faces", C.c_void_p), ("alpha_raw", C.c_void_p), ("scale_raw", C.c_void_p),
+                ("features", C.c_void_p), ("opacity_raw", C.c_void_p), ("eps", C.c_float), ("settings", RasterSettings),
+                ("image", C.c_void_p), ("invdepth", C.c_void_p), ("radii", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)),
+                ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p)]
+
+
+class MetricsArgs(C.Structure):
+    """struct gms_metrics_args"""
+    _fields_ = [("C", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("img", C.c_void_p), ("gt", C.c_void_p),
+                ("quantize", C.c_int32), ("out", C.c_void_p), ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t)]
+
+
 class AdamShArgs(C.Structure):
     _fields_ = [("P", C.c_int32), ("M", C.c_int32), ("sh_degree", C.c_int32), ("R", C.c_int32), ("xyz", C.c_void_p),
                 ("exchange", C.c_void_p), ("slot_floats", C.c_int64), ("grad_scale", C.c_float), ("p", C.c_void_p),
@@ -138,7 +154,8 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_expand_backward", "gms_last_error", "gms_version", "gms_launch_count", "gms_set_option",
                "gms_kernel_times", "gms_loss_scratch_bytes", "gms_l1_ssim_loss", "gms_adam_step",
                "gms_frame_workspace_bytes", "gms_train_frame", "gms_points_expand_forward",
-               "gms_points_prepare_vertices", "gms_image_quantize", "gms_image_dequantize", "gms_adam_sh_factored", "gms_frame_views"]
+               "gms_points_prepare_vertices", "gms_image_quantize", "gms_image_dequantize", "gms_adam_sh_factored", "gms_frame_views",
+               "gms_render_workspace_bytes", "gms_render_frame", "gms_metrics_scratch_bytes", "gms_image_metrics"]
 
 _lib = None
 
@@ -189,6 +206,11 @@ def lib():
     L.gms_frame_workspace_bytes.restype = C.c_size_t
     L.gms_frame_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.gms_train_frame.argtypes = [C.POINTER(FrameArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
+    L.gms_render_workspace_bytes.restype = C.c_size_t
+    L.gms_render_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    L.gms_render_frame.argtypes = [C.POINTER(RenderArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
+    L.gms_metrics_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]
+    L.gms_image_metrics.argtypes = [C.POINTER(MetricsArgs), C.c_void_p]
     _lib = L
     # GMS_OPTIONS="key=value,key=value": tuning knobs applied at load (A/B runs of whole test suites / benches)
     for kv in filter(None, os.environ.get("GMS_OPTIONS", "").split(",")):
@@ -214,7 +236,7 @@ def set_option(key: str, value: int) -> int:
 def kernel_times(reset: bool = True) -> dict:
     """{kernel name: (accumulated ms, launches)} measured by CUDA events on the launching stream."""
     L = lib()
-    n = 16
+    n = 32
     ms = (C.c_double * n)(); cnt = (C.c_int64 * n)(); names = (C.c_char_p * n)()
     k = L.gms_kernel_times(1 if reset else 0, n, ms, cnt, names)
     return {names[i].decode(): (float(ms[i]), int(cnt[i])) for i in range(min(k, n)) if names[i]}

@@ -1,0 +1,111 @@
+"""Per-view binning capacity of the sync-free frames (NativeFrame for training, NativeRenderer for rendering).
+
+A sync-free frame does not read N (the number of tile duplicates) back before it bins: the binning region is sized for a
+PREDICTED capacity, N stays on the device and the range kernel mirrors (N, overflow flag) into a ring of mapped pinned host
+slots that the host polls WITHOUT synchronising.  The prediction is per view: 1.08x the N this camera had at its last visit
+(more when it moved a lot between its last two visits) + 64k; a camera seen for the first time gets 1.25x the largest N
+seen so far + 256k.  A frame whose N exceeds its capacity renders the background; the host notices when it harvests that
+frame's slot, counts it in `overflows`, and the camera's next visit is sized from the true N."""
+from __future__ import annotations
+
+import collections
+import ctypes as C
+
+import torch
+
+
+def grow_only_alloc(dev):
+    """(scratch dict, allocation callback) for the library's scratch regions: grow-only, persistent across frames, so
+    there is no allocator traffic in steady state.  `scratch["requested"]` holds the byte count of the latest request per
+    region."""
+    from . import _lib
+    scratch = {"requested": {}}
+
+    def _alloc(user, which, nbytes):
+        scratch["requested"][int(which)] = int(nbytes)
+        t = scratch.get(int(which))
+        if t is None or t.numel() < nbytes:
+            try:
+                t = torch.empty(int(nbytes * 1.25) + (1 << 20), dtype=torch.uint8, device=dev)
+            except Exception:
+                return 0
+            scratch[int(which)] = t
+        return t.data_ptr()
+
+    return scratch, _lib.ALLOC_FN(_alloc)      # the closure captures `scratch`/`dev` only (no reference cycle through its owner)
+
+
+class SyncFreeCapacity:
+    RING = 64       # mapped (N, flag) slots = frames the host may run ahead of the device before it waits
+
+    def _init_capacity(self, sync_free: bool = True) -> None:
+        self.n_rendered = C.c_int64(0)
+        self.sync_free = bool(sync_free)
+        self.capacity = 0                       # duplicates the most recent frame's binning region was sized for (0: not known yet)
+        self.capacity_override = None           # tests: force the next frames' capacity
+        self.n_host = torch.zeros(self.RING, 2, dtype=torch.int32).pin_memory()   # slot i: (N, overflow flag) of an in-flight frame
+        self._n_np = self.n_host.numpy()
+        self._pending = collections.deque()     # (slot, view key, capacity) of frames whose N has not been harvested yet
+        self._view_n = {}                       # view key -> (N at the last visit, N at the visit before)
+        self._n_max, self._n_last, self._frame_no = 0, 0, 0
+        self.overflows = 0
+
+    @property
+    def last_num_rendered(self) -> int:
+        """N of the most recent frame whose range kernel has run (no synchronisation: may lag behind the queue)."""
+        if self.sync_free and self.capacity > 0:
+            self._harvest()
+            return self._n_last
+        return int(self.n_rendered.value)
+
+    def _harvest(self) -> None:
+        """Collect (N, overflow) of the frames the device has finished binning; their slots become reusable."""
+        while self._pending:
+            slot, key, cap = self._pending[0]
+            n = int(self._n_np[slot, 0])
+            if n < 0:                       # that frame's k_tile_ranges has not run yet
+                break
+            self._pending.popleft()
+            self._note(key, n)
+            if n > cap:
+                self.overflows += 1
+
+    def _note(self, key, n: int) -> None:
+        prev = self._view_n.get(key)
+        self._view_n[key] = (n, prev[0] if prev else 0)
+        self._n_max, self._n_last = max(self._n_max, n), n
+
+    def _predict_capacity(self, key) -> int:
+        if self.capacity_override is not None:
+            return int(self.capacity_override)
+        known = self._view_n.get(key)
+        if known is None:
+            return int(self._n_max * 1.25) + (1 << 18)
+        n1, n0 = known
+        drift = abs(n1 - n0) / max(n1, 1) if n0 else 0.0
+        return int(n1 * (1.0 + max(0.08, 3.0 * drift))) + (1 << 16)
+
+    @staticmethod
+    def _view_key(cam):
+        key = getattr(cam, "uid", None)
+        return id(cam) if key is None else key
+
+    def _sync_free_slot(self, key, dev) -> int:
+        """Capacity and ring slot of the next sync-free frame of view `key`: sets self.capacity, returns the address of the
+        frame's mapped (N, flag) pair."""
+        self._harvest()
+        if len(self._pending) >= self.RING - 1:         # the host is a whole ring ahead of the device: wait for the oldest frames
+            torch.cuda.current_stream(dev).synchronize()
+            self._harvest()
+        slot = self._frame_no % self.RING
+        self._frame_no += 1
+        self.capacity = self._predict_capacity(key)
+        self._n_np[slot, 0], self._n_np[slot, 1] = -1, 0
+        self._pending.append((slot, key, self.capacity))
+        return self.n_host.data_ptr() + 8 * slot
+
+    def _learned_first(self, key) -> None:
+        """After the one synchronising frame: its N sizes the next ones."""
+        n = max(int(self.n_rendered.value), 0)
+        self._note(key, n)
+        self.capacity = n

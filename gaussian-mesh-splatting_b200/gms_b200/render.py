@@ -1,0 +1,156 @@
+"""Render and evaluate views of a gs_mesh model natively: one gms_render_frame call per view, no host synchronisation.
+
+    renderer = NativeRenderer(model, W, H)
+    image, radii, invdepth = renderer.render(cam, bg)                  # scripts/render.py, render_time_animated.py
+    result = renderer.evaluate(test_cams, test_gts, bg)               # training_report / metrics.py
+
+The first render learns N through one 4-byte read-back; every later one is sync-free, with the binning capacity predicted
+per view (SyncFreeCapacity).  An overflowed render (N above its capacity) gives the background image and is counted in
+`overflows`; the view's next render is sized from its true N.  evaluate() never reports an overflowed view's score: it
+re-renders those views before it reads its results."""
+from __future__ import annotations
+
+import ctypes as C
+from dataclasses import dataclass
+from typing import List, Sequence
+
+import torch
+
+from . import _lib, io_image
+from .capacity import SyncFreeCapacity, grow_only_alloc
+from .metrics import METRIC_NAMES, image_metrics, scratch_bytes
+
+
+@dataclass
+class Evaluation:
+    per_view: torch.Tensor      # float64 [n,4] on the host, columns METRIC_NAMES
+    mean: torch.Tensor          # float64 [4]: the mean of the per-view values (PSNR too, as both reference scripts average it)
+    rerun: List[int]            # views whose first render overflowed its capacity and was re-rendered before scoring
+
+
+class NativeRenderer(SyncFreeCapacity):
+    """Forward-only renders of one model at one image size.  The outputs of render() are buffers the renderer owns and the
+    next call overwrites in stream order (ImageSink.write and anything else queued on the same stream read them first)."""
+
+    def __init__(self, model, width: int, height: int):
+        self.model, self.W, self.H = model, int(width), int(height)
+        dev = model.vertices.device
+        self.dev = dev
+        P = model._scale.shape[0]
+        if model.faces.dtype != torch.int64 or not model.faces.is_contiguous():
+            model.faces = model.faces.long().contiguous()
+        self.ws = torch.empty(int(_lib.lib().gms_render_workspace_bytes(P, self.W, self.H)), dtype=torch.uint8, device=dev)
+        self.image = torch.empty(3, self.H, self.W, dtype=torch.float32, device=dev)
+        self.invdepth = torch.empty(1, self.H, self.W, dtype=torch.float32, device=dev)
+        self.radii = torch.empty(P, dtype=torch.int32, device=dev)
+        self._init_capacity(True)
+        self._scratch, self._cb = grow_only_alloc(dev)
+        self._metric_scratch = torch.empty(scratch_bytes(3, self.H, self.W), dtype=torch.uint8, device=dev)
+        self._gt_buf = None
+
+    def _features(self) -> torch.Tensor:
+        m = self.model
+        f = m._features if m._features is not None else m.get_features      # packed SH: zero-copy
+        return f.detach().contiguous()
+
+    def _check(self, cam, bg) -> None:
+        m = self.model
+        for name in ("vertices", "_alpha", "_scale", "_opacity"):
+            t = getattr(m, name)
+            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
+                raise RuntimeError(f"NativeRenderer: model.{name} must be a contiguous float32 CUDA tensor on {self.dev}")
+        if m.faces.device != self.dev:
+            raise RuntimeError("NativeRenderer: model.faces must live on the model's device")
+        if m._scale.shape[0] != self.radii.shape[0]:
+            raise RuntimeError("NativeRenderer: the model's Gaussian count changed; make a new renderer")
+        for t, what in ((bg, "bg"), (cam.world_view_transform, "camera matrices"), (cam.full_proj_transform, "camera matrices"),
+                        (cam.camera_center, "camera centre")):
+            if not t.is_cuda or t.device != self.dev or t.dtype != torch.float32:
+                raise RuntimeError(f"NativeRenderer: {what} must be float32 on {self.dev}")
+        if int(cam.image_width) != self.W or int(cam.image_height) != self.H:
+            raise ValueError(f"NativeRenderer was sized for {self.W}x{self.H}; got a {cam.image_width}x{cam.image_height} camera")
+
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+        """One gms_render_frame into the renderer's buffers: capacity 0 = synchronising, else sync-free with (N, flag) at
+        the mapped address n_host."""
+        self._check(cam, bg)
+        m = self.model
+        feats = self._features()
+        a = _lib.RenderArgs()
+        a.V, a.F, a.K, a.M = m.vertices.shape[0], m._alpha.shape[0], m._alpha.shape[1], feats.shape[1]
+        a.vertices, a.faces, a.alpha_raw, a.scale_raw = m.vertices.data_ptr(), m.faces.data_ptr(), m._alpha.data_ptr(), m._scale.data_ptr()
+        a.features, a.opacity_raw, a.eps = feats.data_ptr(), m._opacity.data_ptr(), m.eps_s0
+        s = a.settings
+        s.image_height, s.image_width, s.tanfovx, s.tanfovy = self.H, self.W, cam.tanfovx, cam.tanfovy
+        s.bg, s.scale_modifier = bg.data_ptr(), float(scale_modifier)
+        s.viewmatrix, s.projmatrix, s.campos = cam.world_view_transform.data_ptr(), cam.full_proj_transform.data_ptr(), cam.camera_center.data_ptr()
+        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = m.active_sh_degree, 0, 0, int(bool(antialiasing))
+        a.image, a.invdepth, a.radii = self.image.data_ptr(), self.invdepth.data_ptr(), self.radii.data_ptr()
+        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
+        a.num_rendered = C.pointer(self.n_rendered)
+        a.binning_capacity, a.n_host_mapped = int(capacity), n_host
+        with torch.cuda.device(self.dev):
+            _lib.check(_lib.lib().gms_render_frame(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream),
+                       "gms_render_frame")
+
+    def render(self, cam, bg: torch.Tensor, scale_modifier: float = 1.0, antialiasing: bool = False):
+        """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view, the reference's render(...)["render"], ["radii"],
+        ["depth"]."""
+        key = self._view_key(cam)
+        if self.capacity == 0:
+            self._render(cam, bg, scale_modifier, antialiasing, 0, None)
+            self._learned_first(key)
+        else:
+            n_host = self._sync_free_slot(key, self.dev)
+            self._render(cam, bg, scale_modifier, antialiasing, self.capacity, n_host)
+        return self.image, self.radii, self.invdepth
+
+    def _gt_float(self, gt: torch.Tensor) -> torch.Tensor:
+        """float [3,H,W] as is; uint8 [H,W,3] (8-bit ground truth) -> byte / 255 in one reused device buffer."""
+        if gt.dtype == torch.uint8:
+            if tuple(gt.shape) != (self.H, self.W, 3):
+                raise ValueError(f"evaluate: uint8 ground truth must be [{self.H},{self.W},3]; got {tuple(gt.shape)}")
+            if self._gt_buf is None:
+                self._gt_buf = torch.empty(3, self.H, self.W, dtype=torch.float32, device=self.dev)
+            return io_image.to_device_float(gt.to(self.dev, non_blocking=True), out=self._gt_buf, hwc=True)
+        if tuple(gt.shape) != (3, self.H, self.W) or gt.dtype != torch.float32:
+            raise ValueError(f"evaluate: float ground truth must be float32 [3,{self.H},{self.W}]; got {gt.dtype} {tuple(gt.shape)}")
+        return gt.to(self.dev, non_blocking=True)
+
+    def evaluate(self, cams: Sequence, gts: Sequence[torch.Tensor], bg: torch.Tensor, protocol: str = "training_report",
+                 scale_modifier: float = 1.0, antialiasing: bool = False) -> Evaluation:
+        """Renders every view and scores it against its ground truth (metrics.METRIC_NAMES under `protocol`, "training_report"
+        or "metrics"), all on the current stream into one device array; the host synchronises once, at the end.  Views whose
+        render overflowed its predicted capacity are then re-rendered, sized from their true N, and re-scored before the
+        array is read."""
+        if len(cams) != len(gts):
+            raise ValueError(f"evaluate: {len(cams)} cameras but {len(gts)} ground-truth images")
+        n = len(cams)
+        out = torch.empty(n, len(METRIC_NAMES), dtype=torch.float64, device=self.dev)
+        slots = torch.full((max(n, 1), 2), -1, dtype=torch.int32).pin_memory()     # per view: (N, overflow flag), mapped
+        slots_np = slots.numpy()
+        keys = [self._view_key(c) for c in cams]
+        caps = []
+
+        def one(v, capacity):
+            self._render(cams[v], bg, scale_modifier, antialiasing, capacity, slots.data_ptr() + 8 * v)
+            image_metrics(self.image, self._gt_float(gts[v]), protocol, out=out[v], scratch=self._metric_scratch)
+
+        for v in range(n):
+            caps.append(self._predict_capacity(keys[v]))
+            one(v, caps[v])
+        torch.cuda.current_stream(self.dev).synchronize()
+        rerun = []
+        for v in range(n):
+            nv = int(slots_np[v, 0])
+            self._note(keys[v], nv)
+            if nv > caps[v]:
+                self.overflows += 1
+                rerun.append(v)
+        for v in rerun:
+            one(v, max(int(slots_np[v, 0]), 1))
+        if n:
+            self.capacity = max(caps)
+        per_view = out.cpu()        # (waits for the re-runs, if any)
+        mean = per_view.mean(0) if n else torch.full((len(METRIC_NAMES),), float("nan"), dtype=torch.float64)
+        return Evaluation(per_view=per_view, mean=mean, rerun=rerun)

@@ -11,8 +11,6 @@ All gradients live in ONE contiguous buffer (param.grad are views into it), so t
 """
 from __future__ import annotations
 
-import collections
-
 import math
 from typing import List, Optional, Sequence
 
@@ -21,6 +19,7 @@ import torch.distributed as dist
 
 import diff_gaussian_rasterization as dgr
 
+from .capacity import SyncFreeCapacity, grow_only_alloc
 from .losses import fused_training_loss
 from .model import MeshGaussianModel
 from .optim import FlatAdam, mesh_model_groups
@@ -48,26 +47,18 @@ def render_frame(model: MeshGaussianModel, cam: Camera, bg: torch.Tensor, fused:
                                                       shs=model.get_features, scales=scales, rotations=rots)
 
 
-class NativeFrame:
+class NativeFrame(SyncFreeCapacity):
     """One training frame through gms_train_frame: expansion, rasterizer, loss and both backward passes issued from ONE C
     call on the current stream -- no autograd graph, no per-op Python.  Gradients land in the parameters' preallocated
     .grad views (FlatAdam's flat buffer); intermediates live in a persistent workspace, rasterizer scratch in grow-only
     buffers served through the allocation callback.
 
     sync_free (default): only the FIRST frame learns N through the stock-style 4-byte read-back; from then on the binning
-    region is capacity-sized, N stays on the device and is mirrored by the range kernel into a ring of mapped pinned host
-    slots (`n_host`: one (N, overflow flag) pair per in-flight frame) that the host polls WITHOUT synchronising.
-    The tile sort runs over the capacity, so the capacity is predicted PER VIEW: 1.08x the N this camera had at its last
-    visit (more when it moved a lot between its last two visits) + 64k; a camera seen for the first time gets 1.25x the
-    largest N seen so far + 256k.  A frame whose N exceeds its capacity renders the background with zero gradients; the
-    host notices when it harvests that frame's slot, counts it in `overflows`, and the camera's next visit is sized from
-    the true N."""
-
-    RING = 64       # mapped (N, flag) slots = frames the host may run ahead of the device before it waits
+    region is sized per view by the capacity prediction of SyncFreeCapacity (gms_b200/capacity.py), and a frame whose N
+    exceeds its capacity renders the background with zero gradients and is counted in `overflows`."""
 
     def __init__(self, model: MeshGaussianModel, width: int, height: int, lambda_dssim: float = 0.2, sync_free: bool = True,
                  world: int = 1, rank: int = 0):
-        import ctypes as C
         from . import _lib
         assert model._features is not None, "NativeFrame needs packed SH features"
         self.model, self.W, self.H, self.lam = model, int(width), int(height), float(lambda_dssim)
@@ -76,16 +67,7 @@ class NativeFrame:
         P = model._scale.shape[0]
         self.ws = torch.empty(int(_lib.lib().gms_frame_workspace_bytes(P, self.W, self.H)), dtype=torch.uint8, device=dev)
         self.loss = torch.zeros(3, dtype=torch.float32, device=dev)
-        self.n_rendered = C.c_int64(0)
-        self.sync_free = bool(sync_free)
-        self.capacity = 0                       # duplicates the most recent frame's binning region was sized for (0: not known yet)
-        self.capacity_override = None           # tests: force the next frames' capacity
-        self.n_host = torch.zeros(self.RING, 2, dtype=torch.int32).pin_memory()   # slot i: (N, overflow flag) of an in-flight frame
-        self._n_np = self.n_host.numpy()
-        self._pending = collections.deque()     # (slot, view key, capacity) of frames whose N has not been harvested yet
-        self._view_n = {}                       # view key -> (N at the last visit, N at the visit before)
-        self._n_max, self._n_last, self._frame_no = 0, 0, 0
-        self.overflows = 0
+        self._init_capacity(sync_free)
         # factored SH gradient (run(..., factored=True)): slot r of `exchange` = [3P colour gradients | camera centre | pad] of
         # rank r's frame; this rank's frame writes slot `rank`, FlatAdam(sh_factored=True) all-gathers and consumes the rest
         self.world, self.rank = int(world), int(rank)
@@ -96,20 +78,7 @@ class NativeFrame:
         self.ev_sh = None           # recorded by gms_train_frame right after the preprocess backward (world > 1: the exchange of the
                                     # colour gradients starts there, on the optimizer's communication stream)
         self._check_model()
-        scratch = {}
-        self._scratch = scratch
-
-        def _alloc(user, which, nbytes):        # grow-only, persistent across frames: no allocator traffic in steady state
-            t = scratch.get(int(which))
-            if t is None or t.numel() < nbytes:
-                try:
-                    t = torch.empty(int(nbytes * 1.25) + (1 << 20), dtype=torch.uint8, device=dev)
-                except Exception:
-                    return 0
-                scratch[int(which)] = t
-            return t.data_ptr()
-
-        self._cb = _lib.ALLOC_FN(_alloc)        # closure captures `scratch`/`dev` only (no reference cycle through self)
+        self._scratch, self._cb = grow_only_alloc(dev)
 
     def _check_model(self):
         """Raw pointers go straight to CUDA kernels: dtype / device / layout are checked here, once, instead of failing
@@ -125,41 +94,6 @@ class NativeFrame:
                 raise RuntimeError(f"NativeFrame: model.{name}.grad must be a preallocated contiguous buffer (FlatAdam provides it)")
         if m.faces.device != self.dev:
             raise RuntimeError("NativeFrame: model.faces must live on the model's device")
-
-    @property
-    def last_num_rendered(self) -> int:
-        """N of the most recent frame whose range kernel has run (no synchronisation: may lag behind the queue)."""
-        if self.sync_free and self.capacity > 0:
-            self._harvest()
-            return self._n_last
-        return int(self.n_rendered.value)
-
-    def _harvest(self) -> None:
-        """Collect (N, overflow) of the frames the device has finished binning; their slots become reusable."""
-        while self._pending:
-            slot, key, cap = self._pending[0]
-            n = int(self._n_np[slot, 0])
-            if n < 0:                       # that frame's k_tile_ranges has not run yet
-                break
-            self._pending.popleft()
-            self._note(key, n)
-            if n > cap:
-                self.overflows += 1
-
-    def _note(self, key, n: int) -> None:
-        prev = self._view_n.get(key)
-        self._view_n[key] = (n, prev[0] if prev else 0)
-        self._n_max, self._n_last = max(self._n_max, n), n
-
-    def _predict_capacity(self, key) -> int:
-        if self.capacity_override is not None:
-            return int(self.capacity_override)
-        known = self._view_n.get(key)
-        if known is None:
-            return int(self._n_max * 1.25) + (1 << 18)
-        n1, n0 = known
-        drift = abs(n1 - n0) / max(n1, 1) if n0 else 0.0
-        return int(n1 * (1.0 + max(0.08, 3.0 * drift))) + (1 << 16)
 
     def read_loss_async(self, loss_host: torch.Tensor, loss_ready: Optional[torch.cuda.Event] = None) -> None:
         """Copy the last frame's loss into pinned host memory from a side stream as soon as the LOSS kernels are done (the
@@ -230,28 +164,16 @@ class NativeFrame:
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
         a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
         a.num_rendered = C.pointer(self.n_rendered)
-        key = getattr(cam, "uid", None)
-        if key is None:
-            key = id(cam)
+        key = self._view_key(cam)
         first = self.capacity == 0
         if self.sync_free and not first:
-            self._harvest()
-            if len(self._pending) >= self.RING - 1:         # the host is a whole ring ahead of the device: wait for the oldest frames
-                torch.cuda.current_stream(self.dev).synchronize()
-                self._harvest()
-            slot = self._frame_no % self.RING
-            self._frame_no += 1
-            self.capacity = self._predict_capacity(key)
-            self._n_np[slot, 0], self._n_np[slot, 1] = -1, 0
-            self._pending.append((slot, key, self.capacity))
-            a.binning_capacity, a.n_host_mapped = self.capacity, self.n_host.data_ptr() + 8 * slot
+            a.n_host_mapped = self._sync_free_slot(key, self.dev)
+            a.binning_capacity = self.capacity
         with torch.cuda.device(self.dev):
             _lib.check(_lib.lib().gms_train_frame(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream),
                        "gms_train_frame")
         if self.sync_free and first:           # the one synchronising frame told us N
-            n = max(int(self.n_rendered.value), 0)
-            self._note(key, n)
-            self.capacity = n
+            self._learned_first(key)
         return self.loss[0]
 
 
@@ -273,6 +195,7 @@ class MeshTrainer:
         self.sync_free = sync_free          # native frames after the first never synchronise with the host (NativeFrame)
         self.loss_fn = loss_fn or fused_training_loss    # fast=False A/B arm: callers may pass an ATen loss (tests/aten_reference.py)
         self._frame = None
+        self._renderer = None
         self.sh_factored = False
         if fast:
             # native frames hand the SH gradient over as factors (12 B instead of 192 B per Gaussian; replicated optimizer);
@@ -351,3 +274,13 @@ class MeshTrainer:
             for p in self.model.parameters():
                 p.grad = None
         return loss.detach()
+
+    def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
+        """L1 / SSIM / PSNR of the current model on held-out views with the trainer's background, the test half of
+        training_report (train.py:183-218): NativeRenderer.evaluate, one host synchronisation for the whole set."""
+        from .render import NativeRenderer
+        W, H = int(cams[0].image_width), int(cams[0].image_height)
+        r = self._renderer
+        if r is None or (r.W, r.H) != (W, H) or r.radii.shape[0] != self.model._scale.shape[0]:
+            r = self._renderer = NativeRenderer(self.model, W, H)
+        return r.evaluate(cams, gts, self.bg, protocol=protocol)

@@ -362,6 +362,55 @@ typedef struct gms_adam_sh_args {
 int gms_adam_sh_factored(const gms_adam_sh_args* a, void* cuda_stream);
 int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
 
+/* ---- rendering and evaluating views ------------------------------------------------------------- */
+
+/* One gs_mesh render in ONE call: the forward half of gms_train_frame (expansion fwd with activated scales / rotations ->
+ * sigmoid(opacity) inside the preprocess -> rasterizer fwd), as a forward-only frame (GMS_FORWARD_ONLY: the binning region
+ * holds the point list only).  Replaces the per-view render of scripts/render.py:25-36 and of the animated sweep,
+ * renderer/gaussian_animated_renderer/__init__.py:61-112 (for scripts/render_time_animated.py the caller moves `vertices`
+ * first, as its :82-84 does).  num_rendered / binning_capacity / n_host_mapped: exactly as in gms_frame_args -- a capacity
+ * of 0 reads N back once (one host synchronisation), a capacity > 0 never synchronises and an overflow (N > capacity)
+ * renders the background with zero inverse depth. */
+typedef struct gms_render_args {
+    int32_t V, F, K, M;
+    const float* vertices; const int64_t* faces; const float* alpha_raw; const float* scale_raw;
+    const float* features;      /* [P,M,3] packed SH (get_features) */
+    const float* opacity_raw;   /* [P,1] logits */
+    float eps;                  /* eps_s0 */
+    gms_raster_settings settings;
+    float* image;               /* out [3,H,W] */
+    float* invdepth;            /* out [1,H,W] */
+    int32_t* radii;             /* out [P] */
+    void* workspace; size_t workspace_bytes;   /* gms_render_workspace_bytes: the expansion outputs and opacities only */
+    int64_t* num_rendered;      /* host, optional (-1 on the sync-free path) */
+    int64_t binning_capacity;
+    uint32_t* n_host_mapped;    /* optional mapped pinned host [2]: N, overflow flag */
+} gms_render_args;
+size_t gms_render_workspace_bytes(int32_t P, int32_t W, int32_t H);
+int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
+
+/* Scores an image against its ground truth, forward only, deterministically (per-tile partial sums added in a fixed order in
+ * double, no atomics: the same inputs give the same bits).  Both images go through the same transform first:
+ *   quantize 0: clamp to [0,1]                                  (training_report, train.py:203-204)
+ *   quantize 1: save_image's 8-bit rounding, back to byte / 255 (scripts/render.py's PNGs as metrics.py reads them)
+ * out (device, double [4]):
+ *   0  L1 = mean |x - y|                                                   (utils/loss_utils.py:17)
+ *   1  SSIM, 11x11 Gaussian window sigma 1.5, zero padding, mean           (utils/loss_utils.py:33-64, metrics.py:72)
+ *   2  PSNR over all channels, -10 log10(mean (x - y)^2)                   (utils/image_utils.py:17-19 on [1,C,H,W], metrics.py:73)
+ *   3  mean over channels of the per-channel PSNR                          (the same psnr on a [C,H,W] tensor, train.py:212)
+ * A PSNR is +inf where the MSE is 0. */
+typedef struct gms_metrics_args {
+    int32_t C, H, W;            /* C <= 4 */
+    const float* img;           /* [C,H,W] */
+    const float* gt;            /* [C,H,W] */
+    int32_t quantize;           /* 0 or 1, see above */
+    double* out;                /* device [4] */
+    void* scratch;              /* gms_metrics_scratch_bytes() bytes */
+    size_t scratch_bytes;
+} gms_metrics_args;
+int gms_metrics_scratch_bytes(int32_t C, int32_t H, int32_t W, size_t* bytes);
+int gms_image_metrics(const gms_metrics_args* a, void* cuda_stream);
+
 /* ---- image sink / source (SURVEY.md section 8(f) rank 4) ---------------------------------------- */
 
 /* float [C,H,W] -> 8-bit interleaved rows, byte = clamp(x * 255 + 0.5, 0, 255) truncated: the device half of

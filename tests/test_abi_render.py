@@ -1,0 +1,25 @@
+"""CPU-only: the ctypes mirrors of gms_render_args (gms_render_frame) and gms_metrics_args (gms_image_metrics) have the size
+and field offsets the C compiler gives the header's structs."""
+import ctypes
+import os
+import subprocess
+
+import pytest
+
+from gms_b200 import _lib
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+@pytest.mark.parametrize("cls,cname", [(_lib.RenderArgs, "gms_render_args"), (_lib.MetricsArgs, "gms_metrics_args")])
+def test_layout_matches_the_ctypes_mirror(tmp_path, cls, cname):
+    body = f'    printf("size %zu\\n", sizeof({cname}));\n'
+    body += "".join(f'    printf("{f[0]} %zu\\n", offsetof({cname}, {f[0]}));\n' for f in cls._fields_)
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "gms_b200.h"\nint main(void) {\n' + body + "    return 0;\n}\n")
+    exe = tmp_path / "layout"
+    subprocess.check_call(["gcc", "-std=c99", "-Wall", "-Wextra", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
+    out = dict(l.split() for l in subprocess.check_output([str(exe)], text=True).strip().split("\n"))
+    assert int(out["size"]) == ctypes.sizeof(cls)
+    for f in cls._fields_:
+        assert int(out[f[0]]) == getattr(cls, f[0]).offset, f[0]
