@@ -1751,27 +1751,40 @@ int gms_expand_backward(const gms_expand_args* a, const gms_expand_grads* g, voi
 
 size_t gms_frame_workspace_bytes(int32_t P, int32_t W, int32_t H) { return frame_layout(nullptr, P, W, H).total + 512; }
 
-// The forward half of a whole frame, shared by gms_train_frame and gms_render_frame: E1-E4 mesh -> Gaussians (activated
-// scales / rotations) into xyz / scales / rots, then the rasterizer forward.  sigmoid(opacity) is computed inside
-// k_preprocess_fwd (which stores it to `opac` for the backward), its derivative inside k_preprocess_bwd: no separate
-// activation launches.  `ea` and `in` are filled for the training frame's backward passes.
+// A whole frame's forward is the model's own expansion step followed by one rasterizer forward, frame_raster_forward, which
+// gms_train_frame, gms_render_frame and gms_points_render_frame share.  The expansion writes activated Gaussians (xyz,
+// scales, unit quaternions) into the frame's workspace.
 struct FrameModel {
     int32_t V, F, K, M;
     const float* vertices; const int64_t* faces; const float* alpha_raw; const float* scale_raw; const float* features;
     const float* opacity_raw; float eps;
 };
 
-static int frame_forward(const FrameModel& m, const gms_raster_settings* s, float* xyz, float* scales, float* rots, float* opac,
-                         gms_raster_outputs* out, gms_alloc_fn alloc, void* user, int64_t binning_capacity, uint32_t* n_host,
-                         void* cuda_stream, gms_expand_args* ea, gms_raster_inputs* in, gms_raster_saved* saved) {
-    int rc;
+// gs_mesh: E1-E4 mesh -> Gaussians (activated scales / rotations) into xyz / scales / rots.  `ea` is filled for the training
+// frame's expansion backward.
+static int mesh_expand_forward(const FrameModel& m, float* xyz, float* scales, float* rots, void* cuda_stream, gms_expand_args* ea) {
     memset(ea, 0, sizeof(*ea));
     ea->V = m.V; ea->F = m.F; ea->K = m.K; ea->vertices = m.vertices; ea->faces = m.faces; ea->alpha_raw = m.alpha_raw;
     ea->scale_raw = m.scale_raw; ea->eps = m.eps; ea->xyz = xyz; ea->scaling_act = scales; ea->rotation_act = rots;
-    if ((rc = gms_expand_forward(ea, cuda_stream))) return rc;
+    return gms_expand_forward(ea, cuda_stream);
+}
+
+// The activated Gaussians an expansion step left in the workspace, with the model's SH features and opacity logits.
+struct FrameGaussians {
+    int32_t P, M;
+    const float* xyz; const float* scales; const float* rots; const float* features; const float* opacity_raw;
+    float* opac;        // [P] sigmoid(opacity_raw), written by the preprocess for the training frame's backward
+};
+
+// The rasterizer forward of a whole frame.  sigmoid(opacity) is computed inside k_preprocess_fwd (which stores it to `opac`),
+// its derivative inside k_preprocess_bwd: no separate activation launches.  `in` is filled for the training frame's backward.
+static int frame_raster_forward(const FrameGaussians& g, const gms_raster_settings* s, gms_raster_outputs* out, gms_alloc_fn alloc,
+                                void* user, int64_t binning_capacity, uint32_t* n_host, void* cuda_stream, gms_raster_inputs* in,
+                                gms_raster_saved* saved) {
     memset(in, 0, sizeof(*in));
-    in->P = m.F * m.K; in->M = m.M; in->means3D = xyz; in->opacities = opac; in->shs = m.features; in->scales = scales; in->rotations = rots;
-    return raster_forward_impl(s, in, out, alloc, user, saved, cuda_stream, binning_capacity, n_host, m.opacity_raw);
+    in->P = g.P; in->M = g.M; in->means3D = g.xyz; in->opacities = g.opac; in->shs = g.features; in->scales = g.scales;
+    in->rotations = g.rots;
+    return raster_forward_impl(s, in, out, alloc, user, saved, cuda_stream, binning_capacity, n_host, g.opacity_raw);
 }
 
 struct RenderLayout { float* xyz; float* scales; float* rots; float* opac; size_t total; };
@@ -1799,9 +1812,38 @@ int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_u
     gms_expand_args ea;
     gms_raster_inputs in;
     gms_raster_saved saved;
-    const int rc = frame_forward(m, &a->settings, RL.xyz, RL.scales, RL.rots, RL.opac, &out, alloc, alloc_user, a->binning_capacity,
-                                 a->n_host_mapped, cuda_stream, &ea, &in, &saved);
-    if (rc) return rc;
+    int rc;
+    if ((rc = mesh_expand_forward(m, RL.xyz, RL.scales, RL.rots, cuda_stream, &ea))) return rc;
+    const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
+    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
+                                   &saved))) return rc;
+    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
+    return GMS_OK;
+}
+
+size_t gms_points_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { return gms_render_workspace_bytes(P, W, H); }
+
+int gms_points_render_frame(const gms_points_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
+    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii)
+        return set_err(GMS_E_ARG, "gms_points_render_frame: null argument%s%s");
+    if (!a->triangles || !a->features || !a->opacity_raw) return set_err(GMS_E_ARG, "gms_points_render_frame: model tensors required%s%s");
+    if (a->P < 0) return set_err(GMS_E_ARG, "gms_points_render_frame: P < 0%s%s");
+    const int P = a->P, W = a->settings.image_width, H = a->settings.image_height;
+    if (a->workspace_bytes < gms_points_render_workspace_bytes(P, W, H))
+        return set_err(GMS_E_ARG, "gms_points_render_frame: workspace too small%s%s");
+    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
+    // pseudo-mesh triangles -> xyz = v1, (eps, exp(log s2), exp(log s3)), normalised quaternion
+    gms_points_args pa;
+    memset(&pa, 0, sizeof(pa));
+    pa.P = P; pa.triangles = a->triangles; pa.eps = a->eps; pa.xyz = RL.xyz; pa.scaling_act = RL.scales; pa.rotation_act = RL.rots;
+    int rc;
+    if ((rc = gms_points_expand_forward(&pa, cuda_stream))) return rc;
+    gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
+    gms_raster_inputs in;
+    gms_raster_saved saved;
+    const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
+    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
+                                   &saved))) return rc;
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;
     return GMS_OK;
 }
@@ -1824,8 +1866,10 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     gms_expand_args ea;
     gms_raster_inputs in;
     gms_raster_saved saved;
-    if ((rc = frame_forward(m, &a->settings, FL.xyz, FL.scales, FL.rots, FL.opac, &out, alloc, alloc_user, a->binning_capacity,
-                            a->n_host_mapped, cuda_stream, &ea, &in, &saved))) return rc;
+    if ((rc = mesh_expand_forward(m, FL.xyz, FL.scales, FL.rots, cuda_stream, &ea))) return rc;
+    const FrameGaussians g = {P, a->M, FL.xyz, FL.scales, FL.rots, a->features, a->opacity_raw, FL.opac};
+    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
+                                   &saved))) return rc;
     // loss + dL/dimage
     gms_loss_args la;
     memset(&la, 0, sizeof(la));

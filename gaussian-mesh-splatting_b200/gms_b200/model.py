@@ -115,6 +115,53 @@ class MeshGaussianModel:
         return self.optimizer
 
 
+class PointsModel:
+    """gs_points pseudo-mesh model for rendering: one triangle per Gaussian (PointsGaussianModel,
+    games/flat_splatting/scene/points_gaussian_model.py, after prepare_vertices).  `triangles` [P,3,3] is what an editing
+    script moves; the SH features stay packed in ONE [P,M,3] tensor (`_features`), so a frame reads them without the
+    reference's per-frame torch.cat; `_opacity` [P,1] holds the logits.  The model carries no scaling / rotation: every
+    frame derives them from the triangles (gms_points_render_frame)."""
+
+    def __init__(self, triangles: torch.Tensor, features: torch.Tensor, opacity: torch.Tensor, active_sh_degree: int = 3,
+                 eps_s0: float = 1e-8):
+        P = triangles.shape[0]
+        if tuple(triangles.shape) != (P, 3, 3) or features.dim() != 3 or tuple(features.shape[::2]) != (P, 3) or \
+                tuple(opacity.shape) != (P, 1):
+            raise ValueError("PointsModel: expected triangles [P,3,3], features [P,M,3], opacity [P,1]")
+        f32 = lambda t: t.detach().float().contiguous()
+        self.triangles, self._features, self._opacity = f32(triangles), f32(features), f32(opacity)
+        self.max_sh_degree = int(round(features.shape[1] ** 0.5)) - 1
+        self.active_sh_degree = min(int(active_sh_degree), self.max_sh_degree)
+        self.eps_s0 = float(eps_s0)         # PointsGaussianModel.eps_s0 (:23), also prepare_scaling_rot's eps (:60)
+
+    @classmethod
+    def from_gaussians(cls, xyz, _scaling, _rotation, features_dc, features_rest, opacity, device="cuda",
+                       active_sh_degree: int = 3) -> "PointsModel":
+        """Flat Gaussians (raw parameters: `_scaling` [P,2|3] log-scales, `_rotation` [P,4]) -> their pseudo-mesh, as
+        PointsGaussianModel.prepare_vertices builds it (expansion.points_prepare_vertices)."""
+        d = lambda t: t.detach().to(device).float().contiguous()
+        tri = expansion.points_prepare_vertices(d(xyz), d(_scaling), d(_rotation))
+        return cls(tri, torch.cat((d(features_dc), d(features_rest)), dim=1), d(opacity), active_sh_degree)
+
+    @classmethod
+    def from_flat_checkpoint(cls, ply_path: str, device="cuda", active_sh_degree: int = 3) -> "PointsModel":
+        """A trained gs_flat (or gs_points) point_cloud.ply -> its pseudo-mesh model: GaussianModel.load_ply, then
+        prepare_vertices, as scripts/render_points_time_animated.py:53-56 loads a checkpoint.  The file's scale_0 column
+        (log eps_s0 of a flat model) is ignored: the triangle spans the last two scales."""
+        from . import io_ply
+        g = io_ply.load_gaussian_ply(ply_path)
+        return cls.from_gaussians(g["_xyz"], g["_scaling"], g["_rotation"], g["_features_dc"], g["_features_rest"], g["_opacity"],
+                                  device, active_sh_degree)
+
+    @property
+    def get_features(self):
+        return self._features
+
+    @property
+    def get_opacity(self):
+        return torch.sigmoid(self._opacity)
+
+
 class MultiMeshGaussianModel(MeshGaussianModel):
     """gs_multi_mesh: several meshes, one Gaussian set (games/multi_mesh_splatting/scene/gaussian_multi_mesh_model.py).
 

@@ -1,8 +1,13 @@
-"""Render and evaluate views of a gs_mesh model natively: one gms_render_frame call per view, no host synchronisation.
+"""Render and evaluate views natively: one gms_render_frame (gs_mesh) or gms_points_render_frame (gs_points pseudo-mesh)
+call per view, no host synchronisation.
 
     renderer = NativeRenderer(model, W, H)
     image, radii, invdepth = renderer.render(cam, bg)                  # scripts/render.py, render_time_animated.py
     result = renderer.evaluate(test_cams, test_gts, bg)               # training_report / metrics.py
+
+    renderer = PointsRenderer(PointsModel.from_flat_checkpoint(ply), W, H)
+    image, radii, invdepth = renderer.render(cam, bg, triangles=transform_hotdog(renderer.model.triangles, t))
+                                                                       # scripts/render_points_time_animated.py
 
 The first render learns N through one 4-byte read-back; every later one is sync-free, with the binning capacity predicted
 per view (SyncFreeCapacity).  An overflowed render (N above its capacity) gives the background image and is counted in
@@ -34,12 +39,9 @@ class NativeRenderer(SyncFreeCapacity):
 
     def __init__(self, model, width: int, height: int):
         self.model, self.W, self.H = model, int(width), int(height)
-        dev = model.vertices.device
+        dev, P = self._adopt(model)
         self.dev = dev
-        P = model._scale.shape[0]
-        if model.faces.dtype != torch.int64 or not model.faces.is_contiguous():
-            model.faces = model.faces.long().contiguous()
-        self.ws = torch.empty(int(_lib.lib().gms_render_workspace_bytes(P, self.W, self.H)), dtype=torch.uint8, device=dev)
+        self.ws = torch.empty(int(self._workspace_bytes(P)), dtype=torch.uint8, device=dev)
         self.image = torch.empty(3, self.H, self.W, dtype=torch.float32, device=dev)
         self.invdepth = torch.empty(1, self.H, self.W, dtype=torch.float32, device=dev)
         self.radii = torch.empty(P, dtype=torch.int32, device=dev)
@@ -47,6 +49,15 @@ class NativeRenderer(SyncFreeCapacity):
         self._scratch, self._cb = grow_only_alloc(dev)
         self._metric_scratch = torch.empty(scratch_bytes(3, self.H, self.W), dtype=torch.uint8, device=dev)
         self._gt_buf = None
+
+    def _adopt(self, model):
+        """(device, Gaussian count) of the model this renderer draws; makes its face indices int64 and contiguous."""
+        if model.faces.dtype != torch.int64 or not model.faces.is_contiguous():
+            model.faces = model.faces.long().contiguous()
+        return model.vertices.device, model._scale.shape[0]
+
+    def _workspace_bytes(self, P: int) -> int:
+        return _lib.lib().gms_render_workspace_bytes(P, self.W, self.H)
 
     def _features(self) -> torch.Tensor:
         m = self.model
@@ -63,12 +74,15 @@ class NativeRenderer(SyncFreeCapacity):
             raise RuntimeError("NativeRenderer: model.faces must live on the model's device")
         if m._scale.shape[0] != self.radii.shape[0]:
             raise RuntimeError("NativeRenderer: the model's Gaussian count changed; make a new renderer")
+        self._check_view(cam, bg)
+
+    def _check_view(self, cam, bg) -> None:
         for t, what in ((bg, "bg"), (cam.world_view_transform, "camera matrices"), (cam.full_proj_transform, "camera matrices"),
                         (cam.camera_center, "camera centre")):
             if not t.is_cuda or t.device != self.dev or t.dtype != torch.float32:
-                raise RuntimeError(f"NativeRenderer: {what} must be float32 on {self.dev}")
+                raise RuntimeError(f"{type(self).__name__}: {what} must be float32 on {self.dev}")
         if int(cam.image_width) != self.W or int(cam.image_height) != self.H:
-            raise ValueError(f"NativeRenderer was sized for {self.W}x{self.H}; got a {cam.image_width}x{cam.image_height} camera")
+            raise ValueError(f"{type(self).__name__} was sized for {self.W}x{self.H}; got a {cam.image_width}x{cam.image_height} camera")
 
     def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
         """One gms_render_frame into the renderer's buffers: capacity 0 = synchronising, else sync-free with (N, flag) at
@@ -80,18 +94,21 @@ class NativeRenderer(SyncFreeCapacity):
         a.V, a.F, a.K, a.M = m.vertices.shape[0], m._alpha.shape[0], m._alpha.shape[1], feats.shape[1]
         a.vertices, a.faces, a.alpha_raw, a.scale_raw = m.vertices.data_ptr(), m.faces.data_ptr(), m._alpha.data_ptr(), m._scale.data_ptr()
         a.features, a.opacity_raw, a.eps = feats.data_ptr(), m._opacity.data_ptr(), m.eps_s0
+        self._call("gms_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
+
+    def _call(self, fn: str, a, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+        """Fills the settings, outputs, workspace and capacity fields shared by every render-args struct and calls `fn`."""
         s = a.settings
         s.image_height, s.image_width, s.tanfovx, s.tanfovy = self.H, self.W, cam.tanfovx, cam.tanfovy
         s.bg, s.scale_modifier = bg.data_ptr(), float(scale_modifier)
         s.viewmatrix, s.projmatrix, s.campos = cam.world_view_transform.data_ptr(), cam.full_proj_transform.data_ptr(), cam.camera_center.data_ptr()
-        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = m.active_sh_degree, 0, 0, int(bool(antialiasing))
+        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = self.model.active_sh_degree, 0, 0, int(bool(antialiasing))
         a.image, a.invdepth, a.radii = self.image.data_ptr(), self.invdepth.data_ptr(), self.radii.data_ptr()
         a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
         a.num_rendered = C.pointer(self.n_rendered)
         a.binning_capacity, a.n_host_mapped = int(capacity), n_host
         with torch.cuda.device(self.dev):
-            _lib.check(_lib.lib().gms_render_frame(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream),
-                       "gms_render_frame")
+            _lib.check(getattr(_lib.lib(), fn)(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream), fn)
 
     def render(self, cam, bg: torch.Tensor, scale_modifier: float = 1.0, antialiasing: bool = False):
         """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view, the reference's render(...)["render"], ["radii"],
@@ -154,3 +171,68 @@ class NativeRenderer(SyncFreeCapacity):
         per_view = out.cpu()        # (waits for the re-runs, if any)
         mean = per_view.mean(0) if n else torch.full((len(METRIC_NAMES),), float("nan"), dtype=torch.float64)
         return Evaluation(per_view=per_view, mean=mean, rerun=rerun)
+
+
+class PointsRenderer(NativeRenderer):
+    """NativeRenderer for a gs_points pseudo-mesh model (model.PointsModel): every render derives the Gaussians from the
+    triangles inside gms_points_render_frame.  evaluate(), the capacity prediction and the overflow re-runs are
+    NativeRenderer's."""
+
+    _frame_triangles = None     # set by render(triangles=...) for that one frame
+
+    def _adopt(self, model):
+        return model.triangles.device, model.triangles.shape[0]
+
+    def _workspace_bytes(self, P: int) -> int:
+        return _lib.lib().gms_points_render_workspace_bytes(P, self.W, self.H)
+
+    def _check(self, cam, bg) -> None:
+        m = self.model
+        for name, t in (("triangles", self._triangles), ("_features", m._features), ("_opacity", m._opacity)):
+            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
+                raise RuntimeError(f"PointsRenderer: {name} must be a contiguous float32 CUDA tensor on {self.dev}")
+        P = self.radii.shape[0]
+        if tuple(self._triangles.shape) != (P, 3, 3) or m._features.shape[0] != P or tuple(m._opacity.shape) != (P, 1):
+            raise RuntimeError(f"PointsRenderer: sized for {P} Gaussians: triangles must be [{P},3,3], features [{P},M,3], "
+                               f"opacity [{P},1]; got {tuple(self._triangles.shape)}")
+        self._check_view(cam, bg)
+
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+        m = self.model
+        self._check(cam, bg)
+        a = _lib.PointsRenderArgs()
+        a.P, a.M = self.radii.shape[0], m._features.shape[1]
+        a.triangles, a.features, a.opacity_raw, a.eps = self._triangles.data_ptr(), m._features.data_ptr(), m._opacity.data_ptr(), m.eps_s0
+        self._call("gms_points_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
+
+    @property
+    def _triangles(self) -> torch.Tensor:
+        return self.model.triangles if self._frame_triangles is None else self._frame_triangles
+
+    def render(self, cam, bg: torch.Tensor, triangles: torch.Tensor = None, scale_modifier: float = 1.0, antialiasing: bool = False):
+        """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view.  `triangles` [P,3,3], when given, are this frame's
+        pseudo-mesh in place of the model's (the `triangles` argument of renderer/gaussian_points_animated_renderer's
+        render); the model is never modified.  (The reference's render calls pc.prepare_scaling_rot(triangles), which
+        overwrites pc._scaling and pc._rotation with those of the frame's triangles.)"""
+        self._frame_triangles = None if triangles is None else triangles.detach()
+        try:
+            return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing)
+        finally:
+            self._frame_triangles = None
+
+
+def render_points_frame(model, cam, bg: torch.Tensor, triangles: torch.Tensor = None, scale_modifier: float = 1.0,
+                        antialiasing: bool = False):
+    """The same render through the autograd shim, as renderer/gaussian_points_animated_renderer/__init__.py:21-114 does it
+    on the library's kernels: expansion.points_prepare_scaling_rot(activated=True), an ATen sigmoid and GaussianRasterizer
+    (whose forward reads N back to the host).  Returns (image, radii, invdepth)."""
+    import diff_gaussian_rasterization as dgr
+    from . import expansion
+    tri = model.triangles if triangles is None else triangles
+    xyz, scales, rots = expansion.points_prepare_scaling_rot(tri, model.eps_s0, activated=True)
+    rs = dgr.GaussianRasterizationSettings(
+        image_height=int(cam.image_height), image_width=int(cam.image_width), tanfovx=cam.tanfovx, tanfovy=cam.tanfovy,
+        bg=bg, scale_modifier=float(scale_modifier), viewmatrix=cam.world_view_transform, projmatrix=cam.full_proj_transform,
+        sh_degree=model.active_sh_degree, campos=cam.camera_center, prefiltered=False, debug=False, antialiasing=antialiasing)
+    return dgr.GaussianRasterizer(raster_settings=rs)(means3D=xyz, means2D=torch.zeros_like(xyz), opacities=model.get_opacity,
+                                                      shs=model.get_features, scales=scales, rotations=rots)

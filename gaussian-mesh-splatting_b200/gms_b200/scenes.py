@@ -251,3 +251,12 @@ def transform_hotdog_fly(vertices: torch.Tensor, t) -> torch.Tensor:
     out = vertices.clone()
     out[:, 2] += t * (vertices[:, 1] ** 2 + vertices[:, 1] ** 2) ** 0.5 * 0.01
     return out
+
+
+def transform_hotdog(triangles: torch.Tensor, t) -> torch.Tensor:
+    """Pseudo-mesh animation of scripts/render_points_time_animated.py:27-30: every triangle vertex moves by
+    z += 0.3 sin(pi x + t).  The reference script sweeps t = linspace(0, 10 pi, len(views)) but renders every view at
+    t[43] (:44); here `t` is the caller's."""
+    out = triangles.clone()
+    out[:, :, 2] += 0.3 * torch.sin(triangles[:, :, 0] * math.pi + t)
+    return out

@@ -389,6 +389,32 @@ typedef struct gms_render_args {
 size_t gms_render_workspace_bytes(int32_t P, int32_t W, int32_t H);
 int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
 
+/* One gs_points (pseudo-mesh) render in ONE call: the pseudo-mesh expansion (gms_points_expand_forward with activated outputs:
+ * xyz = v1, scaling (eps, exp(log s2), exp(log s3)), normalised quaternion) -> sigmoid(opacity) inside the preprocess ->
+ * rasterizer fwd, as a forward-only frame (GMS_FORWARD_ONLY: the binning region holds the point list only).  Replaces the
+ * per-view render of renderer/gaussian_points_animated_renderer/__init__.py:21-114 (prepare_scaling_rot(triangles), the
+ * getters and GaussianRasterizer) as scripts/render_points_time_animated.py, scripts/render_from_object.py and
+ * scripts/render.py --gs_type gs_points call it; the caller transforms `triangles` first, as those scripts do.  Unlike the
+ * reference, nothing of the model is overwritten.  num_rendered / binning_capacity / n_host_mapped: exactly as in
+ * gms_render_args. */
+typedef struct gms_points_render_args {
+    int32_t P, M;
+    const float* triangles;     /* [P,3,3] pseudo-mesh triangles of this frame */
+    const float* features;      /* [P,M,3] packed SH (get_features) */
+    const float* opacity_raw;   /* [P,1] logits */
+    float eps;                  /* eps_s0 = prepare_scaling_rot's eps, 1e-8 */
+    gms_raster_settings settings;
+    float* image;               /* out [3,H,W] */
+    float* invdepth;            /* out [1,H,W] */
+    int32_t* radii;             /* out [P] */
+    void* workspace; size_t workspace_bytes;   /* gms_points_render_workspace_bytes: the expansion outputs and opacities only */
+    int64_t* num_rendered;      /* host, optional (-1 on the sync-free path) */
+    int64_t binning_capacity;
+    uint32_t* n_host_mapped;    /* optional mapped pinned host [2]: N, overflow flag */
+} gms_points_render_args;
+size_t gms_points_render_workspace_bytes(int32_t P, int32_t W, int32_t H);
+int gms_points_render_frame(const gms_points_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
+
 /* Scores an image against its ground truth, forward only, deterministically (per-tile partial sums added in a fixed order in
  * double, no atomics: the same inputs give the same bits).  Both images go through the same transform first:
  *   quantize 0: clamp to [0,1]                                  (training_report, train.py:203-204)
