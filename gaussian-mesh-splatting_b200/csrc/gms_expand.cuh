@@ -336,9 +336,9 @@ GMS_HD void gms_expand_face_bwd(const gms_expand_args& a, const gms_expand_grads
 // PointsGaussianModel.prepare_scaling_rot  games/flat_splatting/scene/points_gaussian_model.py:61-104 and the per-frame
 // call in renderer/gaussian_points_animated_renderer/__init__.py:61-66 (_xyz = triangles[:, 0]).  Forward only: the
 // reference uses it under torch.no_grad() in scripts/render_points_time_animated.py.
-GMS_HD void gms_points_face_fwd(const gms_points_args& a, int i) {
-    const float* t = a.triangles + 9 * (size_t)i;
-    const float* v1 = t; const float* v2 = t + 3; const float* v3 = t + 6;
+// The core takes the triangle's three vertices from wherever the caller holds them (the triangles array, or registers of
+// the mesh-driven kernel); `i` indexes the outputs.
+GMS_HD void gms_points_core_fwd(const gms_points_args& a, int i, const float* v1, const float* v2, const float* v3) {
     float e2[3], e3[3];
 #pragma unroll
     for (int k = 0; k < 3; k++) { e2[k] = v2[k] - v1[k]; e3[k] = v3[k] - v1[k]; }
@@ -373,6 +373,104 @@ GMS_HD void gms_points_face_fwd(const gms_points_args& a, int i) {
     if (a.rotation_act) {
         const float qn = fmaxf(GMS_SQRTN(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
         float* o = a.rotation_act + 4 * (size_t)i; o[0] = GMS_DIVN(q[0], qn); o[1] = GMS_DIVN(q[1], qn); o[2] = GMS_DIVN(q[2], qn); o[3] = GMS_DIVN(q[3], qn);
+    }
+}
+
+GMS_HD void gms_points_face_fwd(const gms_points_args& a, int i) {
+    const float* t = a.triangles + 9 * (size_t)i;
+    gms_points_core_fwd(a, i, t, t + 3, t + 6);
+}
+
+// ---- mesh-driven pseudo-mesh: every pseudo-triangle is bound to the nearest face of a driving mesh and follows it
+// (scripts/edit_pseudomesh_based_on_estimated_mesh.py:8-82).  Every operation is an explicit round-to-nearest one with no
+// contraction, so numpy (float32 / float64) restates each function bit for bit (tests/pseudomesh_oracle.py).
+#if defined(__CUDA_ARCH__)
+#define GMS_DMUL(a, b) __dmul_rn((a), (b))
+#define GMS_DADD(a, b) __dadd_rn((a), (b))
+#define GMS_DSUB(a, b) __dsub_rn((a), (b))
+#define GMS_DDIV(a, b) __ddiv_rn((a), (b))
+#else
+#define GMS_DMUL(a, b) ((a) * (b))
+#define GMS_DADD(a, b) ((a) + (b))
+#define GMS_DSUB(a, b) ((a) - (b))
+#define GMS_DDIV(a, b) ((a) / (b))
+#endif
+
+// A face's frame: the skewed basis (n, e1, e2) of the reference (:32-43, :62-70), n = normalise(cross(v2 - v1, v3 - v1)),
+// e1 = normalise(v2 - v1), e2 = normalise(v3 - v1).  IEEE division and square root: the norms may be 0.  Returns true when
+// the face is degenerate (one of the three norms is exactly 0; its frame is then non-finite).
+struct GmsPmFrame { float n[3], e1[3], e2[3]; };
+
+GMS_HD float gms_pm_norm(const float* v) {
+    return GMS_SQRT(GMS_ADD(GMS_ADD(GMS_MUL(v[0], v[0]), GMS_MUL(v[1], v[1])), GMS_MUL(v[2], v[2])));
+}
+
+GMS_HD bool gms_pm_frame(const float* v1, const float* v2, const float* v3, GmsPmFrame& f) {
+    float a[3], b[3], c[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) { a[k] = GMS_SUB(v2[k], v1[k]); b[k] = GMS_SUB(v3[k], v1[k]); }
+    c[0] = GMS_SUB(GMS_MUL(a[1], b[2]), GMS_MUL(a[2], b[1]));
+    c[1] = GMS_SUB(GMS_MUL(a[2], b[0]), GMS_MUL(a[0], b[2]));
+    c[2] = GMS_SUB(GMS_MUL(a[0], b[1]), GMS_MUL(a[1], b[0]));
+    const float la = gms_pm_norm(a), lb = gms_pm_norm(b), lc = gms_pm_norm(c);
+#pragma unroll
+    for (int k = 0; k < 3; k++) { f.n[k] = GMS_DIV(c[k], lc); f.e1[k] = GMS_DIV(a[k], la); f.e2[k] = GMS_DIV(b[k], lb); }
+    return la == 0.f || lb == 0.f || lc == 0.f;
+}
+
+// Centroid of a pseudo-triangle or a face, ((v0 + v1) + v2) / 3.
+GMS_HD void gms_pm_centroid(const float* v0, const float* v1, const float* v2, float* m) {
+#pragma unroll
+    for (int k = 0; k < 3; k++) m[k] = GMS_DIV(GMS_ADD(GMS_ADD(v0[k], v1[k]), v2[k]), 3.0f);
+}
+
+// Squared distance between two centroids in double, as sklearn's Euclidean rdist sums it: (dx*dx + dy*dy) + dz*dz.
+GMS_HD double gms_pm_dist2(double qx, double qy, double qz, double cx, double cy, double cz) {
+    const double dx = GMS_DSUB(qx, cx), dy = GMS_DSUB(qy, cy), dz = GMS_DSUB(qz, cz);
+    return GMS_DADD(GMS_DADD(GMS_DMUL(dx, dx), GMS_DMUL(dy, dy)), GMS_DMUL(dz, dz));
+}
+
+GMS_HD void gms_pm_dcross(const double* a, const double* b, double* c) {
+    c[0] = GMS_DSUB(GMS_DMUL(a[1], b[2]), GMS_DMUL(a[2], b[1]));
+    c[1] = GMS_DSUB(GMS_DMUL(a[2], b[0]), GMS_DMUL(a[0], b[2]));
+    c[2] = GMS_DSUB(GMS_DMUL(a[0], b[1]), GMS_DMUL(a[1], b[0]));
+}
+
+GMS_HD double gms_pm_ddot(const double* a, const double* b) {
+    return GMS_DADD(GMS_DADD(GMS_DMUL(a[0], b[0]), GMS_DMUL(a[1], b[1])), GMS_DMUL(a[2], b[2]));
+}
+
+// Coefficients of the three pseudo-vertices w_j in the face's frame: [n|e1|e2] c_j = w_j - v1 (the reference's
+// torch.linalg.solve, :52-54), solved in double through the adjugate and rounded to fp32.  c[3*j + k] multiplies n, e1, e2
+// for k = 0, 1, 2.
+GMS_HD void gms_pm_coeffs(const GmsPmFrame& f, const float* v1, const float* w, float* c) {
+    double n[3], e1[3], e2[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) { n[k] = f.n[k]; e1[k] = f.e1[k]; e2[k] = f.e2[k]; }
+    double r0[3], r1[3], r2[3];           // rows of det * inverse
+    gms_pm_dcross(e1, e2, r0);
+    gms_pm_dcross(e2, n, r1);
+    gms_pm_dcross(n, e1, r2);
+    const double det = gms_pm_ddot(n, r0);
+#pragma unroll
+    for (int j = 0; j < 3; j++) {
+        double d[3];
+#pragma unroll
+        for (int k = 0; k < 3; k++) d[k] = GMS_DSUB((double)w[3 * j + k], (double)v1[k]);
+        c[3 * j] = (float)GMS_DDIV(gms_pm_ddot(d, r0), det);
+        c[3 * j + 1] = (float)GMS_DDIV(gms_pm_ddot(d, r1), det);
+        c[3 * j + 2] = (float)GMS_DDIV(gms_pm_ddot(d, r2), det);
+    }
+}
+
+// Re-pose: w_j = ((v1 + c_j0 n) + c_j1 e1) + c_j2 e2 in the (driving) face's frame (calc_new_vertices_position, :8-12).
+GMS_HD void gms_pm_repose(const GmsPmFrame& f, const float* v1, const float* c, float* w) {
+#pragma unroll
+    for (int j = 0; j < 3; j++) {
+#pragma unroll
+        for (int k = 0; k < 3; k++)
+            w[3 * j + k] = GMS_ADD(GMS_ADD(GMS_ADD(v1[k], GMS_MUL(c[3 * j], f.n[k])), GMS_MUL(c[3 * j + 1], f.e1[k])),
+                                   GMS_MUL(c[3 * j + 2], f.e2[k]));
     }
 }
 

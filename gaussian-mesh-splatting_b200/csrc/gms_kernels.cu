@@ -881,6 +881,126 @@ __global__ void __launch_bounds__(128) k_points_vertices(gms_points_vertices_arg
     gms_points_vertices_fwd(a, i);
 }
 
+// ------------------------------------------------------------------------------------------ mesh-driven pseudo-mesh
+// scripts/edit_pseudomesh_based_on_estimated_mesh.py:14-94: bind every pseudo-triangle to the nearest face of a driving mesh
+// (nearest centroid, brute force), then re-pose it from any pose of that mesh (gms_expand.cuh: gms_pm_*).
+#define GMS_PM_BLOCK 128
+#define GMS_PM_TILE 512        // face centroids staged through shared memory per pass
+
+__device__ __forceinline__ void pm_load_face(const float* __restrict__ vertices, const int64_t* __restrict__ faces, int f, float* v) {
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const int64_t vi = faces[3 * (size_t)f + c];
+        v[3 * c] = vertices[3 * vi]; v[3 * c + 1] = vertices[3 * vi + 1]; v[3 * c + 2] = vertices[3 * vi + 2];
+    }
+}
+
+// Per face: (centroid, 1 if degenerate else 0), and the number of degenerate faces.
+__global__ void __launch_bounds__(GMS_PM_BLOCK) k_pseudomesh_faces(int F, const float* __restrict__ vertices,
+                                                                    const int64_t* __restrict__ faces, float4* __restrict__ cent,
+                                                                    uint32_t* __restrict__ n_degenerate) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= F) return;
+    float v[9], m[3];
+    pm_load_face(vertices, faces, f, v);
+    GmsPmFrame fr;
+    const bool deg = gms_pm_frame(v, v + 3, v + 6, fr);
+    gms_pm_centroid(v, v + 3, v + 6, m);
+    cent[f] = make_float4(m[0], m[1], m[2], deg ? 1.f : 0.f);
+    if (deg) atomicAdd(n_degenerate, 1u);
+}
+
+// One thread per pseudo-triangle: nearest non-degenerate face centroid (double distance, lowest index on a tie; the first
+// non-degenerate face is taken whatever its distance, so a non-finite query still binds in range), then the 9 coefficients.
+__global__ void __launch_bounds__(GMS_PM_BLOCK) k_pseudomesh_bind(int P, int F, const float* __restrict__ triangles,
+                                                                   const float* __restrict__ vertices, const int64_t* __restrict__ faces,
+                                                                   const float4* __restrict__ cent, int32_t* __restrict__ face_out,
+                                                                   float* __restrict__ coeffs) {
+    __shared__ double sx[GMS_PM_TILE], sy[GMS_PM_TILE], sz[GMS_PM_TILE];
+    __shared__ uint8_t sdeg[GMS_PM_TILE];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    float w[9], q[3] = {0.f, 0.f, 0.f};
+    if (i < P) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) w[k] = triangles[9 * (size_t)i + k];
+        gms_pm_centroid(w, w + 3, w + 6, q);
+    }
+    const double qx = q[0], qy = q[1], qz = q[2];
+    double best = 0.0;
+    int bi = -1;
+    for (int t0 = 0; t0 < F; t0 += GMS_PM_TILE) {
+        const int n = min(GMS_PM_TILE, F - t0);
+        __syncthreads();
+        for (int j = threadIdx.x; j < n; j += blockDim.x) {
+            const float4 c = cent[t0 + j];
+            sx[j] = c.x; sy[j] = c.y; sz[j] = c.z; sdeg[j] = c.w != 0.f;
+        }
+        __syncthreads();
+        for (int j = 0; j < n; j++) {
+            if (sdeg[j]) continue;
+            const double d = gms_pm_dist2(qx, qy, qz, sx[j], sy[j], sz[j]);
+            if (d < best || bi < 0) { best = d; bi = t0 + j; }
+        }
+    }
+    if (i >= P) return;
+    float v[9], c[9];
+    pm_load_face(vertices, faces, bi, v);
+    GmsPmFrame fr;
+    gms_pm_frame(v, v + 3, v + 6, fr);
+    gms_pm_coeffs(fr, v, w, c);
+    face_out[i] = bi;
+#pragma unroll
+    for (int k = 0; k < 9; k++) coeffs[9 * (size_t)i + k] = c[k];
+}
+
+// The pseudo-triangle of binding i in the driving pose (vertices, faces).
+__device__ __forceinline__ void pm_reposed(const gms_pseudomesh_repose_args& a, int i, float* w) {
+    float v[9], c[9];
+    pm_load_face(a.vertices, a.faces, a.face[i], v);
+#pragma unroll
+    for (int k = 0; k < 9; k++) c[k] = a.coeffs[9 * (size_t)i + k];
+    GmsPmFrame fr;
+    gms_pm_frame(v, v + 3, v + 6, fr);
+    gms_pm_repose(fr, v, c, w);
+}
+
+__global__ void __launch_bounds__(GMS_PM_BLOCK) k_pseudomesh_repose(gms_pseudomesh_repose_args a) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.P) return;
+    float w[9];
+    pm_reposed(a, i, w);
+#pragma unroll
+    for (int k = 0; k < 9; k++) a.triangles[9 * (size_t)i + k] = w[k];
+}
+
+// Re-pose + the gs_points expansion in one pass (the triangles never reach global memory).  The core reads the re-posed
+// triangle from a per-thread slot in shared memory, as k_points_expand_fwd reads it from the triangles array: the core's
+// fp32 expressions leave contraction to the compiler, and reading the vertices from memory in both kernels keeps its
+// choices, and so the Gaussians, bit-identical to the triangles path.  A Gaussian whose re-posed triangle is not finite (its
+// driving face is degenerate in this pose) is placed at the camera centre, -R^T t of the view matrix: its view-space depth
+// is ~0 <= the near plane, so the preprocess's first test culls it (radius 0, no tile) before it reads anything else of it.
+__global__ void __launch_bounds__(GMS_PM_BLOCK) k_points_bound_expand_fwd(gms_pseudomesh_repose_args r, gms_points_args a,
+                                                                           const float* __restrict__ view) {
+    __shared__ float tri[GMS_PM_BLOCK * 9];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= r.P) return;
+    float w[9];
+    pm_reposed(r, i, w);
+    float* t = tri + 9 * threadIdx.x;
+#pragma unroll
+    for (int k = 0; k < 9; k++) t[k] = w[k];
+    asm volatile("" ::: "memory");      // no store-to-load forwarding: the core loads its vertices, as in the triangles path
+    gms_points_core_fwd(a, i, t, t + 3, t + 6);
+    bool finite = true;
+#pragma unroll
+    for (int k = 0; k < 9; k++) finite = finite && isfinite(w[k]);
+    if (!finite) {
+#pragma unroll
+        for (int j = 0; j < 3; j++)
+            a.xyz[3 * (size_t)i + j] = -(view[4 * j] * view[12] + view[4 * j + 1] * view[13] + view[4 * j + 2] * view[14]);
+    }
+}
+
 // ------------------------------------------------------------------------------------------ fused Adam
 // torch.optim.Adam(lr per group, betas, eps=1e-15) of gaussian_mesh_model.py:171-183 over ONE flat parameter buffer:
 // p, g, m, v are flat fp32 arrays; segments carry the per-group learning rates (feature segment: lr0 for the DC
@@ -1842,6 +1962,90 @@ int gms_points_render_frame(const gms_points_render_args* a, gms_alloc_fn alloc,
     gms_raster_inputs in;
     gms_raster_saved saved;
     const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
+    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
+                                   &saved))) return rc;
+    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
+    return GMS_OK;
+}
+
+size_t gms_pseudomesh_bind_scratch_bytes(int32_t F) {
+    return align_up(16 * (size_t)(F > 0 ? F : 1)) + 256 + 512;
+}
+
+int gms_pseudomesh_bind(const gms_pseudomesh_bind_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !a->vertices || !a->faces || !a->n_degenerate || !a->scratch || (a->P > 0 && (!a->triangles || !a->face || !a->coeffs)))
+        return set_err(GMS_E_ARG, "gms_pseudomesh_bind: null argument%s%s");
+    if (a->P < 0 || a->F < 1 || a->V < 1) return set_err(GMS_E_ARG, "gms_pseudomesh_bind: need P >= 0, F >= 1, V >= 1%s%s");
+    if (a->scratch_bytes < gms_pseudomesh_bind_scratch_bytes(a->F)) return set_err(GMS_E_ARG, "gms_pseudomesh_bind: scratch too small%s%s");
+    char* base = reinterpret_cast<char*>(aligned_base_c(a->scratch));
+    float4* cent = carve<float4>(base, a->F);
+    uint32_t* n_deg = carve<uint32_t>(base, 1);
+    GMS_CUDA(cudaMemsetAsync(n_deg, 0, sizeof(uint32_t), st));
+    span_begin(K_MISC, st);
+    k_pseudomesh_faces<<<(a->F + GMS_PM_BLOCK - 1) / GMS_PM_BLOCK, GMS_PM_BLOCK, 0, st>>>(a->F, a->vertices, a->faces, cent, n_deg);
+    GMS_AFTER_LAUNCH("pseudomesh_faces", 0, st);
+    span_end(st);
+    uint32_t nd = 0;
+    GMS_CUDA(cudaMemcpyAsync(&nd, n_deg, sizeof(nd), cudaMemcpyDeviceToHost, st));
+    GMS_CUDA(cudaStreamSynchronize(st));
+    *a->n_degenerate = (int32_t)nd;
+    if ((int64_t)nd >= a->F) return set_err(GMS_E_ARG, "gms_pseudomesh_bind: every face of the mesh is degenerate%s%s");
+    if (a->P == 0) return GMS_OK;
+    span_begin(K_MISC, st);
+    k_pseudomesh_bind<<<(a->P + GMS_PM_BLOCK - 1) / GMS_PM_BLOCK, GMS_PM_BLOCK, 0, st>>>(a->P, a->F, a->triangles, a->vertices, a->faces,
+                                                                                          cent, a->face, a->coeffs);
+    GMS_AFTER_LAUNCH("pseudomesh_bind", 0, st);
+    span_end(st);
+    return GMS_OK;
+}
+
+static bool repose_args_ok(const gms_pseudomesh_repose_args& r) {
+    return r.P >= 0 && r.F >= 1 && r.V >= 1 && (r.P == 0 || (r.face && r.coeffs && r.vertices && r.faces));
+}
+
+int gms_pseudomesh_repose(const gms_pseudomesh_repose_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !repose_args_ok(*a) || (a->P > 0 && !a->triangles)) return set_err(GMS_E_ARG, "gms_pseudomesh_repose: bad arguments%s%s");
+    if (a->P == 0) return GMS_OK;
+    span_begin(K_MISC, st);
+    k_pseudomesh_repose<<<(a->P + GMS_PM_BLOCK - 1) / GMS_PM_BLOCK, GMS_PM_BLOCK, 0, st>>>(*a);
+    GMS_AFTER_LAUNCH("pseudomesh_repose", 0, st);
+    span_end(st);
+    return GMS_OK;
+}
+
+size_t gms_bound_points_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { return gms_render_workspace_bytes(P, W, H); }
+
+int gms_bound_points_render_frame(const gms_bound_points_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii)
+        return set_err(GMS_E_ARG, "gms_bound_points_render_frame: null argument%s%s");
+    if (!a->face || !a->coeffs || !a->vertices || !a->faces || !a->features || !a->opacity_raw || !a->settings.viewmatrix)
+        return set_err(GMS_E_ARG, "gms_bound_points_render_frame: model tensors required%s%s");
+    if (a->P < 0 || a->F < 1 || a->V < 1) return set_err(GMS_E_ARG, "gms_bound_points_render_frame: need P >= 0, F >= 1, V >= 1%s%s");
+    const int P = a->P, W = a->settings.image_width, H = a->settings.image_height;
+    if (a->workspace_bytes < gms_bound_points_render_workspace_bytes(P, W, H))
+        return set_err(GMS_E_ARG, "gms_bound_points_render_frame: workspace too small%s%s");
+    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
+    // binding + driving pose -> re-posed triangle -> xyz = v1, (eps, exp(log s2), exp(log s3)), normalised quaternion
+    if (P > 0) {
+        gms_pseudomesh_repose_args r;
+        memset(&r, 0, sizeof(r));
+        r.P = P; r.face = a->face; r.coeffs = a->coeffs; r.V = a->V; r.F = a->F; r.vertices = a->vertices; r.faces = a->faces;
+        gms_points_args pa;
+        memset(&pa, 0, sizeof(pa));
+        pa.P = P; pa.eps = a->eps; pa.xyz = RL.xyz; pa.scaling_act = RL.scales; pa.rotation_act = RL.rots;
+        span_begin(K_EXP_FWD, st);
+        k_points_bound_expand_fwd<<<(P + GMS_PM_BLOCK - 1) / GMS_PM_BLOCK, GMS_PM_BLOCK, 0, st>>>(r, pa, a->settings.viewmatrix);
+        GMS_AFTER_LAUNCH("points_bound_expand_fwd", 0, st);
+        span_end(st);
+    }
+    gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
+    gms_raster_inputs in;
+    gms_raster_saved saved;
+    const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
+    int rc;
     if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
                                    &saved))) return rc;
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;

@@ -142,6 +142,29 @@ class PointsRenderArgs(C.Structure):
                 ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p)]
 
 
+class PseudomeshBindArgs(C.Structure):
+    """struct gms_pseudomesh_bind_args"""
+    _fields_ = [("P", C.c_int32), ("triangles", C.c_void_p), ("V", C.c_int32), ("F", C.c_int32), ("vertices", C.c_void_p),
+                ("faces", C.c_void_p), ("face", C.c_void_p), ("coeffs", C.c_void_p), ("n_degenerate", C.POINTER(C.c_int32)),
+                ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t)]
+
+
+class PseudomeshReposeArgs(C.Structure):
+    """struct gms_pseudomesh_repose_args"""
+    _fields_ = [("P", C.c_int32), ("face", C.c_void_p), ("coeffs", C.c_void_p), ("V", C.c_int32), ("F", C.c_int32),
+                ("vertices", C.c_void_p), ("faces", C.c_void_p), ("triangles", C.c_void_p)]
+
+
+class BoundPointsRenderArgs(C.Structure):
+    """struct gms_bound_points_render_args"""
+    _fields_ = [("P", C.c_int32), ("M", C.c_int32), ("face", C.c_void_p), ("coeffs", C.c_void_p), ("V", C.c_int32),
+                ("F", C.c_int32), ("vertices", C.c_void_p), ("faces", C.c_void_p), ("features", C.c_void_p),
+                ("opacity_raw", C.c_void_p), ("eps", C.c_float), ("settings", RasterSettings),
+                ("image", C.c_void_p), ("invdepth", C.c_void_p), ("radii", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)),
+                ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p)]
+
+
 class MetricsArgs(C.Structure):
     """struct gms_metrics_args"""
     _fields_ = [("C", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("img", C.c_void_p), ("gt", C.c_void_p),
@@ -165,7 +188,9 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_frame_workspace_bytes", "gms_train_frame", "gms_points_expand_forward",
                "gms_points_prepare_vertices", "gms_image_quantize", "gms_image_dequantize", "gms_adam_sh_factored", "gms_frame_views",
                "gms_render_workspace_bytes", "gms_render_frame", "gms_metrics_scratch_bytes", "gms_image_metrics",
-               "gms_points_render_workspace_bytes", "gms_points_render_frame"]
+               "gms_points_render_workspace_bytes", "gms_points_render_frame", "gms_pseudomesh_bind_scratch_bytes",
+               "gms_pseudomesh_bind", "gms_pseudomesh_repose", "gms_bound_points_render_workspace_bytes",
+               "gms_bound_points_render_frame"]
 
 _lib = None
 
@@ -222,6 +247,13 @@ def lib():
     L.gms_points_render_workspace_bytes.restype = C.c_size_t
     L.gms_points_render_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.gms_points_render_frame.argtypes = [C.POINTER(PointsRenderArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
+    L.gms_pseudomesh_bind_scratch_bytes.restype = C.c_size_t
+    L.gms_pseudomesh_bind_scratch_bytes.argtypes = [C.c_int32]
+    L.gms_pseudomesh_bind.argtypes = [C.POINTER(PseudomeshBindArgs), C.c_void_p]
+    L.gms_pseudomesh_repose.argtypes = [C.POINTER(PseudomeshReposeArgs), C.c_void_p]
+    L.gms_bound_points_render_workspace_bytes.restype = C.c_size_t
+    L.gms_bound_points_render_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    L.gms_bound_points_render_frame.argtypes = [C.POINTER(BoundPointsRenderArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
     L.gms_metrics_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]
     L.gms_image_metrics.argtypes = [C.POINTER(MetricsArgs), C.c_void_p]
     _lib = L

@@ -273,3 +273,84 @@ def patch_points_model(model):
     model.prepare_scaling_rot = types.MethodType(prepare_scaling_rot, model)
     model.prepare_vertices = types.MethodType(prepare_vertices, model)
     return model
+
+
+class PseudomeshBinding:
+    """A pseudo-mesh bound to a driving mesh (bind_pseudomesh): `face` int32 [P] is each pseudo-triangle's face of that mesh,
+    `coeffs` float32 [P,3,3] its three vertices in that face's (n, e1, e2) frame; `faces` int64 [F,3] and `V` fix the mesh
+    every pose must share.  `n_degenerate` counts the faces of the rest pose that were never bound."""
+
+    def __init__(self, face: torch.Tensor, coeffs: torch.Tensor, faces: torch.Tensor, V: int, n_degenerate: int):
+        self.face, self.coeffs, self.faces, self.V, self.n_degenerate = face, coeffs, faces, int(V), int(n_degenerate)
+
+    @property
+    def P(self) -> int:
+        return self.face.shape[0]
+
+    def check_vertices(self, vertices: torch.Tensor) -> torch.Tensor:
+        """A pose of the driving mesh as the kernels read it: contiguous float32 [V,3] on the binding's device."""
+        if not torch.is_tensor(vertices) or tuple(vertices.shape) != (self.V, 3):
+            raise ValueError(f"driving mesh pose: expected vertices [{self.V},3], got "
+                             f"{tuple(vertices.shape) if torch.is_tensor(vertices) else type(vertices).__name__}")
+        if vertices.device != self.face.device:
+            raise ValueError(f"driving mesh pose: vertices must be on {self.face.device}")
+        return _f32(vertices.detach())
+
+
+def bind_pseudomesh(triangles: torch.Tensor, vertices: torch.Tensor, faces: torch.Tensor) -> PseudomeshBinding:
+    """Bind every pseudo-triangle [P,3,3] to the nearest face (by centroid) of the mesh (vertices [V,3], faces [F,3]) and
+    express its vertices in that face's frame: scripts/edit_pseudomesh_based_on_estimated_mesh.py:14-54 on the GPU, once per
+    edit.  Degenerate faces (a zero edge or zero area) are never chosen; ValueError if the mesh has no other face.  Shapes,
+    dtypes, the face-index range and finiteness are validated here, on the host, once."""
+    if not (torch.is_tensor(triangles) and torch.is_tensor(vertices) and torch.is_tensor(faces)):
+        raise TypeError("bind_pseudomesh: triangles, vertices and faces must be tensors")
+    if not vertices.is_cuda:
+        raise RuntimeError("bind_pseudomesh: CUDA tensors required (no CPU path in the product)")
+    dev = vertices.device
+    if triangles.device != dev or faces.device != dev:
+        raise ValueError("bind_pseudomesh: triangles, vertices and faces must be on one device")
+    if triangles.dim() != 3 or tuple(triangles.shape[1:]) != (3, 3) or vertices.dim() != 2 or vertices.shape[1] != 3 or \
+            faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError("bind_pseudomesh: expected triangles [P,3,3], vertices [V,3], faces [F,3]")
+    if not (triangles.is_floating_point() and vertices.is_floating_point()) or faces.is_floating_point() or faces.dtype == torch.bool:
+        raise ValueError("bind_pseudomesh: triangles and vertices must be floating point, faces integer")
+    P, V, F = triangles.shape[0], vertices.shape[0], faces.shape[0]
+    if F < 1 or V < 1:
+        raise ValueError("bind_pseudomesh: the mesh needs at least one face")
+    if P >= 2 ** 31 or F >= 2 ** 31 or V >= 2 ** 31:
+        raise ValueError("bind_pseudomesh: more than 2^31 - 1 triangles, faces or vertices")
+    t, v, f = _f32(triangles.detach()), _f32(vertices.detach()), faces.detach().long().contiguous()
+    if int(f.min()) < 0 or int(f.max()) >= V:
+        raise ValueError(f"bind_pseudomesh: face indices must lie in [0, {V})")
+    if not bool(torch.isfinite(t).all()) or not bool(torch.isfinite(v).all()):
+        raise ValueError("bind_pseudomesh: triangles and vertices must be finite")
+    face = torch.empty(P, dtype=torch.int32, device=dev)
+    coeffs = torch.empty(P, 3, 3, dtype=torch.float32, device=dev)
+    L = _lib.lib()
+    scratch = torch.empty(int(L.gms_pseudomesh_bind_scratch_bytes(F)), dtype=torch.uint8, device=dev)
+    nd = C.c_int32(0)
+    a = _lib.PseudomeshBindArgs()
+    a.P, a.triangles, a.V, a.F, a.vertices, a.faces = P, t.data_ptr(), V, F, v.data_ptr(), f.data_ptr()
+    a.face, a.coeffs, a.n_degenerate = face.data_ptr(), coeffs.data_ptr(), C.pointer(nd)
+    a.scratch, a.scratch_bytes = scratch.data_ptr(), scratch.numel()
+    with torch.cuda.device(dev):
+        rc = L.gms_pseudomesh_bind(C.byref(a), _stream(dev))
+    if rc == _lib.GMS_E_ARG and nd.value >= F:
+        raise ValueError(f"bind_pseudomesh: all {F} faces of the mesh are degenerate (zero edge or zero area)")
+    _lib.check(rc, "gms_pseudomesh_bind")
+    return PseudomeshBinding(face, coeffs, f, V, nd.value)
+
+
+def repose_pseudomesh(binding: PseudomeshBinding, vertices: torch.Tensor) -> torch.Tensor:
+    """The bound pseudo-mesh's triangles [P,3,3] in a pose (vertices [V,3]) of the driving mesh:
+    scripts/edit_pseudomesh_based_on_estimated_mesh.py:58-82 (the `edited_triangles.pt` it saves).  A face degenerate in
+    that pose gives non-finite triangles, as in the reference."""
+    v = binding.check_vertices(vertices)
+    P, dev = binding.P, v.device
+    tri = torch.empty(P, 3, 3, dtype=torch.float32, device=dev)
+    a = _lib.PseudomeshReposeArgs()
+    a.P, a.face, a.coeffs, a.V, a.F = P, binding.face.data_ptr(), binding.coeffs.data_ptr(), binding.V, binding.faces.shape[0]
+    a.vertices, a.faces, a.triangles = v.data_ptr(), binding.faces.data_ptr(), tri.data_ptr()
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().gms_pseudomesh_repose(C.byref(a), _stream(dev)), "gms_pseudomesh_repose")
+    return tri

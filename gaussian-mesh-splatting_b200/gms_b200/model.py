@@ -161,6 +161,68 @@ class PointsModel:
     def get_opacity(self):
         return torch.sigmoid(self._opacity)
 
+    def bind_to_mesh(self, vertices: torch.Tensor, faces: torch.Tensor) -> "MeshBoundPointsModel":
+        """Bind this pseudo-mesh to a driving mesh in its rest pose (vertices [V,3], faces [F,3]; e.g. io_obj.read_obj of the
+        mesh an editor moves): every triangle tracks the nearest face, so any pose of that mesh re-poses the Gaussians
+        (expansion.bind_pseudomesh; scripts/edit_pseudomesh_based_on_estimated_mesh.py)."""
+        dev = self.triangles.device
+        v = vertices.detach().to(dev).float().contiguous()
+        binding = expansion.bind_pseudomesh(self.triangles, v, faces.detach().to(dev))
+        return MeshBoundPointsModel(self, binding, v)
+
+
+class MeshBoundPointsModel:
+    """A gs_points pseudo-mesh driven by a mesh (PointsModel.bind_to_mesh): it shares the PointsModel's `_features` /
+    `_opacity` and holds the binding and a current pose `vertices` [V,3] of the driving mesh, initially the rest pose.
+    Setting `vertices` to an edited or animated pose moves the Gaussians; `triangles` materialises them
+    (expansion.repose_pseudomesh), which MeshBoundPointsRenderer never needs."""
+
+    def __init__(self, points: PointsModel, binding, vertices: torch.Tensor):
+        self.points, self.binding = points, binding
+        self.vertices = vertices
+
+    @property
+    def vertices(self) -> torch.Tensor:
+        return self._vertices
+
+    @vertices.setter
+    def vertices(self, v: torch.Tensor) -> None:
+        """A pose must be [V,3] on the binding's device (ValueError otherwise); it is kept as contiguous float32, without
+        a copy when it already is one, so in-place edits of that tensor move the Gaussians too."""
+        self._vertices = self.binding.check_vertices(v)
+
+    @property
+    def _features(self):
+        return self.points._features
+
+    @property
+    def _opacity(self):
+        return self.points._opacity
+
+    @property
+    def active_sh_degree(self):
+        return self.points.active_sh_degree
+
+    @property
+    def eps_s0(self):
+        return self.points.eps_s0
+
+    @property
+    def faces(self):
+        return self.binding.faces
+
+    @property
+    def triangles(self) -> torch.Tensor:
+        return expansion.repose_pseudomesh(self.binding, self.vertices)
+
+    @property
+    def get_features(self):
+        return self._features
+
+    @property
+    def get_opacity(self):
+        return torch.sigmoid(self._opacity)
+
 
 class MultiMeshGaussianModel(MeshGaussianModel):
     """gs_multi_mesh: several meshes, one Gaussian set (games/multi_mesh_splatting/scene/gaussian_multi_mesh_model.py).

@@ -9,6 +9,10 @@ call per view, no host synchronisation.
     image, radii, invdepth = renderer.render(cam, bg, triangles=transform_hotdog(renderer.model.triangles, t))
                                                                        # scripts/render_points_time_animated.py
 
+    renderer = MeshBoundPointsRenderer(points_model.bind_to_mesh(*io_obj.read_obj(mesh_obj)), W, H)
+    image, radii, invdepth = renderer.render(cam, bg, vertices=edited_vertices)
+                                                                       # scripts/edit_pseudomesh_based_on_estimated_mesh.py
+
 The first render learns N through one 4-byte read-back; every later one is sync-free, with the binning capacity predicted
 per view (SyncFreeCapacity).  An overflowed render (N above its capacity) gives the background image and is counted in
 `overflows`; the view's next render is sized from its true N.  evaluate() never reports an overflowed view's score: it
@@ -219,6 +223,60 @@ class PointsRenderer(NativeRenderer):
             return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing)
         finally:
             self._frame_triangles = None
+
+
+class MeshBoundPointsRenderer(NativeRenderer):
+    """NativeRenderer for a pseudo-mesh bound to a driving mesh (model.MeshBoundPointsModel): every render re-poses the
+    pseudo-triangles from a pose of that mesh and derives the Gaussians from them inside ONE kernel of
+    gms_bound_points_render_frame; the triangles are never written.  Gaussians whose face is degenerate in the pose are not
+    drawn (radius 0).  evaluate(), the capacity prediction and the overflow re-runs are NativeRenderer's."""
+
+    _frame_vertices = None      # set by render(vertices=...) for that one frame
+
+    def _adopt(self, model):
+        return model.binding.face.device, model.binding.P
+
+    def _workspace_bytes(self, P: int) -> int:
+        return _lib.lib().gms_bound_points_render_workspace_bytes(P, self.W, self.H)
+
+    def _check(self, cam, bg) -> None:
+        m, b = self.model, self.model.binding
+        P = self.radii.shape[0]
+        for name, t in (("_features", m._features), ("_opacity", m._opacity), ("binding.coeffs", b.coeffs)):
+            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
+                raise RuntimeError(f"MeshBoundPointsRenderer: {name} must be a contiguous float32 CUDA tensor on {self.dev}")
+        if b.P != P or m._features.shape[0] != P or tuple(m._opacity.shape) != (P, 1):
+            raise RuntimeError(f"MeshBoundPointsRenderer: sized for {P} Gaussians: features must be [{P},M,3], opacity [{P},1]")
+        v = m.vertices if self._frame_vertices is None else self._frame_vertices
+        if not (torch.is_tensor(v) and v.is_cuda and v.dtype == torch.float32 and v.is_contiguous() and v.device == self.dev
+                and tuple(v.shape) == (b.V, 3)):
+            raise RuntimeError(f"MeshBoundPointsRenderer: the pose `vertices` must be a contiguous float32 [{b.V},3] CUDA "
+                               f"tensor on {self.dev}")
+        for name, t in (("binding.face", b.face), ("binding.faces", b.faces)):
+            if not (t.is_cuda and t.is_contiguous() and t.device == self.dev):
+                raise RuntimeError(f"MeshBoundPointsRenderer: {name} must be a contiguous CUDA tensor on {self.dev}")
+        self._check_view(cam, bg)
+
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+        m, b = self.model, self.model.binding
+        self._check(cam, bg)
+        v = m.vertices if self._frame_vertices is None else self._frame_vertices
+        a = _lib.BoundPointsRenderArgs()
+        a.P, a.M = self.radii.shape[0], m._features.shape[1]
+        a.face, a.coeffs, a.V, a.F = b.face.data_ptr(), b.coeffs.data_ptr(), b.V, b.faces.shape[0]
+        a.vertices, a.faces = v.data_ptr(), b.faces.data_ptr()
+        a.features, a.opacity_raw, a.eps = m._features.data_ptr(), m._opacity.data_ptr(), m.eps_s0
+        self._call("gms_bound_points_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
+
+    def render(self, cam, bg: torch.Tensor, vertices: torch.Tensor = None, scale_modifier: float = 1.0, antialiasing: bool = False):
+        """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view.  `vertices` [V,3], when given, is this frame's pose of
+        the driving mesh in place of the model's (an edited mesh, or one frame of an animation); the model is never
+        modified."""
+        self._frame_vertices = None if vertices is None else self.model.binding.check_vertices(vertices)
+        try:
+            return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing)
+        finally:
+            self._frame_vertices = None
 
 
 def render_points_frame(model, cam, bg: torch.Tensor, triangles: torch.Tensor = None, scale_modifier: float = 1.0,

@@ -415,6 +415,74 @@ typedef struct gms_points_render_args {
 size_t gms_points_render_workspace_bytes(int32_t P, int32_t W, int32_t H);
 int gms_points_render_frame(const gms_points_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
 
+/* Mesh-driven pseudo-mesh editing (scripts/edit_pseudomesh_based_on_estimated_mesh.py:14-94, README "Pseudomesh/Triangle
+ * Soup and modifications"): every pseudo-triangle tracks the nearest face of a driving mesh, so moving that mesh's vertices
+ * moves the Gaussians.
+ *
+ * Binding (:25-54), once per pseudo-mesh and rest-pose mesh:
+ *   - face i = the non-degenerate face whose centroid ((v0 + v1) + v2) / 3 (fp32) is nearest to the pseudo-triangle's
+ *     centroid, by the squared distance in double (dx*dx + dy*dy) + dz*dz, the lowest index on an exact tie.  This is the
+ *     reference's sklearn KDTree query except at exact ties.  A face is degenerate when |v2 - v1|, |v3 - v1| or
+ *     |cross(v2 - v1, v3 - v1)| is exactly 0 in fp32; the reference would bind to it and produce NaN.
+ *   - coeffs[i][j] = the solution of [n|e1|e2] c = w_j - v1 for pseudo-vertex w_j, in double, rounded to fp32, with the skewed
+ *     frame n = normalise(cross(v2 - v1, v3 - v1)), e1 = normalise(v2 - v1), e2 = normalise(v3 - v1) of face i.
+ * Every face index must lie in [0, V) (not checked here: the caller's responsibility, as for gms_expand_args).  The call
+ * synchronises the stream once, to count the degenerate faces.  GMS_E_ARG: a null pointer, P < 0, F < 1, V < 1, too
+ * little scratch, or every face degenerate (n_degenerate is still written). */
+typedef struct gms_pseudomesh_bind_args {
+    int32_t P;
+    const float* triangles;     /* [P,3,3] pseudo-mesh (this and the outputs may be NULL when P == 0) */
+    int32_t V, F;
+    const float* vertices;      /* [V,3] rest pose of the driving mesh */
+    const int64_t* faces;       /* [F,3] */
+    int32_t* face;              /* out [P] bound face */
+    float* coeffs;              /* out [P,3,3] coefficients of (n, e1, e2) per pseudo-vertex */
+    int32_t* n_degenerate;      /* out, host: degenerate faces of the mesh (never bound) */
+    void* scratch; size_t scratch_bytes;   /* gms_pseudomesh_bind_scratch_bytes(F) */
+} gms_pseudomesh_bind_args;
+size_t gms_pseudomesh_bind_scratch_bytes(int32_t F);
+int gms_pseudomesh_bind(const gms_pseudomesh_bind_args* a, void* cuda_stream);
+
+/* Re-posing a binding on a pose of the same mesh (same faces; :58-82): w_j = ((v1' + c_j0 n') + c_j1 e1') + c_j2 e2' with the
+ * frame of the bound face in that pose.  A face degenerate in that pose gives non-finite triangles, as in the reference.
+ * Face indices: as in gms_pseudomesh_bind_args. */
+typedef struct gms_pseudomesh_repose_args {
+    int32_t P;
+    const int32_t* face;        /* [P] from gms_pseudomesh_bind, each in [0, F) */
+    const float* coeffs;        /* [P,3,3] */
+    int32_t V, F;
+    const float* vertices;      /* [V,3] driving pose */
+    const int64_t* faces;       /* [F,3] */
+    float* triangles;           /* out [P,3,3] (unused by gms_bound_points_render_frame) */
+} gms_pseudomesh_repose_args;
+int gms_pseudomesh_repose(const gms_pseudomesh_repose_args* a, void* cuda_stream);
+
+/* One gs_points render of a bound pseudo-mesh in a driving pose, in ONE call: the re-pose and the pseudo-mesh expansion of
+ * gms_points_render_frame fused in one kernel (the triangles are never written), then the same forward-only rasterizer
+ * forward.  Gaussians whose bound face is degenerate in this pose are culled (radius 0, no tile).  Workspace, num_rendered /
+ * binning_capacity / n_host_mapped: exactly as in gms_points_render_args. */
+typedef struct gms_bound_points_render_args {
+    int32_t P, M;
+    const int32_t* face;        /* [P] binding */
+    const float* coeffs;        /* [P,3,3] binding */
+    int32_t V, F;
+    const float* vertices;      /* [V,3] driving pose of this frame */
+    const int64_t* faces;       /* [F,3], each index in [0, V) */
+    const float* features;      /* [P,M,3] packed SH (get_features) */
+    const float* opacity_raw;   /* [P,1] logits */
+    float eps;                  /* eps_s0 = prepare_scaling_rot's eps, 1e-8 */
+    gms_raster_settings settings;
+    float* image;               /* out [3,H,W] */
+    float* invdepth;            /* out [1,H,W] */
+    int32_t* radii;             /* out [P] */
+    void* workspace; size_t workspace_bytes;   /* gms_bound_points_render_workspace_bytes */
+    int64_t* num_rendered;      /* host, optional (-1 on the sync-free path) */
+    int64_t binning_capacity;
+    uint32_t* n_host_mapped;    /* optional mapped pinned host [2]: N, overflow flag */
+} gms_bound_points_render_args;
+size_t gms_bound_points_render_workspace_bytes(int32_t P, int32_t W, int32_t H);
+int gms_bound_points_render_frame(const gms_bound_points_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
+
 /* Scores an image against its ground truth, forward only, deterministically (per-tile partial sums added in a fixed order in
  * double, no atomics: the same inputs give the same bits).  Both images go through the same transform first:
  *   quantize 0: clamp to [0,1]                                  (training_report, train.py:203-204)
