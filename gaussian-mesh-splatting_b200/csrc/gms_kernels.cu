@@ -7,6 +7,7 @@
 #include <thrust/iterator/transform_iterator.h>
 #include <stdio.h>
 #include <string.h>
+#include <vector>
 
 #include "../../include/gms_b200.h"
 #define GMS_BRANCHFREE_DIV 1        // the product: branch-free correctly-rounded division / sqrt where operands are provably normal (gms_common.cuh)
@@ -1878,15 +1879,68 @@ struct FrameModel {
     int32_t V, F, K, M;
     const float* vertices; const int64_t* faces; const float* alpha_raw; const float* scale_raw; const float* features;
     const float* opacity_raw; float eps;
+    const gms_mesh_segment* segments; int32_t n_segments;
 };
 
-// gs_mesh: E1-E4 mesh -> Gaussians (activated scales / rotations) into xyz / scales / rots.  `ea` is filled for the training
-// frame's expansion backward.
-static int mesh_expand_forward(const FrameModel& m, float* xyz, float* scales, float* rots, void* cuda_stream, gms_expand_args* ea) {
-    memset(ea, 0, sizeof(*ea));
-    ea->V = m.V; ea->F = m.F; ea->K = m.K; ea->vertices = m.vertices; ea->faces = m.faces; ea->alpha_raw = m.alpha_raw;
-    ea->scale_raw = m.scale_raw; ea->eps = m.eps; ea->xyz = xyz; ea->scaling_act = scales; ea->rotation_act = rots;
-    return gms_expand_forward(ea, cuda_stream);
+// The Gaussian count of a frame: F*K for one mesh, sum F_i*K_i for a segmented model (gms_mesh_segment), whose sizes are
+// validated here, before the frame issues any launch.
+static int frame_gaussian_count(const char* fn, const FrameModel& m, int* P) {
+    if (m.n_segments == 0) {
+        *P = m.F * m.K;
+        return GMS_OK;
+    }
+    if (m.n_segments < 0 || !m.segments) return set_err(GMS_E_ARG, "%s: n_segments < 0, or segments NULL with n_segments > 0%s", fn);
+    if (m.K != 0) return set_err(GMS_E_ARG, "%s: K must be 0 when segments are given%s", fn);
+    int64_t F = 0, n = 0;
+    for (int i = 0; i < m.n_segments; ++i) {
+        if (m.segments[i].F < 1 || m.segments[i].K < 1) return set_err(GMS_E_ARG, "%s: every segment needs F >= 1 and K >= 1%s", fn);
+        F += m.segments[i].F;
+        n += (int64_t)m.segments[i].F * m.segments[i].K;
+    }
+    if (F != m.F) return set_err(GMS_E_ARG, "%s: F must equal the sum of the segments' F%s", fn);
+    if (n > INT32_MAX) return set_err(GMS_E_ARG, "%s: sum of F_i * K_i over the segments exceeds int32%s", fn);
+    *P = (int)n;
+    return GMS_OK;
+}
+
+// gs_mesh: E1-E4 mesh -> Gaussians (activated scales / rotations) into xyz / scales / rots, one launch per mesh segment
+// (one in all without segments).  `ea` receives each launch's arguments for the training frame's expansion backward.
+static int mesh_expand_forward(const FrameModel& m, float* xyz, float* scales, float* rots, void* cuda_stream,
+                               std::vector<gms_expand_args>* ea) {
+    const gms_mesh_segment whole = {m.F, m.K};
+    const gms_mesh_segment* seg = m.n_segments ? m.segments : &whole;
+    const int n = m.n_segments ? m.n_segments : 1;
+    ea->assign(n, gms_expand_args());
+    size_t f0 = 0, g0 = 0;      // first face and first Gaussian of the segment
+    for (int i = 0; i < n; ++i) {
+        gms_expand_args& e = (*ea)[i];
+        memset(&e, 0, sizeof(e));
+        e.V = m.V; e.F = seg[i].F; e.K = seg[i].K; e.vertices = m.vertices; e.faces = m.faces + 3 * f0;
+        e.alpha_raw = m.alpha_raw + 3 * g0; e.scale_raw = m.scale_raw + g0; e.eps = m.eps;
+        e.xyz = xyz + 3 * g0; e.scaling_act = scales + 3 * g0; e.rotation_act = rots + 4 * g0;
+        int rc;
+        if ((rc = gms_expand_forward(&e, cuda_stream))) return rc;
+        f0 += (size_t)seg[i].F;
+        g0 += (size_t)seg[i].F * seg[i].K;
+    }
+    return GMS_OK;
+}
+
+// The expansion backward of mesh_expand_forward's launches: per segment, the incoming gradients and the raw-parameter
+// gradients are offset like the forward's outputs and inputs; the vertex gradient is shared (accumulated with atomics).
+static int mesh_expand_backward(const std::vector<gms_expand_args>& ea, const float* d_xyz, const float* d_scales, const float* d_rots,
+                                float* d_vertices, float* d_alpha_raw, float* d_scale_raw, void* cuda_stream) {
+    size_t g0 = 0;
+    for (const gms_expand_args& e : ea) {
+        gms_expand_grads g;
+        memset(&g, 0, sizeof(g));
+        g.dL_dxyz = d_xyz + 3 * g0; g.dL_dscaling_act = d_scales + 3 * g0; g.dL_drotation_act = d_rots + 4 * g0;
+        g.dL_dvertices = d_vertices; g.dL_dalpha_raw = d_alpha_raw + 3 * g0; g.dL_dscale_raw = d_scale_raw + g0;
+        int rc;
+        if ((rc = gms_expand_backward(&e, &g, cuda_stream))) return rc;
+        g0 += (size_t)e.F * e.K;
+    }
+    return GMS_OK;
 }
 
 // The activated Gaussians an expansion step left in the workspace, with the model's SH features and opacity logits.
@@ -1924,15 +1978,17 @@ int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_u
     if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii) return set_err(GMS_E_ARG, "gms_render_frame: null argument%s%s");
     if (!a->vertices || !a->faces || !a->alpha_raw || !a->scale_raw || !a->features || !a->opacity_raw)
         return set_err(GMS_E_ARG, "gms_render_frame: model tensors required%s%s");
-    const int P = a->F * a->K, W = a->settings.image_width, H = a->settings.image_height;
+    const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps,
+                          a->segments, a->n_segments};
+    int P, rc;
+    if ((rc = frame_gaussian_count("gms_render_frame", m, &P))) return rc;
+    const int W = a->settings.image_width, H = a->settings.image_height;
     if (a->workspace_bytes < gms_render_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_render_frame: workspace too small%s%s");
     RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
-    const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps};
     gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
-    gms_expand_args ea;
+    std::vector<gms_expand_args> ea;
     gms_raster_inputs in;
     gms_raster_saved saved;
-    int rc;
     if ((rc = mesh_expand_forward(m, RL.xyz, RL.scales, RL.rots, cuda_stream, &ea))) return rc;
     const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
     if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
@@ -2061,13 +2117,15 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
         return set_err(GMS_E_ARG, "gms_train_frame: gradient tensors required%s%s");
     if (a->sh_adam && (!a->sh_adam->m || !a->sh_adam->v || a->sh_adam->step < 1 || a->settings.sh_degree < 0 || a->settings.sh_degree > 3))
         return set_err(GMS_E_ARG, "gms_train_frame: bad sh_adam%s%s");
-    const int P = a->F * a->K, W = a->settings.image_width, H = a->settings.image_height;
+    const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps,
+                          a->segments, a->n_segments};
+    int P, rc;
+    if ((rc = frame_gaussian_count("gms_train_frame", m, &P))) return rc;
+    const int W = a->settings.image_width, H = a->settings.image_height;
     if (a->workspace_bytes < gms_frame_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_train_frame: workspace too small%s%s");
     FrameLayout FL = frame_layout(aligned_base_c(a->workspace), P, W, H);
-    int rc;
-    const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps};
     gms_raster_outputs out = {FL.image, FL.radii, FL.invdepth, 0};
-    gms_expand_args ea;
+    std::vector<gms_expand_args> ea;
     gms_raster_inputs in;
     gms_raster_saved saved;
     if ((rc = mesh_expand_forward(m, FL.xyz, FL.scales, FL.rots, cuda_stream, &ea))) return rc;
@@ -2096,11 +2154,8 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
         return rc;
     if (a->event_sh_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_sh_ready), st));
     // expansion backward (vertex gradients are accumulated with atomics: the caller keeps d_vertices zeroed)
-    gms_expand_grads eg;
-    memset(&eg, 0, sizeof(eg));
-    eg.dL_dxyz = FL.d_xyz; eg.dL_dscaling_act = FL.d_scales; eg.dL_drotation_act = FL.d_rots;
-    eg.dL_dvertices = a->d_vertices; eg.dL_dalpha_raw = a->d_alpha_raw; eg.dL_dscale_raw = a->d_scale_raw;
-    if ((rc = gms_expand_backward(&ea, &eg, cuda_stream))) return rc;
+    if ((rc = mesh_expand_backward(ea, FL.d_xyz, FL.d_scales, FL.d_rots, a->d_vertices, a->d_alpha_raw, a->d_scale_raw, cuda_stream)))
+        return rc;
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;
     return GMS_OK;
 }

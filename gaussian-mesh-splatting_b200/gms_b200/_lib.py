@@ -106,6 +106,19 @@ class ShAdam(C.Structure):
                 ("beta2", C.c_double), ("eps", C.c_double), ("step", C.c_int32)]
 
 
+class MeshSegment(C.Structure):
+    """struct gms_mesh_segment"""
+    _fields_ = [("F", C.c_int32), ("K", C.c_int32)]
+
+
+def mesh_segments(segments) -> "C.Array":
+    """[(F_i, K_i), ...] -> the host array gms_frame_args / gms_render_args point `segments` at."""
+    arr = (MeshSegment * len(segments))()
+    for i, (F, K) in enumerate(segments):
+        arr[i].F, arr[i].K = int(F), int(K)
+    return arr
+
+
 class FrameArgs(C.Structure):
     _fields_ = [("V", C.c_int32), ("F", C.c_int32), ("K", C.c_int32), ("M", C.c_int32),
                 ("vertices", C.c_void_p), ("faces", C.c_void_p), ("alpha_raw", C.c_void_p), ("scale_raw", C.c_void_p),
@@ -115,7 +128,8 @@ class FrameArgs(C.Structure):
                 ("settings", RasterSettings), ("gt", C.c_void_p), ("lambda_dssim", C.c_float), ("loss", C.c_void_p),
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)),
                 ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p), ("d_color_sh", C.c_void_p),
-                ("event_sh_ready", C.c_void_p), ("event_loss_ready", C.c_void_p), ("sh_adam", C.POINTER(ShAdam))]
+                ("event_sh_ready", C.c_void_p), ("event_loss_ready", C.c_void_p), ("sh_adam", C.POINTER(ShAdam)),
+                ("segments", C.POINTER(MeshSegment)), ("n_segments", C.c_int32)]
 
 
 class FrameView(C.Structure):
@@ -130,7 +144,8 @@ class RenderArgs(C.Structure):
                 ("features", C.c_void_p), ("opacity_raw", C.c_void_p), ("eps", C.c_float), ("settings", RasterSettings),
                 ("image", C.c_void_p), ("invdepth", C.c_void_p), ("radii", C.c_void_p),
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)),
-                ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p)]
+                ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p),
+                ("segments", C.POINTER(MeshSegment)), ("n_segments", C.c_int32)]
 
 
 class PointsRenderArgs(C.Structure):

@@ -9,6 +9,8 @@ Reads binary_little_endian (plyfile's default) and ascii PLY; writes binary_litt
 from __future__ import annotations
 
 import os
+import pickle
+import types
 from typing import Dict, List, Tuple
 
 import numpy as np
@@ -129,4 +131,69 @@ def save_mesh_model(ply_path: str, model) -> None:
     par = lambda t: torch.nn.Parameter(t.detach().clone().contiguous(), requires_grad=True)
     torch.save({"_alpha": par(model._alpha), "_scale": par(model._scale), "point_cloud": None,
                 "triangles": model.triangles.detach().clone(), "vertices": par(model.vertices), "faces": model.faces.detach().clone()},
+               ply_path.replace("point_cloud.ply", "model_params.pt"))
+
+
+class _Opaque(tuple):
+    """Stand-in for a class of the reference's own code pickled into model_params.pt (the `point_cloud` entries are
+    games.multi_mesh_splatting.utils.graphics_utils.MultiMeshPointCloud named tuples): kept as a plain tuple of its fields."""
+
+    def __new__(cls, *fields):
+        return tuple.__new__(cls, fields)
+
+
+class _Unpickler(pickle.Unpickler):
+    def find_class(self, module, name):
+        try:
+            return super().find_class(module, name)
+        except (ImportError, AttributeError):
+            return _Opaque
+
+
+_pickle_module = types.ModuleType("gms_b200_pickle")
+_pickle_module.__dict__.update({k: getattr(pickle, k) for k in dir(pickle) if not k.startswith("__")})
+_pickle_module.Unpickler = _Unpickler
+
+
+def load_multi_mesh_model(ply_path: str) -> List[MeshGaussianParams]:
+    """point_cloud.ply + model_params.pt of a trained gs_multi_mesh run -> one MeshGaussianParams per mesh, for
+    MultiMeshGaussianModel.from_mesh_params (GaussianMultiMeshModel.load_ply, gaussian_multi_mesh_model.py:245-256).
+    model_params.pt holds LISTS `_alpha` [F_i,K_i,3], `_scale` [F_i*K_i,1], `vertices` [V_i,3] and `faces` [F_i,3] (indices
+    into mesh i's own vertices); the PLY's Gaussians are the meshes' in that order."""
+    g = load_gaussian_ply(ply_path)
+    params = torch.load(ply_path.replace("point_cloud.ply", "model_params.pt"), map_location="cpu", weights_only=False,
+                        pickle_module=_pickle_module)
+    d = lambda x: (x.detach() if isinstance(x, torch.Tensor) else torch.as_tensor(x)).cpu()
+    out, g0 = [], 0
+    for a, s, v, f in zip(params["_alpha"], params["_scale"], params["vertices"], params["faces"]):
+        n = d(s).shape[0]
+        out.append(MeshGaussianParams(d(v).float(), d(f).long(), d(a).float(), d(s).float(), g["_features_dc"][g0:g0 + n],
+                                      g["_features_rest"][g0:g0 + n], g["_opacity"][g0:g0 + n]))
+        g0 += n
+    if g0 != g["_xyz"].shape[0]:
+        raise ValueError(f"{ply_path}: {g['_xyz'].shape[0]} Gaussians in the PLY, {g0} in model_params.pt")
+    return out
+
+
+def save_multi_mesh_model(ply_path: str, model) -> None:
+    """Counterpart of GaussianMultiMeshModel.save_ply (gaussian_multi_mesh_model.py:222-243) for a gms_b200
+    MultiMeshGaussianModel (merged or segmented): point_cloud.ply, and model_params.pt with the reference's per-mesh LISTS
+    `_alpha`, `_scale`, `vertices` (nn.Parameters) and `faces`, on the model's device, and `point_cloud` (empty: the
+    reference's load_ply does not read it)."""
+    model.update_alpha(); model.prepare_scaling_rot()
+    save_gaussian_ply(ply_path, model._xyz, model._features_dc, model._features_rest, model._opacity, model._scaling, model._rotation,
+                      getattr(model, "eps_s0", 1e-8))
+    par = lambda t: torch.nn.Parameter(t.detach().clone().contiguous(), requires_grad=True)
+    if model.segments is not None:
+        views = model.mesh_views()
+    else:
+        views, f0, K = [], 0, model._alpha.shape[1]
+        for F in model.mesh_face_counts:
+            views.append((model.faces[f0:f0 + F], model._alpha[f0:f0 + F], model._scale[f0 * K:(f0 + F) * K]))
+            f0 += F
+    alphas, scales, verts, faces, v0 = [], [], [], [], 0
+    for (f, a, s), nv in zip(views, model.mesh_vertex_counts):
+        alphas.append(par(a)); scales.append(par(s)); verts.append(par(model.vertices[v0:v0 + nv])); faces.append((f - v0).detach().clone())
+        v0 += nv
+    torch.save({"_alpha": alphas, "_scale": scales, "point_cloud": [], "vertices": verts, "faces": faces},
                ply_path.replace("point_cloud.ply", "model_params.pt"))

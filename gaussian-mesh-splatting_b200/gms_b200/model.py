@@ -11,11 +11,13 @@ from __future__ import annotations
 import torch
 from torch import nn
 
-from . import expansion
+from . import _lib, expansion
 from .scenes import MeshGaussianParams
 
 
 class MeshGaussianModel:
+    segments = None     # MultiMeshGaussianModel with a K per mesh: [(F_i, K_i), ...]; None: one K for every face
+
     def __init__(self, sh_degree: int = 3):
         self.active_sh_degree = 0
         self.max_sh_degree = sh_degree
@@ -33,19 +35,29 @@ class MeshGaussianModel:
         become views of it and get_features is zero-copy (the reference's torch.cat re-materialises 192 B/Gaussian
         every frame, scene/gaussian_model.py:107-111).  Needs FlatAdam for the DC / rest learning rates."""
         m = cls(sh_degree)
-        m.active_sh_degree = active_sh_degree
-        m.faces = p.faces.to(device)
-        mk = lambda t: nn.Parameter(t.to(device).float().contiguous().requires_grad_(True))
-        for k in ("vertices", "_alpha", "_scale", "_opacity"):
-            setattr(m, k, mk(getattr(p, k)))
-        if packed_features:
-            m._features = mk(torch.cat((p._features_dc, p._features_rest), dim=1))
-        else:
-            m._features = None
-            m._features_dc, m._features_rest = mk(p._features_dc), mk(p._features_rest)
+        m._adopt_params(p, device, active_sh_degree, packed_features)
         m.update_alpha()
         m.prepare_scaling_rot()
         return m
+
+    def _adopt_params(self, p: MeshGaussianParams, device, active_sh_degree: int, packed_features: bool) -> None:
+        self.active_sh_degree = active_sh_degree
+        self.faces = p.faces.to(device)
+        mk = lambda t: nn.Parameter(t.to(device).float().contiguous().requires_grad_(True))
+        for k in ("vertices", "_alpha", "_scale", "_opacity"):
+            setattr(self, k, mk(getattr(p, k)))
+        if packed_features:
+            self._features = mk(torch.cat((p._features_dc, p._features_rest), dim=1))
+        else:
+            self._features = None
+            self._features_dc, self._features_rest = mk(p._features_dc), mk(p._features_rest)
+
+    def frame_sizes(self):
+        """(F, K, segments) as gms_frame_args / gms_render_args take them: K and no segments for one K per face; K = 0 and
+        the host array of (F_i, K_i) for a segmented MultiMeshGaussianModel."""
+        if self.segments is None:
+            return self._alpha.shape[0], self._alpha.shape[1], None
+        return self.faces.shape[0], 0, self._segment_array
 
     def __getattr__(self, name):   # only called when normal lookup fails: packed-mode views
         if name in ("_features_dc", "_features_rest") and self.__dict__.get("_features") is not None:
@@ -228,27 +240,84 @@ class MultiMeshGaussianModel(MeshGaussianModel):
     """gs_multi_mesh: several meshes, one Gaussian set (games/multi_mesh_splatting/scene/gaussian_multi_mesh_model.py).
 
     The reference keeps per-mesh lists (vertices / faces / _alpha / _scale) and loops `expand -> torch.cat`
-    (:99-119, :121-174, :176-199).  Per-face work is independent of which mesh a face belongs to, so when every mesh
-    uses the same K the meshes are merged ONCE at construction (faces re-indexed into one vertex array) and the whole
-    set runs through the single-mesh kernels: one launch instead of a loop, no concatenation.  Meshes with different K
-    keep the reference's loop (`expand_per_mesh`)."""
+    (:99-119, :121-174, :176-199).  Per-face work is independent of which mesh a face belongs to, so the meshes are merged
+    ONCE at construction (faces re-indexed into one vertex array).  When every mesh uses the same K the whole set runs
+    through the single-mesh kernels: one launch instead of a loop, no concatenation.
+
+    Meshes with different K (train.py --num_splats a b ...) give a SEGMENTED model: `_alpha` is [P,3] and `_scale` [P,1],
+    mesh i's Gaussians being the rows [P_i, P_i + F_i*K_i), P_i = sum_{j<i} F_j*K_j -- the reference's torch.cat order -- and
+    `segments` lists (F_i, K_i).  Every per-Gaussian tensor is flat, so FlatAdam and the native frames (gms_train_frame /
+    gms_render_frame with gms_mesh_segment) see one Gaussian set; the expansion runs once per mesh.  A segmented model
+    computes no expansion at construction: `alpha` (a per-mesh list), `triangles`, `_xyz`, `_scaling` and `_rotation` are
+    set by update_alpha() / prepare_scaling_rot() or expand_fused(activated=False)."""
 
     @classmethod
-    def from_mesh_params(cls, plist, device="cuda", sh_degree: int = 3, active_sh_degree: int = 3, packed_features: bool = False):
-        Ks = {p._alpha.shape[1] for p in plist}
-        if len(Ks) != 1:
-            raise ValueError("merged fast path needs one K; use expand_per_mesh for heterogeneous K")
+    def from_mesh_params(cls, plist, device="cuda", sh_degree: int = 3, active_sh_degree: int = 3, packed_features: bool = False,
+                         segmented: bool = False):
+        """segmented=True keeps one segment per mesh even when every K is equal (what the per-mesh launches cost, against the
+        merged model); meshes with different K are always segmented."""
         off, faces = 0, []
         for p in plist:
             faces.append(p.faces + off)
             off += p.vertices.shape[0]
-        merged = MeshGaussianParams(torch.cat([p.vertices for p in plist]), torch.cat(faces),
-                                    torch.cat([p._alpha for p in plist]), torch.cat([p._scale for p in plist]),
+        segmented = segmented or len({p._alpha.shape[1] for p in plist}) != 1
+        alpha = [p._alpha.reshape(-1, 3) if segmented else p._alpha for p in plist]
+        merged = MeshGaussianParams(torch.cat([p.vertices for p in plist]), torch.cat(faces), torch.cat(alpha),
+                                    torch.cat([p._scale for p in plist]),
                                     torch.cat([p._features_dc for p in plist]), torch.cat([p._features_rest for p in plist]),
                                     torch.cat([p._opacity for p in plist]))
-        m = cls.from_params(merged, device, sh_degree, active_sh_degree, packed_features)
+        if segmented:
+            m = cls(sh_degree)
+            m._adopt_params(merged, device, active_sh_degree, packed_features)
+            m.segments = [(int(p._alpha.shape[0]), int(p._alpha.shape[1])) for p in plist]
+            m._segment_array = _lib.mesh_segments(m.segments)
+        else:
+            m = cls.from_params(merged, device, sh_degree, active_sh_degree, packed_features)
         m.mesh_face_counts = [p.faces.shape[0] for p in plist]
+        m.mesh_vertex_counts = [p.vertices.shape[0] for p in plist]
         return m
+
+    def mesh_views(self):
+        """Segmented model: per mesh, (faces [F_i,3] indexing the merged `vertices`, _alpha view [F_i,K_i,3], _scale view
+        [F_i*K_i,1]).  Views of the current parameter storage (FlatAdam re-points it), so taken afresh on every call."""
+        out, f0, g0 = [], 0, 0
+        for F, K in self.segments:
+            out.append((self.faces[f0:f0 + F], self._alpha[g0:g0 + F * K].view(F, K, 3), self._scale[g0:g0 + F * K]))
+            f0, g0 = f0 + F, g0 + F * K
+        return out
+
+    def update_alpha(self):
+        if self.segments is None:
+            return super().update_alpha()
+        outs = [expansion.update_alpha_op(self.vertices, f, a) for f, a, _ in self.mesh_views()]
+        self.alpha = [o[0] for o in outs]       # per mesh [F_i,K_i,3], as the reference's list
+        self.triangles, self._xyz = torch.cat([o[1] for o in outs]), torch.cat([o[2] for o in outs])
+
+    def prepare_scaling_rot(self):
+        if self.segments is None:
+            return super().prepare_scaling_rot()
+        outs, f0 = [], 0
+        for (F, K), (_, _, s) in zip(self.segments, self.mesh_views()):
+            outs.append(expansion.prepare_scaling_rot_op(self.triangles[f0:f0 + F], s, K, self.eps_s0))
+            f0 += F
+        self._scaling, self._rotation = torch.cat([o[0] for o in outs]), torch.cat([o[1] for o in outs])
+
+    def expand_fused(self, activated: bool = True):
+        """Segmented model: one fused launch per mesh, then cat (the autograd fast path of MeshTrainer(native=False))."""
+        if self.segments is None:
+            return super().expand_fused(activated)
+        outs = [expansion.expand(self.vertices, f, a, s, self.eps_s0, activated) for f, a, s in self.mesh_views()]
+        xyz, sc, rot = (torch.cat([o[i] for o in outs]) for i in range(3))
+        self.alpha, self.triangles = [o[3] for o in outs], torch.cat([o[4] for o in outs])
+        if not activated:
+            self._xyz, self._scaling, self._rotation = xyz, sc, rot
+        return xyz, sc, rot
+
+    def training_setup(self, *args, **kwargs):
+        if self.segments is not None:
+            raise RuntimeError("a MultiMeshGaussianModel with a K per mesh trains with FlatAdam (MeshTrainer(fast=True)); "
+                               "the reference's torch.optim.Adam op sequence (fast=False) is not supported for it")
+        return super().training_setup(*args, **kwargs)
 
     @staticmethod
     def expand_per_mesh(vertices_list, faces_list, alpha_list, scale_list, eps: float = expansion.EPS_S0):

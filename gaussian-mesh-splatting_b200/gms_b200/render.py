@@ -95,7 +95,10 @@ class NativeRenderer(SyncFreeCapacity):
         m = self.model
         feats = self._features()
         a = _lib.RenderArgs()
-        a.V, a.F, a.K, a.M = m.vertices.shape[0], m._alpha.shape[0], m._alpha.shape[1], feats.shape[1]
+        a.V, a.M = m.vertices.shape[0], feats.shape[1]
+        a.F, a.K, seg = m.frame_sizes()
+        if seg is not None:
+            a.segments, a.n_segments = seg, len(seg)
         a.vertices, a.faces, a.alpha_raw, a.scale_raw = m.vertices.data_ptr(), m.faces.data_ptr(), m._alpha.data_ptr(), m._scale.data_ptr()
         a.features, a.opacity_raw, a.eps = feats.data_ptr(), m._opacity.data_ptr(), m.eps_s0
         self._call("gms_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)

@@ -132,7 +132,10 @@ class NativeFrame(SyncFreeCapacity):
             gt = gt.contiguous().float()
         m = self.model
         a = _lib.FrameArgs()
-        a.V, a.F, a.K, a.M = m.vertices.shape[0], m._alpha.shape[0], m._alpha.shape[1], m._features.shape[1]
+        a.V, a.M = m.vertices.shape[0], m._features.shape[1]
+        a.F, a.K, seg = m.frame_sizes()
+        if seg is not None:
+            a.segments, a.n_segments = seg, len(seg)
         a.vertices, a.faces, a.alpha_raw, a.scale_raw = m.vertices.data_ptr(), m.faces.data_ptr(), m._alpha.data_ptr(), m._scale.data_ptr()
         a.features, a.opacity_raw, a.eps = m._features.data_ptr(), m._opacity.data_ptr(), m.eps_s0
         a.d_vertices, a.d_alpha_raw, a.d_scale_raw = m.vertices.grad.data_ptr(), m._alpha.grad.data_ptr(), m._scale.grad.data_ptr()

@@ -308,6 +308,19 @@ typedef struct gms_sh_adam {
  * into caller buffers, e.g. views of the flat gradient buffer gms_adam_step / the NCCL exchange operate on.
  * `workspace` holds the per-frame intermediates (gms_frame_workspace_bytes); the rasterizer's scratch still comes
  * through the allocation callback. */
+/* One mesh of a gs_multi_mesh scene whose meshes use different splat counts (train.py --num_splats a b ...;
+ * games/multi_mesh_splatting/scene/gaussian_multi_mesh_model.py:99-199).  With n_segments > 0 in gms_frame_args /
+ * gms_render_args:
+ *   - `faces` holds the meshes' faces one after another, already re-indexed into the one `vertices` array;
+ *   - F = sum F_i and K = 0; every F_i >= 1 and K_i >= 1; P = sum F_i * K_i must fit int32;
+ *   - mesh i's Gaussians are the contiguous rows [P_i, P_i + F_i*K_i) of every per-Gaussian array, P_i = sum_{j<i} F_j*K_j
+ *     (the reference's torch.cat order): alpha_raw [P,3] holds mesh i's [F_i,K_i,3] at row P_i, scale_raw is [P,1].
+ * The expansion runs once per mesh (forward and backward: one launch each per mesh); everything after it runs once over all
+ * P Gaussians.  Anything else is GMS_E_ARG, returned before any launch. */
+typedef struct gms_mesh_segment {
+    int32_t F, K;
+} gms_mesh_segment;
+
 typedef struct gms_frame_args {
     int32_t V, F, K, M;
     const float* vertices; const int64_t* faces; const float* alpha_raw; const float* scale_raw;
@@ -333,6 +346,8 @@ typedef struct gms_frame_args {
                                    frame while this one's backward pass still runs */
     const gms_sh_adam* sh_adam; /* optional: the frame also takes the Adam step of `features` (updated in place, M = 16) with
                                    this frame's SH gradient; then d_features and d_color_sh may be NULL */
+    const gms_mesh_segment* segments;   /* HOST [n_segments] or NULL: gs_multi_mesh with a K per mesh (see gms_mesh_segment) */
+    int32_t n_segments;                 /* 0: one mesh of F faces x K splats, P = F*K */
 } gms_frame_args;
 size_t gms_frame_workspace_bytes(int32_t P, int32_t W, int32_t H);
 /* Device pointers into a frame workspace (valid after gms_train_frame): this step's expansion outputs and images. */
@@ -385,6 +400,8 @@ typedef struct gms_render_args {
     int64_t* num_rendered;      /* host, optional (-1 on the sync-free path) */
     int64_t binning_capacity;
     uint32_t* n_host_mapped;    /* optional mapped pinned host [2]: N, overflow flag */
+    const gms_mesh_segment* segments;   /* HOST [n_segments] or NULL: as in gms_frame_args */
+    int32_t n_segments;
 } gms_render_args;
 size_t gms_render_workspace_bytes(int32_t P, int32_t W, int32_t H);
 int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
