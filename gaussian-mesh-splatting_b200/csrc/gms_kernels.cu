@@ -20,6 +20,7 @@
 #include "gms_sort.cuh"
 #include "gms_binning.cuh"
 #include "gms_image.cuh"
+#include "gms_free.cuh"
 
 // ------------------------------------------------------------------------------------------ host state
 static thread_local char g_err[512] = "";
@@ -2157,6 +2158,180 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     if ((rc = mesh_expand_backward(ea, FL.d_xyz, FL.d_scales, FL.d_rots, a->d_vertices, a->d_alpha_raw, a->d_scale_raw, cuda_stream)))
         return rc;
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;
+    return GMS_OK;
+}
+
+// ------------------------------------------------------------------------------------------ free Gaussians (gs, gs_flat)
+
+static bool free_model_ok(int P, int M, int cols, const float* xyz, const float* s, const float* r, const float* f, const float* o) {
+    return P >= 0 && M >= 1 && M <= 16 && (cols == 2 || cols == 3) && (P == 0 || (xyz && s && r && f && o));
+}
+
+// The activation kernels move quaternions and their gradients as float4.
+static bool aligned16(const void* p) { return (reinterpret_cast<size_t>(p) & 15) == 0; }
+
+static int free_act_fwd(int P, int cols, const float* scaling_raw, const float* rotation_raw, float eps, float* scales, float* rots,
+                        cudaStream_t st) {
+    if (P == 0) return GMS_OK;
+    span_begin(K_EXP_FWD, st);
+    k_free_act_fwd<<<(P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, st>>>(P, cols, scaling_raw, rotation_raw, eps, scales, rots);
+    GMS_AFTER_LAUNCH("free_act_fwd", 0, st);
+    span_end(st);
+    return GMS_OK;
+}
+
+int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !alloc || !a->workspace || !a->loss || !a->gt) return set_err(GMS_E_ARG, "gms_free_train_frame: null argument%s%s");
+    if (!free_model_ok(a->P, a->M, a->scale_cols, a->xyz, a->scaling_raw, a->rotation_raw, a->features, a->opacity_raw))
+        return set_err(GMS_E_ARG, "gms_free_train_frame: need P >= 0, 1 <= M <= 16, scale_cols 2 or 3 and every model tensor%s%s");
+    const int P = a->P;
+    if (P > 0 && (!a->d_xyz || !a->d_scaling_raw || !a->d_rotation_raw || (!a->d_features && !a->sh_adam) || !a->d_opacity_raw))
+        return set_err(GMS_E_ARG, "gms_free_train_frame: gradient tensors required%s%s");
+    if (!a->accum != !a->denom) return set_err(GMS_E_ARG, "gms_free_train_frame: accum and denom go together%s%s");
+    if (!aligned16(a->rotation_raw) || !aligned16(a->d_rotation_raw))
+        return set_err(GMS_E_ARG, "gms_free_train_frame: rotation_raw and d_rotation_raw must be 16-byte aligned%s%s");
+    if (a->sh_adam && (!a->sh_adam->m || !a->sh_adam->v || a->sh_adam->step < 1 || a->M != 16 || a->settings.sh_degree < 0 ||
+                       a->settings.sh_degree > 3))
+        return set_err(GMS_E_ARG, "gms_free_train_frame: bad sh_adam%s%s");
+    const int W = a->settings.image_width, H = a->settings.image_height;
+    if (W <= 0 || H <= 0) return set_err(GMS_E_ARG, "gms_free_train_frame: bad image size%s%s");
+    if (a->workspace_bytes < gms_frame_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_free_train_frame: workspace too small%s%s");
+    FrameLayout FL = frame_layout(aligned_base_c(a->workspace), P, W, H);
+    gms_raster_outputs out = {FL.image, FL.radii, FL.invdepth, 0};
+    gms_raster_inputs in;
+    gms_raster_saved saved;
+    int rc;
+    if ((rc = free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, FL.scales, FL.rots, st))) return rc;
+    const FrameGaussians g = {P, a->M, a->xyz, FL.scales, FL.rots, a->features, a->opacity_raw, FL.opac};
+    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
+                                   &saved))) return rc;
+    gms_loss_args la;
+    memset(&la, 0, sizeof(la));
+    la.C = 3; la.H = H; la.W = W; la.img = FL.image; la.gt = a->gt; la.lambda_dssim = a->lambda_dssim; la.loss = a->loss;
+    la.dL_dimg = FL.dimage; la.scratch = FL.loss_scratch; la.scratch_bytes = FL.loss_bytes;
+    if ((rc = gms_l1_ssim_loss(&la, cuda_stream))) return rc;
+    if (a->event_loss_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_loss_ready), st));
+    gms_raster_grads gr;
+    memset(&gr, 0, sizeof(gr));
+    gr.dL_dmeans3D = a->d_xyz; gr.dL_dmeans2D = FL.d_m2d; gr.dL_dopacities = FL.d_opac;
+    if (!a->sh_adam) gr.dL_dshs = a->d_features;
+    gr.dL_dscales = FL.d_scales; gr.dL_drotations = FL.d_rots;
+    if ((rc = raster_backward_impl(&a->settings, &in, FL.radii, &saved, FL.dimage, nullptr, &gr, cuda_stream, a->d_opacity_raw, a->sh_adam)))
+        return rc;
+    if (P > 0) {
+        FreeActBwd b;
+        b.P = P; b.cols = a->scale_cols; b.rotation_raw = a->rotation_raw; b.scales = FL.scales;
+        b.d_scales = FL.d_scales; b.d_rots = FL.d_rots; b.d_m2d = FL.d_m2d; b.radii = FL.radii;
+        b.d_scaling_raw = a->d_scaling_raw; b.d_rotation_raw = a->d_rotation_raw; b.accum = a->accum; b.denom = a->denom;
+        b.counters = geom_layout(aligned_base(saved.geom), P).counters;
+        span_begin(K_EXP_BWD, st);
+        k_free_act_bwd<<<(P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, st>>>(b);
+        GMS_AFTER_LAUNCH("free_act_bwd", 0, st);
+        span_end(st);
+    }
+    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
+    return GMS_OK;
+}
+
+int gms_free_render_frame(const gms_free_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii)
+        return set_err(GMS_E_ARG, "gms_free_render_frame: null argument%s%s");
+    if (!free_model_ok(a->P, a->M, a->scale_cols, a->xyz, a->scaling_raw, a->rotation_raw, a->features, a->opacity_raw))
+        return set_err(GMS_E_ARG, "gms_free_render_frame: need P >= 0, 1 <= M <= 16, scale_cols 2 or 3 and every model tensor%s%s");
+    if (!aligned16(a->rotation_raw)) return set_err(GMS_E_ARG, "gms_free_render_frame: rotation_raw must be 16-byte aligned%s%s");
+    const int P = a->P, W = a->settings.image_width, H = a->settings.image_height;
+    if (a->workspace_bytes < gms_render_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_free_render_frame: workspace too small%s%s");
+    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
+    int rc;
+    if ((rc = free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, RL.scales, RL.rots, st))) return rc;
+    gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
+    gms_raster_inputs in;
+    gms_raster_saved saved;
+    const FrameGaussians g = {P, a->M, a->xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
+    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
+                                   &saved))) return rc;
+    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
+    return GMS_OK;
+}
+
+struct DensifyScratch { int4* flags; int4* incl; void* cub; size_t cub_bytes; size_t total; };
+
+static DensifyScratch densify_scratch(void* base, int P) {
+    DensifyScratch S;
+    char* p = reinterpret_cast<char*>(base);
+    const int Pn = P > 0 ? P : 1;
+    S.flags = carve<int4>(p, Pn); S.incl = carve<int4>(p, Pn);
+    S.cub_bytes = 0;
+    cub::DeviceScan::InclusiveScan(nullptr, S.cub_bytes, S.flags, S.incl, Int4Sum(), Pn);
+    S.cub = p;
+    p += align_up(S.cub_bytes);
+    S.total = (size_t)(p - reinterpret_cast<char*>(base));
+    return S;
+}
+
+size_t gms_densify_scratch_bytes(int32_t P) { return densify_scratch(nullptr, P).total + 512; }
+
+int gms_densify_plan(const gms_densify_plan_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !a->result || a->P < 0 || (a->scale_cols != 2 && a->scale_cols != 3))
+        return set_err(GMS_E_ARG, "gms_densify_plan: need result, P >= 0 and scale_cols 2 or 3%s%s");
+    if (a->P > 0 && (!a->accum || !a->denom || !a->scaling_raw || !a->opacity_raw || !a->scratch))
+        return set_err(GMS_E_ARG, "gms_densify_plan: null argument%s%s");
+    if (a->P > 0 && a->scratch_bytes < gms_densify_scratch_bytes(a->P)) return set_err(GMS_E_ARG, "gms_densify_plan: scratch too small%s%s");
+    memset(a->result, 0, 5 * sizeof(int32_t));
+    if (a->P == 0) return GMS_OK;
+    const int P = a->P;
+    DensifyScratch S = densify_scratch(aligned_base_c(a->scratch), P);
+    DensifyPlanK k;
+    k.P = P; k.cols = a->scale_cols; k.accum = a->accum; k.denom = a->denom; k.scaling_raw = a->scaling_raw; k.opacity_raw = a->opacity_raw;
+    k.eps = a->eps; k.grad_threshold = a->grad_threshold; k.split_scale = a->split_scale; k.min_opacity = a->min_opacity;
+    k.max_world_scale = a->max_world_scale; k.flags = S.flags; k.fate = a->fate;
+    span_begin(K_MISC, st);
+    k_densify_plan<<<(P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, st>>>(k);
+    GMS_AFTER_LAUNCH("densify_plan", 0, st);
+    size_t tb = S.cub_bytes;
+    GMS_CUDA(cub::DeviceScan::InclusiveScan(S.cub, tb, S.flags, S.incl, Int4Sum(), P, st));
+    span_end(st);
+    int4 tot;
+    GMS_CUDA(cudaMemcpyAsync(&tot, S.incl + (P - 1), sizeof(int4), cudaMemcpyDeviceToHost, st));
+    GMS_CUDA(cudaStreamSynchronize(st));
+    const int64_t newP = (int64_t)tot.x + tot.y + 2 * (int64_t)tot.z;
+    if (newP > INT32_MAX) return set_err(GMS_E_ARG, "gms_densify_plan: the densified set exceeds int32 rows%s%s");
+    a->result[0] = (int32_t)newP; a->result[1] = tot.x; a->result[2] = tot.y; a->result[3] = tot.z; a->result[4] = tot.w;
+    return GMS_OK;
+}
+
+static bool free_set_ok(const gms_free_set& s) { return s.xyz && s.scaling && s.rotation && s.opacity && s.features; }
+
+int gms_densify_apply(const gms_densify_apply_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !a->result || a->P < 0 || a->M < 1 || a->M > 16 || (a->scale_cols != 2 && a->scale_cols != 3))
+        return set_err(GMS_E_ARG, "gms_densify_apply: need result, P >= 0, 1 <= M <= 16 and scale_cols 2 or 3%s%s");
+    const int32_t* r = a->result;
+    if (a->new_P != r[0] || r[0] != r[1] + r[2] + 2 * r[3]) return set_err(GMS_E_ARG, "gms_densify_apply: new_P is not the plan's%s%s");
+    if (a->P == 0) return GMS_OK;
+    if (!a->scratch || a->scratch_bytes < gms_densify_scratch_bytes(a->P) || !a->normals)
+        return set_err(GMS_E_ARG, "gms_densify_apply: scratch and normals required%s%s");
+    for (int t = 0; t < 3; t++)
+        if (!free_set_ok(a->src[t]) || (a->new_P > 0 && !free_set_ok(a->dst[t])))
+            return set_err(GMS_E_ARG, "gms_densify_apply: every source and destination tensor is required%s%s");
+    if (a->new_P == 0) return GMS_OK;
+    DensifyScratch S = densify_scratch(const_cast<void*>(aligned_base_c(const_cast<void*>(a->scratch))), a->P);
+    DensifyApplyK k;
+    k.P = a->P; k.cols = a->scale_cols; k.F = 3 * a->M; k.eps = a->eps; k.incl = S.incl;
+    k.kept = r[1]; k.clones = r[2]; k.splits = r[3]; k.normals = a->normals;
+    for (int t = 0; t < 3; t++) {
+        const gms_free_set& s = a->src[t];
+        const gms_free_set& d = a->dst[t];
+        k.src[t] = {s.xyz, s.scaling, s.rotation, s.opacity, s.features};
+        k.dst[t] = {d.xyz, d.scaling, d.rotation, d.opacity, d.features};
+    }
+    span_begin(K_MISC, st);
+    k_densify_apply<<<(a->P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, st>>>(k);
+    GMS_AFTER_LAUNCH("densify_apply", 0, st);
+    span_end(st);
     return GMS_OK;
 }
 

@@ -180,6 +180,50 @@ class BoundPointsRenderArgs(C.Structure):
                 ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p)]
 
 
+class FreeFrameArgs(C.Structure):
+    """struct gms_free_frame_args"""
+    _fields_ = [("P", C.c_int32), ("M", C.c_int32), ("scale_cols", C.c_int32), ("xyz", C.c_void_p), ("scaling_raw", C.c_void_p),
+                ("rotation_raw", C.c_void_p), ("features", C.c_void_p), ("opacity_raw", C.c_void_p), ("eps", C.c_float),
+                ("d_xyz", C.c_void_p), ("d_scaling_raw", C.c_void_p), ("d_rotation_raw", C.c_void_p), ("d_features", C.c_void_p),
+                ("d_opacity_raw", C.c_void_p), ("accum", C.c_void_p), ("denom", C.c_void_p), ("settings", RasterSettings),
+                ("gt", C.c_void_p), ("lambda_dssim", C.c_float), ("loss", C.c_void_p), ("workspace", C.c_void_p),
+                ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)), ("binning_capacity", C.c_int64),
+                ("n_host_mapped", C.c_void_p), ("event_loss_ready", C.c_void_p), ("sh_adam", C.POINTER(ShAdam))]
+
+
+class FreeRenderArgs(C.Structure):
+    """struct gms_free_render_args"""
+    _fields_ = [("P", C.c_int32), ("M", C.c_int32), ("scale_cols", C.c_int32), ("xyz", C.c_void_p), ("scaling_raw", C.c_void_p),
+                ("rotation_raw", C.c_void_p), ("features", C.c_void_p), ("opacity_raw", C.c_void_p), ("eps", C.c_float),
+                ("settings", RasterSettings), ("image", C.c_void_p), ("invdepth", C.c_void_p), ("radii", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)),
+                ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p)]
+
+
+FATE_CLONE, FATE_SPLIT, FATE_PRUNE, FATE_PRUNE_CHILDREN = 1, 2, 4, 8     # gms_densify_plan_args.fate bits
+
+
+class DensifyPlanArgs(C.Structure):
+    """struct gms_densify_plan_args"""
+    _fields_ = [("P", C.c_int32), ("scale_cols", C.c_int32), ("accum", C.c_void_p), ("denom", C.c_void_p),
+                ("scaling_raw", C.c_void_p), ("opacity_raw", C.c_void_p), ("eps", C.c_float), ("grad_threshold", C.c_float),
+                ("split_scale", C.c_float), ("min_opacity", C.c_float), ("max_world_scale", C.c_float), ("fate", C.c_void_p),
+                ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t), ("result", C.POINTER(C.c_int32))]
+
+
+class FreeSet(C.Structure):
+    """struct gms_free_set"""
+    _fields_ = [("xyz", C.c_void_p), ("scaling", C.c_void_p), ("rotation", C.c_void_p), ("opacity", C.c_void_p),
+                ("features", C.c_void_p)]
+
+
+class DensifyApplyArgs(C.Structure):
+    """struct gms_densify_apply_args"""
+    _fields_ = [("P", C.c_int32), ("new_P", C.c_int32), ("scale_cols", C.c_int32), ("M", C.c_int32), ("eps", C.c_float),
+                ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t), ("result", C.POINTER(C.c_int32)),
+                ("normals", C.c_void_p), ("src", FreeSet * 3), ("dst", FreeSet * 3)]
+
+
 class MetricsArgs(C.Structure):
     """struct gms_metrics_args"""
     _fields_ = [("C", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("img", C.c_void_p), ("gt", C.c_void_p),
@@ -205,7 +249,8 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_render_workspace_bytes", "gms_render_frame", "gms_metrics_scratch_bytes", "gms_image_metrics",
                "gms_points_render_workspace_bytes", "gms_points_render_frame", "gms_pseudomesh_bind_scratch_bytes",
                "gms_pseudomesh_bind", "gms_pseudomesh_repose", "gms_bound_points_render_workspace_bytes",
-               "gms_bound_points_render_frame"]
+               "gms_bound_points_render_frame", "gms_free_train_frame", "gms_free_render_frame", "gms_densify_scratch_bytes",
+               "gms_densify_plan", "gms_densify_apply"]
 
 _lib = None
 
@@ -269,6 +314,12 @@ def lib():
     L.gms_bound_points_render_workspace_bytes.restype = C.c_size_t
     L.gms_bound_points_render_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.gms_bound_points_render_frame.argtypes = [C.POINTER(BoundPointsRenderArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
+    L.gms_free_train_frame.argtypes = [C.POINTER(FreeFrameArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
+    L.gms_free_render_frame.argtypes = [C.POINTER(FreeRenderArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
+    L.gms_densify_scratch_bytes.restype = C.c_size_t
+    L.gms_densify_scratch_bytes.argtypes = [C.c_int32]
+    L.gms_densify_plan.argtypes = [C.POINTER(DensifyPlanArgs), C.c_void_p]
+    L.gms_densify_apply.argtypes = [C.POINTER(DensifyApplyArgs), C.c_void_p]
     L.gms_metrics_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]
     L.gms_image_metrics.argtypes = [C.POINTER(MetricsArgs), C.c_void_p]
     _lib = L

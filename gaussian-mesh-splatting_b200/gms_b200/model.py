@@ -325,3 +325,91 @@ class MultiMeshGaussianModel(MeshGaussianModel):
         outs = [expansion.expand(v, f, a, s, eps, activated=False)[:3] for v, f, a, s in
                 zip(vertices_list, faces_list, alpha_list, scale_list)]
         return tuple(torch.cat([o[i] for o in outs]) for i in range(3))
+
+
+class FreeGaussianModel:
+    """gs / gs_flat: free Gaussians, raw parameters activated every frame (scene/gaussian_model.py:95-122;
+    games/flat_splatting/scene/flat_gaussian_model.py:32-35 for gs_flat).  `_xyz` [P,3], `_scaling` [P,3] (gs) or [P,2]
+    (gs_flat: the in-plane log-scales; get_scaling prepends the constant eps_s0), `_rotation` [P,4], `_opacity` [P,1] logits,
+    and the SH coefficients packed in ONE [P,M,3] tensor `_features` (`_features_dc` / `_features_rest` are views of it)."""
+
+    KINDS = ("gs", "gs_flat")
+    NAMES = ("_xyz", "_scaling", "_rotation", "_opacity", "_features")
+
+    def __init__(self, xyz, scaling, rotation, features, opacity, kind: str = "gs_flat", device="cuda", active_sh_degree: int = 0,
+                 eps_s0: float = 1e-8):
+        if kind not in self.KINDS:
+            raise ValueError(f"FreeGaussianModel: kind must be one of {self.KINDS}; got {kind!r}")
+        P = xyz.shape[0]
+        cols = 3 if kind == "gs" else 2
+        if scaling.dim() == 2 and scaling.shape[1] == 3 and cols == 2:
+            scaling = scaling[:, 1:]            # a gs_flat checkpoint's scale_0 column is log(eps_s0): not a parameter
+        if tuple(xyz.shape) != (P, 3) or tuple(scaling.shape) != (P, cols) or tuple(rotation.shape) != (P, 4) or \
+                features.dim() != 3 or tuple(features.shape[::2]) != (P, 3) or tuple(opacity.shape) != (P, 1):
+            raise ValueError(f"FreeGaussianModel({kind}): expected xyz [P,3], scaling [P,{cols}], rotation [P,4], features [P,M,3], "
+                             "opacity [P,1]")
+        self.kind, self.eps_s0 = kind, float(eps_s0)
+        self.max_sh_degree = int(round(features.shape[1] ** 0.5)) - 1
+        self.active_sh_degree = min(int(active_sh_degree), self.max_sh_degree)
+        mk = lambda t: nn.Parameter(t.detach().to(device).float().contiguous().requires_grad_(True))
+        self._xyz, self._scaling, self._rotation, self._features, self._opacity = map(mk, (xyz, scaling, rotation, features, opacity))
+
+    @classmethod
+    def from_checkpoint(cls, ply_path: str, kind: str = "gs_flat", device="cuda", active_sh_degree: int = 3) -> "FreeGaussianModel":
+        """A point_cloud.ply the reference (or save()) wrote: GaussianModel.load_ply (scene/gaussian_model.py:224-262)."""
+        from . import io_ply
+        g = io_ply.load_gaussian_ply(ply_path)
+        return cls(g["_xyz"], g["_scaling"], g["_rotation"], torch.cat((g["_features_dc"], g["_features_rest"]), dim=1), g["_opacity"],
+                   kind, device, active_sh_degree)
+
+    def save(self, ply_path: str) -> None:
+        """The reference's point_cloud.ply (GaussianModel.save_ply; gs_flat gets the log(eps_s0) scale_0 column)."""
+        from . import io_ply
+        io_ply.save_gaussian_ply(ply_path, self._xyz, self._features_dc, self._features_rest, self._opacity, self._scaling,
+                                 self._rotation, self.eps_s0)
+
+    @property
+    def P(self) -> int:
+        return self._xyz.shape[0]
+
+    @property
+    def scale_cols(self) -> int:
+        return self._scaling.shape[1]
+
+    @property
+    def _features_dc(self):
+        return self._features[:, :1]
+
+    @property
+    def _features_rest(self):
+        return self._features[:, 1:]
+
+    @property
+    def get_xyz(self):
+        return self._xyz
+
+    @property
+    def get_scaling(self):
+        s = torch.exp(self._scaling)
+        if self.kind == "gs":
+            return s
+        return torch.cat([torch.full((s.shape[0], 1), self.eps_s0, dtype=s.dtype, device=s.device), s], dim=1)
+
+    @property
+    def get_rotation(self):
+        return torch.nn.functional.normalize(self._rotation)
+
+    @property
+    def get_opacity(self):
+        return torch.sigmoid(self._opacity)
+
+    @property
+    def get_features(self):
+        return self._features
+
+    def oneupSHdegree(self):
+        if self.active_sh_degree < self.max_sh_degree:
+            self.active_sh_degree += 1
+
+    def parameters(self):
+        return [getattr(self, n) for n in self.NAMES]

@@ -7,6 +7,7 @@ same pass.  The flat gradient buffer is also what the data-parallel all-reduce s
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import List, Sequence, Tuple
 
 import torch
@@ -56,9 +57,86 @@ class FlatAdam:
             p.grad = self.g[off:off + k].view(p.shape)
             off += pad(k)
             self.ends.append(off)
-        self.betas, self.eps, self.t = betas, eps, 0
+        self.betas, self.eps = betas, eps
+        # Adam step count per group (torch.optim.Adam keeps one per parameter): a group whose update is skipped -- the
+        # reference's reset_opacity replaces the opacity parameter by one without a gradient -- lags the others from then on
+        self.steps = [0] * len(self.groups)
         self._kernel = kernel or self._cuda_kernel       # `kernel`: test hook (a callable taking the _adam_desc dict)
         self._comm = None                                # side stream of the factored exchange (created on first use)
+
+    @property
+    def t(self) -> int:
+        """The step count, when every group has the same one (every mesh training path); else the largest."""
+        return max(self.steps)
+
+    @t.setter
+    def t(self, value: int) -> None:
+        self.steps = [int(value)] * len(self.groups)
+
+    def group_index(self, name: str) -> int:
+        return next(i for i, g in enumerate(self.groups) if g.get("name") == name)
+
+    def _launch_runs(self, groups, zero_grad, zero_end):
+        """One gms_adam_step per run of consecutive groups in `groups` with equal step counts, each over its flat sub-range
+        (p/g/m/v at the run's first element, `offset` = its flat index; the segment table stays the whole buffer's)."""
+        if self.world != 1:
+            raise ValueError("per-group step counts need a single-GPU FlatAdam")
+        runs = []
+        for i in groups:
+            if runs and runs[-1][-1] == i - 1 and self.steps[i] == self.steps[runs[-1][0]]:
+                runs[-1].append(i)
+            else:
+                runs.append([i])
+        for r in runs:
+            off, end = (self.ends[r[0] - 1] if r[0] else 0), self.ends[r[-1]]
+            d = self._adam_desc(end - off, off, self.p[off:], self.g[off:], zero_grad, zero_end)
+            d.update(m=self.m[off:], v=self.v[off:], step=self.steps[r[0]])
+            self._kernel(d)
+
+    def _step_groups(self, groups, zero_end, skip):
+        """Advances and updates `groups` minus the names in `skip`.  Returns False when that is every group with equal counts
+        (the caller then issues its single launch)."""
+        skipped = [self.group_index(n) for n in skip]
+        active = [i for i in groups if i not in skipped]
+        for i in active:
+            self.steps[i] += 1
+        for i in skipped:           # the frame's gradient of a skipped group is discarded
+            self.g[(self.ends[i - 1] if i else 0):self.ends[i]].zero_()
+        if not skipped and len({self.steps[i] for i in groups}) == 1:
+            return False
+        self._launch_runs(active, 1 if zero_end is None else 2, 0 if zero_end is None else zero_end)
+        return True
+
+    def resize(self, shapes, fill) -> None:
+        """Re-homes the flat buffers for new group shapes (a densification changes every group's row count).
+        fill(old, new) writes the new rows: `old` / `new` map "p", "m", "v" to per-group views of the old / new buffers in
+        the group's shape.  param.data and .grad become views of the new buffers, the gradient is zero, the step counts stay."""
+        if self.world != 1:
+            raise ValueError("FlatAdam.resize needs a single-GPU optimizer")
+        pad = lambda k: (k + 63) // 64 * 64
+        ends, off = [], 0
+        for sh in shapes:
+            off += pad(math.prod(sh))
+            ends.append(off)
+        n = (off + 63) // 64 * 64
+        dev = self.p.device
+        new = {k: torch.zeros(n, dtype=torch.float32, device=dev) for k in ("p", "m", "v")}
+
+        def views(bufs, ends_, shapes_):
+            return {k: [b[(ends_[i - 1] if i else 0):(ends_[i - 1] if i else 0) + math.prod(sh)].view(sh) for i, sh in enumerate(shapes_)]
+                    for k, b in bufs.items()}
+
+        old_shapes = [tuple(g["param"].shape) for g in self.groups]
+        fill(views({"p": self.p, "m": self.m, "v": self.v}, self.ends, old_shapes), views(new, ends, shapes))
+        self.p, self.m, self.v = new["p"], new["m"], new["v"]
+        self.g = torch.zeros(n, dtype=torch.float32, device=dev)
+        self.n = self.shard = n
+        self.ends = ends
+        for i, (g, sh) in enumerate(zip(self.groups, shapes)):
+            o = ends[i - 1] if i else 0
+            k = math.prod(sh)
+            g["param"].data = self.p[o:o + k].view(sh)
+            g["param"].grad = self.g[o:o + k].view(sh)
 
     @property
     def flat_grad(self) -> torch.Tensor:
@@ -154,28 +232,32 @@ class FlatAdam:
         self._adam_sh(sh)
         if reduced is not None:
             torch.cuda.current_stream(self.p.device).wait_event(reduced)
-        self.step_rest(zero_end)
+        self.step_rest(zero_end, _advance=False)
 
-    def step_rest(self, zero_end=None):
-        """Adam on every group but the SH group (one launch, gradient zeroed as in step())."""
+    def step_rest(self, zero_end=None, skip=(), _advance=True):
+        """Adam on every group but the SH group (one launch, gradient zeroed as in step()).  skip: names of groups that take
+        no step (their step count does not advance, their gradient is discarded); with unequal counts, one launch per run."""
+        if _advance and self._step_groups(range(len(self.groups) - 1), zero_end, skip):
+            return
         d = self._adam_desc(self.ends[-2], 0, self.p, self.g, 1 if zero_end is None else 2, 0 if zero_end is None else zero_end)
         for k in ("seg_end", "lr0", "lr1", "inner", "period"):
             d[k] = d[k][:-1]
+        d["step"] = self.steps[0]
         self._kernel(d)
 
     def begin_fused_sh_step(self) -> "_lib.ShAdam":
         """Single-GPU factored optimizer: the next frame applies the SH group's Adam step itself, inside its preprocess backward
         (gms_train_frame with this gms_sh_adam descriptor: the parameter rows are read once and no colour gradient goes
-        through memory).  Advances the step count; step_rest() then updates the other groups."""
+        through memory).  Advances the SH group's step count; step_rest() then updates the other groups."""
         if not self.sh_factored or self.world != 1:
             raise ValueError("the fused SH step needs a single-GPU FlatAdam built with sh_factored=True")
-        self.t += 1
+        self.steps[-1] += 1
         gsh = self.groups[-1]
         off = self.ends[-2]
         a = _lib.ShAdam()
         a.m, a.v = self.m[off:].data_ptr(), self.v[off:].data_ptr()
         a.lr_dc, a.lr_rest = float(gsh["lr0"]), float(gsh["lr1"])
-        a.beta1, a.beta2, a.eps, a.step = self.betas[0], self.betas[1], self.eps, self.t
+        a.beta1, a.beta2, a.eps, a.step = self.betas[0], self.betas[1], self.eps, self.steps[-1]
         return a
 
     def _adam_sh(self, sh):
@@ -188,18 +270,24 @@ class FlatAdam:
         a.xyz, a.exchange, a.slot_floats, a.grad_scale = int(sh["xyz"]), ex.data_ptr(), ex.shape[1], 1.0 / ex.shape[0]
         a.p, a.m, a.v = f.data_ptr(), self.m[off:].data_ptr(), self.v[off:].data_ptr()
         a.lr_dc, a.lr_rest = float(gsh["lr0"]), float(gsh["lr1"])
-        a.beta1, a.beta2, a.eps, a.step = self.betas[0], self.betas[1], self.eps, self.t
+        a.beta1, a.beta2, a.eps, a.step = self.betas[0], self.betas[1], self.eps, self.steps[-1]
         dev = f.device
         with torch.cuda.device(dev):
             _lib.check(_lib.lib().gms_adam_sh_factored(C.byref(a), torch.cuda.current_stream(dev).cuda_stream), "gms_adam_sh_factored")
 
-    def step(self, zero_end=None, sh=None):
+    def step(self, zero_end=None, sh=None, skip=()):
         """sh given (sh_factored optimizers): see _step_factored.  Otherwise:
         world == 1: one launch over the whole flat buffer (gradient zeroed in the same pass).
         world > 1: reduce-scatter(mean) -> Adam on the local slice -> all-gather of the parameters; the full gradient
         buffer is re-zeroed with one memset.
         zero_end: when the producer of the gradients OVERWRITES everything at flat indices >= zero_end each frame
-        (gms_train_frame: all but the atomically accumulated vertex gradients), only [0, zero_end) is zeroed."""
+        (gms_train_frame: all but the atomically accumulated vertex gradients), only [0, zero_end) is zeroed.
+        skip: names of groups that take no step this time (single GPU, dense mode); while every group's step count is the
+        same, the step is the one launch above, otherwise one launch per run of equal counts."""
+        if skip or len(set(self.steps)) != 1:
+            if self.sh_factored or not self._step_groups(range(len(self.groups)), zero_end, skip):
+                raise ValueError("skipped groups / unequal step counts need a single-GPU FlatAdam in dense mode")
+            return
         self.t += 1
         if self.sh_factored:
             if sh is None:
@@ -230,3 +318,16 @@ def mesh_model_groups(model, lrs=REFERENCE_LRS, features_last: bool = False) -> 
         feats += [dict(param=model._features_dc, lr=lrs["f_dc"], name="f_dc"), dict(param=model._features_rest, lr=lrs["f_rest"], name="f_rest")]
     rest = [dict(param=model._opacity, lr=lrs["opacity"], name="opacity"), dict(param=model._scale, lr=lrs["scaling"], name="scaling")]
     return g + (rest + feats if features_last else feats + rest)
+
+
+def free_model_groups(model, xyz_lr: float, feature_lr: float = 0.0025, opacity_lr: float = 0.05, scaling_lr: float = 0.005,
+                      rotation_lr: float = 0.001) -> List[dict]:
+    """Parameter groups of a FreeGaussianModel (gs / gs_flat) with the reference's learning rates (GaussianModel.training_setup,
+    scene/gaussian_model.py:149-167; arguments/__init__.py:72-91): xyz (its lr follows the schedule), scaling, rotation,
+    opacity, and the packed SH tensor last (f_dc at feature_lr, f_rest at feature_lr / 20), as FlatAdam(sh_factored=True)
+    needs it.  Opacity is the last group before the SH tensor: once a lone opacity reset has made its step count lag, the
+    other groups still form one run of equal counts, so the step takes two gms_adam_step launches instead of three."""
+    M = model._features.shape[1]
+    return [dict(param=model._xyz, lr=xyz_lr, name="xyz"), dict(param=model._scaling, lr=scaling_lr, name="scaling"),
+            dict(param=model._rotation, lr=rotation_lr, name="rotation"), dict(param=model._opacity, lr=opacity_lr, name="opacity"),
+            dict(param=model._features, lr0=feature_lr, lr1=feature_lr / 20.0, inner=3, period=M, name="features")]

@@ -297,3 +297,30 @@ def render_points_frame(model, cam, bg: torch.Tensor, triangles: torch.Tensor = 
         sh_degree=model.active_sh_degree, campos=cam.camera_center, prefiltered=False, debug=False, antialiasing=antialiasing)
     return dgr.GaussianRasterizer(raster_settings=rs)(means3D=xyz, means2D=torch.zeros_like(xyz), opacities=model.get_opacity,
                                                       shs=model.get_features, scales=scales, rotations=rots)
+
+
+class NativeFreeRenderer(NativeRenderer):
+    """NativeRenderer for free Gaussians (model.FreeGaussianModel, gs / gs_flat): every render activates the raw parameters
+    inside gms_free_render_frame.  evaluate(), the capacity prediction and the overflow re-runs are NativeRenderer's."""
+
+    def _adopt(self, model):
+        return model._xyz.device, model.P
+
+    def _check(self, cam, bg) -> None:
+        m = self.model
+        for name in m.NAMES:
+            t = getattr(m, name)
+            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
+                raise RuntimeError(f"NativeFreeRenderer: model.{name} must be a contiguous float32 CUDA tensor on {self.dev}")
+        if m.P != self.radii.shape[0]:
+            raise RuntimeError("NativeFreeRenderer: the model's Gaussian count changed; make a new renderer")
+        self._check_view(cam, bg)
+
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+        m = self.model
+        self._check(cam, bg)
+        a = _lib.FreeRenderArgs()
+        a.P, a.M, a.scale_cols = m.P, m._features.shape[1], m.scale_cols
+        a.xyz, a.scaling_raw, a.rotation_raw = m._xyz.data_ptr(), m._scaling.data_ptr(), m._rotation.data_ptr()
+        a.features, a.opacity_raw, a.eps = m._features.data_ptr(), m._opacity.data_ptr(), m.eps_s0
+        self._call("gms_free_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)

@@ -260,3 +260,13 @@ def transform_hotdog(triangles: torch.Tensor, t) -> torch.Tensor:
     out = triangles.clone()
     out[:, :, 2] += 0.3 * torch.sin(triangles[:, :, 0] * math.pi + t)
     return out
+
+
+def camera_extent(cams) -> float:
+    """scene.cameras_extent: getNerfppNorm's radius (scene/dataset_readers.py:45-66) -- 1.1 times the largest distance of a
+    camera centre from their mean.  The arithmetic stays in the centres' dtype, as the reference's numpy keeps it (its
+    centres come from getWorld2View2's float32 matrices)."""
+    c = np.stack([np.asarray(cam.camera_center.detach().cpu().numpy() if torch.is_tensor(cam.camera_center) else cam.camera_center
+                             ).reshape(3, 1) for cam in cams], axis=1)[:, :, 0]
+    center = np.mean(c, axis=1, keepdims=True)
+    return float(np.max(np.linalg.norm(c - center, axis=0, keepdims=True)) * 1.1)

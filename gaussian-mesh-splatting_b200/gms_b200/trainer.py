@@ -12,8 +12,10 @@ All gradients live in ONE contiguous buffer (param.grad are views into it), so t
 from __future__ import annotations
 
 import math
+from dataclasses import dataclass
 from typing import List, Optional, Sequence
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -286,4 +288,280 @@ class MeshTrainer:
         r = self._renderer
         if r is None or (r.W, r.H) != (W, H) or r.radii.shape[0] != self.model._scale.shape[0]:
             r = self._renderer = NativeRenderer(self.model, W, H)
+        return r.evaluate(cams, gts, self.bg, protocol=protocol)
+
+
+# ---------------------------------------------------------------------------------------------- free Gaussians (gs, gs_flat)
+
+@dataclass
+class FreeOptimizationParams:
+    """OptimizationParams of the reference (arguments/__init__.py:72-91) that a gs / gs_flat run reads."""
+    iterations: int = 30_000
+    position_lr_init: float = 0.00016
+    position_lr_final: float = 0.0000016
+    position_lr_delay_mult: float = 0.01
+    position_lr_max_steps: int = 30_000
+    feature_lr: float = 0.0025
+    opacity_lr: float = 0.05
+    scaling_lr: float = 0.005
+    rotation_lr: float = 0.001
+    percent_dense: float = 0.01
+    lambda_dssim: float = 0.2
+    densification_interval: int = 100
+    opacity_reset_interval: int = 3000
+    densify_from_iter: int = 500
+    densify_until_iter: int = 15_000
+    densify_grad_threshold: float = 0.0002
+    min_opacity: float = 0.005          # densify_and_prune's second argument (train.py:143)
+
+
+def expon_lr(step: int, lr_init: float, lr_final: float, lr_delay_steps: int = 0, lr_delay_mult: float = 1.0,
+             max_steps: int = 1_000_000) -> float:
+    """get_expon_lr_func (utils/general_utils.py:109-145) evaluated at `step`."""
+    if step < 0 or (lr_init == 0.0 and lr_final == 0.0):
+        return 0.0
+    delay = lr_delay_mult + (1 - lr_delay_mult) * np.sin(0.5 * np.pi * np.clip(step / lr_delay_steps, 0, 1)) if lr_delay_steps > 0 else 1.0
+    t = np.clip(step / max_steps, 0, 1)
+    return float(delay * np.exp(np.log(lr_init) * (1 - t) + np.log(lr_final) * t))
+
+
+class NativeFreeFrame(SyncFreeCapacity):
+    """One gs / gs_flat training frame through gms_free_train_frame: activation, rasterizer, loss, backward and (optionally)
+    the densification statistics in ONE C call.  Gradients land in the parameters' .grad views (FlatAdam's flat buffer).
+
+    Sync-free like NativeFrame, with one addition: after the model's Gaussian count changed (resize()), every view's next
+    frame learns its N with one read-back, so a growing model loses no frame to an overflowed capacity."""
+
+    def __init__(self, model, width: int, height: int, lambda_dssim: float = 0.2, sync_free: bool = True):
+        self.model, self.W, self.H, self.lam = model, int(width), int(height), float(lambda_dssim)
+        self.dev = model._xyz.device
+        self.loss = torch.zeros(3, dtype=torch.float32, device=self.dev)
+        self._init_capacity(sync_free)
+        self._scratch, self._cb = grow_only_alloc(self.dev)
+        self.ws = None
+        self._epoch, self._view_epoch = 0, {}
+        self.ev_loss = None
+        self.resize()
+
+    def resize(self) -> None:
+        """The model's P changed: grow the workspace, zero the statistics, forget every view's N."""
+        from . import _lib
+        P = self.model.P
+        need = int(_lib.lib().gms_frame_workspace_bytes(P, self.W, self.H))
+        if self.ws is None or self.ws.numel() < need:
+            self.ws = torch.empty(need, dtype=torch.uint8, device=self.dev)
+        self.accum = torch.zeros(P, dtype=torch.float32, device=self.dev)
+        self.denom = torch.zeros(P, dtype=torch.float32, device=self.dev)
+        self._harvest()
+        self._epoch += 1
+        self._view_n.clear()
+        self._n_max = 0
+
+    def _check(self, gt, bg, cam):
+        m = self.model
+        for n in m.NAMES:
+            t = getattr(m, n)
+            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
+                raise RuntimeError(f"NativeFreeFrame: model.{n} must be a contiguous float32 CUDA tensor on {self.dev}")
+            if t.grad is None or not t.grad.is_contiguous() or t.grad.shape != t.shape:
+                raise RuntimeError(f"NativeFreeFrame: model.{n}.grad must be a preallocated contiguous buffer (FlatAdam provides it)")
+        if self.accum.shape[0] != m.P:
+            raise RuntimeError("NativeFreeFrame: the model's Gaussian count changed; call resize()")
+        for t, what in ((gt, "gt"), (bg, "bg"), (cam.world_view_transform, "camera matrices"), (cam.full_proj_transform, "camera matrices"),
+                        (cam.camera_center, "camera centre")):
+            if not t.is_cuda or t.device != self.dev or t.dtype != torch.float32:
+                raise RuntimeError(f"NativeFreeFrame.run: {what} must be float32 on {self.dev}")
+        if int(cam.image_width) != self.W or int(cam.image_height) != self.H or tuple(gt.shape) != (3, self.H, self.W):
+            raise ValueError(f"NativeFreeFrame was sized for {self.W}x{self.H}; got a {cam.image_width}x{cam.image_height} camera")
+
+    def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, stats: bool = True, sh_adam=None) -> torch.Tensor:
+        """stats: add this frame's densification statistics to `accum` / `denom`.  sh_adam (FlatAdam.begin_fused_sh_step()):
+        the frame also applies the SH parameters' Adam step and writes no SH gradient."""
+        import ctypes as C
+        from . import _lib
+        gt = gt.contiguous()
+        self._check(gt, bg, cam)
+        m = self.model
+        a = _lib.FreeFrameArgs()
+        a.P, a.M, a.scale_cols = m.P, m._features.shape[1], m.scale_cols
+        a.xyz, a.scaling_raw, a.rotation_raw = m._xyz.data_ptr(), m._scaling.data_ptr(), m._rotation.data_ptr()
+        a.features, a.opacity_raw, a.eps = m._features.data_ptr(), m._opacity.data_ptr(), m.eps_s0
+        a.d_xyz, a.d_scaling_raw, a.d_rotation_raw = m._xyz.grad.data_ptr(), m._scaling.grad.data_ptr(), m._rotation.grad.data_ptr()
+        a.d_features, a.d_opacity_raw = m._features.grad.data_ptr(), m._opacity.grad.data_ptr()
+        if sh_adam is not None:
+            a.d_features, a.sh_adam = None, C.pointer(sh_adam)
+        if stats:
+            a.accum, a.denom = self.accum.data_ptr(), self.denom.data_ptr()
+        if self.ev_loss is None:
+            self.ev_loss = torch.cuda.Event()
+            self.ev_loss.record(torch.cuda.current_stream(self.dev))
+        a.event_loss_ready = self.ev_loss.cuda_event
+        s = a.settings
+        s.image_height, s.image_width, s.tanfovx, s.tanfovy = self.H, self.W, cam.tanfovx, cam.tanfovy
+        s.bg, s.scale_modifier = bg.data_ptr(), 1.0
+        s.viewmatrix, s.projmatrix, s.campos = cam.world_view_transform.data_ptr(), cam.full_proj_transform.data_ptr(), cam.camera_center.data_ptr()
+        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = m.active_sh_degree, 0, 0, 0
+        a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
+        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
+        a.num_rendered = C.pointer(self.n_rendered)
+        key = self._view_key(cam)
+        learn = self.capacity == 0 or self._view_epoch.get(key) != self._epoch
+        if self.sync_free and not learn:
+            a.n_host_mapped = self._sync_free_slot(key, self.dev)
+            a.binning_capacity = self.capacity
+        with torch.cuda.device(self.dev):
+            _lib.check(_lib.lib().gms_free_train_frame(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream),
+                       "gms_free_train_frame")
+        if self.sync_free and learn:
+            self._learned_first(key)
+            self._view_epoch[key] = self._epoch
+        return self.loss[0]
+
+
+def densify_plan(model, accum, denom, extent: float, opt: FreeOptimizationParams, size_prune: bool):
+    """gms_densify_plan on the model's current rows: (result [new P, kept, clones, split pairs, pruned], fate [P] uint8,
+    scratch).  One host synchronisation."""
+    import ctypes as C
+    from . import _lib
+    P = model.P
+    scratch = torch.empty(int(_lib.lib().gms_densify_scratch_bytes(P)), dtype=torch.uint8, device=model._xyz.device)
+    fate = torch.empty(max(P, 1), dtype=torch.uint8, device=model._xyz.device)
+    res = (C.c_int32 * 5)()
+    a = _lib.DensifyPlanArgs()
+    a.P, a.scale_cols = P, model.scale_cols
+    a.accum, a.denom, a.scaling_raw, a.opacity_raw = accum.data_ptr(), denom.data_ptr(), model._scaling.data_ptr(), model._opacity.data_ptr()
+    a.eps, a.grad_threshold = model.eps_s0, opt.densify_grad_threshold
+    a.split_scale, a.min_opacity = opt.percent_dense * extent, opt.min_opacity
+    a.max_world_scale = 0.1 * extent if size_prune else 0.0
+    a.fate, a.scratch, a.scratch_bytes, a.result = fate.data_ptr(), scratch.data_ptr(), scratch.numel(), res
+    with torch.cuda.device(model._xyz.device):
+        _lib.check(_lib.lib().gms_densify_plan(C.byref(a), torch.cuda.current_stream(model._xyz.device).cuda_stream), "gms_densify_plan")
+    return list(res), fate[:P], scratch
+
+
+def densify_apply(model, plan, normals, old: dict, new: dict) -> None:
+    """gms_densify_apply: `old` / `new` map "p", "m", "v" to per-tensor lists in FreeGaussianModel.NAMES order."""
+    import ctypes as C
+    from . import _lib
+    res, _, scratch = plan
+    a = _lib.DensifyApplyArgs()
+    a.P, a.new_P, a.scale_cols, a.M, a.eps = model.P, res[0], model.scale_cols, model._features.shape[1], model.eps_s0
+    a.scratch, a.scratch_bytes, a.result = scratch.data_ptr(), scratch.numel(), (C.c_int32 * 5)(*res)
+    a.normals = normals.data_ptr()
+    for t, k in enumerate(("p", "m", "v")):
+        for dst, src in ((a.dst[t], new[k]), (a.src[t], old[k])):
+            dst.xyz, dst.scaling, dst.rotation, dst.opacity, dst.features = (x.data_ptr() for x in src)
+    with torch.cuda.device(model._xyz.device):
+        _lib.check(_lib.lib().gms_densify_apply(C.byref(a), torch.cuda.current_stream(model._xyz.device).cuda_stream), "gms_densify_apply")
+
+
+class FreeTrainer:
+    """A whole iteration of the reference's train.py:83-157 for gs / gs_flat, on one GPU:
+
+        update_learning_rate (xyz schedule) -> oneupSHdegree every 1000 -> gms_free_train_frame with the densification
+        statistics -> densify_and_prune / reset_opacity at the reference's schedule -> Adam.
+
+    Reproduced quirks of the reference:
+      - max_radii2D is not tracked: densification_postfix zeroes it on every densify_and_prune before it is read, so the
+        screen-size prune never fires; only the world-size prune (max scale > 0.1 * extent, after opacity_reset_interval) does.
+      - On a densification iteration every parameter is replaced by one without a gradient, so optimizer.step() updates
+        nothing and no step count advances; the frame then runs without the fused SH step.  A lone opacity reset (white
+        background at densify_from_iter) skips the opacity group only, whose bias correction lags by one from then on.
+      - Appended rows start with zero Adam moments; reset_opacity zeroes the opacity moments.
+    The split samples come from torch.randn on the device (`generator`)."""
+
+    def __init__(self, model, bg: torch.Tensor, extent: float, opt: FreeOptimizationParams = None, white_background: bool = None,
+                 sync_free: bool = True, world: int = 1, generator: torch.Generator = None):
+        if world != 1:
+            raise ValueError("FreeTrainer trains on one GPU: data-parallel densification (all-reduced statistics) is not implemented")
+        from .optim import free_model_groups
+        self.model, self.bg, self.extent = model, bg, float(extent)
+        self.opt = opt or FreeOptimizationParams()
+        self.white_background = bool((bg == 1).all()) if white_background is None else bool(white_background)
+        self.sync_free, self.generator = sync_free, generator
+        o = self.opt
+        self.fused_sh = model._features.shape[1] == 16
+        self.adam = FlatAdam(free_model_groups(model, self._xyz_lr(0), o.feature_lr, o.opacity_lr, o.scaling_lr, o.rotation_lr),
+                             sh_factored=self.fused_sh)
+        self.iteration = 0
+        self.frame = None
+        self._renderer = None
+        self.densifications = []        # (iteration, P before, result of the plan)
+
+    def _xyz_lr(self, it: int) -> float:
+        o = self.opt
+        return expon_lr(it, o.position_lr_init * self.extent, o.position_lr_final * self.extent, lr_delay_mult=o.position_lr_delay_mult,
+                        max_steps=o.position_lr_max_steps)
+
+    def schedule(self, it: int):
+        """(statistics, densify, reset_opacity) of iteration `it` (1-based), train.py:133-149."""
+        o = self.opt
+        if it >= o.densify_until_iter:
+            return False, False, False
+        densify = it > o.densify_from_iter and it % o.densification_interval == 0
+        reset = it % o.opacity_reset_interval == 0 or (self.white_background and it == o.densify_from_iter)
+        return True, densify, reset
+
+    def step(self, cam: Camera, gt: torch.Tensor) -> torch.Tensor:
+        it = self.iteration + 1
+        self.adam.groups[0]["lr"] = self._xyz_lr(it)
+        if it % 1000 == 0:
+            self.model.oneupSHdegree()
+        stats, densify, reset = self.schedule(it)
+        if self.frame is None:
+            self.frame = NativeFreeFrame(self.model, cam.image_width, cam.image_height, self.opt.lambda_dssim, sync_free=self.sync_free)
+        sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and not densify else None
+        loss = self.frame.run(cam, gt, self.bg, stats=stats, sh_adam=sh_adam)
+        if densify:
+            self.densify(size_prune=it > self.opt.opacity_reset_interval)
+        if reset:
+            self.reset_opacity()
+        if not densify and it < self.opt.iterations:     # train.py steps the optimizer on every iteration but the last
+            skip = ("opacity",) if reset else ()
+            if self.fused_sh:
+                self.adam.step_rest(zero_end=0, skip=skip)
+            else:
+                self.adam.step(zero_end=0, skip=skip)
+        self.iteration = it
+        return loss
+
+    def densify(self, size_prune: bool, normals: torch.Tensor = None) -> list:
+        """densify_and_prune(densify_grad_threshold, min_opacity, extent, 20 if size_prune else None) on the statistics
+        gathered so far; the frame's gradients are discarded.  normals [P,2,3]: the split draws (default torch.randn)."""
+        m, f = self.model, self.frame
+        P0 = m.P
+        plan = densify_plan(m, f.accum, f.denom, self.extent, self.opt, size_prune)
+        if normals is None:
+            normals = torch.randn(max(P0, 1), 2, 3, device=m._xyz.device, generator=self.generator)
+        newP = plan[0][0]
+        names = [g["name"] for g in self.adam.groups]
+        tensor_of = {"xyz": "_xyz", "opacity": "_opacity", "scaling": "_scaling", "rotation": "_rotation", "features": "_features"}
+        order = [names.index(k) for k in ("xyz", "scaling", "rotation", "opacity", "features")]     # FreeGaussianModel.NAMES order
+
+        def fill(old, new):
+            densify_apply(m, plan, normals, {k: [old[k][i] for i in order] for k in old}, {k: [new[k][i] for i in order] for k in new})
+
+        self.adam.resize([(newP,) + tuple(getattr(m, tensor_of[n]).shape[1:]) for n in names], fill)
+        f.resize()
+        self.densifications.append((self.iteration + 1, P0, plan[0]))
+        return plan[0]
+
+    def reset_opacity(self) -> None:
+        """reset_opacity (scene/gaussian_model.py:218-221) on the flat views: opacity = inverse_sigmoid(min(sigmoid, 0.01)),
+        opacity moments zeroed."""
+        i = self.adam.group_index("opacity")
+        op = self.model._opacity.data
+        x = torch.min(torch.sigmoid(op), torch.ones_like(op) * 0.01)
+        op.copy_(torch.log(x / (1 - x)))
+        o0, o1 = (self.adam.ends[i - 1] if i else 0), self.adam.ends[i]
+        self.adam.m[o0:o1].zero_()
+        self.adam.v[o0:o1].zero_()
+
+    def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
+        """L1 / SSIM / PSNR of the current model on held-out views (NativeFreeRenderer.evaluate)."""
+        from .render import NativeFreeRenderer
+        W, H = int(cams[0].image_width), int(cams[0].image_height)
+        r = self._renderer
+        if r is None or (r.W, r.H) != (W, H) or r.radii.shape[0] != self.model.P:
+            r = self._renderer = NativeFreeRenderer(self.model, W, H)
         return r.evaluate(cams, gts, self.bg, protocol=protocol)

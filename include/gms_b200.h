@@ -500,6 +500,114 @@ typedef struct gms_bound_points_render_args {
 size_t gms_bound_points_render_workspace_bytes(int32_t P, int32_t W, int32_t H);
 int gms_bound_points_render_frame(const gms_bound_points_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
 
+/* ---- free Gaussians: gs and gs_flat ----------------------------------------------------------------- */
+
+/* One gs / gs_flat training frame in ONE call: gms_train_frame with the mesh expansion replaced by the per-Gaussian
+ * activation of scene/gaussian_model.py:95-101 (games/flat_splatting/scene/flat_gaussian_model.py:32-35 for gs_flat):
+ *   scales = exp(scaling_raw) (gs, scale_cols 3) or (eps, exp(scaling_raw[:,0]), exp(scaling_raw[:,1])) (gs_flat, scale_cols 2),
+ *   rotations = rotation_raw / max(|rotation_raw|, 1e-12); xyz is the raw parameter itself.
+ * -> sigmoid(opacity) -> rasterizer fwd -> L1+SSIM -> rasterizer bwd -> raw gradients of scaling (none for the eps column)
+ * and rotation.  d_xyz receives dL/dxyz directly.  With accum / denom ([P] float) the same pass adds the densification
+ * statistics of add_densification_stats (scene/gaussian_model.py:416-418): accum += |dL/dmeans2D.xy|, denom += 1 where
+ * radii > 0 -- except on an overflowed sync-free frame, which adds nothing.  num_rendered / binning_capacity / n_host_mapped /
+ * event_loss_ready / sh_adam: as in gms_frame_args; the workspace is gms_frame_workspace_bytes(P, W, H).  As many launches as
+ * gms_train_frame.  Quaternion rows move as float4: rotation_raw and d_rotation_raw must be 16-byte aligned. */
+typedef struct gms_free_frame_args {
+    int32_t P, M;
+    int32_t scale_cols;         /* 3 (gs) or 2 (gs_flat) */
+    const float* xyz;           /* [P,3] _xyz */
+    const float* scaling_raw;   /* [P,scale_cols] _scaling */
+    const float* rotation_raw;  /* [P,4] _rotation, 16-byte aligned (GMS_E_ARG otherwise) */
+    const float* features;      /* [P,M,3] packed SH */
+    const float* opacity_raw;   /* [P,1] logits */
+    float eps;                  /* gs_flat eps_s0 = 1e-8 (unused for gs) */
+    float* d_xyz; float* d_scaling_raw; float* d_rotation_raw /* 16-byte aligned */; float* d_features; float* d_opacity_raw;
+    float* accum; float* denom; /* optional [P]: xyz_gradient_accum, denom (both or neither) */
+    gms_raster_settings settings;
+    const float* gt;            /* [3,H,W] */
+    float lambda_dssim;
+    float* loss;                /* device [3]: loss, L1, SSIM */
+    void* workspace; size_t workspace_bytes;
+    int64_t* num_rendered;
+    int64_t binning_capacity;
+    uint32_t* n_host_mapped;
+    void* event_loss_ready;
+    const gms_sh_adam* sh_adam; /* optional: fused Adam step of `features` (M = 16); then d_features may be NULL */
+} gms_free_frame_args;
+int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
+
+/* The forward half of gms_free_train_frame as a forward-only frame (GMS_FORWARD_ONLY), with gms_render_frame's capacity
+ * semantics; the workspace is gms_render_workspace_bytes(P, W, H). */
+typedef struct gms_free_render_args {
+    int32_t P, M, scale_cols;
+    const float* xyz; const float* scaling_raw; const float* rotation_raw /* 16-byte aligned */; const float* features;
+    const float* opacity_raw;
+    float eps;
+    gms_raster_settings settings;
+    float* image;               /* out [3,H,W] */
+    float* invdepth;            /* out [1,H,W] */
+    int32_t* radii;             /* out [P] */
+    void* workspace; size_t workspace_bytes;
+    int64_t* num_rendered;
+    int64_t binning_capacity;
+    uint32_t* n_host_mapped;
+} gms_free_render_args;
+int gms_free_render_frame(const gms_free_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
+
+/* densify_and_prune (scene/gaussian_model.py:360-414; flat_gaussian_model.py:62-88) in two calls.
+ * gms_densify_plan decides every row's fate from grads = accum / denom (0 / 0 -> 0) and S = max(get_scaling):
+ *   clone  grads >= grad_threshold and S <= split_scale (percent_dense * extent)
+ *   split  grads >= grad_threshold and S >  split_scale (the original is removed; two children replace it)
+ *   prune  sigmoid(opacity) < min_opacity, or (max_world_scale > 0) get_scaling.max > max_world_scale (0.1 * extent, the
+ *          reference's big_points_ws when max_screen_size is set) -- for originals, clones, and split children (judged by
+ *          their own scaling).  The screen-space prune never fires in the reference (max_radii2D is all zeros there) and
+ *          is not offered.
+ * A scan gives every surviving row its position in the reference's order: kept originals, clones, split copy 0 of every
+ * split row, split copy 1.  The call synchronises the stream ONCE and writes result[5] (host): the new P, the kept
+ * originals, the surviving clones, the surviving split pairs (each gives two rows) and the pruned rows.  P = 0 is valid. */
+#define GMS_FATE_CLONE 1
+#define GMS_FATE_SPLIT 2
+#define GMS_FATE_PRUNE 4            /* the row (and its clone) fails the prune */
+#define GMS_FATE_PRUNE_CHILDREN 8   /* its split children fail the prune */
+typedef struct gms_densify_plan_args {
+    int32_t P, scale_cols;
+    const float* accum; const float* denom;   /* [P] */
+    const float* scaling_raw;                 /* [P,scale_cols] */
+    const float* opacity_raw;                 /* [P,1] */
+    float eps;                                /* gs_flat eps_s0 */
+    float grad_threshold, split_scale, min_opacity, max_world_scale;
+    uint8_t* fate;                            /* optional out [P]: GMS_FATE_* bits */
+    void* scratch; size_t scratch_bytes;      /* gms_densify_scratch_bytes(P); gms_densify_apply reads the plan from it */
+    int32_t* result;                          /* host [5] */
+} gms_densify_plan_args;
+size_t gms_densify_scratch_bytes(int32_t P);
+int gms_densify_plan(const gms_densify_plan_args* a, void* cuda_stream);
+
+/* One set of per-Gaussian rows: the raw parameters, or one Adam moment of each of them. */
+typedef struct gms_free_set {
+    float* xyz;       /* [P,3] */
+    float* scaling;   /* [P,scale_cols] */
+    float* rotation;  /* [P,4] */
+    float* opacity;   /* [P,1] */
+    float* features;  /* [P,M,3] */
+} gms_free_set;
+
+/* Builds the densified set the plan in `scratch` describes into caller-allocated rows of the new size (result[0] of that
+ * plan): parameters and both Adam moments (src/dst[0] parameters, [1] exp_avg, [2] exp_avg_sq).  Kept originals carry
+ * their moments, clones and split children get zero moments.  Split child c of row i: xyz = R(q_i) (get_scaling_i *
+ * normals[i][c]) + xyz_i, scaling = log(get_scaling_i / 1.6) (columns [1,2] of it for gs_flat); normals [P,2,3] are
+ * standard-normal draws.  Sources are read only; destinations may not overlap them. */
+typedef struct gms_densify_apply_args {
+    int32_t P, new_P, scale_cols, M;
+    float eps;
+    const void* scratch; size_t scratch_bytes;   /* as left by gms_densify_plan for the same P */
+    const int32_t* result;                       /* host [5], gms_densify_plan's */
+    const float* normals;                        /* [P,2,3] */
+    gms_free_set src[3];
+    gms_free_set dst[3];
+} gms_densify_apply_args;
+int gms_densify_apply(const gms_densify_apply_args* a, void* cuda_stream);
+
 /* Scores an image against its ground truth, forward only, deterministically (per-tile partial sums added in a fixed order in
  * double, no atomics: the same inputs give the same bits).  Both images go through the same transform first:
  *   quantize 0: clamp to [0,1]                                  (training_report, train.py:203-204)

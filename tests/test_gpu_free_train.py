@@ -1,0 +1,420 @@
+"""-m gpu: native training of free Gaussians (gs, gs_flat): gms_free_train_frame against the float64 oracle, the fused
+densification statistics, gms_densify_plan / gms_densify_apply against the reference's own densification
+(tests/golden/densify.npz) and its restatement (densify_oracle.py), the lagged opacity group of FlatAdam, and a scaled-down
+white-background training run through FreeTrainer."""
+import ctypes as C
+
+import numpy as np
+import pytest
+import torch
+
+import aten_reference
+import densify_oracle as D
+from gms_b200 import _lib, scenes
+from gms_b200.model import FreeGaussianModel, PointsModel
+from gms_b200.optim import FlatAdam, free_model_groups
+from gms_b200.render import NativeFreeRenderer, PointsRenderer
+from gms_b200.trainer import FreeOptimizationParams, FreeTrainer, NativeFreeFrame
+from gpu_helpers import assert_image_parity
+from helpers import random_gaussians, settings_from_camera
+from oracle import raster
+
+pytestmark = pytest.mark.gpu
+
+LAMBDA = 0.2
+BG = (0.2, 0.5, 0.9)
+W = H = 256
+SIZES = [(240, 272), (256, 256), (400, 300)]      # T = 15 x 17 = 255, 16 x 16 = 256, 25 x 19 = 475 (300 = 18.75 tiles)
+OPTION_SETS = [{}, {"sort_impl": 1}, {"bin_impl": 1}, {"bin_impl": 1, "sort_impl": 1}, {"key16": 0}, {"key16": 0, "sort_impl": 1},
+               {"composite_fwd": 3}, {"composite_bwd": 3}, {"tile_order": 0}, {"sh_staged": 0}, {"sh_staged": 2},
+               {"expand_staged": 0}]
+# max err / max |ref| of the raw gradients; scales and rotations go through the near-singular 2D covariance (DESIGN.md 2.2)
+# run-to-run spread of the gradients between two frames of one camera, max |diff| / max |grad|: the composite backward adds
+# with float atomics; scales and rotations amplify it through the near-singular 2D covariance.  Largest spread measured over
+# the twelve option sets on an H100: xyz 5.7e-5, scaling 1.7e-3, rotation 5.5e-4, opacity 3.4e-7, features 2.9e-7; the
+# bounds are about 2.5x that
+SYNC_NOISE = {"_xyz": 1.5e-4, "_scaling": 4e-3, "_rotation": 1.5e-3, "_opacity": 1e-6, "_features": 1e-6}
+RAW_TOL = {"_xyz": 5e-4, "_scaling": 5e-3, "_rotation": 5e-3, "_opacity": 2e-4, "_features": 2e-4}
+
+
+def _opt_id(opts):
+    return ",".join(f"{k}={v}" for k, v in opts.items()) or "defaults"
+
+
+class _Options:
+    def __init__(self, opts):
+        self.opts = opts
+
+    def __enter__(self):
+        self.old = {k: _lib.set_option(k, v) for k, v in self.opts.items()}
+
+    def __exit__(self, *exc):
+        for k, v in self.old.items():
+            _lib.set_option(k, v)
+
+
+def _raw(kind, P=3000, seed=3):
+    """Raw parameters of a free-Gaussian scene: un-normalised quaternions (the normalisation's backward is exercised)."""
+    g = random_gaussians(P, seed=seed, extent=0.8, flat_frac=0.0)
+    gen = torch.Generator().manual_seed(seed + 1)
+    s = torch.log(g["scales"])
+    if kind == "gs_flat":
+        s = s[:, 1:]
+    rot = g["rotations"] * (0.5 + torch.rand(P, 1, generator=gen))
+    return dict(xyz=g["means3D"], scaling=s.contiguous(), rotation=rot, features=g["shs"], opacity=torch.logit(g["opacities"]))
+
+
+def _model(raw, kind, degree):
+    m = FreeGaussianModel(raw["xyz"], raw["scaling"], raw["rotation"], raw["features"], raw["opacity"], kind, "cuda", degree)
+    opt = FlatAdam(free_model_groups(m, 1e-3))
+    return m, opt
+
+
+def _cam(i=0, W=W, H=H):
+    return scenes.ring_cameras(8, 2.5, W, H)[i]
+
+
+def _gt(seed=0, W=W, H=H):
+    return torch.rand(3, H, W, generator=torch.Generator().manual_seed(seed))
+
+
+def _views(fr, P):
+    v = _lib.FrameView()
+    _lib.check(_lib.lib().gms_frame_views(fr.ws.data_ptr(), P, fr.W, fr.H, C.byref(v)), "gms_frame_views")
+
+    def take(ptr, shape, dtype=torch.float32):
+        off = ptr - fr.ws.data_ptr()
+        return fr.ws[off:off + 4 * int(np.prod(shape))].view(dtype).view(shape).clone()
+
+    al = lambda b: (b + 255) // 256 * 256
+    HW = fr.W * fr.H
+    d_m2d = v.invdepth + al(4 * HW) + al(12 * HW) + al(12 * P)     # frame_layout: invdepth, dimage, d_xyz, d_m2d
+    return dict(scales=take(v.scales, (P, 3)), rotations=take(v.rotations, (P, 4)), radii=take(v.radii, (P,), torch.int32),
+                image=take(v.image, (3, fr.H, fr.W)), d_m2d=take(d_m2d, (P, 3)))
+
+
+def _grads(m):
+    return {n: getattr(m, n).grad.detach().clone() for n in m.NAMES}
+
+
+def _oracle_raw(raw, kind, out, dC, S):
+    """Oracle image and float64 gradients of sum(image * dC) with respect to the raw parameters."""
+    t = {k: v.double().clone().requires_grad_(True) for k, v in raw.items()}
+    s = torch.exp(t["scaling"])
+    if kind == "gs_flat":
+        s = torch.cat([torch.full((s.shape[0], 1), 1e-8, dtype=torch.float64), s], 1)
+    rot = torch.nn.functional.normalize(t["rotation"])
+    op = torch.sigmoid(t["opacity"])
+    gs, gr = out["scales"].cpu(), out["rotations"].cpu()
+    assert float(((gs.double() - s.detach()).abs() / s.detach()).max()) <= 1e-6
+    assert float((gr.double() - rot.detach()).abs().max()) <= 1e-6
+    st = raster.forward(S, raw["xyz"], op.detach().float(), shs=raw["features"].contiguous(), scales=gs, rotations=gr)
+    g = raster.backward(st, dC)
+    outs = [(t["xyz"], g["dL_dmeans3D"]), (s, g["dL_dscales"]), (rot, g["dL_drotations"]), (op, g["dL_dopacity"])]
+    torch.autograd.backward([a for a, _ in outs], [torch.tensor(b, dtype=torch.float64).reshape(a.shape) for a, b in outs])
+    return st, dict(_xyz=t["xyz"].grad, _scaling=t["scaling"].grad, _rotation=t["rotation"].grad, _opacity=t["opacity"].grad,
+                    _features=torch.tensor(g["dL_dsh"]))
+
+
+def _check_against_oracle(kind, degree, W, H, opts=None, tag=""):
+    """The second (sync-free) frame of a camera against the float64 oracle chain: radii and N bit-exact, image, loss and the
+    raw gradients; gms_free_render_frame gives the train frame's image and radii bit for bit."""
+    raw = _raw(kind)
+    cam, gt, bg = _cam(1, W, H).to("cuda"), _gt(1, W, H).cuda(), torch.tensor(BG, device="cuda")
+    with _Options(opts or {}):
+        m, opt = _model(raw, kind, degree)
+        fr = NativeFreeFrame(m, W, H, LAMBDA)
+        fr.run(cam, gt, bg, stats=False)
+        n_first = fr.last_num_rendered
+        loss = float(fr.run(cam, gt, bg, stats=False))
+        torch.cuda.synchronize()
+        assert fr.overflows == 0 and fr.capacity > n_first > 0
+        P = m.P
+        out = _views(fr, P)
+        r = NativeFreeRenderer(m, W, H)
+        image, radii, _ = r.render(cam, bg)
+        torch.cuda.synchronize()
+    assert torch.equal(image, out["image"]) and torch.equal(radii, out["radii"])
+    img = out["image"].cpu().double().requires_grad_(True)
+    aten_reference.training_loss(img, gt.cpu().double(), LAMBDA).backward()
+    S = settings_from_camera(_cam(1, W, H), sh_degree=degree, bg=BG)
+    st, og = _oracle_raw(raw, kind, out, img.grad.float().numpy(), S)
+    np.testing.assert_array_equal(out["radii"].cpu().numpy(), st.radii)
+    assert fr.last_num_rendered == st.N
+    assert_image_parity(st, out["image"].cpu().numpy())
+    ref_loss = float(aten_reference.training_loss(torch.tensor(st.color, dtype=torch.float64), gt.cpu().double(), LAMBDA))
+    assert abs(loss - ref_loss) <= 1e-5 * max(1.0, abs(ref_loss))
+    got = _grads(m)
+    errs = {}
+    for k, ref in og.items():
+        a = got[k].cpu().double().reshape(ref.shape)
+        errs[k] = float((a - ref).abs().max()) / max(float(ref.abs().max()), 1e-20)
+    print(f"[free frame {kind} deg {degree} {W}x{H} {tag}] P={P} N={st.N} grad err/max: " +
+          ", ".join(f"{k} {e:.2e}" for k, e in errs.items()))
+    for k, e in errs.items():
+        assert e <= RAW_TOL[k], (k, e)
+
+
+@pytest.mark.parametrize("W,H", SIZES)
+@pytest.mark.parametrize("degree", [0, 1, 2, 3])
+@pytest.mark.parametrize("kind", ["gs", "gs_flat"])
+def test_free_frame_matches_oracle(kind, degree, W, H):
+    _check_against_oracle(kind, degree, W, H)
+
+
+@pytest.mark.parametrize("opts", OPTION_SETS, ids=_opt_id)
+def test_free_frame_matches_oracle_under_every_option(opts):
+    """Every binning / sort / compositing option at the ragged size (400 x 300: 475 tiles, two passes of the hand-written sort)."""
+    _check_against_oracle("gs_flat", 3, 400, 300, opts, _opt_id(opts))
+
+
+@pytest.mark.parametrize("opts", OPTION_SETS, ids=_opt_id)
+def test_sync_free_frame_equals_synchronising_frame(opts):
+    """Under every binning / sort / compositing option: the sync-free frame (capacity predicted) renders the synchronising
+    frame's image and radii bit for bit; its gradients agree within the run-to-run noise of the float atomics of the
+    composite backward."""
+    raw = _raw("gs_flat", seed=5)
+    cam, gt, bg = _cam(2).to("cuda"), _gt(2).cuda(), torch.tensor(BG, device="cuda")
+    with _Options(opts):
+        m, opt = _model(raw, "gs_flat", 3)
+        fr = NativeFreeFrame(m, W, H, LAMBDA)
+        fr.run(cam, gt, bg, stats=False)
+        torch.cuda.synchronize()
+        a, ga = _views(fr, m.P), _grads(m)
+        fr.run(cam, gt, bg, stats=False)
+        torch.cuda.synchronize()
+        b, gb = _views(fr, m.P), _grads(m)
+    assert fr.overflows == 0 and fr.capacity > fr.last_num_rendered
+    assert torch.equal(a["image"], b["image"]) and torch.equal(a["radii"], b["radii"])
+    spread = {k: float((ga[k] - gb[k]).abs().max()) / max(float(ga[k].abs().max()), 1e-20) for k in ga}
+    print(f"[sync-free vs synchronising {_opt_id(opts)}] grad |diff| / max|grad|: " + ", ".join(f"{k} {e:.2e}" for k, e in spread.items()))
+    for k, e in spread.items():
+        assert e <= SYNC_NOISE[k], (k, e)
+
+
+def test_statistics_match_restatement_and_skip_overflowed_frames():
+    raw = _raw("gs_flat", seed=7)
+    raw["xyz"][:100] = 1000.0           # beyond zfar of every camera: never visible, denom stays 0
+    m, opt = _model(raw, "gs_flat", 3)
+    bg = torch.tensor(BG, device="cuda")
+    fr = NativeFreeFrame(m, W, H, LAMBDA)
+    acc, den = torch.zeros(m.P, device="cuda"), torch.zeros(m.P, device="cuda")
+    cams = [_cam(i).to("cuda") for i in range(4)]
+    for i in range(8):
+        fr.run(cams[i % 4], _gt(i % 4).cuda(), bg)
+        torch.cuda.synchronize()
+        v = _views(fr, m.P)
+        acc, den = D.add_stats(acc, den, v["d_m2d"], v["radii"])
+        torch.testing.assert_close(fr.accum, acc, rtol=2.4e-7 * (i + 1), atol=0)
+        assert torch.equal(fr.denom, den)
+    assert fr.overflows == 0 and (den > 0).any() and (den == 0).any()
+    # an overflowed frame adds nothing; the view's next frame adds again
+    before_a, before_d = fr.accum.clone(), fr.denom.clone()
+    fr.capacity_override = 1
+    fr.run(cams[0], _gt(0).cuda(), bg)
+    torch.cuda.synchronize()
+    assert fr.last_num_rendered > 1 and fr.overflows == 1        # (reading N harvests the frame's overflow flag)
+    assert torch.equal(fr.accum, before_a) and torch.equal(fr.denom, before_d)
+    fr.capacity_override = None
+    fr.run(cams[0], _gt(0).cuda(), bg)
+    torch.cuda.synchronize()
+    v = _views(fr, m.P)
+    acc, den = D.add_stats(acc, den, v["d_m2d"], v["radii"])
+    assert fr.overflows == 1
+    torch.testing.assert_close(fr.accum, acc, rtol=2.4e-6, atol=0)
+    assert torch.equal(fr.denom, den)
+
+
+def _trainer_from_state(st, kind, accum, denom, extent):
+    feats = st["features"]
+    m = FreeGaussianModel(st["xyz"], st["scaling"], st["rotation"], feats, st["opacity"], kind, "cuda", 3)
+    tr = FreeTrainer(m, torch.ones(3, device="cuda"), extent, FreeOptimizationParams())
+    idx = {g["name"]: i for i, g in enumerate(tr.adam.groups)}
+    for n in D.NAMES:
+        i = idx[n]
+        o0 = tr.adam.ends[i - 1] if i else 0
+        k = st[n].numel()
+        tr.adam.m[o0:o0 + k] = st["m_" + n].reshape(-1).cuda()
+        tr.adam.v[o0:o0 + k] = st["v_" + n].reshape(-1).cuda()
+    tr.frame = NativeFreeFrame(m, 64, 64, LAMBDA)
+    tr.frame.accum.copy_(accum)
+    tr.frame.denom.copy_(denom)
+    return tr
+
+
+def _native_state(tr):
+    idx = {g["name"]: i for i, g in enumerate(tr.adam.groups)}
+    out = {}
+    for n in D.NAMES:
+        p = getattr(tr.model, "_" + n)
+        out[n] = p.detach().cpu()
+        i = idx[n]
+        o0 = tr.adam.ends[i - 1] if i else 0
+        out["m_" + n] = tr.adam.m[o0:o0 + p.numel()].view(p.shape).cpu()
+        out["v_" + n] = tr.adam.v[o0:o0 + p.numel()].view(p.shape).cpu()
+    return out
+
+
+def _compare_densified(got, ref, counts, tag):
+    """Rows [0, kept + clones) and every moment bit for bit; split children: xyz / scaling within a few ulp of max(|value|, 1)
+    (the exp / log / sqrt of the device and the host, and the reference's bmm, round differently)."""
+    c = counts[1] + counts[2]
+    worst = {}
+    for k, r in ref.items():
+        g = got[k]
+        assert g.shape == r.shape, (tag, k, g.shape, r.shape)
+        if k in ("xyz", "scaling"):
+            assert torch.equal(g[:c], r[:c]), (tag, k)
+            d = (g[c:].double() - r[c:].double()).abs()
+            ulp = torch.finfo(torch.float32).eps * r[c:].double().abs().clamp_min(1.0)     # ulps of max(|value|, 1)
+            worst[k] = float((d / ulp).max()) if d.numel() else 0.0
+        else:
+            assert torch.equal(g, r), (tag, k)
+    print(f"[densify {tag}] new P {counts[0]}, split children: max |native - reference| in ulp of the value: {worst}")
+    assert all(v <= 8 for v in worst.values()), worst
+
+
+@pytest.mark.parametrize("kind,size", [(k, s) for k in ("gs", "gs_flat") for s in ("none", "20")])
+def test_densify_matches_the_reference(golden_dir, kind, size):
+    gold = dict(np.load(f"{golden_dir}/densify.npz"))
+    tag = f"{kind}_{size}_"
+    st = {k[len(tag) + 3:]: torch.from_numpy(v) for k, v in gold.items() if k.startswith(tag + "in_")}
+    tr = _trainer_from_state(st, kind, torch.from_numpy(gold[tag + "accum"]).cuda(), torch.from_numpy(gold[tag + "denom"]).cuda(), 4.0)
+    steps = list(tr.adam.steps)
+    counts = tr.densify(size_prune=size != "none", normals=torch.from_numpy(gold[tag + "normals"]).cuda())
+    ref = {k[len(tag) + 4:]: torch.from_numpy(v) for k, v in gold.items() if k.startswith(tag + "out_") and k != tag + "out_accum"}
+    assert counts[0] == ref["xyz"].shape[0] and tr.adam.steps == steps
+    _, _, ocounts = D.densify(st, torch.from_numpy(gold[tag + "accum"]), torch.from_numpy(gold[tag + "denom"]),
+                              torch.from_numpy(gold[tag + "normals"]), 4.0, size_prune=size != "none")
+    assert counts == ocounts
+    _compare_densified(_native_state(tr), ref, counts, tag)
+    assert not tr.frame.accum.any() and tr.frame.accum.shape[0] == counts[0]
+
+
+def _big_state(kind, P, seed):
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    cols = 3 if kind == "gs" else 2
+    r = lambda *s: torch.randn(*s, device="cuda", generator=g)
+    st = dict(xyz=r(P, 3), scaling=math_log(0.05) + 1.2 * r(P, cols), rotation=r(P, 4), opacity=2 * r(P, 1), features=r(P, 16, 3))
+    for n in D.NAMES:
+        st["m_" + n], st["v_" + n] = 1e-3 * r(*st[n].shape), 1e-6 * r(*st[n].shape).abs()
+    accum = 3e-4 * r(P).abs() * 4
+    denom = torch.randint(0, 5, (P,), device="cuda", generator=g).float()
+    accum[denom == 0] = 0
+    return st, accum, denom, r(P, 2, 3)
+
+
+def math_log(x):
+    return float(np.log(x))
+
+
+@pytest.mark.parametrize("kind", ["gs", "gs_flat"])
+@pytest.mark.parametrize("P", [200_000, 0])
+def test_densify_matches_restatement_at_scale(kind, P):
+    st, accum, denom, normals = _big_state(kind, P, seed=P + len(kind))
+    extent = 3.0
+    for size_prune in (False, True):
+        tr = _trainer_from_state({k: v.cpu() for k, v in st.items()}, kind, accum, denom, extent)
+        counts = tr.densify(size_prune=size_prune, normals=normals)
+        ref, _, rcounts = D.densify(st, accum, denom, normals, extent, size_prune=size_prune)
+        assert counts == rcounts
+        if P:
+            assert min(counts[1:4]) > 0
+        _compare_densified(_native_state(tr), {k: v.cpu() for k, v in ref.items()}, counts, f"{kind} P={P} size_prune={size_prune}")
+
+
+def test_lagged_opacity_group_matches_torch_adam(golden_dir):
+    """A lone opacity reset skips the opacity group's step once; 20 steps against torch.optim.Adam on the same groups."""
+    raw = _raw("gs_flat", P=500, seed=11)
+    m, opt = _model(raw, "gs_flat", 3)
+    ref = {n: torch.nn.Parameter(getattr(m, n).detach().clone()) for n in m.NAMES}
+    names = {"xyz": "_xyz", "opacity": "_opacity", "scaling": "_scaling", "rotation": "_rotation"}
+    groups = [dict(params=[ref[names[g["name"]]]], lr=g["lr"]) for g in opt.groups[:-1]]
+    f = ref["_features"]
+    fdc, frest = torch.nn.Parameter(f.detach()[:, :1].clone()), torch.nn.Parameter(f.detach()[:, 1:].clone())
+    groups += [dict(params=[fdc], lr=opt.groups[-1]["lr0"]), dict(params=[frest], lr=opt.groups[-1]["lr1"])]
+    adam = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
+    gen = torch.Generator(device="cuda").manual_seed(3)
+    for it in range(20):
+        grads = {n: 1e-2 * torch.randn(getattr(m, n).shape, device="cuda", generator=gen) for n in m.NAMES}
+        for n in m.NAMES:
+            getattr(m, n).grad.copy_(grads[n])
+        skip = ("opacity",) if it == 1 else ()
+        opt.step(skip=skip)
+        for n in m.NAMES:
+            if n == "_features":
+                fdc.grad, frest.grad = grads[n][:, :1].clone(), grads[n][:, 1:].clone()
+            else:
+                ref[n].grad = None if (skip and n == "_opacity") else grads[n].clone()
+        adam.step()
+    assert opt.steps == [20, 20, 20, 19, 20]
+    for n in m.NAMES:
+        want = torch.cat([fdc.detach(), frest.detach()], 1) if n == "_features" else ref[n].detach()
+        torch.testing.assert_close(getattr(m, n).detach(), want, rtol=1e-5, atol=1e-7)
+
+
+def test_white_background_training_run(tmp_path):
+    """Densify from 200 every 100, opacity reset at 600, 1200 iterations at 256x256 from 10k flat Gaussians: no overflowed
+    frame, P changes at every densification, each densification equals the restated reference's on the same state and
+    draws, the loss falls, and the saved checkpoint renders as a gs_points pseudo-mesh."""
+    cams = [c.to("cuda") for c in scenes.ring_cameras(8, 2.5, W, H)]
+    for i, c in enumerate(cams):
+        c.uid = i
+    white = torch.ones(3, device="cuda")
+    target = FreeGaussianModel(**{k: v for k, v in zip(("xyz", "scaling", "rotation", "features", "opacity"),
+                                                      _raw("gs_flat", P=4000, seed=21).values())}, kind="gs_flat", active_sh_degree=0)
+    rt = NativeFreeRenderer(target, W, H)
+    gts = [rt.render(c, white)[0].clone() for c in cams]
+    raw = _raw("gs_flat", P=10_000, seed=22)
+    model = FreeGaussianModel(raw["xyz"], raw["scaling"], raw["rotation"], raw["features"], raw["opacity"], "gs_flat", "cuda", 0)
+    o = FreeOptimizationParams(iterations=1200, densify_from_iter=200, densification_interval=100, opacity_reset_interval=600,
+                               densify_until_iter=1100)
+    checked = []
+
+    class Checked(FreeTrainer):
+        def densify(self, size_prune, normals=None):
+            P = self.model.P
+            st = {n: getattr(self.model, "_" + n).detach().clone() for n in D.NAMES}
+            nat = _native_state(self)
+            for n in D.NAMES:
+                st["m_" + n], st["v_" + n] = nat["m_" + n].cuda(), nat["v_" + n].cuda()
+            acc, den = self.frame.accum.clone(), self.frame.denom.clone()
+            normals = torch.randn(max(P, 1), 2, 3, device="cuda")
+            counts = super().densify(size_prune, normals)
+            ref, _, rc = D.densify(st, acc, den, normals, self.extent, size_prune=size_prune)
+            assert counts == rc
+            _compare_densified(_native_state(self), {k: v.cpu() for k, v in ref.items()}, counts, f"run it {self.iteration + 1}")
+            checked.append((P, counts[0]))
+            return counts
+
+    tr = Checked(model, white, scenes.camera_extent(cams), o)
+    losses, launches = [], {}
+    for it in range(1, 1201):
+        v = it % len(cams)
+        _lib.launch_count(reset=True)
+        losses.append(tr.step(cams[v], gts[v]).clone())
+        launches[it] = _lib.launch_count(reset=True)
+    losses = torch.stack(losses).cpu()
+    assert tr.frame.overflows == 0
+    assert len(checked) == 8 and all(a != b for a, b in checked), checked
+    # no step on a densification iteration (8) nor on the last one; the lone reset at densify_from_iter skips opacity once
+    assert tr.adam.steps[0] == 1200 - 8 - 1 and tr.adam.steps[tr.adam.group_index("opacity")] == tr.adam.steps[0] - 1
+    # launches: the frame (12) + one Adam launch while every group's count is equal; after the lone reset, two (the lagging
+    # opacity group is a run of its own); a densification: the frame + plan + apply; the last iteration: the frame alone
+    densify_its = set(range(300, 1001, 100))
+    assert all(launches[it] == 13 for it in range(1, 200)), launches
+    assert all(launches[it] == 14 for it in range(201, 1200) if it not in densify_its), launches
+    assert all(launches[it] == 14 for it in densify_its) and launches[200] == 13 and launches[1200] == 12, launches
+    first, last = float(losses[:100].mean()), float(losses[-100:].mean())
+    print(f"[free training] P {raw['xyz'].shape[0]} -> {model.P}, densifications {checked}, loss {first:.4f} -> {last:.4f}")
+    assert last < 0.9 * first
+    ev = tr.evaluate(cams[:2], gts[:2])
+    assert torch.isfinite(ev.mean).all()
+    ply = str(tmp_path / "point_cloud.ply")
+    model.save(ply)
+    pm = PointsModel.from_flat_checkpoint(ply, "cuda", active_sh_degree=model.active_sh_degree)
+    image, radii, _ = PointsRenderer(pm, W, H).render(cams[0], white)
+    torch.cuda.synchronize()
+    assert pm.triangles.shape[0] == model.P and torch.isfinite(image).all() and (radii > 0).any()
+    back = FreeGaussianModel.from_checkpoint(ply, "gs_flat", "cuda")
+    assert torch.equal(back._scaling, model._scaling.detach()) and torch.equal(back._xyz, model._xyz.detach())
