@@ -21,6 +21,7 @@
 #include "gms_binning.cuh"
 #include "gms_image.cuh"
 #include "gms_free.cuh"
+#include "gms_knn.cuh"
 
 // ------------------------------------------------------------------------------------------ host state
 static thread_local char g_err[512] = "";
@@ -2331,6 +2332,67 @@ int gms_densify_apply(const gms_densify_apply_args* a, void* cuda_stream) {
     span_begin(K_MISC, st);
     k_densify_apply<<<(a->P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, st>>>(k);
     GMS_AFTER_LAUNCH("densify_apply", 0, st);
+    span_end(st);
+    return GMS_OK;
+}
+
+// ---- three-nearest-neighbour mean squared distance (gms_knn.cuh)
+
+struct KnnLayout {
+    KnnBounds* part;                    // [GMS_KNN_BOUNDS_BLOCKS] partial bounding boxes
+    KnnBounds* bounds;                  // [1] bounding box of the cloud
+    uint32_t* code; uint32_t* code_s;   // [P] Morton codes, unsorted / sorted
+    uint32_t* idx; uint32_t* idx_s;     // [P] point indices, unsorted / sorted
+    float4* sorted;                     // [P] points in Morton order, w = original index
+    float4* blo; float4* bhi;           // [boxes] per-box bounds
+    void* cub; size_t cub_bytes; size_t total;
+};
+
+static KnnLayout knn_layout(void* base, int P) {
+    KnnLayout L;
+    char* p = reinterpret_cast<char*>(base);
+    const int Pn = P > 0 ? P : 1, nbox = (Pn + GMS_KNN_BOX - 1) / GMS_KNN_BOX;
+    L.part = carve<KnnBounds>(p, GMS_KNN_BOUNDS_BLOCKS);
+    L.bounds = carve<KnnBounds>(p, 1);
+    L.code = carve<uint32_t>(p, Pn); L.code_s = carve<uint32_t>(p, Pn);
+    L.idx = carve<uint32_t>(p, Pn); L.idx_s = carve<uint32_t>(p, Pn);
+    L.sorted = carve<float4>(p, Pn);
+    L.blo = carve<float4>(p, nbox); L.bhi = carve<float4>(p, nbox);
+    L.cub_bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, L.cub_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr,
+                                    Pn, 0, 30);
+    L.cub = p;
+    p += align_up(L.cub_bytes);
+    L.total = (size_t)(p - reinterpret_cast<char*>(base));
+    return L;
+}
+
+size_t gms_knn_scratch_bytes(int32_t P) { return knn_layout(nullptr, P).total + 512; }
+
+int gms_knn_dist2(const gms_knn_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || a->P < 0 || (a->P >= 1 && a->P <= 3) || a->P > INT32_MAX - GMS_KNN_BOX)
+        return set_err(GMS_E_ARG, "gms_knn_dist2: need P == 0 or 4 <= P <= INT32_MAX - GMS_KNN_BOX (three other points)%s%s");
+    if (a->P == 0) return GMS_OK;
+    if (!a->points || !a->dist2 || !a->scratch) return set_err(GMS_E_ARG, "gms_knn_dist2: null argument%s%s");
+    if (a->scratch_bytes < gms_knn_scratch_bytes(a->P)) return set_err(GMS_E_ARG, "gms_knn_dist2: scratch too small%s%s");
+    const int P = a->P, nbox = (P + GMS_KNN_BOX - 1) / GMS_KNN_BOX;
+    KnnLayout L = knn_layout(aligned_base_c(a->scratch), P);
+    span_begin(K_MISC, st);
+    k_knn_bounds<<<GMS_KNN_BOUNDS_BLOCKS, 256, 0, st>>>(P, a->points, L.part);
+    GMS_AFTER_LAUNCH("knn_bounds", 0, st);
+    k_knn_bounds_fold<<<1, 256, 0, st>>>(L.part, L.bounds);
+    GMS_AFTER_LAUNCH("knn_bounds_fold", 0, st);
+    k_knn_morton<<<(P + 255) / 256, 256, 0, st>>>(P, a->points, L.bounds, L.code, L.idx);
+    GMS_AFTER_LAUNCH("knn_morton", 0, st);
+    size_t tb = L.cub_bytes;
+    GMS_CUDA(cub::DeviceRadixSort::SortPairs(L.cub, tb, L.code, L.code_s, L.idx, L.idx_s, P, 0, 30, st));
+    k_knn_gather<<<(P + 255) / 256, 256, 0, st>>>(P, a->points, L.idx_s, L.sorted);
+    GMS_AFTER_LAUNCH("knn_gather", 0, st);
+    k_knn_box_bounds<<<(nbox + 7) / 8, 256, 0, st>>>(P, nbox, L.sorted, L.blo, L.bhi);
+    GMS_AFTER_LAUNCH("knn_box_bounds", 0, st);
+    k_knn_search<<<nbox, GMS_KNN_BOX, 0, st>>>(P, nbox, L.sorted, L.blo, L.bhi, a->dist2);
+    GMS_AFTER_LAUNCH("knn_search", 0, st);
     span_end(st);
     return GMS_OK;
 }

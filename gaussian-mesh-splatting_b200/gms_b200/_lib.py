@@ -237,6 +237,14 @@ class AdamShArgs(C.Structure):
                 ("beta2", C.c_double), ("eps", C.c_double), ("step", C.c_int32)]
 
 
+KNN_BOX = 64        # GMS_KNN_BOX: points per box of the three-nearest-neighbour search
+
+
+class KnnArgs(C.Structure):
+    """struct gms_knn_args"""
+    _fields_ = [("P", C.c_int32), ("points", C.c_void_p), ("dist2", C.c_void_p), ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t)]
+
+
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_int, C.c_size_t)
 
 # every symbol include/gms_b200.h declares (tests/test_abi.py checks the library exports all of them)
@@ -250,7 +258,7 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_points_render_workspace_bytes", "gms_points_render_frame", "gms_pseudomesh_bind_scratch_bytes",
                "gms_pseudomesh_bind", "gms_pseudomesh_repose", "gms_bound_points_render_workspace_bytes",
                "gms_bound_points_render_frame", "gms_free_train_frame", "gms_free_render_frame", "gms_densify_scratch_bytes",
-               "gms_densify_plan", "gms_densify_apply"]
+               "gms_densify_plan", "gms_densify_apply", "gms_knn_scratch_bytes", "gms_knn_dist2"]
 
 _lib = None
 
@@ -320,6 +328,9 @@ def lib():
     L.gms_densify_scratch_bytes.argtypes = [C.c_int32]
     L.gms_densify_plan.argtypes = [C.POINTER(DensifyPlanArgs), C.c_void_p]
     L.gms_densify_apply.argtypes = [C.POINTER(DensifyApplyArgs), C.c_void_p]
+    L.gms_knn_scratch_bytes.restype = C.c_size_t
+    L.gms_knn_scratch_bytes.argtypes = [C.c_int32]
+    L.gms_knn_dist2.argtypes = [C.POINTER(KnnArgs), C.c_void_p]
     L.gms_metrics_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]
     L.gms_image_metrics.argtypes = [C.POINTER(MetricsArgs), C.c_void_p]
     _lib = L

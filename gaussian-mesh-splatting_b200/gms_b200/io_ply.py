@@ -197,3 +197,52 @@ def save_multi_mesh_model(ply_path: str, model) -> None:
         v0 += nv
     torch.save({"_alpha": alphas, "_scale": scales, "point_cloud": [], "vertices": verts, "faces": faces},
                ply_path.replace("point_cloud.ply", "model_params.pt"))
+
+
+# ---- point clouds (points3d.ply): scene/dataset_readers.py:107-130
+
+_PCD_DTYPE = [("x", "f4"), ("y", "f4"), ("z", "f4"), ("nx", "f4"), ("ny", "f4"), ("nz", "f4"), ("red", "u1"), ("green", "u1"),
+              ("blue", "u1")]
+
+
+def point_cloud_elements(xyz, rgb) -> np.ndarray:
+    """The `vertex` rows storePly builds (scene/dataset_readers.py:115-126): xyz and zero normals cast to f4, rgb cast to u1
+    by numpy's float -> uint8 conversion, which truncates (127.9 -> 127)."""
+    xyz, rgb = np.asarray(xyz), np.asarray(rgb)
+    el = np.empty(xyz.shape[0], dtype=_PCD_DTYPE)
+    for k, n in enumerate(("x", "y", "z")):
+        el[n] = xyz[:, k]
+    for n in ("nx", "ny", "nz"):
+        el[n] = 0
+    for k, n in enumerate(("red", "green", "blue")):
+        el[n] = rgb[:, k]
+    return el
+
+
+def point_cloud_arrays(data) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """`vertex` rows -> (points [P,3], colors [P,3] = rgb / 255 in float64, normals [P,3]) as fetchPly returns them
+    (scene/dataset_readers.py:107-113)."""
+    points = np.vstack([data["x"], data["y"], data["z"]]).T
+    colors = np.vstack([data["red"], data["green"], data["blue"]]).T / 255.0
+    normals = np.vstack([data["nx"], data["ny"], data["nz"]]).T
+    return points, colors, normals
+
+
+def load_point_cloud(path: str) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """points3d.ply (COLMAP's converted cloud, or the random cloud of a NeRF-synthetic scene) -> (points [P,3] float32,
+    colors [P,3] = rgb / 255, normals [P,3]): fetchPly (scene/dataset_readers.py:107-113).  Binary or ASCII."""
+    data, _ = read_ply_vertices(path)
+    return point_cloud_arrays(data)
+
+
+def save_point_cloud(path: str, xyz, rgb) -> None:
+    """storePly (scene/dataset_readers.py:115-130): binary little-endian `x y z nx ny nz` float (normals zero) and
+    `red green blue` uchar, the colours truncated to bytes."""
+    el = point_cloud_elements(xyz, rgb)
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    with open(path, "wb") as f:
+        f.write(("ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % el.shape[0]).encode())
+        for n, t in _PCD_DTYPE:
+            f.write(f"property {'float' if t == 'f4' else 'uchar'} {n}\n".encode())
+        f.write(b"end_header\n")
+        el.tofile(f)

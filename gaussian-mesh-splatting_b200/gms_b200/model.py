@@ -12,7 +12,7 @@ import torch
 from torch import nn
 
 from . import _lib, expansion
-from .scenes import MeshGaussianParams
+from .scenes import SH_C0, MeshGaussianParams
 
 
 class MeshGaussianModel:
@@ -361,6 +361,30 @@ class FreeGaussianModel:
         g = io_ply.load_gaussian_ply(ply_path)
         return cls(g["_xyz"], g["_scaling"], g["_rotation"], torch.cat((g["_features_dc"], g["_features_rest"]), dim=1), g["_opacity"],
                    kind, device, active_sh_degree)
+
+    @classmethod
+    def from_point_cloud(cls, points, colors, kind: str = "gs_flat", sh_degree: int = 3, device="cuda") -> "FreeGaussianModel":
+        """create_from_pcd (scene/gaussian_model.py:124-147; flat_gaussian_model.py:37-60 for gs_flat): points [P,3] and
+        colors [P,3] in [0,1] (io_ply.load_point_cloud, scenes.random_point_cloud) ->
+          _xyz = points.float(); DC = RGB2SH(colors), rest 0; _rotation = (1,0,0,0); _opacity = inverse_sigmoid(0.1);
+          _scaling = log(sqrt(clamp_min(dist2, 1e-7))) over 3 columns (gs) or 2 (gs_flat), dist2 = knn.mean_dist2(_xyz);
+          active_sh_degree = 0.
+        RGB2SH is evaluated in float32 on the host, where the colours arrive; the scale and opacity maths is ATen on the device."""
+        from . import knn
+        xyz = torch.as_tensor(points).detach().float().to(device)
+        rgb = torch.as_tensor(colors).detach().cpu().float()
+        if xyz.dim() != 2 or xyz.shape[1] != 3 or tuple(rgb.shape) != tuple(xyz.shape):
+            raise ValueError("from_point_cloud: expected points [P,3] and colors [P,3]")
+        P, M = xyz.shape[0], (int(sh_degree) + 1) ** 2
+        features = torch.zeros(P, M, 3)
+        features[:, 0] = (rgb - 0.5) / SH_C0
+        dist2 = torch.clamp_min(knn.mean_dist2(xyz), 0.0000001)
+        scaling = torch.log(torch.sqrt(dist2))[..., None].repeat(1, 3 if kind == "gs" else 2)
+        rotation = torch.zeros(P, 4, device=xyz.device)
+        rotation[:, 0] = 1
+        x = 0.1 * torch.ones(P, 1, dtype=torch.float, device=xyz.device)
+        opacity = torch.log(x / (1 - x))
+        return cls(xyz, scaling, rotation, features, opacity, kind, device, active_sh_degree=0)
 
     def save(self, ply_path: str) -> None:
         """The reference's point_cloud.ply (GaussianModel.save_ply; gs_flat gets the log(eps_s0) scale_0 column)."""

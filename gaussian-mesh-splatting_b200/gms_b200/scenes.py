@@ -262,6 +262,19 @@ def transform_hotdog(triangles: torch.Tensor, t) -> torch.Tensor:
     return out
 
 
+def random_point_cloud(num_pts: int = 100_000, seed: int = 0) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """The cloud a NeRF-synthetic scene without points3d.ply trains from (readNerfSyntheticInfo, scene/dataset_readers.py:
+    233-246, after safe_state's np.random.seed(0); RandomState(seed) draws the same stream): xyz = U * 2.6 - 1.3,
+    shs = U / 255, colours SH2RGB(shs).  The reference stores that cloud (storePly) and trains from the file it reads back
+    (fetchPly), so it is returned after the same round trip: points cast to float32, and colours truncated to bytes, which
+    makes every colour 127/255 (SH2RGB(shs) * 255 lies in [127.5, 127.79)).  -> (points, colors, normals) as fetchPly."""
+    from . import io_ply
+    rng = np.random.RandomState(seed)
+    xyz = rng.random_sample((num_pts, 3)) * 2.6 - 1.3
+    shs = rng.random_sample((num_pts, 3)) / 255.0
+    return io_ply.point_cloud_arrays(io_ply.point_cloud_elements(xyz, (shs * SH_C0 + 0.5) * 255))
+
+
 def camera_extent(cams) -> float:
     """scene.cameras_extent: getNerfppNorm's radius (scene/dataset_readers.py:45-66) -- 1.1 times the largest distance of a
     camera centre from their mean.  The arithmetic stays in the centres' dtype, as the reference's numpy keeps it (its

@@ -608,6 +608,28 @@ typedef struct gms_densify_apply_args {
 } gms_densify_apply_args;
 int gms_densify_apply(const gms_densify_apply_args* a, void* cuda_stream);
 
+/* ---- point-cloud initialisation ------------------------------------------------------------------ */
+
+/* simple-knn's distCUDA2 (the initial scales of create_from_pcd, scene/gaussian_model.py:124-147): for every point, the mean
+ * squared distance to its three nearest OTHER points, exactly.
+ *   d(q,p)   = (dx*dx + dy*dy) + dz*dz, dx = q.x - p.x, each operation one round-to-nearest fp32 op (no FMA)
+ *   b0 <= b1 <= b2: the three smallest d(points[i], points[j]) over j != i; tied values (duplicate points at 0) count
+ *   separately
+ *   dist2[i] = ((b0 + b1) + b2) / 3, round-to-nearest
+ * The result depends only on the multiset of distances: two calls give the same bits, whatever the launch order.  The search
+ * prunes with Morton-ordered boxes of GMS_KNN_BOX points whose lower bounds round as d does, so pruning is exact (DESIGN.md
+ * 4.4).  P = 0 is a no-op; 1 <= P <= 3 (no three neighbours), a null pointer or too little scratch is GMS_E_ARG.  No host
+ * synchronisation. */
+#define GMS_KNN_BOX 64
+typedef struct gms_knn_args {
+    int32_t P;
+    const float* points;                   /* [P,3] device, every coordinate finite (not checked here) */
+    float* dist2;                          /* out [P] */
+    void* scratch; size_t scratch_bytes;   /* gms_knn_scratch_bytes(P) */
+} gms_knn_args;
+size_t gms_knn_scratch_bytes(int32_t P);
+int gms_knn_dist2(const gms_knn_args* a, void* cuda_stream);
+
 /* Scores an image against its ground truth, forward only, deterministically (per-tile partial sums added in a fixed order in
  * double, no atomics: the same inputs give the same bits).  Both images go through the same transform first:
  *   quantize 0: clamp to [0,1]                                  (training_report, train.py:203-204)
