@@ -187,10 +187,203 @@ GMS_HD void gms_face_frame_backward(const float* t, float eps, const GmsFrame& f
 #define GMS_ATOMIC_ADD(p, v) (*(p) += (v))
 #endif
 
+// Barycentric weights of one splat from its three raw parameters (gms_expand_args.alpha_activation):
+//   GMS_ALPHA_RELU     r_j = relu(x_j) + 1e-8, alpha_j = r_j / sum r   (GaussianMeshModel.update_alpha, gaussian_mesh_model.py:166-167)
+//   GMS_ALPHA_SOFTMAX  alpha = softmax(x)                               (GaussianFlameModel.update_alpha_func, gaussian_flame_model.py:34,195)
+// The softmax subtracts the row maximum first, so logits far above 88 cannot overflow expf: e_j = exp(x_j - m) lies in
+// (0, 1] and the largest is exactly 1, so s = (e0 + e1) + e2 lies in [1, 3].
+
 // `f` indexes the per-FACE arrays (faces / triangles_in / triangles); `fl` indexes the per-GAUSSIAN streams (alpha_raw,
 // scale_raw and every output row): fl == f when they are the caller's arrays, fl == the face's slot in the block when the
 // kernel has redirected those pointers to its shared-memory staging buffers (k_expand_fwd / k_expand_bwd).
-GMS_HD void gms_expand_face_fwd(const gms_expand_args& a, int f, int fl) {
+// A face is read, its frame and quaternion formed once (gms_expand_face_load / gms_expand_face_frame), then every splat is one call of
+// gms_expand_splat_fwd / gms_expand_splat_bwd: the per-thread kernels loop over the face's K splats, the wide kernels
+// (k_expand_wide_*) spread them over a warp's lanes.  Either way each splat's arithmetic is the same sequence of operations.
+struct GmsFaceState {
+    float t[9];
+    int64_t vi[3];
+    GmsFrame fr;
+    float q[4];
+    GmsQuatAux ax;
+    float qnorm, qn;
+};
+
+GMS_HD void gms_expand_face_load(const gms_expand_args& a, int f, GmsFaceState& s) {
+    s.vi[0] = s.vi[1] = s.vi[2] = 0;
+    if (a.triangles_in) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) s.t[k] = a.triangles_in[9 * (size_t)f + k];
+    } else {
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            s.vi[c] = a.faces[3 * (size_t)f + c];
+            s.t[3 * c] = a.vertices[3 * s.vi[c]]; s.t[3 * c + 1] = a.vertices[3 * s.vi[c] + 1]; s.t[3 * c + 2] = a.vertices[3 * s.vi[c] + 2];
+        }
+    }
+}
+
+GMS_HD void gms_expand_face_frame(const gms_expand_args& a, GmsFaceState& s) {
+    gms_face_frame(s.t, a.eps, s.fr);
+    gms_frame_quat(s.fr, s.q, s.ax);
+    s.qnorm = GMS_SQRTN(s.q[0] * s.q[0] + s.q[1] * s.q[1] + s.q[2] * s.q[2] + s.q[3] * s.q[3]);
+    s.qn = fmaxf(s.qnorm, 1e-12f);
+}
+
+template <int ACT>
+GMS_HD void gms_alpha_fwd(float x0, float x1, float x2, float& al0, float& al1, float& al2) {
+    if constexpr (ACT == GMS_ALPHA_SOFTMAX) {
+        const float m = fmaxf(fmaxf(x0, x1), x2);
+        const float e0 = expf(x0 - m), e1 = expf(x1 - m), e2 = expf(x2 - m);
+        const float s = (e0 + e1) + e2;                                                       // s in [1, 3]
+        al0 = GMS_DIVN(e0, s); al1 = GMS_DIVN(e1, s); al2 = GMS_DIVN(e2, s);
+    } else {
+        const float r0 = fmaxf(x0, 0.f) + 1e-8f, r1 = fmaxf(x1, 0.f) + 1e-8f, r2 = fmaxf(x2, 0.f) + 1e-8f;
+        const float S = r0 + r1 + r2;
+        al0 = GMS_DIVN(r0, S); al1 = GMS_DIVN(r1, S); al2 = GMS_DIVN(r2, S);        // S >= 3e-8
+    }
+}
+
+// Splat p of a face whose frame is in `s`.
+template <int ACT>
+GMS_HD void gms_expand_splat_fwd(const gms_expand_args& a, const GmsFaceState& s, size_t p) {
+    const float* t = s.t;
+    float al0, al1, al2;
+    gms_alpha_fwd<ACT>(a.alpha_raw[3 * p], a.alpha_raw[3 * p + 1], a.alpha_raw[3 * p + 2], al0, al1, al2);
+    if (a.alpha) { a.alpha[3 * p] = al0; a.alpha[3 * p + 1] = al1; a.alpha[3 * p + 2] = al2; }
+    if (a.xyz) {
+#pragma unroll
+        for (int c = 0; c < 3; c++) a.xyz[3 * p + c] = al0 * t[c] + al1 * t[3 + c] + al2 * t[6 + c];
+    }
+    const float cs = a.scale_raw[p];
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const float inner = fmaxf(cs * s.fr.s[c], 0.f) + a.eps;
+        if (a.scaling_log) a.scaling_log[3 * p + c] = logf(inner);
+        if (a.scaling_act) a.scaling_act[3 * p + c] = expf(logf(inner));
+    }
+    const float* q = s.q;
+    const float qn = s.qn;
+    if (a.rotation_raw) { float* o = a.rotation_raw + 4 * p; o[0] = q[0]; o[1] = q[1]; o[2] = q[2]; o[3] = q[3]; }
+    if (a.rotation_act) { float* o = a.rotation_act + 4 * p; o[0] = GMS_DIVN(q[0], qn); o[1] = GMS_DIVN(q[1], qn); o[2] = GMS_DIVN(q[2], qn); o[3] = GMS_DIVN(q[3], qn); }
+}
+
+template <int ACT>
+GMS_HD void gms_expand_face_fwd_act(const gms_expand_args& a, int f, int fl) {
+    GmsFaceState s;
+    gms_expand_face_load(a, f, s);
+    if (a.triangles) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) a.triangles[9 * (size_t)f + k] = s.t[k];
+    }
+    gms_expand_face_frame(a, s);
+    for (int k = 0; k < a.K; k++) gms_expand_splat_fwd<ACT>(a, s, (size_t)fl * a.K + k);
+}
+
+// The backward of splat p: writes its dL/d_alpha and dL/d_scale rows and ADDS its share of the face's corner, quaternion
+// and in-plane scale gradients to dt / dq / ds1 / ds2.
+template <int ACT>
+GMS_HD void gms_expand_splat_bwd(const gms_expand_args& a, const gms_expand_grads& g, const GmsFaceState& s, size_t p,
+                                 float* dt, float* dq, float& ds1, float& ds2) {
+    const float* t = s.t;
+    const float* q = s.q;
+    const float qnorm = s.qnorm, qn = s.qn;
+    // --- xyz = alpha @ triangle
+    float dx[3] = {0.f, 0.f, 0.f};
+    if (g.dL_dxyz) { dx[0] = g.dL_dxyz[3 * p]; dx[1] = g.dL_dxyz[3 * p + 1]; dx[2] = g.dL_dxyz[3 * p + 2]; }
+    const float ar[3] = {a.alpha_raw[3 * p], a.alpha_raw[3 * p + 1], a.alpha_raw[3 * p + 2]};
+    float al[3];
+    gms_alpha_fwd<ACT>(ar[0], ar[1], ar[2], al[0], al[1], al[2]);
+    float dal[3];
+#pragma unroll
+    for (int j = 0; j < 3; j++) {
+        dal[j] = dx[0] * t[3 * j] + dx[1] * t[3 * j + 1] + dx[2] * t[3 * j + 2];
+#pragma unroll
+        for (int c = 0; c < 3; c++) dt[3 * j + c] += al[j] * dx[c];
+    }
+    const float dsum = dal[0] * al[0] + dal[1] * al[1] + dal[2] * al[2];
+    if (g.dL_dalpha_raw) {
+        if constexpr (ACT == GMS_ALPHA_SOFTMAX) {
+#pragma unroll
+            for (int j = 0; j < 3; j++) g.dL_dalpha_raw[3 * p + j] = al[j] * (dal[j] - dsum);
+        } else {
+            const float S = (fmaxf(ar[0], 0.f) + 1e-8f) + (fmaxf(ar[1], 0.f) + 1e-8f) + (fmaxf(ar[2], 0.f) + 1e-8f);
+#pragma unroll
+            for (int j = 0; j < 3; j++) g.dL_dalpha_raw[3 * p + j] = ar[j] > 0.f ? GMS_DIVN(dal[j] - dsum, S) : 0.f;
+        }
+    }
+    // --- scaling
+    const float cs = a.scale_raw[p];
+    float dcs = 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        float gl = g.dL_dscaling_log ? g.dL_dscaling_log[3 * p + c] : 0.f;
+        const float prod = cs * s.fr.s[c];
+        const float inner = fmaxf(prod, 0.f) + a.eps;
+        if (g.dL_dscaling_act) gl += g.dL_dscaling_act[3 * p + c] * expf(logf(inner));
+        const float dprod = prod > 0.f ? GMS_DIVN(gl, inner) : 0.f;       // inner >= eps
+        dcs += dprod * s.fr.s[c];
+        if (c == 1) ds1 += dprod * cs;
+        if (c == 2) ds2 += dprod * cs;
+    }
+    if (g.dL_dscale_raw) g.dL_dscale_raw[p] = dcs;
+    // --- rotation (same quaternion for the K splats of the face: sum the incoming rows)
+    if (g.dL_drotation_raw) {
+        const float* d = g.dL_drotation_raw + 4 * p;
+        dq[0] += d[0]; dq[1] += d[1]; dq[2] += d[2]; dq[3] += d[3];
+    }
+    if (g.dL_drotation_act) {
+        const float* dp = g.dL_drotation_act + 4 * p;
+        const float d_x = dp[0], d_y = dp[1], d_z = dp[2], d_w = dp[3];
+        if (qnorm >= 1e-12f) {
+            const float u[4] = {GMS_DIVN(q[0], qn), GMS_DIVN(q[1], qn), GMS_DIVN(q[2], qn), GMS_DIVN(q[3], qn)};       // qn >= 1e-12
+            const float dd = d_x * u[0] + d_y * u[1] + d_z * u[2] + d_w * u[3];
+            dq[0] += GMS_DIVN(d_x - u[0] * dd, qn); dq[1] += GMS_DIVN(d_y - u[1] * dd, qn);
+            dq[2] += GMS_DIVN(d_z - u[2] * dd, qn); dq[3] += GMS_DIVN(d_w - u[3] * dd, qn);
+        } else {
+            dq[0] += GMS_DIVN(d_x, qn); dq[1] += GMS_DIVN(d_y, qn); dq[2] += GMS_DIVN(d_z, qn); dq[3] += GMS_DIVN(d_w, qn);
+        }
+    }
+}
+
+// The face's share once every splat's has been summed: through the quaternion and the frame to the corners, then
+// dL_dtriangles and the vertex atomics.
+GMS_HD void gms_expand_face_bwd_tail(const gms_expand_args& a, const gms_expand_grads& g, const GmsFaceState& s, int f, float* dt,
+                                     const float* dq, float ds1, float ds2) {
+    float dv0[3] = {0.f, 0.f, 0.f}, dv1[3] = {0.f, 0.f, 0.f}, dv2[3] = {0.f, 0.f, 0.f};
+    gms_frame_quat_backward(s.ax, dq, dv0, dv1, dv2);
+    gms_face_frame_backward(s.t, a.eps, s.fr, dv0, dv1, dv2, ds1, ds2, dt);
+    if (g.dL_dtriangles) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) g.dL_dtriangles[9 * (size_t)f + k] = dt[k];
+    }
+    if (g.dL_dvertices && !a.triangles_in) {
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            GMS_ATOMIC_ADD(&g.dL_dvertices[3 * s.vi[c]], dt[3 * c]);
+            GMS_ATOMIC_ADD(&g.dL_dvertices[3 * s.vi[c] + 1], dt[3 * c + 1]);
+            GMS_ATOMIC_ADD(&g.dL_dvertices[3 * s.vi[c] + 2], dt[3 * c + 2]);
+        }
+    }
+}
+
+template <int ACT>
+GMS_HD void gms_expand_face_bwd_act(const gms_expand_args& a, const gms_expand_grads& g, int f, int fl) {
+    GmsFaceState s;
+    gms_expand_face_load(a, f, s);
+    gms_expand_face_frame(a, s);
+    float dt[9];
+#pragma unroll
+    for (int k = 0; k < 9; k++) dt[k] = 0.f;
+    float dq[4] = {0.f, 0.f, 0.f, 0.f};
+    float ds1 = 0.f, ds2 = 0.f;
+    for (int k = 0; k < a.K; k++) gms_expand_splat_bwd<ACT>(a, g, s, (size_t)fl * a.K + k, dt, dq, ds1, ds2);
+    gms_expand_face_bwd_tail(a, g, s, f, dt, dq, ds1, ds2);
+}
+
+// The relu weights' whole-face functions as the per-thread gs_mesh kernels have always compiled them (k_expand_fwd /
+// k_expand_bwd): the same arithmetic as gms_expand_face_*_act<GMS_ALPHA_RELU>, written as one loop, kept as it is so those
+// kernels' machine code does not change.
+GMS_HD void gms_expand_face_fwd_relu(const gms_expand_args& a, int f, int fl) {
     float t[9];
     if (a.triangles_in) {
 #pragma unroll
@@ -235,7 +428,7 @@ GMS_HD void gms_expand_face_fwd(const gms_expand_args& a, int f, int fl) {
     }
 }
 
-GMS_HD void gms_expand_face_bwd(const gms_expand_args& a, const gms_expand_grads& g, int f, int fl) {
+GMS_HD void gms_expand_face_bwd_relu(const gms_expand_args& a, const gms_expand_grads& g, int f, int fl) {
     float t[9];
     int64_t vi[3] = {0, 0, 0};
     if (a.triangles_in) {
@@ -329,6 +522,18 @@ GMS_HD void gms_expand_face_bwd(const gms_expand_args& a, const gms_expand_grads
             GMS_ATOMIC_ADD(&g.dL_dvertices[3 * vi[c] + 2], dt[3 * c + 2]);
         }
     }
+}
+
+// Whole face with the activation the arguments select (the host shim's entry points; the per-thread kernels call the
+// functions above directly).
+GMS_HD void gms_expand_face_fwd(const gms_expand_args& a, int f, int fl) {
+    if (a.alpha_activation == GMS_ALPHA_SOFTMAX) gms_expand_face_fwd_act<GMS_ALPHA_SOFTMAX>(a, f, fl);
+    else gms_expand_face_fwd_relu(a, f, fl);
+}
+
+GMS_HD void gms_expand_face_bwd(const gms_expand_args& a, const gms_expand_grads& g, int f, int fl) {
+    if (a.alpha_activation == GMS_ALPHA_SOFTMAX) gms_expand_face_bwd_act<GMS_ALPHA_SOFTMAX>(a, g, f, fl);
+    else gms_expand_face_bwd_relu(a, g, f, fl);
 }
 
 

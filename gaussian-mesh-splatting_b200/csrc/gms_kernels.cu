@@ -41,6 +41,8 @@ static int g_opt_sh_staged = 1;     // preprocess fwd/bwd: SH rows through a per
 static int g_opt_pre_bwd_minb = 4;  // k_preprocess_bwd min CTAs/SM (1: 2.67 ms, 3: 2.67 ms, 4: default)
 static int g_opt_expand_staged = 1; // expansion kernels, per-Gaussian streams staged through shared memory (coalesced): bit 0 forward
                                     // (0: 2.74 ms), bit 1 backward (3: 2.67 ms, off)
+static int g_opt_expand_wide = 1;  // expansion kernels, one warp per face (k_expand_wide_*): 0 never, 1 softmax weights with K >=
+                                    // GMS_EXP_WIDE_MIN_K (default; relu meshes keep the per-thread kernels), 2 always (A/B runs, tests)
 static int g_opt_sort = 0;         // depth sort (and the emit + sort path's tile sort): 0 cub::DeviceRadixSort, 1 hand-written radix sort
                                    //    with device-side N clamped to the capacity (gms_sort.cuh; bit-identical order through the
                                    //    synchronising entry points and the sync-free frame; 2.67-2.70 ms against 2.40-2.42 ms
@@ -812,11 +814,22 @@ static int exp_bwd_stage_width(const gms_expand_grads& g) {
            (g.dL_drotation_raw ? 4 : 0) + (g.dL_drotation_act ? 4 : 0) + (g.dL_dalpha_raw ? 3 : 0) + (g.dL_dscale_raw ? 1 : 0);
 }
 
-template <bool STAGED>
-__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_fwd(gms_expand_args a) {
+template <int ACT>
+__device__ __forceinline__ void expand_face_fwd(const gms_expand_args& a, int f, int fl) {
+    if constexpr (ACT == GMS_ALPHA_RELU) gms_expand_face_fwd_relu(a, f, fl);
+    else gms_expand_face_fwd_act<ACT>(a, f, fl);
+}
+template <int ACT>
+__device__ __forceinline__ void expand_face_bwd(const gms_expand_args& a, const gms_expand_grads& g, int f, int fl) {
+    if constexpr (ACT == GMS_ALPHA_RELU) gms_expand_face_bwd_relu(a, g, f, fl);
+    else gms_expand_face_bwd_act<ACT>(a, g, f, fl);
+}
+
+template <bool STAGED, int ACT>
+__device__ __forceinline__ void expand_fwd_block(const gms_expand_args& a) {
     const int f0 = blockIdx.x * GMS_EXP_BLOCK, f = f0 + threadIdx.x;
     if (!STAGED) {
-        if (f < a.F) gms_expand_face_fwd(a, f, f);
+        if (f < a.F) expand_face_fwd<ACT>(a, f, f);
         return;
     }
     extern __shared__ float4 exp_smem4[];
@@ -833,7 +846,7 @@ __global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_fwd(gms_expand_args a)
     l.rotation_raw = exp_stage_out(a.rotation_raw, 4, cap, sm);
     l.rotation_act = exp_stage_out(a.rotation_act, 4, cap, sm);
     __syncthreads();
-    if (f < a.F) gms_expand_face_fwd(l, f, threadIdx.x);
+    if (f < a.F) expand_face_fwd<ACT>(l, f, threadIdx.x);
     __syncthreads();
     exp_stage_flush(a.alpha, l.alpha, 3, g0, ng);
     exp_stage_flush(a.xyz, l.xyz, 3, g0, ng);
@@ -844,10 +857,15 @@ __global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_fwd(gms_expand_args a)
 }
 
 template <bool STAGED>
-__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_bwd(gms_expand_args a, gms_expand_grads g) {
+__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_fwd(gms_expand_args a) { expand_fwd_block<STAGED, GMS_ALPHA_RELU>(a); }
+template <bool STAGED>
+__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_softmax_fwd(gms_expand_args a) { expand_fwd_block<STAGED, GMS_ALPHA_SOFTMAX>(a); }
+
+template <bool STAGED, int ACT>
+__device__ __forceinline__ void expand_bwd_block(const gms_expand_args& a, const gms_expand_grads& g) {
     const int f0 = blockIdx.x * GMS_EXP_BLOCK, f = f0 + threadIdx.x;
     if (!STAGED) {
-        if (f < a.F) gms_expand_face_bwd(a, g, f, f);
+        if (f < a.F) expand_face_bwd<ACT>(a, g, f, f);
         return;
     }
     extern __shared__ float4 exp_smem4[];
@@ -866,10 +884,62 @@ __global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_bwd(gms_expand_args a,
     lg.dL_dalpha_raw = exp_stage_out(g.dL_dalpha_raw, 3, cap, sm);
     lg.dL_dscale_raw = exp_stage_out(g.dL_dscale_raw, 1, cap, sm);
     __syncthreads();
-    if (f < a.F) gms_expand_face_bwd(l, lg, f, threadIdx.x);     // per-face outputs (dL_dtriangles, vertex atomics) stay global
+    if (f < a.F) expand_face_bwd<ACT>(l, lg, f, threadIdx.x);     // per-face outputs (dL_dtriangles, vertex atomics) stay global
     __syncthreads();
     exp_stage_flush(g.dL_dalpha_raw, lg.dL_dalpha_raw, 3, g0, ng);
     exp_stage_flush(g.dL_dscale_raw, lg.dL_dscale_raw, 1, g0, ng);
+}
+
+template <bool STAGED>
+__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_bwd(gms_expand_args a, gms_expand_grads g) {
+    expand_bwd_block<STAGED, GMS_ALPHA_RELU>(a, g);
+}
+template <bool STAGED>
+__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_softmax_bwd(gms_expand_args a, gms_expand_grads g) {
+    expand_bwd_block<STAGED, GMS_ALPHA_SOFTMAX>(a, g);
+}
+
+// Splat-parallel expansion for many splats per face (gs_flame: K = 100 on ~10k faces).  One warp per face: every lane reads
+// the face and evaluates its frame and quaternion in lockstep (one instruction stream per face, as cheap as one lane
+// computing them and broadcasting the result, without the shuffles), then lane j handles splats j, j + 32, ...: consecutive
+// lanes touch consecutive rows, so every per-Gaussian stream is read and written coalesced without staging.  Each splat is
+// the per-thread kernel's gms_expand_splat_* call, so the forward is bit-identical to it.  The backward sums each lane's
+// dt / dq / ds1 / ds2 partials over its splats, reduces them across the warp (butterfly), and lane 0 finishes the face: one
+// set of vertex atomics per face, as in the per-thread kernel.  Only the order of the sum over K differs.
+constexpr int GMS_EXP_WIDE_BLOCK = 128;                     // 4 faces per block
+constexpr int GMS_EXP_WIDE_MIN_K = 16;                      // expand_wide = 1: softmax weights with K >= this (DESIGN.md 4.5)
+
+template <int ACT>
+__global__ void __launch_bounds__(GMS_EXP_WIDE_BLOCK) k_expand_wide_fwd(gms_expand_args a) {
+    const int f = blockIdx.x * (GMS_EXP_WIDE_BLOCK / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (f >= a.F) return;
+    GmsFaceState s;
+    gms_expand_face_load(a, f, s);
+    if (a.triangles && lane == 0) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) a.triangles[9 * (size_t)f + k] = s.t[k];
+    }
+    gms_expand_face_frame(a, s);
+    for (int k = lane; k < a.K; k += 32) gms_expand_splat_fwd<ACT>(a, s, (size_t)f * a.K + k);
+}
+
+template <int ACT>
+__global__ void __launch_bounds__(GMS_EXP_WIDE_BLOCK) k_expand_wide_bwd(gms_expand_args a, gms_expand_grads g) {
+    const int f = blockIdx.x * (GMS_EXP_WIDE_BLOCK / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (f >= a.F) return;                                   // whole warps: f is uniform across the warp
+    GmsFaceState s;
+    gms_expand_face_load(a, f, s);
+    gms_expand_face_frame(a, s);
+    float acc[15];                                          // dt[9], dq[4], ds1, ds2
+#pragma unroll
+    for (int i = 0; i < 15; i++) acc[i] = 0.f;
+    for (int k = lane; k < a.K; k += 32) gms_expand_splat_bwd<ACT>(a, g, s, (size_t)f * a.K + k, acc, acc + 9, acc[13], acc[14]);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+#pragma unroll
+        for (int i = 0; i < 15; i++) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
+    }
+    if (lane == 0) gms_expand_face_bwd_tail(a, g, s, f, acc, acc + 9, acc[13], acc[14]);
 }
 
 __global__ void __launch_bounds__(128) k_points_expand_fwd(gms_points_args a) {
@@ -1364,6 +1434,7 @@ int gms_set_option(const char* key, int value) {
     else if (!strcmp(key, "sort_impl")) p = &g_opt_sort;
     else if (!strcmp(key, "bin_impl")) p = &g_opt_bin;
     else if (!strcmp(key, "expand_staged")) p = &g_opt_expand_staged;
+    else if (!strcmp(key, "expand_wide")) p = &g_opt_expand_wide;
     else if (!strcmp(key, "sh_staged")) p = &g_opt_sh_staged;
     else if (!strcmp(key, "pre_bwd_minblocks")) p = &g_opt_pre_bwd_minb;
     if (!p) return -1;
@@ -1810,17 +1881,33 @@ int gms_debug_unpack(const gms_raster_saved* saved, int32_t P, const int32_t* ra
     return GMS_OK;
 }
 
+// Which expansion kernels a call runs: the warp-per-face ones (option "expand_wide") or the per-thread ones.
+static bool expand_wide(const gms_expand_args& a) {
+    return g_opt_expand_wide == 2 || (g_opt_expand_wide == 1 && a.alpha_activation == GMS_ALPHA_SOFTMAX && a.K >= GMS_EXP_WIDE_MIN_K);
+}
+
 int gms_expand_forward(const gms_expand_args* a, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (!a || a->F < 0 || a->K <= 0) return set_err(GMS_E_ARG, "bad expansion sizes%s%s");
     if (!a->triangles_in && (!a->vertices || !a->faces)) return set_err(GMS_E_ARG, "vertices/faces or triangles_in required%s%s");
     if (!a->alpha_raw || !a->scale_raw) return set_err(GMS_E_ARG, "_alpha and _scale required%s%s");
+    if (a->alpha_activation != GMS_ALPHA_RELU && a->alpha_activation != GMS_ALPHA_SOFTMAX)
+        return set_err(GMS_E_ARG, "alpha_activation must be 0 (relu) or 1 (softmax)%s%s");
     if (a->F == 0) return GMS_OK;
     span_begin(K_EXP_FWD, st);
-    {
+    const bool softmax = a->alpha_activation == GMS_ALPHA_SOFTMAX;
+    if (expand_wide(*a)) {
+        const int grid = (a->F + GMS_EXP_WIDE_BLOCK / 32 - 1) / (GMS_EXP_WIDE_BLOCK / 32);
+        if (softmax) k_expand_wide_fwd<GMS_ALPHA_SOFTMAX><<<grid, GMS_EXP_WIDE_BLOCK, 0, st>>>(*a);
+        else k_expand_wide_fwd<GMS_ALPHA_RELU><<<grid, GMS_EXP_WIDE_BLOCK, 0, st>>>(*a);
+    } else {
         const int grid = (a->F + GMS_EXP_BLOCK - 1) / GMS_EXP_BLOCK;
         const size_t smem = (size_t)GMS_EXP_BLOCK * a->K * exp_fwd_stage_width(*a) * sizeof(float);
-        if ((g_opt_expand_staged & 1) && smem <= 48 * 1024) k_expand_fwd<true><<<grid, GMS_EXP_BLOCK, smem, st>>>(*a);
+        const bool staged = (g_opt_expand_staged & 1) && smem <= 48 * 1024;
+        if (softmax) {
+            if (staged) k_expand_softmax_fwd<true><<<grid, GMS_EXP_BLOCK, smem, st>>>(*a);
+            else k_expand_softmax_fwd<false><<<grid, GMS_EXP_BLOCK, 0, st>>>(*a);
+        } else if (staged) k_expand_fwd<true><<<grid, GMS_EXP_BLOCK, smem, st>>>(*a);
         else k_expand_fwd<false><<<grid, GMS_EXP_BLOCK, 0, st>>>(*a);
     }
     GMS_AFTER_LAUNCH("expand_fwd", 0, st);
@@ -1858,12 +1945,23 @@ int gms_expand_backward(const gms_expand_args* a, const gms_expand_grads* g, voi
     if (!a || !g || a->F < 0 || a->K <= 0) return set_err(GMS_E_ARG, "bad expansion sizes%s%s");
     if (!a->triangles_in && (!a->vertices || !a->faces)) return set_err(GMS_E_ARG, "vertices/faces or triangles_in required%s%s");
     if (!a->alpha_raw || !a->scale_raw) return set_err(GMS_E_ARG, "_alpha and _scale required%s%s");
+    if (a->alpha_activation != GMS_ALPHA_RELU && a->alpha_activation != GMS_ALPHA_SOFTMAX)
+        return set_err(GMS_E_ARG, "alpha_activation must be 0 (relu) or 1 (softmax)%s%s");
     if (a->F == 0) return GMS_OK;
     span_begin(K_EXP_BWD, st);
-    {
+    const bool softmax = a->alpha_activation == GMS_ALPHA_SOFTMAX;
+    if (expand_wide(*a)) {
+        const int grid = (a->F + GMS_EXP_WIDE_BLOCK / 32 - 1) / (GMS_EXP_WIDE_BLOCK / 32);
+        if (softmax) k_expand_wide_bwd<GMS_ALPHA_SOFTMAX><<<grid, GMS_EXP_WIDE_BLOCK, 0, st>>>(*a, *g);
+        else k_expand_wide_bwd<GMS_ALPHA_RELU><<<grid, GMS_EXP_WIDE_BLOCK, 0, st>>>(*a, *g);
+    } else {
         const int grid = (a->F + GMS_EXP_BLOCK - 1) / GMS_EXP_BLOCK;
         const size_t smem = (size_t)GMS_EXP_BLOCK * a->K * exp_bwd_stage_width(*g) * sizeof(float);
-        if ((g_opt_expand_staged & 2) && smem <= 48 * 1024) k_expand_bwd<true><<<grid, GMS_EXP_BLOCK, smem, st>>>(*a, *g);
+        const bool staged = (g_opt_expand_staged & 2) && smem <= 48 * 1024;
+        if (softmax) {
+            if (staged) k_expand_softmax_bwd<true><<<grid, GMS_EXP_BLOCK, smem, st>>>(*a, *g);
+            else k_expand_softmax_bwd<false><<<grid, GMS_EXP_BLOCK, 0, st>>>(*a, *g);
+        } else if (staged) k_expand_bwd<true><<<grid, GMS_EXP_BLOCK, smem, st>>>(*a, *g);
         else k_expand_bwd<false><<<grid, GMS_EXP_BLOCK, 0, st>>>(*a, *g);
     }
     GMS_AFTER_LAUNCH("expand_bwd", 0, st);
@@ -1882,11 +1980,14 @@ struct FrameModel {
     const float* vertices; const int64_t* faces; const float* alpha_raw; const float* scale_raw; const float* features;
     const float* opacity_raw; float eps;
     const gms_mesh_segment* segments; int32_t n_segments;
+    int32_t alpha_activation;
 };
 
 // The Gaussian count of a frame: F*K for one mesh, sum F_i*K_i for a segmented model (gms_mesh_segment), whose sizes are
 // validated here, before the frame issues any launch.
 static int frame_gaussian_count(const char* fn, const FrameModel& m, int* P) {
+    if (m.alpha_activation != GMS_ALPHA_RELU && m.alpha_activation != GMS_ALPHA_SOFTMAX)
+        return set_err(GMS_E_ARG, "%s: alpha_activation must be 0 (relu) or 1 (softmax)%s", fn);
     if (m.n_segments == 0) {
         *P = m.F * m.K;
         return GMS_OK;
@@ -1920,6 +2021,7 @@ static int mesh_expand_forward(const FrameModel& m, float* xyz, float* scales, f
         e.V = m.V; e.F = seg[i].F; e.K = seg[i].K; e.vertices = m.vertices; e.faces = m.faces + 3 * f0;
         e.alpha_raw = m.alpha_raw + 3 * g0; e.scale_raw = m.scale_raw + g0; e.eps = m.eps;
         e.xyz = xyz + 3 * g0; e.scaling_act = scales + 3 * g0; e.rotation_act = rots + 4 * g0;
+        e.alpha_activation = m.alpha_activation;
         int rc;
         if ((rc = gms_expand_forward(&e, cuda_stream))) return rc;
         f0 += (size_t)seg[i].F;
@@ -1981,7 +2083,7 @@ int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_u
     if (!a->vertices || !a->faces || !a->alpha_raw || !a->scale_raw || !a->features || !a->opacity_raw)
         return set_err(GMS_E_ARG, "gms_render_frame: model tensors required%s%s");
     const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps,
-                          a->segments, a->n_segments};
+                          a->segments, a->n_segments, a->alpha_activation};
     int P, rc;
     if ((rc = frame_gaussian_count("gms_render_frame", m, &P))) return rc;
     const int W = a->settings.image_width, H = a->settings.image_height;
@@ -2120,7 +2222,7 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     if (a->sh_adam && (!a->sh_adam->m || !a->sh_adam->v || a->sh_adam->step < 1 || a->settings.sh_degree < 0 || a->settings.sh_degree > 3))
         return set_err(GMS_E_ARG, "gms_train_frame: bad sh_adam%s%s");
     const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps,
-                          a->segments, a->n_segments};
+                          a->segments, a->n_segments, a->alpha_activation};
     int P, rc;
     if ((rc = frame_gaussian_count("gms_train_frame", m, &P))) return rc;
     const int W = a->settings.image_width, H = a->settings.image_height;
@@ -2251,6 +2353,68 @@ int gms_free_render_frame(const gms_free_render_args* a, gms_alloc_fn alloc, voi
     gms_raster_inputs in;
     gms_raster_saved saved;
     const FrameGaussians g = {P, a->M, a->xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
+    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
+                                   &saved))) return rc;
+    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
+    return GMS_OK;
+}
+
+// ------------------------------------------------------------------------------------------ gs_flame checkpoint render
+
+// xyz from the checkpoint's activated weights and the driving pose (the product of the expansion forward, same operation
+// order), scales and rotations from the checkpoint's rows as k_free_act_fwd activates them.
+__global__ void __launch_bounds__(GMS_FREE_BLOCK) k_flame_act(int P, int K, const float* __restrict__ alpha, const int64_t* __restrict__ faces,
+                                                              const float* __restrict__ vertices, const float* __restrict__ scaling_log,
+                                                              const float* __restrict__ rotation_raw, float* __restrict__ xyz,
+                                                              float* __restrict__ scales, float* __restrict__ rots) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P) return;
+    const size_t f = (size_t)(i / K);
+    float t[9];
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const int64_t vi = faces[3 * f + c];
+        t[3 * c] = vertices[3 * vi]; t[3 * c + 1] = vertices[3 * vi + 1]; t[3 * c + 2] = vertices[3 * vi + 2];
+    }
+    const float al0 = alpha[3 * (size_t)i], al1 = alpha[3 * (size_t)i + 1], al2 = alpha[3 * (size_t)i + 2];
+#pragma unroll
+    for (int c = 0; c < 3; c++) xyz[3 * (size_t)i + c] = al0 * t[c] + al1 * t[3 + c] + al2 * t[6 + c];
+    const float* s = scaling_log + 3 * (size_t)i;
+    float* so = scales + 3 * (size_t)i;
+    so[0] = expf(s[0]); so[1] = expf(s[1]); so[2] = expf(s[2]);
+    const float4 r = reinterpret_cast<const float4*>(rotation_raw)[i];
+    const float q[4] = {r.x, r.y, r.z, r.w};
+    const float n = gms_quat_norm(q);
+    reinterpret_cast<float4*>(rots)[i] = make_float4(q[0] / n, q[1] / n, q[2] / n, q[3] / n);
+}
+
+size_t gms_flame_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { return gms_render_workspace_bytes(P, W, H); }
+
+int gms_flame_render_frame(const gms_flame_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii)
+        return set_err(GMS_E_ARG, "gms_flame_render_frame: null argument%s%s");
+    if (!a->vertices || !a->faces || !a->alpha || !a->scaling_log || !a->rotation_raw || !a->features || !a->opacity_raw)
+        return set_err(GMS_E_ARG, "gms_flame_render_frame: model tensors required%s%s");
+    if (a->F < 0 || a->K < 1 || a->V < 1 || a->M < 1 || a->M > 16 || (int64_t)a->F * a->K > INT32_MAX)
+        return set_err(GMS_E_ARG, "gms_flame_render_frame: need F >= 0, K >= 1, V >= 1, 1 <= M <= 16 and F*K < 2^31%s%s");
+    if (!aligned16(a->rotation_raw)) return set_err(GMS_E_ARG, "gms_flame_render_frame: rotation_raw must be 16-byte aligned%s%s");
+    const int P = a->F * a->K, W = a->settings.image_width, H = a->settings.image_height;
+    if (a->workspace_bytes < gms_flame_render_workspace_bytes(P, W, H))
+        return set_err(GMS_E_ARG, "gms_flame_render_frame: workspace too small%s%s");
+    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
+    if (P > 0) {
+        span_begin(K_EXP_FWD, st);
+        k_flame_act<<<(P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, st>>>(P, a->K, a->alpha, a->faces, a->vertices,
+                                                                                       a->scaling_log, a->rotation_raw, RL.xyz, RL.scales, RL.rots);
+        GMS_AFTER_LAUNCH("flame_act", 0, st);
+        span_end(st);
+    }
+    gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
+    gms_raster_inputs in;
+    gms_raster_saved saved;
+    const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
+    int rc;
     if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
                                    &saved))) return rc;
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;

@@ -12,6 +12,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgms_b200.so")
 
+ALPHA_RELU, ALPHA_SOFTMAX = 0, 1   # gms_*_args.alpha_activation: relu + 1e-8, normalised (gs_mesh); softmax (gs_flame)
 FORWARD_ONLY = 1        # gms_raster_outputs.flags: no backward will follow (skip the survivor lists)
 GMS_OK, GMS_E_ARG, GMS_E_CUDA, GMS_E_ALLOC, GMS_E_UNSUPPORTED = 0, -1, -2, -3, -4
 BUF_GEOM, BUF_BINNING, BUF_IMAGE = 0, 1, 2
@@ -65,7 +66,8 @@ class ExpandArgs(C.Structure):
                 ("faces", C.c_void_p), ("triangles_in", C.c_void_p), ("alpha_raw", C.c_void_p),
                 ("scale_raw", C.c_void_p), ("eps", C.c_float), ("alpha", C.c_void_p),
                 ("triangles", C.c_void_p), ("xyz", C.c_void_p), ("scaling_log", C.c_void_p),
-                ("rotation_raw", C.c_void_p), ("scaling_act", C.c_void_p), ("rotation_act", C.c_void_p)]
+                ("rotation_raw", C.c_void_p), ("scaling_act", C.c_void_p), ("rotation_act", C.c_void_p),
+                ("alpha_activation", C.c_int32)]
 
 
 class ExpandGrads(C.Structure):
@@ -129,7 +131,7 @@ class FrameArgs(C.Structure):
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)),
                 ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p), ("d_color_sh", C.c_void_p),
                 ("event_sh_ready", C.c_void_p), ("event_loss_ready", C.c_void_p), ("sh_adam", C.POINTER(ShAdam)),
-                ("segments", C.POINTER(MeshSegment)), ("n_segments", C.c_int32)]
+                ("segments", C.POINTER(MeshSegment)), ("n_segments", C.c_int32), ("alpha_activation", C.c_int32)]
 
 
 class FrameView(C.Structure):
@@ -145,7 +147,16 @@ class RenderArgs(C.Structure):
                 ("image", C.c_void_p), ("invdepth", C.c_void_p), ("radii", C.c_void_p),
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)),
                 ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p),
-                ("segments", C.POINTER(MeshSegment)), ("n_segments", C.c_int32)]
+                ("segments", C.POINTER(MeshSegment)), ("n_segments", C.c_int32), ("alpha_activation", C.c_int32)]
+
+
+class FlameRenderArgs(C.Structure):
+    """struct gms_flame_render_args"""
+    _fields_ = [("V", C.c_int32), ("F", C.c_int32), ("K", C.c_int32), ("M", C.c_int32), ("vertices", C.c_void_p), ("faces", C.c_void_p),
+                ("alpha", C.c_void_p), ("scaling_log", C.c_void_p), ("rotation_raw", C.c_void_p), ("features", C.c_void_p),
+                ("opacity_raw", C.c_void_p), ("settings", RasterSettings), ("image", C.c_void_p), ("invdepth", C.c_void_p),
+                ("radii", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
+                ("num_rendered", C.POINTER(C.c_int64)), ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p)]
 
 
 class PointsRenderArgs(C.Structure):
@@ -258,7 +269,8 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_points_render_workspace_bytes", "gms_points_render_frame", "gms_pseudomesh_bind_scratch_bytes",
                "gms_pseudomesh_bind", "gms_pseudomesh_repose", "gms_bound_points_render_workspace_bytes",
                "gms_bound_points_render_frame", "gms_free_train_frame", "gms_free_render_frame", "gms_densify_scratch_bytes",
-               "gms_densify_plan", "gms_densify_apply", "gms_knn_scratch_bytes", "gms_knn_dist2"]
+               "gms_densify_plan", "gms_densify_apply", "gms_knn_scratch_bytes", "gms_knn_dist2",
+               "gms_flame_render_workspace_bytes", "gms_flame_render_frame"]
 
 _lib = None
 
@@ -312,6 +324,9 @@ def lib():
     L.gms_render_workspace_bytes.restype = C.c_size_t
     L.gms_render_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.gms_render_frame.argtypes = [C.POINTER(RenderArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
+    L.gms_flame_render_workspace_bytes.restype = C.c_size_t
+    L.gms_flame_render_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    L.gms_flame_render_frame.argtypes = [C.POINTER(FlameRenderArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
     L.gms_points_render_workspace_bytes.restype = C.c_size_t
     L.gms_points_render_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.gms_points_render_frame.argtypes = [C.POINTER(PointsRenderArgs), ALLOC_FN, C.c_void_p, C.c_void_p]

@@ -36,8 +36,9 @@ def _p(t):
     return None if t is None else t.data_ptr()
 
 
-def _args(V, F, K, vertices, faces, triangles_in, alpha_raw, scale_raw, eps, **outs):
+def _args(V, F, K, vertices, faces, triangles_in, alpha_raw, scale_raw, eps, alpha_activation=_lib.ALPHA_RELU, **outs):
     a = _lib.ExpandArgs()
+    a.alpha_activation = int(alpha_activation)
     a.V, a.F, a.K = int(V), int(F), int(K)
     a.vertices, a.faces, a.triangles_in = _p(vertices), _p(faces), _p(triangles_in)
     a.alpha_raw, a.scale_raw, a.eps = _p(alpha_raw), _p(scale_raw), float(eps)
@@ -50,7 +51,7 @@ class _Expand(torch.autograd.Function):
     """vertices [V,3], faces [F,3] int64, _alpha [F,K,3], _scale [P,1] -> xyz, scaling, rotation (+alpha, triangles)."""
 
     @staticmethod
-    def forward(ctx, vertices, faces, alpha_raw, scale_raw, eps, activated):
+    def forward(ctx, vertices, faces, alpha_raw, scale_raw, eps, activated, alpha_activation):
         if not vertices.is_cuda:
             raise RuntimeError("gms_b200.expand: CUDA tensors required (no CPU path in the product)")
         L = _lib.lib()
@@ -63,11 +64,11 @@ class _Expand(torch.autograd.Function):
         alpha, tri, xyz, sc, rot = e(F, K, 3), e(F, 3, 3), e(P, 3), e(P, 3), e(P, 4)
         outs = dict(alpha=alpha, triangles=tri, xyz=xyz)
         outs.update(dict(scaling_act=sc, rotation_act=rot) if activated else dict(scaling_log=sc, rotation_raw=rot))
-        args = _args(v.shape[0], F, K, v, f, None, a, s, eps, **outs)
+        args = _args(v.shape[0], F, K, v, f, None, a, s, eps, alpha_activation, **outs)
         with torch.cuda.device(dev):
             _lib.check(L.gms_expand_forward(C.byref(args), _stream(dev)), "gms_expand_forward")
         ctx.save_for_backward(v, f, a, s)
-        ctx.eps, ctx.activated = float(eps), bool(activated)
+        ctx.eps, ctx.activated, ctx.alpha_activation = float(eps), bool(activated), int(alpha_activation)
         ctx.mark_non_differentiable(alpha, tri)
         return xyz, sc, rot, alpha, tri
 
@@ -90,16 +91,17 @@ class _Expand(torch.autograd.Function):
         da = torch.empty_like(a)
         ds = torch.empty_like(s)
         g.dL_dvertices, g.dL_dalpha_raw, g.dL_dscale_raw = dv.data_ptr(), da.data_ptr(), ds.data_ptr()
-        args = _args(v.shape[0], F, K, v, f, None, a, s, ctx.eps)
+        args = _args(v.shape[0], F, K, v, f, None, a, s, ctx.eps, ctx.alpha_activation)
         with torch.cuda.device(dev):
             _lib.check(L.gms_expand_backward(C.byref(args), C.byref(g), _stream(dev)), "gms_expand_backward")
-        return dv, None, da, ds, None, None
+        return dv, None, da, ds, None, None, None
 
 
-def expand(vertices, faces, _alpha, _scale, eps: float = EPS_S0, activated: bool = True):
+def expand(vertices, faces, _alpha, _scale, eps: float = EPS_S0, activated: bool = True, alpha_activation: int = _lib.ALPHA_RELU):
     """One-launch expansion.  Returns (xyz [P,3], scaling [P,3], rotation [P,4], alpha [F,K,3], triangles [F,3,3]);
-    scaling/rotation are ACTIVATED (exp / normalised) when `activated`, else the raw `_scaling` / `_rotation`."""
-    return _Expand.apply(vertices, faces, _alpha, _scale, eps, activated)
+    scaling/rotation are ACTIVATED (exp / normalised) when `activated`, else the raw `_scaling` / `_rotation`.
+    alpha_activation: _lib.ALPHA_RELU (gs_mesh: relu + 1e-8, normalised) or _lib.ALPHA_SOFTMAX (gs_flame: softmax)."""
+    return _Expand.apply(vertices, faces, _alpha, _scale, eps, activated, alpha_activation)
 
 
 class _UpdateAlpha(torch.autograd.Function):

@@ -246,3 +246,51 @@ def save_point_cloud(path: str, xyz, rgb) -> None:
             f.write(f"property {'float' if t == 'f4' else 'uchar'} {n}\n".encode())
         f.write(b"end_header\n")
         el.tofile(f)
+
+
+# ---- gs_flame checkpoints: GaussianFlameModel.save_ply / load_ply (games/flame_splatting/scene/gaussian_flame_model.py:230-265)
+
+FLAME_KEYS = ("_flame_shape", "_flame_exp", "_flame_pose", "_flame_neck_pose", "_flame_trans", "_vertices_enlargement", "faces",
+              "alpha", "point_cloud")
+
+
+def load_flame_model(ply_path: str) -> Dict[str, object]:
+    """point_cloud.ply + flame_params.pt of a trained gs_flame run -> dict with load_gaussian_ply's tensors (_xyz,
+    _features_dc, _features_rest, _opacity, _scaling, _rotation) and flame_params.pt's entries (FLAME_KEYS) as CPU tensors;
+    `alpha` is the ACTIVATED weights [F,K,3] the reference stores, and there is no `_scales` (the reference does not save it).
+    `point_cloud` is read through the unpickler that keeps classes of the reference's code as opaque tuples, so the reference
+    need not be importable."""
+    out = dict(load_gaussian_ply(ply_path))
+    params = torch.load(ply_path.replace("point_cloud.ply", "flame_params.pt"), map_location="cpu", weights_only=False,
+                        pickle_module=_pickle_module)
+    d = lambda x: (x.detach() if isinstance(x, torch.Tensor) else torch.as_tensor(x)).cpu()
+    for k in FLAME_KEYS[:-1]:
+        out[k] = d(params[k]).long() if k == "faces" else d(params[k]).float()
+    out["point_cloud"] = params.get("point_cloud")
+    return out
+
+
+def save_flame_model(ply_path: str, model, point_cloud=None) -> None:
+    """Counterpart of GaussianFlameModel.save_ply for a gms_b200 FlameGaussianModel at its current parameters: point_cloud.ply
+    (the expansion's _xyz, raw _scaling / _rotation, SH, opacity) and flame_params.pt with exactly the reference's keys --
+    the six FLAME tensors as nn.Parameters, `faces`, the activated `alpha` and `point_cloud` (pickled as given) -- on the
+    model's device, as the reference's writer leaves them."""
+    from . import _lib, expansion
+    verts = model.refresh_vertices()
+    xyz, sc, rot, alpha, _ = expansion.expand(verts, model.faces, model._alpha.detach(), model._scales.detach(), model.eps_s0,
+                                              activated=False, alpha_activation=_lib.ALPHA_SOFTMAX)
+    f = model._features.detach()
+    write_flame_checkpoint(ply_path, xyz, f[:, :1], f[:, 1:], model._opacity, sc, rot, {k: getattr(model, k) for k in FLAME_KEYS[:6]},
+                           model.faces, alpha, point_cloud, model.eps_s0)
+
+
+def write_flame_checkpoint(ply_path: str, xyz, features_dc, features_rest, opacity, scaling, rotation, flame: dict, faces, alpha,
+                           point_cloud=None, eps_s0: float = 1e-8) -> None:
+    """The two files of a gs_flame checkpoint from expanded tensors: point_cloud.ply (save_gaussian_ply) and flame_params.pt
+    with the reference's keys -- the six FLAME tensors (`flame`) as nn.Parameters, `faces`, the activated `alpha`,
+    `point_cloud` -- each where the caller holds it."""
+    save_gaussian_ply(ply_path, xyz, features_dc, features_rest, opacity, scaling, rotation, eps_s0)
+    par = lambda t: torch.nn.Parameter(torch.as_tensor(t).detach().clone().contiguous(), requires_grad=True)
+    save = {k: par(flame[k]) for k in FLAME_KEYS[:6]}
+    save.update(faces=torch.as_tensor(faces).detach().clone(), alpha=torch.as_tensor(alpha).detach().clone(), point_cloud=point_cloud)
+    torch.save(save, ply_path.replace("point_cloud.ply", "flame_params.pt"))

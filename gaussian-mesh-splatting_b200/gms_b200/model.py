@@ -8,6 +8,7 @@ patched in place with expansion.patch_mesh_model().
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 from torch import nn
 
@@ -17,6 +18,7 @@ from .scenes import SH_C0, MeshGaussianParams
 
 class MeshGaussianModel:
     segments = None     # MultiMeshGaussianModel with a K per mesh: [(F_i, K_i), ...]; None: one K for every face
+    alpha_activation = _lib.ALPHA_RELU      # barycentric weights from _alpha: relu + 1e-8, normalised (gaussian_mesh_model.py:166-167)
 
     def __init__(self, sh_degree: int = 3):
         self.active_sh_degree = 0
@@ -437,3 +439,173 @@ class FreeGaussianModel:
 
     def parameters(self):
         return [getattr(self, n) for n in self.NAMES]
+
+
+# ---------------------------------------------------------------------------------------------- gs_flame (FLAME-driven mesh)
+
+FLAME_ENLARGEMENT = 8.35        # FlameConfig.vertices_enlargement (games/flame_splatting/FLAME/config.py:28)
+
+
+def flame_transform_vertices(vertices: torch.Tensor, enlargement) -> torch.Tensor:
+    """transform_vertices_function (games/flame_splatting/scene/dataset_readers.py:40-45) out of place: the driver's
+    [1,V,3] (or [V,3]) vertices as (x, -z, y) times `enlargement` ([V,3] or a scalar), element for element the same
+    rounding as the reference's in-place version (a negation is exact)."""
+    v = vertices.reshape(-1, 3)
+    sign = torch.tensor([1.0, -1.0, 1.0], dtype=v.dtype, device=v.device)
+    return v[:, [0, 2, 1]] * sign * enlargement
+
+
+class FlameGaussianModel:
+    """gs_flame: K Gaussians on every face of a FLAME head mesh (GaussianFlameModel,
+    games/flame_splatting/scene/gaussian_flame_model.py).  The Gaussian parameters are `_alpha` [F,K,3] (barycentric logits,
+    weighted through a softmax), `_scales` [P,1], the packed SH `_features` [P,M,3] and `_opacity` [P,1]; the mesh is the
+    output of a caller-supplied FLAME `driver` with the reference's FLAME.forward signature
+        driver(shape_params, expression_params, pose_params, neck_pose, transl) -> (vertices [1,V,3], landmarks)
+    at the model's six FLAME tensors, through flame_transform_vertices.  The library never looks inside the driver: it runs
+    in ATen with autograd, and the frame's vertex gradient is pushed back through it (FlameTrainer).
+
+    `vertices` [V,3] is the pose the native frames and NativeRenderer read; refresh_vertices() sets it from the current
+    parameters."""
+    alpha_activation = _lib.ALPHA_SOFTMAX
+    segments = None
+    FLAME_NAMES = ("_flame_shape", "_flame_exp", "_flame_pose", "_flame_neck_pose", "_flame_trans", "_vertices_enlargement")
+
+    def __init__(self, driver, faces: torch.Tensor, _alpha: torch.Tensor, _scales: torch.Tensor, features: torch.Tensor,
+                 opacity: torch.Tensor, flame: dict, active_sh_degree: int = 0, eps_s0: float = expansion.EPS_S0):
+        F, K = _alpha.shape[:2]
+        P = F * K
+        if _alpha.dim() != 3 or _alpha.shape[2] != 3 or tuple(_scales.shape) != (P, 1) or features.dim() != 3 or \
+                tuple(features.shape[::2]) != (P, 3) or tuple(opacity.shape) != (P, 1) or tuple(faces.shape) != (F, 3):
+            raise ValueError("FlameGaussianModel: expected faces [F,3], _alpha [F,K,3], _scales / _opacity [F*K,1], features [F*K,M,3]")
+        dev = _alpha.device
+        mk = lambda t: nn.Parameter(t.detach().to(dev).float().contiguous().requires_grad_(True))
+        self.driver = driver
+        self.faces = faces.detach().to(dev).long().contiguous()
+        self._alpha, self._scales, self._features, self._opacity = mk(_alpha), mk(_scales), mk(features), mk(opacity)
+        for n in self.FLAME_NAMES:
+            setattr(self, n, mk(flame[n]))
+        self.max_sh_degree = int(round(features.shape[1] ** 0.5)) - 1
+        self.active_sh_degree = min(int(active_sh_degree), self.max_sh_degree)
+        self.eps_s0 = float(eps_s0)
+        V = self._vertices_enlargement.shape[0]
+        self.vertices = torch.zeros(V, 3, dtype=torch.float32, device=dev)
+        self.vertices.grad = torch.zeros_like(self.vertices)     # the frames' dL/dvertices (accumulated with atomics)
+        self.refresh_vertices()
+
+    @classmethod
+    def create(cls, driver, faces: torch.Tensor, K: int = 100, sh_degree: int = 3, seed: int = 0, device="cuda",
+               n_shape: int = 100, n_exp: int = 50) -> "FlameGaussianModel":
+        """A new model as readNerfSyntheticFlameInfo + create_from_pcd build it (games/flame_splatting/scene/
+        dataset_readers.py:48-120, gaussian_flame_model.py:58-105): FLAME parameters zero, enlargement 8.35 per vertex
+        coordinate, `_alpha` ~ U[0,1) [F,K,3], colours np.random.random / 255 through SH2RGB / RGB2SH, `_scales` 1 and
+        opacity inverse_sigmoid(0.1).  The draws come from torch / numpy generators seeded with `seed`."""
+        dev = torch.device(device)
+        zeros = lambda n: torch.zeros(1, n, dtype=torch.float32, device=dev)
+        flame = dict(_flame_shape=zeros(n_shape), _flame_exp=zeros(n_exp), _flame_pose=zeros(6), _flame_neck_pose=zeros(3),
+                     _flame_trans=zeros(3))
+        with torch.no_grad():
+            v0, _ = driver(shape_params=flame["_flame_shape"], expression_params=flame["_flame_exp"], pose_params=flame["_flame_pose"],
+                           neck_pose=flame["_flame_neck_pose"], transl=flame["_flame_trans"])
+        V = v0.reshape(-1, 3).shape[0]
+        flame["_vertices_enlargement"] = FLAME_ENLARGEMENT * torch.ones(V, 3, dtype=torch.float32, device=dev)
+        F = faces.shape[0]
+        P = F * K
+        g = torch.Generator().manual_seed(int(seed))
+        alpha = torch.rand(F, K, 3, generator=g)
+        shs = np.random.RandomState(seed).random_sample((P, 3)) / 255.0
+        colors = shs * SH_C0 + 0.5                                        # SH2RGB
+        fused = (torch.tensor(colors).float() - 0.5) / SH_C0              # RGB2SH
+        M = (sh_degree + 1) ** 2
+        features = torch.zeros(P, M, 3)
+        features[:, 0, :] = fused
+        opacity = torch.full((P, 1), 0.1)
+        opacity = torch.log(opacity / (1 - opacity))                      # inverse_sigmoid
+        return cls(driver, faces.to(dev), alpha.to(dev), torch.ones(P, 1, device=dev), features.to(dev), opacity.to(dev), flame)
+
+    # -- the mesh
+    def driver_vertices(self) -> torch.Tensor:
+        """update_alpha's mesh (gaussian_flame_model.py:196-205): the driver at the FLAME parameters, transformed; [V,3] with
+        autograd to the six FLAME tensors."""
+        v, _ = self.driver(shape_params=self._flame_shape, expression_params=self._flame_exp, pose_params=self._flame_pose,
+                           neck_pose=self._flame_neck_pose, transl=self._flame_trans)
+        return flame_transform_vertices(v, self._vertices_enlargement)
+
+    def refresh_vertices(self) -> torch.Tensor:
+        with torch.no_grad():
+            self.vertices.copy_(self.driver_vertices())
+        return self.vertices
+
+    # -- what the native frames read (MeshGaussianModel's surface)
+    @property
+    def _scale(self):
+        return self._scales
+
+    @property
+    def P(self) -> int:
+        return self._scales.shape[0]
+
+    def frame_sizes(self):
+        return self._alpha.shape[0], self._alpha.shape[1], None
+
+    @property
+    def alpha(self) -> torch.Tensor:
+        """The activated barycentric weights softmax(_alpha) [F,K,3] (update_alpha_func, gaussian_flame_model.py:195)."""
+        return expansion.expand(self.vertices, self.faces, self._alpha.detach(), self._scales.detach(), self.eps_s0,
+                                alpha_activation=_lib.ALPHA_SOFTMAX)[3]
+
+    @property
+    def get_features(self):
+        return self._features
+
+    @property
+    def get_opacity(self):
+        return torch.sigmoid(self._opacity)
+
+    def oneupSHdegree(self):
+        if self.active_sh_degree < self.max_sh_degree:
+            self.active_sh_degree += 1
+
+    def parameters(self):
+        return [getattr(self, n) for n in self.FLAME_NAMES] + [self._alpha, self._features, self._opacity, self._scales]
+
+
+class FlameCheckpoint:
+    """A trained gs_flame checkpoint as scripts/render_flame.py renders it (io_ply.load_flame_model): the activated weights
+    `alpha` [F,K,3], `faces`, the raw `_scaling` [P,3] / `_rotation` [P,4] rows, packed `_features` [P,M,3], `_opacity`
+    and the six FLAME tensors.  `vertices` [V,3] is the pose FlameRenderer draws when render() is given none (None until
+    set, e.g. to flame_transform_vertices(driver(...), ckpt._vertices_enlargement))."""
+
+    def __init__(self, ckpt: dict, device="cuda", active_sh_degree: int = 3):
+        d = lambda t: torch.as_tensor(t).detach().to(device).float().contiguous()
+        self.faces = torch.as_tensor(ckpt["faces"]).to(device).long().contiguous()
+        self.alpha, self._scaling, self._rotation, self._opacity = (d(ckpt[k]) for k in ("alpha", "_scaling", "_rotation", "_opacity"))
+        self._features = torch.cat((d(ckpt["_features_dc"]), d(ckpt["_features_rest"])), dim=1).contiguous()
+        for n in FlameGaussianModel.FLAME_NAMES:
+            setattr(self, n, d(ckpt[n]))
+        self.max_sh_degree = int(round(self._features.shape[1] ** 0.5)) - 1
+        self.active_sh_degree = min(int(active_sh_degree), self.max_sh_degree)
+        self.vertices = None
+        F, K = self.alpha.shape[:2]
+        P = F * K
+        if tuple(self._scaling.shape) != (P, 3) or tuple(self._rotation.shape) != (P, 4) or self._features.shape[0] != P or \
+                tuple(self._opacity.shape) != (P, 1):
+            raise ValueError(f"FlameCheckpoint: alpha [{F},{K},3] needs {P} Gaussian rows")
+
+    @classmethod
+    def load(cls, ply_path: str, device="cuda", active_sh_degree: int = 3) -> "FlameCheckpoint":
+        from . import io_ply
+        return cls(io_ply.load_flame_model(ply_path), device, active_sh_degree)
+
+    @property
+    def P(self) -> int:
+        return self._opacity.shape[0]
+
+    def driver_vertices(self, driver, **overrides) -> torch.Tensor:
+        """The pose render_flame.py draws (:23-33): the driver at the checkpoint's FLAME parameters, any of them replaced by
+        `overrides` (shape_params, expression_params, pose_params, neck_pose, transl -- e.g. the --animated expressions)."""
+        kw = dict(shape_params=self._flame_shape, expression_params=self._flame_exp, pose_params=self._flame_pose,
+                  neck_pose=self._flame_neck_pose, transl=self._flame_trans)
+        kw.update(overrides)
+        with torch.no_grad():
+            v, _ = driver(**kw)
+            return flame_transform_vertices(v, self._vertices_enlargement).contiguous()

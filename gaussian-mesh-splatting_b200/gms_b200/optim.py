@@ -34,7 +34,6 @@ class FlatAdam:
         self.sh_factored = bool(sh_factored)
         if self.sh_factored and not ("period" in self.groups[-1] and self.groups[-1]["param"].dim() == 3):
             raise ValueError("sh_factored needs the packed SH tensor as the last group (mesh_model_groups(features_last=True))")
-        assert 1 <= len(self.groups) <= 8
         params = [g["param"] for g in self.groups]
         dev = params[0].device
         pad = lambda k: (k + 63) // 64 * 64     # every segment starts 256-byte aligned (the kernels use 128-bit accesses)
@@ -57,6 +56,8 @@ class FlatAdam:
             p.grad = self.g[off:off + k].view(p.shape)
             off += pad(k)
             self.ends.append(off)
+        if not self.groups or len(self._segments()[0]) > 8:
+            raise ValueError("FlatAdam: gms_adam_step takes at most 8 segments of distinct hyper-parameters")
         self.betas, self.eps = betas, eps
         # Adam step count per group (torch.optim.Adam keeps one per parameter): a group whose update is skipped -- the
         # reference's reset_opacity replaces the opacity parameter by one without a gradient -- lags the others from then on
@@ -162,13 +163,24 @@ class FlatAdam:
             self.g_shard.copy_(self.g[off:off + self.shard]).mul_(1.0 / self.world)
         return self.g_shard, p_local, off
 
+    def _segments(self):
+        """(seg_end, lr0, lr1, inner, period) of gms_adam_step: one segment per group.  With more than 8 groups (gs_flame has
+        ten), neighbouring groups with the same hyper-parameters share one segment; Adam is element-wise, so the update is
+        the same."""
+        hp = [(float(g_.get("lr0", g_.get("lr", 0.0))), float(g_.get("lr1", g_.get("lr", 0.0))), int(g_.get("inner", 1)),
+               int(g_.get("period", 0))) for g_ in self.groups]
+        ends = list(self.ends)
+        if len(self.groups) > 8:
+            keep = [i for i in range(len(hp)) if i == len(hp) - 1 or hp[i] != hp[i + 1]]
+            hp, ends = [hp[i] for i in keep], [ends[i] for i in keep]
+        return [ends] + [[h[k] for h in hp] for k in range(4)]
+
     def _adam_desc(self, n, offset, p, g, zero_grad, zero_end):
         """Everything gms_adam_step needs, as plain Python (the stub kernel of the CPU tests reads the same dict)."""
-        return dict(n=int(n), offset=int(offset), p=p, g=g, m=self.m, v=self.v, seg_end=list(self.ends),
-                    lr0=[float(g_.get("lr0", g_.get("lr", 0.0))) for g_ in self.groups],
-                    lr1=[float(g_.get("lr1", g_.get("lr", 0.0))) for g_ in self.groups],
-                    inner=[int(g_.get("inner", 1)) for g_ in self.groups], period=[int(g_.get("period", 0)) for g_ in self.groups],
-                    beta1=self.betas[0], beta2=self.betas[1], eps=self.eps, step=self.t, zero_grad=int(zero_grad), zero_end=int(zero_end))
+        seg_end, lr0, lr1, inner, period = self._segments()
+        return dict(n=int(n), offset=int(offset), p=p, g=g, m=self.m, v=self.v, seg_end=seg_end, lr0=lr0, lr1=lr1, inner=inner,
+                    period=period, beta1=self.betas[0], beta2=self.betas[1], eps=self.eps, step=self.t, zero_grad=int(zero_grad),
+                    zero_end=int(zero_end))
 
     def _cuda_kernel(self, d):
         a = _lib.AdamArgs()

@@ -39,7 +39,9 @@ class Evaluation:
 
 class NativeRenderer(SyncFreeCapacity):
     """Forward-only renders of one model at one image size.  The outputs of render() are buffers the renderer owns and the
-    next call overwrites in stream order (ImageSink.write and anything else queued on the same stream read them first)."""
+    next call overwrites in stream order (ImageSink.write and anything else queued on the same stream read them first).
+    A FlameGaussianModel is drawn at its `vertices`, which FlameTrainer.step leaves at the pose that step rendered (before
+    its Adam update); call model.refresh_vertices() first to draw the current parameters (FlameTrainer.evaluate does)."""
 
     def __init__(self, model, width: int, height: int):
         self.model, self.W, self.H = model, int(width), int(height)
@@ -101,6 +103,7 @@ class NativeRenderer(SyncFreeCapacity):
             a.segments, a.n_segments = seg, len(seg)
         a.vertices, a.faces, a.alpha_raw, a.scale_raw = m.vertices.data_ptr(), m.faces.data_ptr(), m._alpha.data_ptr(), m._scale.data_ptr()
         a.features, a.opacity_raw, a.eps = feats.data_ptr(), m._opacity.data_ptr(), m.eps_s0
+        a.alpha_activation = getattr(m, "alpha_activation", _lib.ALPHA_RELU)
         self._call("gms_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
 
     def _call(self, fn: str, a, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
@@ -324,3 +327,53 @@ class NativeFreeRenderer(NativeRenderer):
         a.xyz, a.scaling_raw, a.rotation_raw = m._xyz.data_ptr(), m._scaling.data_ptr(), m._rotation.data_ptr()
         a.features, a.opacity_raw, a.eps = m._features.data_ptr(), m._opacity.data_ptr(), m.eps_s0
         self._call("gms_free_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
+
+
+class FlameRenderer(NativeRenderer):
+    """Renders of a trained gs_flame checkpoint (model.FlameCheckpoint) by the protocol of scripts/render_flame.py, in ONE call
+    per view (gms_flame_render_frame): xyz from the stored activated weights and a driving pose, scales and rotations from
+    the checkpoint's rows (they do not follow the pose, as in the reference).  evaluate(), the capacity prediction and the
+    overflow re-runs are NativeRenderer's; evaluate() draws the checkpoint's `vertices` pose."""
+
+    _frame_vertices = None
+
+    def _adopt(self, model):
+        return model.alpha.device, model.P
+
+    def _workspace_bytes(self, P: int) -> int:
+        return _lib.lib().gms_flame_render_workspace_bytes(P, self.W, self.H)
+
+    def _check(self, cam, bg) -> None:
+        m = self.model
+        v = m.vertices if self._frame_vertices is None else self._frame_vertices
+        V = m._vertices_enlargement.shape[0]
+        if not (torch.is_tensor(v) and v.is_cuda and v.dtype == torch.float32 and v.is_contiguous() and v.device == self.dev
+                and tuple(v.shape) == (V, 3)):
+            raise RuntimeError(f"FlameRenderer: the pose `vertices` must be a contiguous float32 [{V},3] CUDA tensor on {self.dev}")
+        for name in ("alpha", "_scaling", "_rotation", "_features", "_opacity"):
+            t = getattr(m, name)
+            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
+                raise RuntimeError(f"FlameRenderer: {name} must be a contiguous float32 CUDA tensor on {self.dev}")
+        if m.P != self.radii.shape[0]:
+            raise RuntimeError("FlameRenderer: the checkpoint's Gaussian count changed; make a new renderer")
+        self._check_view(cam, bg)
+
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+        m = self.model
+        self._check(cam, bg)
+        v = m.vertices if self._frame_vertices is None else self._frame_vertices
+        a = _lib.FlameRenderArgs()
+        a.V, a.F, a.K, a.M = v.shape[0], m.alpha.shape[0], m.alpha.shape[1], m._features.shape[1]
+        a.vertices, a.faces, a.alpha = v.data_ptr(), m.faces.data_ptr(), m.alpha.data_ptr()
+        a.scaling_log, a.rotation_raw = m._scaling.data_ptr(), m._rotation.data_ptr()
+        a.features, a.opacity_raw = m._features.data_ptr(), m._opacity.data_ptr()
+        self._call("gms_flame_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
+
+    def render(self, cam, bg: torch.Tensor, vertices: torch.Tensor = None, scale_modifier: float = 1.0, antialiasing: bool = False):
+        """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view at the pose `vertices` [V,3] (default: the checkpoint's
+        `vertices`); the checkpoint is never modified."""
+        self._frame_vertices = None if vertices is None else vertices.detach().float().contiguous()
+        try:
+            return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing)
+        finally:
+            self._frame_vertices = None

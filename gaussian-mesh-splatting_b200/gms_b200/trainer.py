@@ -140,6 +140,7 @@ class NativeFrame(SyncFreeCapacity):
             a.segments, a.n_segments = seg, len(seg)
         a.vertices, a.faces, a.alpha_raw, a.scale_raw = m.vertices.data_ptr(), m.faces.data_ptr(), m._alpha.data_ptr(), m._scale.data_ptr()
         a.features, a.opacity_raw, a.eps = m._features.data_ptr(), m._opacity.data_ptr(), m.eps_s0
+        a.alpha_activation = getattr(m, "alpha_activation", _lib.ALPHA_RELU)
         a.d_vertices, a.d_alpha_raw, a.d_scale_raw = m.vertices.grad.data_ptr(), m._alpha.grad.data_ptr(), m._scale.grad.data_ptr()
         a.d_features, a.d_opacity_raw = m._features.grad.data_ptr(), m._opacity.grad.data_ptr()
         if factored:        # no SH gradient rows: the colour gradient + camera centre go to this rank's exchange slot
@@ -564,4 +565,96 @@ class FreeTrainer:
         r = self._renderer
         if r is None or (r.W, r.H) != (W, H) or r.radii.shape[0] != self.model.P:
             r = self._renderer = NativeFreeRenderer(self.model, W, H)
+        return r.evaluate(cams, gts, self.bg, protocol=protocol)
+
+
+# ---------------------------------------------------------------------------------------------- gs_flame
+
+@dataclass
+class FlameOptimizationParams:
+    """OptimizationParamsFlame of the reference (arguments_games/__init__.py:32-49)."""
+    iterations: int = 30_000
+    alpha_lr: float = 0.001
+    feature_lr: float = 0.0025
+    opacity_lr: float = 0.05
+    scaling_lr: float = 0.005
+    flame_shape_lr: float = 0.01
+    flame_exp_lr: float = 0.001
+    flame_pose_lr: float = 0.001
+    flame_neck_pose_lr: float = 0.001
+    flame_trans_lr: float = 0.001
+    vertices_enlargement_lr: float = 0.0002
+    lambda_dssim: float = 0.2
+
+
+def flame_model_groups(model, o: FlameOptimizationParams) -> List[dict]:
+    """GaussianFlameModel.training_setup's groups (gaussian_flame_model.py:209-224) in its order, f_dc / f_rest as the one
+    packed SH group moved to the end (what FlatAdam(sh_factored=True) needs; the order of Adam groups has no numerical
+    meaning)."""
+    M = model._features.shape[1]
+    return [dict(param=model._flame_shape, lr=o.flame_shape_lr, name="shape"),
+            dict(param=model._flame_exp, lr=o.flame_exp_lr, name="expression"),
+            dict(param=model._flame_pose, lr=o.flame_pose_lr, name="pose"),
+            dict(param=model._flame_neck_pose, lr=o.flame_neck_pose_lr, name="neck_pose"),
+            dict(param=model._flame_trans, lr=o.flame_trans_lr, name="transl"),
+            dict(param=model._vertices_enlargement, lr=o.vertices_enlargement_lr, name="vertices_enlargement"),
+            dict(param=model._alpha, lr=o.alpha_lr, name="alpha"),
+            dict(param=model._opacity, lr=o.opacity_lr, name="opacity"),
+            dict(param=model._scales, lr=o.scaling_lr, name="scaling"),
+            dict(param=model._features, lr0=o.feature_lr, lr1=o.feature_lr / 20.0, inner=3, period=M, name="features")]
+
+
+class FlameTrainer:
+    """A whole iteration of the reference's train.py:83-157 for gs_flame (FlameGaussianModel), on one GPU:
+
+        oneupSHdegree every 1000 -> the driver's forward (ATen, autograd graph kept) -> gms_train_frame with softmax
+        weights on the detached vertices -> dL/dvertices back through the driver (torch.autograd.backward) -> Adam over the
+        reference's groups (FlatAdam; the SH step fused into the frame when M = 16).
+
+    No densification (train.py densifies gs / gs_flat only), a constant learning rate per group (update_learning_rate is a
+    no-op, gaussian_flame_model.py:226-228), and no optimizer step at the last iteration.  After step(), model.vertices
+    holds the pose the step rendered, not the updated parameters' (model.refresh_vertices() moves it; evaluate() does)."""
+
+    def __init__(self, model, bg: torch.Tensor, opt: FlameOptimizationParams = None, sync_free: bool = True):
+        self.model, self.bg = model, bg
+        self.opt = opt or FlameOptimizationParams()
+        self.sync_free = sync_free
+        self.fused_sh = model._features.shape[1] == 16
+        self.adam = FlatAdam(flame_model_groups(model, self.opt), sh_factored=self.fused_sh)
+        self.iteration = 0
+        self.frame = None
+        self._renderer = None
+
+    def step(self, cam: Camera, gt: torch.Tensor) -> torch.Tensor:
+        it = self.iteration + 1
+        m = self.model
+        if it % 1000 == 0:
+            m.oneupSHdegree()
+        verts = m.driver_vertices()
+        with torch.no_grad():
+            m.vertices.copy_(verts)
+        m.vertices.grad.zero_()
+        if self.frame is None:
+            self.frame = NativeFrame(m, cam.image_width, cam.image_height, self.opt.lambda_dssim, sync_free=self.sync_free)
+        take_step = it < self.opt.iterations         # train.py steps the optimizer on every iteration but the last
+        sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and take_step else None
+        loss = self.frame.run(cam, gt, self.bg, sh_adam=sh_adam)
+        torch.autograd.backward(verts, m.vertices.grad)      # accumulates into the FLAME tensors' flat .grad views
+        if not take_step:
+            self.adam.zero_grad()
+        elif self.fused_sh:
+            self.adam.step_rest()
+        else:
+            self.adam.step()
+        self.iteration = it
+        return loss
+
+    def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
+        """L1 / SSIM / PSNR of the current model (at its current pose) on held-out views (NativeRenderer.evaluate)."""
+        from .render import NativeRenderer
+        self.model.refresh_vertices()
+        W, H = int(cams[0].image_width), int(cams[0].image_height)
+        r = self._renderer
+        if r is None or (r.W, r.H) != (W, H):
+            r = self._renderer = NativeRenderer(self.model, W, H)
         return r.evaluate(cams, gts, self.bg, protocol=protocol)

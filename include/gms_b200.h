@@ -186,6 +186,9 @@ int gms_debug_unpack(const gms_raster_saved* saved, int32_t P, const int32_t* ra
 
 /* ---- mesh -> Gaussian expansion --------------------------------------------------------------- */
 
+#define GMS_ALPHA_RELU 0
+#define GMS_ALPHA_SOFTMAX 1
+
 typedef struct gms_expand_args {
     int32_t V, F, K;             /* vertices, faces, splats per face (P = F*K) */
     const float* vertices;       /* [V,3] */
@@ -203,6 +206,9 @@ typedef struct gms_expand_args {
     float* rotation_raw;         /* [P,4] (pc._rotation) */
     float* scaling_act;          /* [P,3] = exp(_scaling)        (get_scaling, fused E4) */
     float* rotation_act;         /* [P,4] = normalize(_rotation) (get_rotation, fused E4) */
+    int32_t alpha_activation;    /* barycentric weights from _alpha: GMS_ALPHA_RELU (0) relu + 1e-8, normalised (gs_mesh,
+                                    gaussian_mesh_model.py:166-167); GMS_ALPHA_SOFTMAX (1) softmax over the three
+                                    (gs_flame, gaussian_flame_model.py:34,195); anything else is GMS_E_ARG */
 } gms_expand_args;
 
 int gms_expand_forward(const gms_expand_args* a, void* cuda_stream);
@@ -348,6 +354,7 @@ typedef struct gms_frame_args {
                                    this frame's SH gradient; then d_features and d_color_sh may be NULL */
     const gms_mesh_segment* segments;   /* HOST [n_segments] or NULL: gs_multi_mesh with a K per mesh (see gms_mesh_segment) */
     int32_t n_segments;                 /* 0: one mesh of F faces x K splats, P = F*K */
+    int32_t alpha_activation;           /* as gms_expand_args.alpha_activation (every segment): 0 gs_mesh, 1 gs_flame */
 } gms_frame_args;
 size_t gms_frame_workspace_bytes(int32_t P, int32_t W, int32_t H);
 /* Device pointers into a frame workspace (valid after gms_train_frame): this step's expansion outputs and images. */
@@ -402,9 +409,35 @@ typedef struct gms_render_args {
     uint32_t* n_host_mapped;    /* optional mapped pinned host [2]: N, overflow flag */
     const gms_mesh_segment* segments;   /* HOST [n_segments] or NULL: as in gms_frame_args */
     int32_t n_segments;
+    int32_t alpha_activation;           /* as gms_expand_args.alpha_activation */
 } gms_render_args;
 size_t gms_render_workspace_bytes(int32_t P, int32_t W, int32_t H);
 int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
+
+/* One gs_flame render of a trained checkpoint in ONE call, the protocol of scripts/render_flame.py
+ * (renderer/flame_gaussian_renderer/__init__.py:59-80): xyz = alpha [F,K,3] (the ACTIVATED weights flame_params.pt stores)
+ * times vertices[faces] of the driving pose; scales = exp(_scaling) and rotations = normalize(_rotation) from the
+ * checkpoint's rows -- they do not follow the pose, as in the reference; sigmoid(opacity) inside the preprocess.  One
+ * activation launch, then the rasterizer forward of gms_render_frame.  Capacity semantics, outputs and validation as in
+ * gms_render_args; P = F*K; rotation_raw must be 16-byte aligned. */
+typedef struct gms_flame_render_args {
+    int32_t V, F, K, M;
+    const float* vertices;      /* [V,3] driving pose */
+    const int64_t* faces;       /* [F,3] */
+    const float* alpha;         /* [F,K,3] activated barycentric weights */
+    const float* scaling_log;   /* [P,3] _scaling of the checkpoint */
+    const float* rotation_raw;  /* [P,4] _rotation of the checkpoint */
+    const float* features;      /* [P,M,3] packed SH */
+    const float* opacity_raw;   /* [P,1] logits */
+    gms_raster_settings settings;
+    float* image; float* invdepth; int32_t* radii;
+    void* workspace; size_t workspace_bytes;   /* gms_flame_render_workspace_bytes */
+    int64_t* num_rendered;
+    int64_t binning_capacity;
+    uint32_t* n_host_mapped;
+} gms_flame_render_args;
+size_t gms_flame_render_workspace_bytes(int32_t P, int32_t W, int32_t H);
+int gms_flame_render_frame(const gms_flame_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
 
 /* One gs_points (pseudo-mesh) render in ONE call: the pseudo-mesh expansion (gms_points_expand_forward with activated outputs:
  * xyz = v1, scaling (eps, exp(log s2), exp(log s3)), normalised quaternion) -> sigmoid(opacity) inside the preprocess ->
@@ -673,8 +706,8 @@ int64_t gms_launch_count(int reset);
  * returns the number of kernel slots. */
 int gms_kernel_times(int reset, int max_kernels, double* ms_out, int64_t* count_out, const char** names_out);
 /* Tuning knobs (round-over-round experiments): "quad_masks", "warp_emit", "time_kernels", "composite_version",
- * "composite_fwd", "composite_bwd", "bwd_minblocks", "tile_order", "sort_impl", "expand_staged", "sh_staged"
- * (DESIGN.md lists what each selects).  Returns the previous value; unknown keys return -1. */
+ * "composite_fwd", "composite_bwd", "bwd_minblocks", "tile_order", "sort_impl", "expand_staged", "sh_staged",
+ * "expand_wide" (DESIGN.md lists what each selects).  Returns the previous value; unknown keys return -1. */
 int gms_set_option(const char* key, int value);
 
 #ifdef __cplusplus
