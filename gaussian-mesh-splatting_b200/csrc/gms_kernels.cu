@@ -1391,6 +1391,52 @@ int gms_image_dequantize(const uint8_t* src, int32_t src_is_hwc, float* chw, int
     return GMS_OK;
 }
 
+int gms_image_composite_rgba(const uint8_t* rgba, uint8_t* rgb, int32_t H, int32_t W, int32_t white_background, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!rgba || !rgb || H <= 0 || W <= 0 || (white_background != 0 && white_background != 1) ||
+        reinterpret_cast<size_t>(rgba) % 4 != 0)
+        return set_err(GMS_E_ARG, "gms_image_composite_rgba: bad arguments%s%s");
+    const long long npix = (long long)H * W;
+    k_image_composite_rgba<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(reinterpret_cast<const uchar4*>(rgba), rgb, npix,
+                                                                           white_background ? 1.0 : 0.0);
+    GMS_AFTER_LAUNCH("image_composite_rgba", 0, st);
+    return GMS_OK;
+}
+
+int gms_image_resize_u8(const gms_resize_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !a->src || !a->dst || a->C != 3 || a->in_w <= 0 || a->in_h <= 0 || a->out_w <= 0 || a->out_h <= 0 ||
+        a->out_w > 65535 * 256 || a->out_h > 65535 || a->in_h > 65535)
+        return set_err(GMS_E_ARG, "gms_image_resize_u8: bad sizes%s%s");
+    const bool horiz = a->out_w != a->in_w, vert = a->out_h != a->in_h;
+    if ((horiz && (!a->bounds_h || !a->coeffs_h || a->ksize_h <= 0)) || (vert && (!a->bounds_v || !a->coeffs_v || a->ksize_v <= 0)))
+        return set_err(GMS_E_ARG, "gms_image_resize_u8: missing coefficient table%s%s");
+    if (!horiz && !vert) {      // Image.resize to the same size is a copy
+        GMS_CUDA(cudaMemcpyAsync(a->dst, a->src, (size_t)a->in_w * a->in_h * 3, cudaMemcpyDeviceToDevice, st));
+        return GMS_OK;
+    }
+    if (horiz && vert) {        // the horizontal pass covers only the source rows the vertical pass reads
+        if (a->row0 < 0 || a->rows <= 0 || a->row0 + a->rows > a->in_h || !a->scratch ||
+            a->scratch_bytes < (size_t)a->out_w * a->rows * 3)
+            return set_err(GMS_E_ARG, "gms_image_resize_u8: bad row range or scratch too small%s%s");
+    }
+    if (horiz) {
+        uint8_t* out = vert ? a->scratch : a->dst;
+        const int row0 = vert ? a->row0 : 0, rows = vert ? a->rows : a->in_h;
+        k_resize_h_u8<<<dim3((a->out_w + 255) / 256, rows), 256, 0, st>>>(a->src, a->in_w, out, a->out_w, row0, a->bounds_h,
+                                                                          a->coeffs_h, a->ksize_h);
+        GMS_AFTER_LAUNCH("resize_h_u8", 0, st);
+    }
+    if (vert) {
+        const uint8_t* in = horiz ? a->scratch : a->src;
+        const int row0 = horiz ? a->row0 : 0;
+        k_resize_v_u8<<<dim3((a->out_w + 255) / 256, a->out_h), 256, 0, st>>>(in, a->out_w, a->dst, row0, a->bounds_v,
+                                                                              a->coeffs_v, a->ksize_v);
+        GMS_AFTER_LAUNCH("resize_v_u8", 0, st);
+    }
+    return GMS_OK;
+}
+
 int gms_adam_sh_factored(const gms_adam_sh_args* a, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (!a || !a->xyz || !a->exchange || !a->p || !a->m || !a->v || a->P < 0 || a->M != 16 || a->R < 1 || a->step < 1 ||

@@ -248,6 +248,14 @@ class AdamShArgs(C.Structure):
                 ("beta2", C.c_double), ("eps", C.c_double), ("step", C.c_int32)]
 
 
+class ResizeArgs(C.Structure):
+    """struct gms_resize_args"""
+    _fields_ = [("in_w", C.c_int32), ("in_h", C.c_int32), ("out_w", C.c_int32), ("out_h", C.c_int32), ("C", C.c_int32),
+                ("src", C.c_void_p), ("dst", C.c_void_p), ("bounds_h", C.c_void_p), ("coeffs_h", C.c_void_p), ("ksize_h", C.c_int32),
+                ("bounds_v", C.c_void_p), ("coeffs_v", C.c_void_p), ("ksize_v", C.c_int32), ("row0", C.c_int32), ("rows", C.c_int32),
+                ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t)]
+
+
 KNN_BOX = 64        # GMS_KNN_BOX: points per box of the three-nearest-neighbour search
 
 
@@ -270,7 +278,7 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_pseudomesh_bind", "gms_pseudomesh_repose", "gms_bound_points_render_workspace_bytes",
                "gms_bound_points_render_frame", "gms_free_train_frame", "gms_free_render_frame", "gms_densify_scratch_bytes",
                "gms_densify_plan", "gms_densify_apply", "gms_knn_scratch_bytes", "gms_knn_dist2",
-               "gms_flame_render_workspace_bytes", "gms_flame_render_frame"]
+               "gms_flame_render_workspace_bytes", "gms_flame_render_frame", "gms_image_composite_rgba", "gms_image_resize_u8"]
 
 _lib = None
 
@@ -316,6 +324,8 @@ def lib():
     L.gms_points_prepare_vertices.argtypes = [C.POINTER(PointsVerticesArgs), C.c_void_p]
     L.gms_image_quantize.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     L.gms_image_dequantize.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+    L.gms_image_composite_rgba.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+    L.gms_image_resize_u8.argtypes = [C.POINTER(ResizeArgs), C.c_void_p]
     L.gms_adam_sh_factored.argtypes = [C.POINTER(AdamShArgs), C.c_void_p]
     L.gms_frame_views.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(FrameView)]
     L.gms_frame_workspace_bytes.restype = C.c_size_t

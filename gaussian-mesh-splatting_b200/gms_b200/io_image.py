@@ -123,6 +123,22 @@ def to_device_float(image_u8: torch.Tensor, out: Optional[torch.Tensor] = None, 
     return out
 
 
+class GroundTruthBuffer:
+    """The float [3,H,W] ground truth the loss and metric kernels read, from 8-bit [H,W,3] images (dataset.load_scene's
+    resident views): byte / 255 into ONE reused device buffer per frame or renderer, in stream order."""
+
+    def __init__(self, height: int, width: int, device):
+        self.H, self.W, self.dev = int(height), int(width), torch.device(device)
+        self.buf = None
+
+    def __call__(self, gt_u8: torch.Tensor, who: str) -> torch.Tensor:
+        if tuple(gt_u8.shape) != (self.H, self.W, 3):
+            raise ValueError(f"{who}: uint8 ground truth must be [{self.H},{self.W},3]; got {tuple(gt_u8.shape)}")
+        if self.buf is None:
+            self.buf = torch.empty(3, self.H, self.W, dtype=torch.float32, device=self.dev)
+        return to_device_float(gt_u8.to(self.dev, non_blocking=True), out=self.buf, hwc=True)
+
+
 def load_image_u8(path: str) -> torch.Tensor:
     """PNG / PPM file -> pinned uint8 [H,W,C] host tensor (the data-loader side of the 8-bit ground-truth path)."""
     data = open(path, "rb").read()

@@ -54,7 +54,7 @@ class NativeRenderer(SyncFreeCapacity):
         self._init_capacity(True)
         self._scratch, self._cb = grow_only_alloc(dev)
         self._metric_scratch = torch.empty(scratch_bytes(3, self.H, self.W), dtype=torch.uint8, device=dev)
-        self._gt_buf = None
+        self._gt_u8 = io_image.GroundTruthBuffer(self.H, self.W, dev)
 
     def _adopt(self, model):
         """(device, Gaussian count) of the model this renderer draws; makes its face indices int64 and contiguous."""
@@ -135,11 +135,7 @@ class NativeRenderer(SyncFreeCapacity):
     def _gt_float(self, gt: torch.Tensor) -> torch.Tensor:
         """float [3,H,W] as is; uint8 [H,W,3] (8-bit ground truth) -> byte / 255 in one reused device buffer."""
         if gt.dtype == torch.uint8:
-            if tuple(gt.shape) != (self.H, self.W, 3):
-                raise ValueError(f"evaluate: uint8 ground truth must be [{self.H},{self.W},3]; got {tuple(gt.shape)}")
-            if self._gt_buf is None:
-                self._gt_buf = torch.empty(3, self.H, self.W, dtype=torch.float32, device=self.dev)
-            return io_image.to_device_float(gt.to(self.dev, non_blocking=True), out=self._gt_buf, hwc=True)
+            return self._gt_u8(gt, "evaluate")
         if tuple(gt.shape) != (3, self.H, self.W) or gt.dtype != torch.float32:
             raise ValueError(f"evaluate: float ground truth must be float32 [3,{self.H},{self.W}]; got {gt.dtype} {tuple(gt.shape)}")
         return gt.to(self.dev, non_blocking=True)

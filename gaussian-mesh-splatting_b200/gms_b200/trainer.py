@@ -22,6 +22,7 @@ import torch.distributed as dist
 import diff_gaussian_rasterization as dgr
 
 from .capacity import SyncFreeCapacity, grow_only_alloc
+from .io_image import GroundTruthBuffer
 from .losses import fused_training_loss
 from .model import MeshGaussianModel
 from .optim import FlatAdam, mesh_model_groups
@@ -81,6 +82,7 @@ class NativeFrame(SyncFreeCapacity):
                                     # colour gradients starts there, on the optimizer's communication stream)
         self._check_model()
         self._scratch, self._cb = grow_only_alloc(dev)
+        self._gt_u8 = GroundTruthBuffer(self.H, self.W, dev)
 
     def _check_model(self):
         """Raw pointers go straight to CUDA kernels: dtype / device / layout are checked here, once, instead of failing
@@ -121,9 +123,12 @@ class NativeFrame(SyncFreeCapacity):
 
     def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, factored: bool = False, sh_adam=None) -> torch.Tensor:
         """sh_adam (FlatAdam.begin_fused_sh_step()): the frame also applies the SH parameters' Adam step, and writes no SH
-        gradient (unless `factored` asks for the colour gradient as well)."""
+        gradient (unless `factored` asks for the colour gradient as well).  gt: float32 [3,H,W], or uint8 [H,W,3] (dequantized
+        on the device into the frame's buffer)."""
         import ctypes as C
         from . import _lib
+        if gt.dtype == torch.uint8:
+            gt = self._gt_u8(gt, "NativeFrame.run")
         for t, what in ((gt, "gt"), (bg, "bg"), (cam.world_view_transform, "camera matrices"), (cam.full_proj_transform, "camera matrices"),
                         (cam.camera_center, "camera centre")):
             if not t.is_cuda or t.device != self.dev or t.dtype != torch.float32:
@@ -202,6 +207,7 @@ class MeshTrainer:
         self.loss_fn = loss_fn or fused_training_loss    # fast=False A/B arm: callers may pass an ATen loss (tests/aten_reference.py)
         self._frame = None
         self._renderer = None
+        self._gt_u8 = None      # the autograd arm's buffer for 8-bit ground truth
         self.sh_factored = False
         if fast:
             # native frames hand the SH gradient over as factors (12 B instead of 192 B per Gaussian; replicated optimizer);
@@ -232,7 +238,7 @@ class MeshTrainer:
         """One optimisation step.  If `loss_host` (pinned) / `loss_ready` are given, the loss is copied to the host from a side
         stream as soon as the loss kernels have run (native frames: NativeFrame.read_loss_async; otherwise right after the
         backward pass, before the optimizer kernels are queued): a caller that logs the loss every step gets it while the
-        backward pass is still running and queues its next step in that time."""
+        backward pass is still running and queues its next step in that time.  gt: float32 [3,H,W] or uint8 [H,W,3]."""
         if self.native:
             if self._frame is None:
                 self._frame = NativeFrame(self.model, cam.image_width, cam.image_height, self.lambda_dssim, sync_free=self.sync_free,
@@ -256,6 +262,10 @@ class MeshTrainer:
             else:
                 self.opt.zero_grad_partial(self.opt.ends[0])
             return loss
+        if gt.dtype == torch.uint8:
+            if self._gt_u8 is None:
+                self._gt_u8 = GroundTruthBuffer(cam.image_height, cam.image_width, self.model.vertices.device)
+            gt = self._gt_u8(gt, "MeshTrainer.step")
         from . import rasterizer as _r
         prev = _r.DIRECT_SH_GRAD
         _r.DIRECT_SH_GRAD = self.fast      # FlatAdam keeps .grad preallocated and zeroed: write dL/dshs in place
@@ -342,6 +352,7 @@ class NativeFreeFrame(SyncFreeCapacity):
         self.ws = None
         self._epoch, self._view_epoch = 0, {}
         self.ev_loss = None
+        self._gt_u8 = GroundTruthBuffer(self.H, self.W, self.dev)
         self.resize()
 
     def resize(self) -> None:
@@ -377,9 +388,12 @@ class NativeFreeFrame(SyncFreeCapacity):
 
     def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, stats: bool = True, sh_adam=None) -> torch.Tensor:
         """stats: add this frame's densification statistics to `accum` / `denom`.  sh_adam (FlatAdam.begin_fused_sh_step()):
-        the frame also applies the SH parameters' Adam step and writes no SH gradient."""
+        the frame also applies the SH parameters' Adam step and writes no SH gradient.  gt: float32 [3,H,W], or uint8 [H,W,3]
+        (dequantized on the device into the frame's buffer)."""
         import ctypes as C
         from . import _lib
+        if gt.dtype == torch.uint8:
+            gt = self._gt_u8(gt, "NativeFreeFrame.run")
         gt = gt.contiguous()
         self._check(gt, bg, cam)
         m = self.model

@@ -695,6 +695,39 @@ int gms_image_quantize(const float* chw, uint8_t* out, int32_t C, int32_t H, int
  * utils/general_utils.py:105-112): ground-truth images can stay 8-bit on the host and on the device. */
 int gms_image_dequantize(const uint8_t* src, int32_t src_is_hwc, float* chw, int32_t C, int32_t H, int32_t W, void* cuda_stream);
 
+/* ---- ground-truth preparation (the dataset loader, DESIGN.md 4.6) -------------------------------- */
+
+/* uint8 RGBA [H,W,4] (4-byte aligned) -> uint8 RGB [H,W,3] over a black (white_background 0) or white (1) background,
+ * bit-identical to readCamerasFromTransforms' numpy sequence (scene/dataset_readers.py:204-210): u / 255.0 in double,
+ * rgb * a + bg * (1 - a), * 255.0, truncated to a byte.  Bad sizes, a null or misaligned pointer or another background
+ * value are GMS_E_ARG, returned without a launch.  Caller's stream, no host synchronisation. */
+int gms_image_composite_rgba(const uint8_t* rgba, uint8_t* rgb, int32_t H, int32_t W, int32_t white_background, void* cuda_stream);
+
+/* Bicubic resample of a uint8 [in_h,in_w,3] image to [out_h,out_w,3], bit-exact to Pillow's Image.resize with its default
+ * filter (PILtoTorch, utils/general_utils.py:101-107, as loadCam calls it, utils/camera_utils.py:19-52): Pillow's two-pass
+ * ImagingResample, 8-bit path.  A pass runs only when its dimension changes; the horizontal pass runs first, and when both
+ * run it covers only the source rows [row0, row0 + rows) the vertical pass reads, into `scratch` (out_w * rows * 3 bytes).
+ * The per-axis tables come from the host (gms_b200/dataset.py resize_coeffs): bounds [out,2] = (first source index, taps),
+ * coeffs [out,ksize] int32 weights in 22-bit fixed point; the kernels only do integer multiply-adds.  A table is read only
+ * when its axis changes; the same size on both axes is a device copy.  Bad sizes (C != 3, a size < 1, out_h, in_h > 65535),
+ * a missing table or a bad row range / short scratch are GMS_E_ARG, returned without a launch.  The tables' contents are not
+ * checked.  Caller's stream, no host synchronisation. */
+typedef struct gms_resize_args {
+    int32_t in_w, in_h, out_w, out_h, C;
+    const uint8_t* src;          /* [in_h,in_w,C] */
+    uint8_t* dst;                /* [out_h,out_w,C] */
+    const int32_t* bounds_h;     /* [out_w,2] */
+    const int32_t* coeffs_h;     /* [out_w,ksize_h] */
+    int32_t ksize_h;
+    const int32_t* bounds_v;     /* [out_h,2], source rows of the original image */
+    const int32_t* coeffs_v;     /* [out_h,ksize_v] */
+    int32_t ksize_v;
+    int32_t row0, rows;          /* both passes: bounds_v[0] and bounds_v[last] + taps - bounds_v[0] */
+    uint8_t* scratch;
+    size_t scratch_bytes;
+} gms_resize_args;
+int gms_image_resize_u8(const gms_resize_args* a, void* cuda_stream);
+
 /* ---- misc ------------------------------------------------------------------------------------- */
 const char* gms_last_error(void);
 const char* gms_version(void);
