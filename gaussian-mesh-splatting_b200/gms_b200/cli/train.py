@@ -1,0 +1,383 @@
+"""python -m gms_b200.cli.train -s <scene> [-m <output>] [--gs_type gs_mesh|gs_flat|gs] ...: the reference's train.py on the
+native trainers.
+
+Flags, defaults and the output directory are the reference's (cfg_args, cameras.json, input.ply,
+point_cloud/iteration_N/point_cloud.ply [+ model_params.pt], chkpnt<N>.pth).  One iteration, in train.py's order
+(train.py:61-157):
+
+    SH degree up every 1000 -> the view from the Scene's view order -> background (torch.rand(3) on the device under
+    --random_background) -> the one-call training frame -> training_report at --test_iterations -> Scene.save at
+    --save_iterations -> densify / opacity reset (gs, gs_flat) -> Adam on every iteration but the last -> checkpoint at
+    --checkpoint_iterations.
+
+The report and the save run inside the trainer's `before_update` callback, so they see the parameters after N-1 updates,
+as the reference's do.  The loop itself never synchronises with the host: the loss reaches the progress display's moving
+average through pinned host slots and CUDA events that are polled, not waited on.
+
+Deliberate differences:
+  * chkpnt<N>.pth holds (state, N) with the library's own state (the trainer's state_dict(), the view-order stream and the
+    background generator), not the reference's capture() tuple; a resumed run continues the uninterrupted run's sequence of
+    views and backgrounds, where the reference re-shuffles.
+  * --seed (default 0) seeds what safe_state seeds: the view shuffle and order, the initial model and the backgrounds.
+  * Not built, refused by name: gs_flame, gs_multi_mesh, --antialiasing, --debug, --debug_from, --detect_anomaly,
+    --convert_SHs_python, --compute_cov3D_python, --save_xyz, --data_device other than cuda.  --ip / --port are accepted and
+    ignored (the reference does not start its viewer either)."""
+from __future__ import annotations
+
+import collections
+import json
+import os
+import random
+import shutil
+import sys
+import uuid
+from argparse import ArgumentParser, Namespace
+from types import SimpleNamespace
+from typing import List
+
+import numpy as np
+import torch
+
+from .. import dataset, io_ply
+from ..model import FreeGaussianModel, MeshGaussianModel
+from ..scenes import MeshGaussianParams
+from ..trainer import FreeOptimizationParams, FreeTrainer, MeshTrainer
+from . import options
+
+GS_TYPES = ("gs_mesh", "gs_flat", "gs")
+FREE_TYPES = ("gs", "gs_flat")
+# flags of the reference that the native training frames do not implement: (name, default)
+REFUSED = (("debug_from", -1), ("detect_anomaly", False), ("save_xyz", False), ("convert_SHs_python", False),
+           ("compute_cov3D_python", False), ("debug", False), ("antialiasing", False))
+
+
+def build_parser(gs_type: str) -> ArgumentParser:
+    """train.py's parser for `gs_type`, in its declaration order, plus --seed."""
+    p = ArgumentParser(description="Training script parameters")
+    p.add_argument("--ip", type=str, default="127.0.0.1")
+    p.add_argument("--port", type=int, default=6009)
+    p.add_argument("--gs_type", type=str, default="gs_mesh")
+    p.add_argument("--num_splats", nargs="+", type=int, default=[2])
+    p.add_argument("--meshes", nargs="+", type=str, default=[])
+    p.add_argument("--debug_from", type=int, default=-1)
+    p.add_argument("--detect_anomaly", action="store_true", default=False)
+    p.add_argument("--test_iterations", nargs="+", type=int, default=[7_000, 20_000, 30_000, 60_000, 90_000])
+    p.add_argument("--save_iterations", nargs="+", type=int, default=[7_000, 20_000, 30_000, 60_000, 90_000])
+    p.add_argument("--quiet", action="store_true")
+    p.add_argument("--checkpoint_iterations", nargs="+", type=int, default=[])
+    p.add_argument("--start_checkpoint", type=str, default=None)
+    p.add_argument("--save_xyz", action="store_true")
+    options.add_group(p, "Loading Parameters", options.MODEL_PARAMS)
+    options.add_group(p, "Optimization Parameters", options.OPT_PARAMS_MESH if gs_type == "gs_mesh" else options.OPT_PARAMS_FREE)
+    options.add_group(p, "Pipeline Parameters", options.PIPELINE_PARAMS)
+    p.add_argument("--seed", type=int, default=0, help="seeds the view shuffle and order, the initial model and the backgrounds")
+    return p
+
+
+def parse_args(argv) -> Namespace:
+    """train.py's argument handling: --gs_type first (it picks the optimisation group), then everything; --iterations is
+    appended to --save_iterations.  Unsupported types and flags exit with an error that names them."""
+    argv = list(argv)
+    pre = ArgumentParser(add_help=False)
+    pre.add_argument("--gs_type", type=str, default="gs_mesh")
+    gs_type = pre.parse_known_args(argv)[0].gs_type
+    parser = build_parser(gs_type if gs_type in GS_TYPES else "gs_mesh")
+    if gs_type not in GS_TYPES:
+        parser.error(f"--gs_type {gs_type} is not supported (supported: {', '.join(GS_TYPES)}); gs_flame needs the FLAME model "
+                     f"files and gs_multi_mesh a COLMAP mesh reader")
+    args = parser.parse_args(argv)
+    for name, default in REFUSED:
+        if getattr(args, name) != default:
+            parser.error(f"--{name} is not supported by the native training frames")
+    if args.data_device != "cuda":
+        parser.error(f"--data_device {args.data_device} is not supported: images stay resident on the GPU (--data_device cuda)")
+    args.save_iterations.append(args.iterations)
+    return args
+
+
+def set_default_model_path(args: Namespace) -> None:
+    """prepare_output_and_logger's default -m: ./output/ + the first ten characters of $OAR_JOB_ID or a random UUID."""
+    if not args.model_path:
+        unique = os.getenv("OAR_JOB_ID") or str(uuid.uuid4())
+        args.model_path = os.path.join("./output/", unique[0:10])
+
+
+def iteration_events(it: int, args: Namespace) -> List[str]:
+    """What train.py does at iteration `it` besides the frame, in its order: "report", "save", "densify", "reset", "step",
+    "checkpoint"."""
+    ev = []
+    if it in args.test_iterations:
+        ev.append("report")
+    if it in args.save_iterations:
+        ev.append("save")
+    if args.gs_type in FREE_TYPES:
+        _, densify, reset = FreeTrainer.schedule(SimpleNamespace(opt=free_params(args), white_background=args.white_background), it)
+        ev += ["densify"] * densify + ["reset"] * reset
+    if it < args.iterations:
+        ev.append("step")
+    if it in args.checkpoint_iterations:
+        ev.append("checkpoint")
+    return ev
+
+
+def free_params(args: Namespace) -> FreeOptimizationParams:
+    return FreeOptimizationParams(**{k: getattr(args, k) for k in FreeOptimizationParams.__dataclass_fields__ if k != "min_opacity"})
+
+
+class ViewOrder:
+    """train.py's viewpoint_stack.pop(randint(0, len - 1)) on the Random stream that shuffled the scene (Scene.view_order),
+    drawn one view at a time, with a state a checkpoint can hold."""
+
+    def __init__(self, scene: dataset.Scene):
+        self.rng = random.Random()
+        self.rng.setstate(scene._rng_state)
+        self.n = len(scene.train_cameras)
+        self.stack = []
+
+    def next(self) -> int:
+        if not self.stack:
+            self.stack = list(range(self.n))
+        return self.stack.pop(self.rng.randint(0, len(self.stack) - 1))
+
+    def state_dict(self) -> dict:
+        version, internal, gauss = self.rng.getstate()
+        return {"rng": [version, list(internal), gauss], "stack": list(self.stack)}
+
+    def load_state_dict(self, state: dict) -> None:
+        version, internal, gauss = state["rng"]
+        self.rng.setstate((int(version), tuple(int(x) for x in internal), gauss))
+        self.stack = [int(x) for x in state["stack"]]
+
+
+def unshuffled_views(scene: dataset.Scene, seed: int):
+    """(train, test) ViewInfos in file order: read_scene shuffled both lists with random.Random(seed), train first; the same
+    draws on index lists give the permutations to undo."""
+    rng = random.Random(seed)
+    out = []
+    for views in (scene.train_views, scene.test_views):
+        perm = list(range(len(views)))
+        rng.shuffle(perm)
+        orig = [None] * len(views)
+        for i, p in enumerate(perm):
+            orig[p] = views[i]
+        out.append(orig)
+    return out[0], out[1]
+
+
+def camera_json(idx: int, v: dataset.ViewInfo) -> dict:
+    """camera_to_JSON (utils/camera_utils.py): the camera-to-world position and rotation, the file's size, focal lengths."""
+    Rt = np.zeros((4, 4))
+    Rt[:3, :3] = v.R.transpose()
+    Rt[:3, 3] = v.T
+    Rt[3, 3] = 1.0
+    C2W = np.linalg.inv(Rt)
+    return {"id": idx, "img_name": v.name, "width": v.width, "height": v.height, "position": C2W[:3, 3].tolist(),
+            "rotation": [x.tolist() for x in C2W[:3, :3]], "fy": dataset.fov2focal(v.FovY, v.height),
+            "fx": dataset.fov2focal(v.FovX, v.width)}
+
+
+def write_cameras_json(path: str, scene: dataset.Scene, seed: int) -> None:
+    train, test = unshuffled_views(scene, seed)
+    with open(path, "w") as f:
+        json.dump([camera_json(i, v) for i, v in enumerate(test + train)], f)
+
+
+def write_input_ply(path: str, scene: dataset.Scene, source_path: str, gs_type: str, seed: int) -> None:
+    """Scene.__init__'s input.ply: a byte copy of the dataset's own cloud file where it has one, else the cloud the
+    reference's reader would have stored (the random NeRF-synthetic cloud, the converted COLMAP points, the gs_mesh cloud)."""
+    if gs_type == "gs_mesh":
+        io_ply.save_point_cloud(path, *dataset.mesh_input_cloud(scene.mesh, seed))
+        return
+    for src in (os.path.join(source_path, "points3d.ply"), os.path.join(source_path, "sparse", "0", "points3D.ply")):
+        if os.path.exists(src):
+            shutil.copyfile(src, path)
+            return
+    points, colors, _ = scene.point_cloud
+    io_ply.save_point_cloud(path, points, np.round(colors * 255.0))      # colors are bytes / 255: the round trip is exact
+
+
+def _mesh_params(p: MeshGaussianParams, sh_degree: int) -> MeshGaussianParams:
+    """create_from_pcd's features for max_sh_degree `sh_degree` (the loader builds degree 3: the rest is zero anyway)."""
+    M = (int(sh_degree) + 1) ** 2
+    rest = torch.zeros(p._features_dc.shape[0], M - 1, 3)
+    return MeshGaussianParams(p.vertices, p.faces, p._alpha, p._scale, p._features_dc, rest, p._opacity)
+
+
+class _Progress:
+    def __init__(self, first: int, last: int, quiet: bool):
+        self.bar = None
+        if not quiet:
+            try:
+                from tqdm import tqdm
+                self.bar = tqdm(range(first, last), desc="Training progress")
+            except ImportError:
+                pass
+
+    def show(self, ema: float) -> None:
+        if self.bar is not None:
+            self.bar.set_postfix({"Loss": f"{ema:.{7}f}"})
+            self.bar.update(10)
+
+    def close(self) -> None:
+        if self.bar is not None:
+            self.bar.close()
+
+
+class Training:
+    """One train.py run: prepare() builds the output directory, scene, model and trainer (and restores --start_checkpoint);
+    run() iterates.  Attributes the tests read: trainer, model, scene, order (ViewOrder), ema (per consumed iteration:
+    (iteration, loss, moving average)), reports ((iteration, split, L1, PSNR)), events (per iteration: iteration_events)."""
+
+    LOSS_SLOTS = 64
+
+    def __init__(self, args: Namespace, device="cuda", scene: dataset.Scene = None):
+        """scene: the load_scene result for these arguments, when the caller already has it (loaded on `device`)."""
+        self.args, self.dev = args, torch.device(device)
+        self.ema, self.reports, self.events = [], [], []
+        self.first_iter = 0
+        self.scene = scene
+
+    def log(self, msg: str) -> None:
+        if not self.args.quiet:
+            print(msg)
+
+    # ---- set-up (prepare_output_and_logger, Scene.__init__, training_setup, restore)
+    def prepare(self) -> "Training":
+        a = self.args
+        set_default_model_path(a)
+        self.log(f"Output folder: {a.model_path}")
+        os.makedirs(a.model_path, exist_ok=True)
+        with open(os.path.join(a.model_path, "cfg_args"), "w") as f:
+            f.write(options.cfg_args_string(a))
+        if self.scene is None:
+            self.scene = dataset.load_scene(a.source_path, a.gs_type, a.white_background, a.eval, a.resolution, a.images,
+                                            a.num_splats[0], a.seed, device=self.dev)
+        sc = self.scene
+        write_input_ply(os.path.join(a.model_path, "input.ply"), sc, a.source_path, a.gs_type, a.seed)
+        write_cameras_json(os.path.join(a.model_path, "cameras.json"), sc, a.seed)
+        sizes = {(c.image_width, c.image_height) for c in sc.train_cameras + sc.test_cameras}
+        if len(sizes) > 1:
+            raise ValueError(f"training needs every view at one size; this scene has {sorted(sizes)} (-r sets a common width)")
+        self.bg = torch.tensor([1.0, 1.0, 1.0] if a.white_background else [0.0, 0.0, 0.0], dtype=torch.float32, device=self.dev)
+        self.bg_gen = torch.Generator(device=self.dev).manual_seed(a.seed) if a.random_background else None
+        if a.gs_type == "gs_mesh":
+            self.model = MeshGaussianModel.from_params(_mesh_params(sc.mesh, a.sh_degree), self.dev, sh_degree=a.sh_degree,
+                                                       active_sh_degree=0, packed_features=True)
+            tr = self.trainer = MeshTrainer(self.model, self.bg, a.lambda_dssim, native=True)
+            lrs = {"vertices": a.vertices_lr, "alpha": a.alpha_lr, "opacity": a.opacity_lr, "scaling": a.scaling_lr}
+            for g in tr.opt.groups:         # OptimizationParamsMesh's learning rates (mesh_model_groups' f_rest = f_dc / 20)
+                if g["name"] == "features":
+                    g["lr0"], g["lr1"] = a.feature_lr, a.feature_lr / 20.0
+                else:
+                    g["lr"] = lrs[g["name"]]
+        else:
+            points, colors, _ = sc.point_cloud
+            self.model = FreeGaussianModel.from_point_cloud(points, colors, a.gs_type, a.sh_degree, self.dev)
+            gen = torch.Generator(device=self.dev).manual_seed(a.seed)
+            self.trainer = FreeTrainer(self.model, self.bg, sc.cameras_extent, free_params(a), white_background=a.white_background,
+                                       generator=gen)
+        self.order = ViewOrder(sc)
+        if a.start_checkpoint:
+            state, self.first_iter = torch.load(a.start_checkpoint, map_location="cpu", weights_only=True)
+            self.load_state_dict(state)
+        return self
+
+    def state_dict(self) -> dict:
+        return {"gs_type": self.args.gs_type, "trainer": self.trainer.state_dict(), "view_order": self.order.state_dict(),
+                "bg_generator": self.bg_gen.get_state() if self.bg_gen is not None else None}
+
+    def load_state_dict(self, state: dict) -> None:
+        if state.get("gs_type") != self.args.gs_type:
+            raise ValueError(f"--start_checkpoint holds a {state.get('gs_type')} run, not {self.args.gs_type}")
+        self.trainer.load_state_dict(state["trainer"])
+        self.order.load_state_dict(state["view_order"])
+        if self.bg_gen is not None and state["bg_generator"] is not None:
+            self.bg_gen.set_state(state["bg_generator"])
+
+    # ---- what happens at an iteration besides the frame
+    def report(self, it: int) -> None:
+        """training_report at a test iteration: the test views and train views 5, 10, ..., 25 (mod n) with the fixed
+        background; mean L1 and mean per-channel PSNR, as the reference prints them."""
+        sc = self.scene
+        n = len(sc.train_cameras)
+        configs = (("test", sc.test_cameras, sc.test_images),
+                   ("train", [sc.train_cameras[i % n] for i in range(5, 30, 5)], [sc.train_images[i % n] for i in range(5, 30, 5)]))
+        for name, cams, gts in configs:
+            if cams:
+                r = self.trainer.evaluate(cams, gts)
+                l1, psnr = float(r.mean[0]), float(r.mean[3])
+                self.reports.append((it, name, l1, psnr))
+                self.log(f"\n[ITER {it}] Evaluating {name}: L1 {l1} PSNR {psnr}")
+
+    def save(self, it: int) -> None:
+        self.log(f"\n[ITER {it}] Saving Gaussians")
+        path = os.path.join(self.args.model_path, "point_cloud", f"iteration_{it}", "point_cloud.ply")
+        if self.args.gs_type == "gs_mesh":
+            io_ply.save_mesh_model(path, self.model)
+        else:
+            self.model.save(path)
+
+    def checkpoint(self, it: int) -> None:
+        self.log(f"\n[ITER {it}] Saving Checkpoint")
+        torch.save((self.state_dict(), it), os.path.join(self.args.model_path, f"chkpnt{it}.pth"))
+
+    # ---- the loss, read without synchronising
+    def _consume(self, block: bool = False) -> None:
+        while self._pending and (block or self._pending[0][2].query()):
+            it, i, ev = self._pending.popleft()
+            ev.synchronize()
+            loss = float(self._slots_np[i])
+            self._ema = 0.4 * loss + 0.6 * self._ema
+            self.ema.append((it, loss, self._ema))
+            if it % 10 == 0:
+                self._progress.show(self._ema)
+
+    def run(self) -> "Training":
+        a, sc, dev = self.args, self.scene, self.dev
+        slots = torch.zeros(self.LOSS_SLOTS, dtype=torch.float32).pin_memory()
+        self._slots_np = slots.numpy()
+        events = [torch.cuda.Event() for _ in range(self.LOSS_SLOTS)]
+        self._pending, self._ema = collections.deque(), 0.0
+        self._progress = _Progress(self.first_iter, a.iterations, a.quiet)
+        mesh = a.gs_type == "gs_mesh"
+        for it in range(self.first_iter + 1, a.iterations + 1):
+            ev = iteration_events(it, a)
+            self.events.append((it, ev))
+            if mesh and it % 1000 == 0:
+                self.model.oneupSHdegree()
+            v = self.order.next()
+            bg = torch.rand(3, device=dev, generator=self.bg_gen) if self.bg_gen is not None else None
+            hooks = [f for name, f in (("report", self.report), ("save", self.save)) if name in ev]
+            # the last iteration takes no Adam step: never let the frame fuse one in
+            before = (lambda: [f(it) for f in hooks]) if hooks or "step" not in ev else None
+            if len(self._pending) == self.LOSS_SLOTS:
+                self._pending[0][2].synchronize()
+                self._consume()
+            slot = it % self.LOSS_SLOTS
+            if mesh:
+                self.trainer.optimizer_step = "step" in ev
+                self.trainer.step(sc.train_cameras[v], sc.train_images[v], loss_host=slots[slot:slot + 1], loss_ready=events[slot],
+                                  bg=bg, before_update=before)
+            else:
+                loss = self.trainer.step(sc.train_cameras[v], sc.train_images[v], bg=bg, before_update=before)
+                slots[slot:slot + 1].copy_(loss.reshape(1), non_blocking=True)
+                events[slot].record(torch.cuda.current_stream(dev))
+            self._pending.append((it, slot, events[slot]))
+            self._consume()
+            if "checkpoint" in ev:
+                self.checkpoint(it)
+        self._consume(block=True)
+        self._progress.close()
+        self.log("\nTraining complete.")
+        return self
+
+
+def main(argv=None) -> Training:
+    args = parse_args(sys.argv[1:] if argv is None else argv)
+    if not torch.cuda.is_available():
+        raise RuntimeError("gms_b200.cli.train needs a CUDA device")
+    return Training(args).prepare().run()
+
+
+if __name__ == "__main__":
+    main()

@@ -489,6 +489,18 @@ def mesh_gaussians_from_obj(obj_path: str, num_splats: int, seed: int = 0) -> Me
     return MeshGaussianParams(vertices.contiguous(), faces, alpha, torch.ones(P, 1), fdc, torch.zeros(P, 15, 3), opacity)
 
 
+def mesh_input_cloud(mesh: MeshGaussianParams, seed: int = 0) -> Tuple[np.ndarray, np.ndarray]:
+    """The cloud readNerfSyntheticMeshInfo stores (storePly, the `input.ply` of a gs_mesh run) for mesh_gaussians_from_obj's
+    parameters: points = torch.rand alpha (not normalised) @ the face's float32 triangle, colours SH2RGB(shs) * 255 in float64
+    (save_point_cloud truncates them to bytes).  -> (points float32 [F*K,3], colours float64 [F*K,3])."""
+    alpha = mesh._alpha.detach().cpu()
+    F, K = alpha.shape[0], alpha.shape[1]
+    triangles = mesh.vertices.detach().cpu()[mesh.faces.detach().cpu().long()].float()
+    xyz = torch.matmul(alpha, triangles).reshape(F * K, 3)
+    shs = np.random.RandomState(seed).random_sample((F * K, 3)) / 255.0
+    return xyz.numpy(), (shs * SH_C0 + 0.5) * 255
+
+
 SUPPORTED = {"blender": ("gs", "gs_flat", "gs_mesh"), "colmap": ("gs", "gs_flat")}
 
 

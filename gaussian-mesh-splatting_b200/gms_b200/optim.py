@@ -316,6 +316,40 @@ class FlatAdam:
     def zero_grad_partial(self, zero_end=None):
         (self.g if zero_end is None else self.g[:int(zero_end)]).zero_()
 
+    def step_dense(self, zero_end=None, skip=()):
+        """Single GPU: Adam on every group from a gradient the frame materialised in full, SH group included, whether or not
+        the optimizer was built sh_factored (a step whose frame did not apply the fused SH update).  skip as in step()."""
+        if self.world != 1:
+            raise ValueError("step_dense needs a single-GPU FlatAdam")
+        groups = range(len(self.groups))
+        if not self._step_groups(groups, zero_end, skip):
+            self._launch_runs(groups, 1 if zero_end is None else 2, 0 if zero_end is None else zero_end)
+
+    def state_dict(self) -> dict:
+        """Copies of the flat parameters and moments, the group shapes and the per-group step counts (single GPU)."""
+        if self.world != 1:
+            raise ValueError("FlatAdam.state_dict needs a single-GPU optimizer")
+        return {"p": self.p.detach().clone(), "m": self.m.detach().clone(), "v": self.v.detach().clone(), "steps": list(self.steps),
+                "shapes": [tuple(g["param"].shape) for g in self.groups]}
+
+    def load_state_dict(self, state: dict) -> None:
+        """Restores state_dict(); group shapes that differ from the current ones (a densified model) re-home the buffers
+        first.  The gradient is zeroed."""
+        if self.world != 1:
+            raise ValueError("FlatAdam.load_state_dict needs a single-GPU optimizer")
+        shapes = [tuple(s) for s in state["shapes"]]
+        if len(shapes) != len(self.groups):
+            raise ValueError(f"FlatAdam.load_state_dict: {len(shapes)} groups in the state, {len(self.groups)} here")
+        if shapes != [tuple(g["param"].shape) for g in self.groups]:
+            self.resize(shapes, lambda old, new: None)
+        if state["p"].numel() != self.p.numel() or state["m"].numel() != self.m.numel():
+            raise ValueError("FlatAdam.load_state_dict: the flat buffers do not match this optimizer's layout")
+        self.p.copy_(state["p"])
+        self.m.copy_(state["m"])
+        self.v.copy_(state["v"])
+        self.g.zero_()
+        self.steps = [int(s) for s in state["steps"]]
+
 
 def mesh_model_groups(model, lrs=REFERENCE_LRS, features_last: bool = False) -> List[dict]:
     """Parameter groups of a MeshGaussianModel with the reference's learning rates; the reference's order (vertices, alpha,

@@ -234,11 +234,15 @@ class MeshTrainer:
                     p.grad.mul_(1.0 / self.world)
 
     def step(self, cam: Camera, gt: torch.Tensor, loss_host: Optional[torch.Tensor] = None,
-             loss_ready: Optional[torch.cuda.Event] = None) -> torch.Tensor:
+             loss_ready: Optional[torch.cuda.Event] = None, bg: Optional[torch.Tensor] = None, before_update=None) -> torch.Tensor:
         """One optimisation step.  If `loss_host` (pinned) / `loss_ready` are given, the loss is copied to the host from a side
         stream as soon as the loss kernels have run (native frames: NativeFrame.read_loss_async; otherwise right after the
         backward pass, before the optimizer kernels are queued): a caller that logs the loss every step gets it while the
-        backward pass is still running and queues its next step in that time.  gt: float32 [3,H,W] or uint8 [H,W,3]."""
+        backward pass is still running and queues its next step in that time.  gt: float32 [3,H,W] or uint8 [H,W,3].
+        bg: this step's background instead of the trainer's (train.py's --random_background).  before_update: called after
+        the frame and before any parameter changes (train.py's training_report and Scene.save see the parameters before the
+        iteration's Adam step); the step then does not fuse the SH Adam update into the frame."""
+        bg = self.bg if bg is None else bg
         if self.native:
             if self._frame is None:
                 self._frame = NativeFrame(self.model, cam.image_width, cam.image_height, self.lambda_dssim, sync_free=self.sync_free,
@@ -246,13 +250,15 @@ class MeshTrainer:
             factored = self.sh_factored and self.optimizer_step      # without an optimizer step the full gradient is materialised
             # one GPU: the frame applies the SH Adam step itself (no colour-gradient slot, no second read of the SH rows);
             # data parallel: the colour gradients are exchanged first and k_adam_sh consumes them
-            fused = factored and self.world == 1
+            fused = factored and self.world == 1 and before_update is None
             sh_adam = self.opt.begin_fused_sh_step() if fused else None
-            loss = self._frame.run(cam, gt, self.bg, factored=factored and not fused, sh_adam=sh_adam)
+            loss = self._frame.run(cam, gt, bg, factored=factored and not fused, sh_adam=sh_adam)
             from . import rasterizer as _r
             _r.last_num_rendered = self._frame.last_num_rendered
             if loss_host is not None:
                 self._frame.read_loss_async(loss_host, loss_ready)
+            if before_update is not None:
+                before_update()
             self._all_reduce()
             # gms_train_frame overwrites every gradient except the atomically accumulated vertex segment (group 0)
             if fused:
@@ -270,7 +276,7 @@ class MeshTrainer:
         prev = _r.DIRECT_SH_GRAD
         _r.DIRECT_SH_GRAD = self.fast      # FlatAdam keeps .grad preallocated and zeroed: write dL/dshs in place
         try:
-            image, radii, _ = render_frame(self.model, cam, self.bg, fused=self.fast)
+            image, radii, _ = render_frame(self.model, cam, bg, fused=self.fast)
             loss = fused_training_loss(image, gt, self.lambda_dssim) if self.fast else self.loss_fn(image, gt, self.lambda_dssim)
             loss.backward()
         finally:
@@ -279,6 +285,8 @@ class MeshTrainer:
             loss_host.copy_(loss.detach().reshape(loss_host.shape), non_blocking=True)
             if loss_ready is not None:
                 loss_ready.record(torch.cuda.current_stream(loss.device))
+        if before_update is not None:
+            before_update()
         self._all_reduce()
         if self.optimizer_step:
             self.opt.step()
@@ -300,6 +308,19 @@ class MeshTrainer:
         if r is None or (r.W, r.H) != (W, H) or r.radii.shape[0] != self.model._scale.shape[0]:
             r = self._renderer = NativeRenderer(self.model, W, H)
         return r.evaluate(cams, gts, self.bg, protocol=protocol)
+
+    def state_dict(self) -> dict:
+        """What resuming needs (single GPU, fast=True): FlatAdam's flat parameters, moments and step counts, and the active
+        SH degree.  Copies on the device."""
+        if not self.fast:
+            raise ValueError("MeshTrainer.state_dict needs the FlatAdam trainer (fast=True)")
+        return {"adam": self.opt.state_dict(), "active_sh_degree": int(self.model.active_sh_degree)}
+
+    def load_state_dict(self, state: dict) -> None:
+        if not self.fast:
+            raise ValueError("MeshTrainer.load_state_dict needs the FlatAdam trainer (fast=True)")
+        self.opt.load_state_dict(state["adam"])
+        self.model.active_sh_degree = int(state["active_sh_degree"])
 
 
 # ---------------------------------------------------------------------------------------------- free Gaussians (gs, gs_flat)
@@ -501,6 +522,7 @@ class FreeTrainer:
         self.iteration = 0
         self.frame = None
         self._renderer = None
+        self._loaded_stats = None       # (accum, denom) of load_state_dict, until the first frame exists
         self.densifications = []        # (iteration, P before, result of the plan)
 
     def _xyz_lr(self, it: int) -> float:
@@ -517,7 +539,11 @@ class FreeTrainer:
         reset = it % o.opacity_reset_interval == 0 or (self.white_background and it == o.densify_from_iter)
         return True, densify, reset
 
-    def step(self, cam: Camera, gt: torch.Tensor) -> torch.Tensor:
+    def step(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor = None, before_update=None) -> torch.Tensor:
+        """One iteration.  bg: this step's background instead of the trainer's (train.py's --random_background).
+        before_update: called after the frame and before densify / opacity reset / Adam (train.py's training_report and
+        Scene.save see the parameters before the iteration's update); the step then does not fuse the SH Adam update into
+        the frame."""
         it = self.iteration + 1
         self.adam.groups[0]["lr"] = self._xyz_lr(it)
         if it % 1000 == 0:
@@ -525,20 +551,64 @@ class FreeTrainer:
         stats, densify, reset = self.schedule(it)
         if self.frame is None:
             self.frame = NativeFreeFrame(self.model, cam.image_width, cam.image_height, self.opt.lambda_dssim, sync_free=self.sync_free)
-        sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and not densify else None
-        loss = self.frame.run(cam, gt, self.bg, stats=stats, sh_adam=sh_adam)
+            if self._loaded_stats is not None:      # load_state_dict before the first frame existed
+                self.frame.accum.copy_(self._loaded_stats[0])
+                self.frame.denom.copy_(self._loaded_stats[1])
+                self._loaded_stats = None
+        sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and not densify and before_update is None else None
+        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, stats=stats, sh_adam=sh_adam)
+        if before_update is not None:
+            before_update()
         if densify:
             self.densify(size_prune=it > self.opt.opacity_reset_interval)
         if reset:
             self.reset_opacity()
         if not densify and it < self.opt.iterations:     # train.py steps the optimizer on every iteration but the last
             skip = ("opacity",) if reset else ()
-            if self.fused_sh:
+            if sh_adam is not None:
                 self.adam.step_rest(zero_end=0, skip=skip)
+            elif self.fused_sh:
+                self.adam.step_dense(zero_end=0, skip=skip)
             else:
                 self.adam.step(zero_end=0, skip=skip)
         self.iteration = it
         return loss
+
+    def state_dict(self) -> dict:
+        """What resuming needs: FlatAdam's flat parameters, moments, group shapes and step counts, the active SH degree, the
+        iteration, P, the frame's densification statistics and the split generator's state.  Copies on the device."""
+        dev = self.model._xyz.device
+        f = self.frame
+        if f is not None:
+            accum, denom = f.accum.detach().clone(), f.denom.detach().clone()
+        elif self._loaded_stats is not None:
+            accum, denom = (t.detach().clone() for t in self._loaded_stats)
+        else:
+            accum = torch.zeros(self.model.P, dtype=torch.float32, device=dev)
+            denom = torch.zeros(self.model.P, dtype=torch.float32, device=dev)
+        gen = self.generator.get_state() if self.generator is not None else torch.cuda.get_rng_state(dev)
+        return {"adam": self.adam.state_dict(), "active_sh_degree": int(self.model.active_sh_degree), "iteration": int(self.iteration),
+                "P": int(self.model.P), "accum": accum, "denom": denom, "generator": gen}
+
+    def load_state_dict(self, state: dict) -> None:
+        """Restores state_dict(), also when the state's P differs from the model's (densified before it was captured)."""
+        dev = self.model._xyz.device
+        self.adam.load_state_dict(state["adam"])
+        if self.model.P != int(state["P"]):
+            raise ValueError(f"FreeTrainer.load_state_dict: the state holds P = {state['P']} but its parameters {self.model.P}")
+        self.model.active_sh_degree = int(state["active_sh_degree"])
+        self.iteration = int(state["iteration"])
+        accum, denom = state["accum"].to(dev), state["denom"].to(dev)
+        if self.frame is not None:
+            self.frame.resize()
+            self.frame.accum.copy_(accum)
+            self.frame.denom.copy_(denom)
+        else:
+            self._loaded_stats = (accum, denom)
+        if self.generator is not None:
+            self.generator.set_state(state["generator"].cpu())
+        else:
+            torch.cuda.set_rng_state(state["generator"].cpu(), dev)
 
     def densify(self, size_prune: bool, normals: torch.Tensor = None) -> list:
         """densify_and_prune(densify_grad_threshold, min_opacity, extent, 20 if size_prune else None) on the statistics
