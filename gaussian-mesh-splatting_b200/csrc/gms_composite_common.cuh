@@ -45,8 +45,15 @@ __device__ __forceinline__ GmsTileGeom gms_tile_geom(int tile, int gx, int W, in
     return g;
 }
 
+// Rounding margin of the quad cull, relative to the term magnitude S = 0.5*(|cx| dx^2 + |cz| dy^2) + |cy dx dy| at the
+// evaluated point: 18 units of 2^-24 by the bound in DESIGN.md 3.4 (6 for this evaluation, 12 for the canonical power of a
+// pixel of the quad, whose S is at most 2 S + 2 S(7, 7)), rounded up to 24.
+#define GMS_CULL_REL 1.430511474609375e-6f
+
 // Can this splat reach alpha >= 1/255 anywhere in the pixel rectangle [rx0, rx0+7] x [ry0, ry0+7]?
-// i.e. min over the rectangle of 0.5*(cx dx^2 + cz dy^2) + cy dx dy  <=  tau   (tau carries the safety margin).
+// i.e. min over the rectangle of 0.5*(cx dx^2 + cz dy^2) + cy dx dy - GMS_CULL_REL * S  <=  tau   (tau carries the
+// exp / log margin and the constant part of the rounding bound).  Edge-on slivers have S up to ~1e9 where the form is < 10:
+// there the per-pixel power and this evaluation both carry rounding errors of thousands, which S bounds.
 __device__ __forceinline__ bool gms_reaches_quad(float x, float y, float cx, float cy, float cz, float tau, float rx0, float ry0) {
     if (!(tau > 0.f)) return false;                 // opacity < 1/255: never blends
     if (!(cx > 0.f) || !(cz > 0.f)) return true;    // degenerate conic: be conservative
@@ -60,13 +67,15 @@ __device__ __forceinline__ bool gms_reaches_quad(float x, float y, float cx, flo
             const float dy = y - (e ? ry1 : ry0);
             const float t = fminf(fmaxf(x + cy * dy * icx, rx0), rx1);
             const float dx = x - t;
-            best = fminf(best, 0.5f * (cx * dx * dx + cz * dy * dy) + cy * dx * dy);
+            const float h = 0.5f * (cx * dx * dx + cz * dy * dy), m = cy * dx * dy;
+            best = fminf(best, (h + m) - GMS_CULL_REL * (h + fabsf(m)));
         }
         {   // vertical edge
             const float dx = x - (e ? rx1 : rx0);
             const float t = fminf(fmaxf(y + cy * dx * icz, ry0), ry1);
             const float dy = y - t;
-            best = fminf(best, 0.5f * (cx * dx * dx + cz * dy * dy) + cy * dx * dy);
+            const float h = 0.5f * (cx * dx * dx + cz * dy * dy), m = cy * dx * dy;
+            best = fminf(best, (h + m) - GMS_CULL_REL * (h + fabsf(m)));
         }
     }
     return best <= tau;

@@ -385,9 +385,12 @@ k_preprocess_fwd(PreArgs a, int* __restrict__ radii, float4* __restrict__ rec, f
         rgb[0] = a.colors_pre[3 * i]; rgb[1] = a.colors_pre[3 * i + 1]; rgb[2] = a.colors_pre[3 * i + 2];
     }
     // tau' = ln(255 * opacity) + margin: a pixel can blend (alpha >= 1/255) only where 0.5 d^T Q d <= tau'.  The composite
-    // kernels test each tile quad against that ellipse before visiting the splat.  Margin: 1% + 0.1 covers the fp32
-    // cancellation error of the quadratic form for edge-on flat Gaussians (terms up to ~1e5).
-    const float tau = (o.opac >= GMS_ALPHA_MIN) ? 1.01f * logf(255.0f * o.opac) + 0.1f : -1.0f;
+    // kernels test each tile quad against that ellipse before visiting the splat (gms_reaches_quad).  Margin (DESIGN.md 3.4):
+    // 1% + 1e-3 for ex2.approx and logf; 1e-3 * (|cx| + |cz| + 2|cy|) for the rounding of the per-pixel power across the
+    // 7 x 7 px of a quad and for the cull's own edge minimiser.  The part that grows with the magnitude of the quadratic form's
+    // terms (edge-on slivers: up to ~1e9) is subtracted inside the cull, point by point.
+    const float tau = (o.opac >= GMS_ALPHA_MIN)
+        ? 1.01f * logf(255.0f * o.opac) + 1e-3f * (1.0f + fabsf(o.conx) + fabsf(o.conz) + 2.0f * fabsf(o.cony)) : -1.0f;
     rec[3 * (size_t)i] = make_float4(o.px, o.py, o.conx, o.cony);
     rec[3 * (size_t)i + 1] = make_float4(o.conz, o.opac, rgb[0], rgb[1]);
     rec[3 * (size_t)i + 2] = make_float4(rgb[2], GMS_DIVP(1.f, o.depth), tau, 0.f);

@@ -232,7 +232,10 @@ GMS_HD void gms_preprocess_backward_geom(const float* mean, const float* scale, 
     }
     const float dcx = gi.dconic[0], dcy = gi.dconic[1], dcz = gi.dconic[2];
     const float denom = det;
-    const float denom2inv = GMS_DIVP(1.0f, (denom * denom) + 0.0000001f);
+    // det^2 overflows to +inf for footprints beyond ~6e4 px; IEEE 1/inf = 0 then skips the conic term below.  The branch-free
+    // reciprocal is exact only for normal divisors (it gives NaN for inf), so the overflow is taken out by the select.
+    const float denom2 = (denom * denom) + 0.0000001f;
+    const float denom2inv = denom2 <= 3.402823466e+38f ? GMS_DIVP(1.0f, denom2) : 0.f;
     if (denom2inv != 0.f) {
         dL_da += denom2inv * (-c * c * dcx + 2.f * b * c * dcy + (denom - a * c) * dcz);
         dL_dc += denom2inv * (-a * a * dcz + 2.f * a * b * dcy + (denom - a * c) * dcx);

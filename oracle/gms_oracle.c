@@ -201,12 +201,22 @@ static inline float quad_power(const float* co, float dx, float dy) {
 static inline int imin(int a, int b) { return a < b ? a : b; }
 static inline int imax(int a, int b) { return a > b ? a : b; }
 
+/* float -> int32 with the device's cvt.rzi.s32.f32 semantics: truncate toward zero, saturate to [INT32_MIN, INT32_MAX],
+ * NaN -> 0.  A C cast is undefined outside the int32 range (x86 returns INT32_MIN at either end), so a radius beyond
+ * int32 or a rect bound of a centre far off-screen would otherwise disagree with the kernels for no reason of theirs. */
+int32_t gmso_f2i_sat(float v) {
+    if (v != v) return 0;
+    if (v >= 2147483648.0f) return INT32_MAX;
+    if (v <= -2147483648.0f) return INT32_MIN;
+    return (int32_t)v;
+}
+
 static inline void get_rect(float px, float py, int radius, int gx, int gy, int* rmin, int* rmax) {
     float r = (float)radius;
-    rmin[0] = imin(gx, imax(0, (int)((px - r) / (float)GMSO_BLOCK)));
-    rmin[1] = imin(gy, imax(0, (int)((py - r) / (float)GMSO_BLOCK)));
-    rmax[0] = imin(gx, imax(0, (int)((px + r + (float)(GMSO_BLOCK - 1)) / (float)GMSO_BLOCK)));
-    rmax[1] = imin(gy, imax(0, (int)((py + r + (float)(GMSO_BLOCK - 1)) / (float)GMSO_BLOCK)));
+    rmin[0] = imin(gx, imax(0, gmso_f2i_sat((px - r) / (float)GMSO_BLOCK)));
+    rmin[1] = imin(gy, imax(0, gmso_f2i_sat((py - r) / (float)GMSO_BLOCK)));
+    rmax[0] = imin(gx, imax(0, gmso_f2i_sat((px + r + (float)(GMSO_BLOCK - 1)) / (float)GMSO_BLOCK)));
+    rmax[1] = imin(gy, imax(0, gmso_f2i_sat((py + r + (float)(GMSO_BLOCK - 1)) / (float)GMSO_BLOCK)));
 }
 
 /* SH basis, utils/sh_utils.py:74-100 (degree <= 3) */
@@ -325,7 +335,7 @@ int gmso_preprocess_forward(const gmso_settings* s,
         float mid = 0.5f * (a + c);
         float disc = sqrtf(fmaxf(0.1f, fmaf(mid, mid, -det)));
         float lambda1 = mid + disc, lambda2 = mid - disc;
-        int my_radius = (int)ceilf(3.f * sqrtf(fmaxf(lambda1, lambda2)));
+        int my_radius = gmso_f2i_sat(ceilf(3.f * sqrtf(fmaxf(lambda1, lambda2))));
         float pixx = fmaf(pprojx + 1.0f, (float)W, -1.0f) * 0.5f;
         float pixy = fmaf(pprojy + 1.0f, (float)H, -1.0f) * 0.5f;
         int rmin[2], rmax[2];

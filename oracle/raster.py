@@ -53,7 +53,14 @@ def lib():
         _lib = ctypes.CDLL(_LIB_PATH)
         _lib.gmso_bin.restype = ctypes.c_int64
         _lib.gmso_num_threads.restype = ctypes.c_int
+        _lib.gmso_f2i_sat.restype = ctypes.c_int32
+        _lib.gmso_f2i_sat.argtypes = [ctypes.c_float]
     return _lib
+
+
+def f2i_sat(v: float) -> int:
+    """The oracle's float -> int32 conversion (device cvt.rzi.s32.f32 semantics: saturating, NaN -> 0)."""
+    return int(lib().gmso_f2i_sat(float(v)))
 
 
 def num_threads() -> int:
