@@ -22,6 +22,7 @@
 #include "gms_image.cuh"
 #include "gms_free.cuh"
 #include "gms_knn.cuh"
+#include "gms_flame.cuh"
 
 // ------------------------------------------------------------------------------------------ host state
 static thread_local char g_err[512] = "";
@@ -2606,6 +2607,92 @@ int gms_knn_dist2(const gms_knn_args* a, void* cuda_stream) {
     GMS_AFTER_LAUNCH("knn_box_bounds", 0, st);
     k_knn_search<<<nbox, GMS_KNN_BOX, 0, st>>>(P, nbox, L.sorted, L.blo, L.bhi, a->dist2);
     GMS_AFTER_LAUNCH("knn_search", 0, st);
+    span_end(st);
+    return GMS_OK;
+}
+
+// ------------------------------------------------------------------------------------------ FLAME linear blend skinning
+
+size_t gms_flame_lbs_workspace_bytes(int32_t V) {
+    if (V <= 0) return 0;
+    return gms_flame_ws(nullptr, V).floats * sizeof(float) + 256;
+}
+
+static int flame_lbs_check(const gms_flame_lbs_args* a, bool backward) {
+    if (!a) return set_err(GMS_E_ARG, "gms_flame_lbs: null argument%s%s");
+    if (a->V <= 0 || a->n_shape < 0 || a->n_shape > 300 || a->n_exp < 0 || a->n_exp > 100)
+        return set_err(GMS_E_ARG, "gms_flame_lbs: need V > 0, 0 <= n_shape <= 300, 0 <= n_exp <= 100%s%s");
+    if (a->n_joints != GMS_FLAME_NJ || a->parents[0] != -1)
+        return set_err(GMS_E_ARG, "gms_flame_lbs: need 5 joints with parents[0] = -1%s%s");
+    for (int j = 1; j < GMS_FLAME_NJ; j++)
+        if (a->parents[j] < 0 || a->parents[j] >= j) return set_err(GMS_E_ARG, "gms_flame_lbs: need 0 <= parents[j] < j%s%s");
+    const int B = a->n_shape + a->n_exp;
+    const void* need[] = {a->v_template, a->posedirs, a->J_regressor, a->lbs_weights, a->pose, a->neck_pose, a->transl,
+                          a->enlargement, a->workspace};
+    for (const void* p : need)
+        if (!p || (reinterpret_cast<size_t>(p) & 3)) return set_err(GMS_E_ARG, "gms_flame_lbs: null or misaligned pointer%s%s");
+    const void* opt[] = {a->shapedirs, a->shape, a->expression, a->vertices_grad};
+    for (const void* p : opt)
+        if (reinterpret_cast<size_t>(p) & 3) return set_err(GMS_E_ARG, "gms_flame_lbs: misaligned pointer%s%s");
+    if ((B > 0 && !a->shapedirs) || (a->n_shape > 0 && !a->shape) || (a->n_exp > 0 && !a->expression))
+        return set_err(GMS_E_ARG, "gms_flame_lbs: null shape or expression pointer%s%s");
+    if (a->workspace_bytes < gms_flame_lbs_workspace_bytes(a->V)) return set_err(GMS_E_ARG, "gms_flame_lbs: workspace too small%s%s");
+    if (!backward) {
+        if (!a->vertices || (reinterpret_cast<size_t>(a->vertices) & 3)) return set_err(GMS_E_ARG, "gms_flame_lbs: null or misaligned vertices%s%s");
+        return GMS_OK;
+    }
+    float* const g[] = {a->d_pose, a->d_neck_pose, a->d_transl, a->d_enlargement, a->vertices_grad};
+    for (float* p : g)
+        if (!p || (reinterpret_cast<size_t>(p) & 3)) return set_err(GMS_E_ARG, "gms_flame_lbs: null or misaligned gradient pointer%s%s");
+    if ((a->n_shape > 0 && (!a->d_shape || (reinterpret_cast<size_t>(a->d_shape) & 3))) ||
+        (a->n_exp > 0 && (!a->d_expression || (reinterpret_cast<size_t>(a->d_expression) & 3))))
+        return set_err(GMS_E_ARG, "gms_flame_lbs: null or misaligned shape / expression gradient%s%s");
+    return GMS_OK;
+}
+
+int gms_flame_lbs_forward(const gms_flame_lbs_args* a, void* cuda_stream) {
+    const int rc = flame_lbs_check(a, false);
+    if (rc != GMS_OK) return rc;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    const int V = a->V;
+    const int nsb = (V + GMS_FLAME_SB - 1) / GMS_FLAME_SB, nvb = (V + GMS_FLAME_VB - 1) / GMS_FLAME_VB;
+    GmsFlameWs w = gms_flame_ws(reinterpret_cast<float*>(aligned_base_c(a->workspace)), V);
+    GmsFlameParents par;
+    for (int j = 0; j < GMS_FLAME_NJ; j++) par.p[j] = a->parents[j];
+    span_begin(K_MISC, st);
+    k_flame_shape<<<nsb, 3 * GMS_FLAME_SB, 0, st>>>(V, a->n_shape, a->n_exp, a->v_template, a->shapedirs, a->shape, a->expression,
+                                                    a->J_regressor, w.vs, w.jpart);
+    GMS_AFTER_LAUNCH("flame_shape", 0, st);
+    k_flame_joints<<<1, 128, 0, st>>>(nsb, w.jpart, a->pose, a->neck_pose, par, w.J, w.state);
+    GMS_AFTER_LAUNCH("flame_joints", 0, st);
+    k_flame_skin<<<nvb, GMS_FLAME_VB, 0, st>>>(V, w.vs, a->posedirs, a->lbs_weights, a->transl, a->enlargement, w.state, w.vp,
+                                               a->vertices, a->vertices_grad);
+    GMS_AFTER_LAUNCH("flame_skin", 0, st);
+    span_end(st);
+    return GMS_OK;
+}
+
+int gms_flame_lbs_backward(const gms_flame_lbs_args* a, void* cuda_stream) {
+    const int rc = flame_lbs_check(a, true);
+    if (rc != GMS_OK) return rc;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    const int V = a->V, B = a->n_shape + a->n_exp;
+    const int nvb = (V + GMS_FLAME_VB - 1) / GMS_FLAME_VB;
+    GmsFlameWs w = gms_flame_ws(reinterpret_cast<float*>(aligned_base_c(a->workspace)), V);
+    GmsFlameParents par;
+    for (int j = 0; j < GMS_FLAME_NJ; j++) par.p[j] = a->parents[j];
+    span_begin(K_MISC, st);
+    k_flame_skin_bwd<<<nvb, GMS_FLAME_VB, 0, st>>>(V, w.vp, a->posedirs, a->lbs_weights, a->transl, a->enlargement, w.state,
+                                                   a->vertices_grad, a->d_enlargement, w.dvp, w.bpart);
+    GMS_AFTER_LAUNCH("flame_skin_bwd", 0, st);
+    k_flame_joints_bwd<<<1, 128, 0, st>>>(nvb, w.bpart, a->pose, a->neck_pose, par, w.J, w.state, a->d_pose, a->d_neck_pose,
+                                          a->d_transl, w.dJ);
+    GMS_AFTER_LAUNCH("flame_joints_bwd", 0, st);
+    if (B > 0) {
+        k_flame_betas_bwd<<<B, GMS_FLAME_CB, 0, st>>>(V, a->n_shape, a->shapedirs, a->J_regressor, w.dvp, w.dJ, a->d_shape,
+                                                      a->d_expression);
+        GMS_AFTER_LAUNCH("flame_betas_bwd", 0, st);
+    }
     span_end(st);
     return GMS_OK;
 }

@@ -264,6 +264,19 @@ class KnnArgs(C.Structure):
     _fields_ = [("P", C.c_int32), ("points", C.c_void_p), ("dist2", C.c_void_p), ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t)]
 
 
+FLAME_JOINTS = 5    # GMS_FLAME_JOINTS
+
+
+class FlameLbsArgs(C.Structure):
+    """struct gms_flame_lbs_args"""
+    _fields_ = [("V", C.c_int32), ("n_shape", C.c_int32), ("n_exp", C.c_int32), ("n_joints", C.c_int32),
+                ("parents", C.c_int32 * FLAME_JOINTS)] + \
+               [(n, C.c_void_p) for n in ("v_template", "shapedirs", "posedirs", "J_regressor", "lbs_weights", "shape", "expression",
+                                          "pose", "neck_pose", "transl", "enlargement", "vertices", "vertices_grad", "d_shape",
+                                          "d_expression", "d_pose", "d_neck_pose", "d_transl", "d_enlargement", "workspace")] + \
+               [("workspace_bytes", C.c_size_t)]
+
+
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_int, C.c_size_t)
 
 # every symbol include/gms_b200.h declares (tests/test_abi.py checks the library exports all of them)
@@ -278,7 +291,8 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_pseudomesh_bind", "gms_pseudomesh_repose", "gms_bound_points_render_workspace_bytes",
                "gms_bound_points_render_frame", "gms_free_train_frame", "gms_free_render_frame", "gms_densify_scratch_bytes",
                "gms_densify_plan", "gms_densify_apply", "gms_knn_scratch_bytes", "gms_knn_dist2",
-               "gms_flame_render_workspace_bytes", "gms_flame_render_frame", "gms_image_composite_rgba", "gms_image_resize_u8"]
+               "gms_flame_render_workspace_bytes", "gms_flame_render_frame", "gms_image_composite_rgba", "gms_image_resize_u8",
+               "gms_flame_lbs_workspace_bytes", "gms_flame_lbs_forward", "gms_flame_lbs_backward"]
 
 _lib = None
 
@@ -356,6 +370,10 @@ def lib():
     L.gms_knn_scratch_bytes.restype = C.c_size_t
     L.gms_knn_scratch_bytes.argtypes = [C.c_int32]
     L.gms_knn_dist2.argtypes = [C.POINTER(KnnArgs), C.c_void_p]
+    L.gms_flame_lbs_workspace_bytes.restype = C.c_size_t
+    L.gms_flame_lbs_workspace_bytes.argtypes = [C.c_int32]
+    L.gms_flame_lbs_forward.argtypes = [C.POINTER(FlameLbsArgs), C.c_void_p]
+    L.gms_flame_lbs_backward.argtypes = [C.POINTER(FlameLbsArgs), C.c_void_p]
     L.gms_metrics_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]
     L.gms_image_metrics.argtypes = [C.POINTER(MetricsArgs), C.c_void_p]
     _lib = L

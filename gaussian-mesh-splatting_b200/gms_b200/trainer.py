@@ -22,6 +22,7 @@ import torch.distributed as dist
 import diff_gaussian_rasterization as dgr
 
 from .capacity import SyncFreeCapacity, grow_only_alloc
+from .flame import NativeFlame
 from .io_image import GroundTruthBuffer
 from .losses import fused_training_loss
 from .model import MeshGaussianModel
@@ -695,6 +696,9 @@ class FlameTrainer:
         weights on the detached vertices -> dL/dvertices back through the driver (torch.autograd.backward) -> Adam over the
         reference's groups (FlatAdam; the SH step fused into the frame when M = 16).
 
+    With a NativeFlame driver there is no autograd graph: gms_flame_lbs_forward writes model.vertices, and
+    gms_flame_lbs_backward writes the FLAME gradients into FlatAdam's slots (no host synchronisation after the first step).
+
     No densification (train.py densifies gs / gs_flat only), a constant learning rate per group (update_learning_rate is a
     no-op, gaussian_flame_model.py:226-228), and no optimizer step at the last iteration.  After step(), model.vertices
     holds the pose the step rendered, not the updated parameters' (model.refresh_vertices() moves it; evaluate() does)."""
@@ -708,22 +712,32 @@ class FlameTrainer:
         self.iteration = 0
         self.frame = None
         self._renderer = None
+        self._lbs = None
 
     def step(self, cam: Camera, gt: torch.Tensor) -> torch.Tensor:
         it = self.iteration + 1
         m = self.model
         if it % 1000 == 0:
             m.oneupSHdegree()
-        verts = m.driver_vertices()
-        with torch.no_grad():
-            m.vertices.copy_(verts)
-        m.vertices.grad.zero_()
+        native = isinstance(m.driver, NativeFlame)
+        if native:
+            if self._lbs is None:
+                self._lbs = m.driver.bind(m)
+            self._lbs.forward()                  # into model.vertices; zeroes model.vertices.grad
+        else:
+            verts = m.driver_vertices()
+            with torch.no_grad():
+                m.vertices.copy_(verts)
+            m.vertices.grad.zero_()
         if self.frame is None:
             self.frame = NativeFrame(m, cam.image_width, cam.image_height, self.opt.lambda_dssim, sync_free=self.sync_free)
         take_step = it < self.opt.iterations         # train.py steps the optimizer on every iteration but the last
         sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and take_step else None
         loss = self.frame.run(cam, gt, self.bg, sh_adam=sh_adam)
-        torch.autograd.backward(verts, m.vertices.grad)      # accumulates into the FLAME tensors' flat .grad views
+        if native:
+            self._lbs.backward()                 # writes the FLAME tensors' flat .grad views
+        else:
+            torch.autograd.backward(verts, m.vertices.grad)      # accumulates into the FLAME tensors' flat .grad views
         if not take_step:
             self.adam.zero_grad()
         elif self.fused_sh:

@@ -663,6 +663,52 @@ typedef struct gms_knn_args {
 size_t gms_knn_scratch_bytes(int32_t P);
 int gms_knn_dist2(const gms_knn_args* a, void* cuda_stream);
 
+/* ---- FLAME's vertex model (gs_flame) ----------------------------------------------------------- */
+
+/* FLAME.forward's vertices (games/flame_splatting/FLAME/FLAME.py:204-248 with smplx.lbs.lbs, landmarks left out) followed by
+ * transform_vertices_function (games/flame_splatting/scene/dataset_readers.py:40-45), for one frame:
+ *   betas    = [shape, expression] (the active columns; the reference's zero-padded ones contribute nothing)
+ *   v_shaped = v_template + shapedirs^T betas;  J = J_regressor . v_shaped
+ *   R_j      = batch_rodrigues(full_pose_j), full_pose = [pose[:3], neck_pose, pose[3:], eye_pose = 0]
+ *   v_posed  = v_shaped + ((R_1..4 - I) flattened) . posedirs
+ *   A_j      = batch_rigid_transform's relative transforms over `parents`
+ *   o        = (sum_j lbs_weights[v,j] A_j) [v_posed, 1] + transl
+ *   vertices = (o_x, -o_z, o_y) * enlargement
+ * Forward: three launches; writes `vertices` and zeroes `vertices_grad` when that is not NULL.  Backward: three launches; reads
+ * dL/dvertices from `vertices_grad` and WRITES (does not accumulate) the six parameter gradients.  The backward reads the
+ * workspace the forward filled, so it must follow a forward with the same arguments.  Fixed-order reductions, no float
+ * atomics: the same inputs give the same bits.  GMS_E_ARG before any launch: n_joints != 5, parents[0] != -1 or
+ * parents[j] not in [0, j), V <= 0, n_shape outside [0, 300], n_exp outside [0, 100], a null or non-4-byte-aligned
+ * pointer that the call reads or writes, or a short workspace.  Caller's stream, no host synchronisation. */
+#define GMS_FLAME_JOINTS 5
+typedef struct gms_flame_lbs_args {
+    int32_t V, n_shape, n_exp, n_joints;
+    int32_t parents[GMS_FLAME_JOINTS];  /* kintree_table[0] with parents[0] = -1 */
+    const float* v_template;     /* [V,3] */
+    const float* shapedirs;      /* [n_shape + n_exp, 3V]: the active columns of FLAME's [V,3,400], packed row-major */
+    const float* posedirs;       /* [36, 3V] (FLAME.__init__'s layout) */
+    const float* J_regressor;    /* [5, V] dense */
+    const float* lbs_weights;    /* [V, 5] */
+    const float* shape;          /* [n_shape] */
+    const float* expression;     /* [n_exp] */
+    const float* pose;           /* [6]: global rotation, jaw */
+    const float* neck_pose;      /* [3] */
+    const float* transl;         /* [3] */
+    const float* enlargement;    /* [V,3] _vertices_enlargement */
+    float* vertices;             /* [V,3] forward output */
+    float* vertices_grad;        /* [V,3] forward: zeroed (may be NULL); backward: dL/dvertices */
+    float* d_shape;              /* [n_shape] */
+    float* d_expression;         /* [n_exp] */
+    float* d_pose;               /* [6] */
+    float* d_neck_pose;          /* [3] */
+    float* d_transl;             /* [3] */
+    float* d_enlargement;        /* [V,3] */
+    void* workspace; size_t workspace_bytes;   /* gms_flame_lbs_workspace_bytes(V) */
+} gms_flame_lbs_args;
+size_t gms_flame_lbs_workspace_bytes(int32_t V);
+int gms_flame_lbs_forward(const gms_flame_lbs_args* a, void* cuda_stream);
+int gms_flame_lbs_backward(const gms_flame_lbs_args* a, void* cuda_stream);
+
 /* Scores an image against its ground truth, forward only, deterministically (per-tile partial sums added in a fixed order in
  * double, no atomics: the same inputs give the same bits).  Both images go through the same transform first:
  *   quantize 0: clamp to [0,1]                                  (training_report, train.py:203-204)
