@@ -121,7 +121,7 @@ static int set_err(int code, const char* fmt, const char* a = "", const char* b 
 
 static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
-static inline void* aligned_base_c(void* p) { return reinterpret_cast<void*>(align_up(reinterpret_cast<size_t>(p))); }
+static inline void* aligned_base(void* p) { return reinterpret_cast<void*>(align_up(reinterpret_cast<size_t>(p))); }
 
 template <typename T>
 static T* carve(char*& p, size_t count) {
@@ -1253,16 +1253,29 @@ extern "C" int gms_loss_scratch_bytes(int32_t C, int32_t H, int32_t W, size_t* b
 
 // ------------------------------------------------------------------------------------------ whole-frame orchestration
 
+// The workspace of a forward-only frame: the activated Gaussians an expansion step writes, and sigmoid(opacity).
+struct RenderLayout { float* xyz; float* scales; float* rots; float* opac; size_t total; };
+
+static RenderLayout render_layout(void* base, int P) {
+    RenderLayout L;
+    char* p = reinterpret_cast<char*>(base);
+    const size_t Pn = (size_t)(P > 0 ? P : 1);
+    L.xyz = carve<float>(p, 3 * Pn); L.scales = carve<float>(p, 3 * Pn); L.rots = carve<float>(p, 4 * Pn); L.opac = carve<float>(p, Pn);
+    L.total = (size_t)(p - reinterpret_cast<char*>(base));
+    return L;
+}
+
+// The workspace of a training frame: a forward-only frame's, then the frame's own outputs, gradients and loss scratch.
 struct FrameLayout {
-    float* xyz; float* scales; float* rots; float* opac; int32_t* radii; float* image; float* invdepth; float* dimage;
+    RenderLayout g; int32_t* radii; float* image; float* invdepth; float* dimage;
     float* d_xyz; float* d_m2d; float* d_opac; float* d_scales; float* d_rots; float* loss_scratch; size_t loss_bytes; size_t total;
 };
 
 static FrameLayout frame_layout(void* base, int P, int W, int H) {
     FrameLayout L;
-    char* p = reinterpret_cast<char*>(base);
+    L.g = render_layout(base, P);
+    char* p = reinterpret_cast<char*>(base) + L.g.total;
     const size_t Pn = (size_t)(P > 0 ? P : 1), HW = (size_t)W * H;
-    L.xyz = carve<float>(p, 3 * Pn); L.scales = carve<float>(p, 3 * Pn); L.rots = carve<float>(p, 4 * Pn); L.opac = carve<float>(p, Pn);
     L.radii = carve<int32_t>(p, Pn);
     L.image = carve<float>(p, 3 * HW); L.invdepth = carve<float>(p, HW); L.dimage = carve<float>(p, 3 * HW);
     L.d_xyz = carve<float>(p, 3 * Pn); L.d_m2d = carve<float>(p, 3 * Pn); L.d_opac = carve<float>(p, Pn);
@@ -1299,7 +1312,7 @@ int gms_l1_ssim_loss(const gms_loss_args* a, void* cuda_stream) {
     size_t need = 0;
     gms_loss_scratch_bytes(C, H, W, &need);
     if (a->scratch_bytes < need) return set_err(GMS_E_ARG, "gms_l1_ssim_loss: scratch too small%s%s");
-    char* base = reinterpret_cast<char*>(aligned_base_c(a->scratch));
+    char* base = reinterpret_cast<char*>(aligned_base(a->scratch));
     float* acc = reinterpret_cast<float*>(base);
     float* dmap = reinterpret_cast<float*>(base + 256);
     const GmsGaussWin win = ssim_window();
@@ -1339,7 +1352,7 @@ int gms_image_metrics(const gms_metrics_args* a, void* cuda_stream) {
     int rc = gms_metrics_scratch_bytes(C, H, W, &need);
     if (rc) return rc;
     if (a->scratch_bytes < need) return set_err(GMS_E_ARG, "gms_image_metrics: scratch too small%s%s");
-    float* part = reinterpret_cast<float*>(aligned_base_c(a->scratch));
+    float* part = reinterpret_cast<float*>(aligned_base(a->scratch));
     const GmsGaussWin win = ssim_window();
     dim3 grid((W + GMS_SSIM_T - 1) / GMS_SSIM_T, (H + GMS_SSIM_T - 1) / GMS_SSIM_T, C);
     span_begin(K_METRICS, st);
@@ -1461,8 +1474,8 @@ int gms_adam_sh_factored(const gms_adam_sh_args* a, void* cuda_stream) {
 
 int gms_frame_views(void* workspace, int32_t P, int32_t W, int32_t H, gms_frame_view* v) {
     if (!workspace || !v) return set_err(GMS_E_ARG, "gms_frame_views: null argument%s%s");
-    FrameLayout FL = frame_layout(aligned_base_c(workspace), P, W, H);
-    v->xyz = FL.xyz; v->scales = FL.scales; v->rotations = FL.rots; v->opacities = FL.opac; v->radii = FL.radii;
+    FrameLayout FL = frame_layout(aligned_base(workspace), P, W, H);
+    v->xyz = FL.g.xyz; v->scales = FL.g.scales; v->rotations = FL.g.rots; v->opacities = FL.g.opac; v->radii = FL.radii;
     v->image = FL.image; v->invdepth = FL.invdepth;
     return GMS_OK;
 }
@@ -1541,7 +1554,30 @@ static PreArgs make_pre_args(const gms_raster_settings* s, const gms_raster_inpu
     return a;
 }
 
-static void* aligned_base(void* p) { return reinterpret_cast<void*>(align_up(reinterpret_cast<size_t>(p))); }
+// The end of a forward with a binned point list: tiles in launch order, then the composite forward, which writes the
+// per-quad survivor lists to `surv` when `emit`.
+static int composite_forward(const gms_raster_settings* s, const gms_raster_outputs* out, const ImageLayout& IL, const float4* rec,
+                             const uint32_t* point_list, bool emit, uint32_t* surv, int T, cudaStream_t st) {
+    const int W = s->image_width, H = s->image_height, gx = (W + GMS_TILE - 1) / GMS_TILE;
+    const int dbg = s->debug;
+    if (g_opt_tile_order) {
+        k_tile_order<<<1, 1024, 0, st>>>(T, IL.ranges, IL.tile_order);
+        GMS_AFTER_LAUNCH("tile_order", dbg, st);
+    }
+    span_begin(K_COMP_FWD, st);
+    if (g_opt_fwd == 3)
+        k_composite_fwd3<<<T, GMS_CB, 0, st>>>(IL.ranges, g_opt_tile_order ? IL.tile_order : nullptr, point_list, rec, W, H, gx, s->bg,
+                                              out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth);
+    else if (emit)
+        k_composite_fwd2<true><<<T, GMS_CB, 0, st>>>(IL.ranges, g_opt_tile_order ? IL.tile_order : nullptr, point_list, rec, W, H, gx, s->bg,
+                                                    out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth, surv, IL.nsurv);
+    else
+        k_composite_fwd2<false><<<T, GMS_CB, 0, st>>>(IL.ranges, g_opt_tile_order ? IL.tile_order : nullptr, point_list, rec, W, H, gx, s->bg,
+                                                     out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth, nullptr, nullptr);
+    GMS_AFTER_LAUNCH("composite_fwd", dbg, st);
+    span_end(st);
+    return GMS_OK;
+}
 
 // nosync_capacity > 0: never synchronise with the host -- the binning region is requested for that many duplicates, N stays
 // on the device (and, when n_host is given, is mirrored into mapped pinned host memory by the kernel that computes it).
@@ -1661,22 +1697,7 @@ static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_in
             GMS_CUDA(cudaLaunchCooperativeKernel((void*)k_bin_tiles, dim3(G), dim3(GMS_BIN_THREADS), kargs, bin_smem, st));
             GMS_AFTER_LAUNCH("bin_tiles", dbg, st);
             span_end(st);
-            if (g_opt_tile_order) {
-                k_tile_order<<<1, 1024, 0, st>>>(T, IL.ranges, IL.tile_order);
-                GMS_AFTER_LAUNCH("tile_order", dbg, st);
-            }
-            span_begin(K_COMP_FWD, st);
-            if (g_opt_fwd == 3)
-                k_composite_fwd3<<<T, GMS_CB, 0, st>>>(IL.ranges, g_opt_tile_order ? IL.tile_order : nullptr, point_list, GL.rec, W, H, gx, s->bg,
-                                                      out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth);
-            else if (emit)
-                k_composite_fwd2<true><<<T, GMS_CB, 0, st>>>(IL.ranges, g_opt_tile_order ? IL.tile_order : nullptr, point_list, GL.rec, W, H, gx, s->bg,
-                                                            out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth, surv, IL.nsurv);
-            else
-                k_composite_fwd2<false><<<T, GMS_CB, 0, st>>>(IL.ranges, g_opt_tile_order ? IL.tile_order : nullptr, point_list, GL.rec, W, H, gx, s->bg,
-                                                             out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth, nullptr, nullptr);
-            GMS_AFTER_LAUNCH("composite_fwd", dbg, st);
-            span_end(st);
+            return composite_forward(s, out, IL, GL.rec, point_list, emit, surv, T, st);
         } else {
             const size_t HW = (size_t)W * H;
             k_fill_background<<<(unsigned)((HW + 255) / 256), 256, 0, st>>>(W, H, s->bg, out->out_color, out->out_invdepth);
@@ -1755,22 +1776,7 @@ static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_in
         else k_tile_ranges<uint32_t><<<(unsigned)((cap + 255) / 256), 256, 0, st>>>(cap, BL.keys_out, IL.ranges, (uint32_t)T, GL.offs + (P - 1), GL.counters, n_host);
         GMS_AFTER_LAUNCH("tile_ranges", dbg, st);
         span_end(st);
-        if (g_opt_tile_order) {
-            k_tile_order<<<1, 1024, 0, st>>>(T, IL.ranges, IL.tile_order);
-            GMS_AFTER_LAUNCH("tile_order", dbg, st);
-        }
-        span_begin(K_COMP_FWD, st);
-        if (g_opt_fwd == 3)
-            k_composite_fwd3<<<T, GMS_CB, 0, st>>>(IL.ranges, g_opt_tile_order ? IL.tile_order : nullptr, BL.vals_out, GL.rec, W, H, gx, s->bg,
-                                                  out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth);
-        else if (emit)
-            k_composite_fwd2<true><<<T, GMS_CB, 0, st>>>(IL.ranges, g_opt_tile_order ? IL.tile_order : nullptr, BL.vals_out, GL.rec, W, H, gx, s->bg,
-                                                        out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth, BL.surv, IL.nsurv);
-        else
-            k_composite_fwd2<false><<<T, GMS_CB, 0, st>>>(IL.ranges, g_opt_tile_order ? IL.tile_order : nullptr, BL.vals_out, GL.rec, W, H, gx, s->bg,
-                                                         out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth, nullptr, nullptr);
-        GMS_AFTER_LAUNCH("composite_fwd", dbg, st);
-        span_end(st);
+        return composite_forward(s, out, IL, GL.rec, BL.vals_out, emit, BL.surv, T, st);
     } else {
         const size_t HW = (size_t)W * H;
         k_fill_background<<<(unsigned)((HW + 255) / 256), 256, 0, st>>>(W, H, s->bg, out->out_color, out->out_invdepth);
@@ -2023,8 +2029,8 @@ int gms_expand_backward(const gms_expand_args* a, const gms_expand_grads* g, voi
 size_t gms_frame_workspace_bytes(int32_t P, int32_t W, int32_t H) { return frame_layout(nullptr, P, W, H).total + 512; }
 
 // A whole frame's forward is the model's own expansion step followed by one rasterizer forward, frame_raster_forward, which
-// gms_train_frame, gms_render_frame and gms_points_render_frame share.  The expansion writes activated Gaussians (xyz,
-// scales, unit quaternions) into the frame's workspace.
+// every one-call frame shares.  The expansion writes activated Gaussians (xyz, scales, unit quaternions) into the frame's
+// workspace.
 struct FrameModel {
     int32_t V, F, K, M;
     const float* vertices; const int64_t* faces; const float* alpha_raw; const float* scale_raw; const float* features;
@@ -2115,67 +2121,95 @@ static int frame_raster_forward(const FrameGaussians& g, const gms_raster_settin
     return raster_forward_impl(s, in, out, alloc, user, saved, cuda_stream, binning_capacity, n_host, g.opacity_raw);
 }
 
-struct RenderLayout { float* xyz; float* scales; float* rots; float* opac; size_t total; };
-
-static RenderLayout render_layout(void* base, int P) {
-    RenderLayout L;
-    char* p = reinterpret_cast<char*>(base);
-    const size_t Pn = (size_t)(P > 0 ? P : 1);
-    L.xyz = carve<float>(p, 3 * Pn); L.scales = carve<float>(p, 3 * Pn); L.rots = carve<float>(p, 4 * Pn); L.opac = carve<float>(p, Pn);
-    L.total = (size_t)(p - reinterpret_cast<char*>(base));
-    return L;
-}
-
 size_t gms_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { (void)W; (void)H; return render_layout(nullptr, P).total + 512; }
 
-int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
-    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii) return set_err(GMS_E_ARG, "gms_render_frame: null argument%s%s");
-    if (!a->vertices || !a->faces || !a->alpha_raw || !a->scale_raw || !a->features || !a->opacity_raw)
-        return set_err(GMS_E_ARG, "gms_render_frame: model tensors required%s%s");
-    const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps,
-                          a->segments, a->n_segments, a->alpha_activation};
+extern "C++" {      // templates need C++ linkage
+
+// A forward-only frame around the model's own checks and expansion step: the output checks; check_model(&P), which checks
+// the model and gives its Gaussian count; the workspace check; expand(P, RL, &xyz) into the render layout (free Gaussians
+// point xyz at the model's own centres); one rasterizer forward; num_rendered.  Every gms_*_render_args names its
+// settings, output, workspace and capacity fields alike.
+template <typename Args, typename CheckModel, typename Expand>
+static int render_frame(const char* fn, const Args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream, CheckModel check_model,
+                        Expand expand) {
+    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii) return set_err(GMS_E_ARG, "%s: null argument%s", fn);
     int P, rc;
-    if ((rc = frame_gaussian_count("gms_render_frame", m, &P))) return rc;
-    const int W = a->settings.image_width, H = a->settings.image_height;
-    if (a->workspace_bytes < gms_render_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_render_frame: workspace too small%s%s");
-    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
+    if ((rc = check_model(&P))) return rc;
+    if (a->workspace_bytes < gms_render_workspace_bytes(P, a->settings.image_width, a->settings.image_height))
+        return set_err(GMS_E_ARG, "%s: workspace too small%s", fn);
+    const RenderLayout RL = render_layout(aligned_base(a->workspace), P);
+    const float* xyz = RL.xyz;
+    if ((rc = expand(P, RL, &xyz))) return rc;
     gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
-    std::vector<gms_expand_args> ea;
     gms_raster_inputs in;
     gms_raster_saved saved;
-    if ((rc = mesh_expand_forward(m, RL.xyz, RL.scales, RL.rots, cuda_stream, &ea))) return rc;
-    const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
+    const FrameGaussians g = {P, a->M, xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
     if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
                                    &saved))) return rc;
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;
     return GMS_OK;
+}
+
+// What both training frames do after their forward: the L1+SSIM loss and dL/dimage, event_loss_ready, then the rasterizer
+// backward into the workspace's gradients, dL/dmeans3D into d_xyz.  dL/dshs goes to d_features; with d_color_sh, the
+// factored colour gradient goes there instead, with this camera's centre right behind it (for gms_adam_sh_factored); with
+// sh_adam, neither: the preprocess backward updates `features` in place.
+template <typename Args>
+static int frame_loss_backward(const Args* a, const FrameLayout& FL, const gms_raster_inputs& in, const gms_raster_saved& saved,
+                               float* d_xyz, float* d_color_sh, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    gms_loss_args la;
+    memset(&la, 0, sizeof(la));
+    la.C = 3; la.H = a->settings.image_height; la.W = a->settings.image_width; la.img = FL.image; la.gt = a->gt;
+    la.lambda_dssim = a->lambda_dssim; la.loss = a->loss;
+    la.dL_dimg = FL.dimage; la.scratch = FL.loss_scratch; la.scratch_bytes = FL.loss_bytes;
+    int rc;
+    if ((rc = gms_l1_ssim_loss(&la, cuda_stream))) return rc;
+    if (a->event_loss_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_loss_ready), st));
+    gms_raster_grads gr;
+    memset(&gr, 0, sizeof(gr));
+    gr.dL_dmeans3D = d_xyz; gr.dL_dmeans2D = FL.d_m2d; gr.dL_dopacities = FL.d_opac;
+    if (d_color_sh) {
+        gr.dL_dcolors_sh = d_color_sh;
+        GMS_CUDA(cudaMemcpyAsync(d_color_sh + 3 * (size_t)in.P, a->settings.campos, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    } else if (!a->sh_adam) gr.dL_dshs = a->d_features;
+    gr.dL_dscales = FL.d_scales; gr.dL_drotations = FL.d_rots;
+    return raster_backward_impl(&a->settings, &in, FL.radii, &saved, FL.dimage, nullptr, &gr, cuda_stream, a->d_opacity_raw, a->sh_adam);
+}
+
+}   // extern "C++"
+
+int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
+    FrameModel m;
+    std::vector<gms_expand_args> ea;
+    return render_frame("gms_render_frame", a, alloc, alloc_user, cuda_stream,
+        [&](int* P) {
+            if (!a->vertices || !a->faces || !a->alpha_raw || !a->scale_raw || !a->features || !a->opacity_raw)
+                return set_err(GMS_E_ARG, "gms_render_frame: model tensors required%s%s");
+            m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps,
+                 a->segments, a->n_segments, a->alpha_activation};
+            return frame_gaussian_count("gms_render_frame", m, P);
+        },
+        [&](int, const RenderLayout& RL, const float**) { return mesh_expand_forward(m, RL.xyz, RL.scales, RL.rots, cuda_stream, &ea); });
 }
 
 size_t gms_points_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { return gms_render_workspace_bytes(P, W, H); }
 
 int gms_points_render_frame(const gms_points_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
-    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii)
-        return set_err(GMS_E_ARG, "gms_points_render_frame: null argument%s%s");
-    if (!a->triangles || !a->features || !a->opacity_raw) return set_err(GMS_E_ARG, "gms_points_render_frame: model tensors required%s%s");
-    if (a->P < 0) return set_err(GMS_E_ARG, "gms_points_render_frame: P < 0%s%s");
-    const int P = a->P, W = a->settings.image_width, H = a->settings.image_height;
-    if (a->workspace_bytes < gms_points_render_workspace_bytes(P, W, H))
-        return set_err(GMS_E_ARG, "gms_points_render_frame: workspace too small%s%s");
-    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
-    // pseudo-mesh triangles -> xyz = v1, (eps, exp(log s2), exp(log s3)), normalised quaternion
-    gms_points_args pa;
-    memset(&pa, 0, sizeof(pa));
-    pa.P = P; pa.triangles = a->triangles; pa.eps = a->eps; pa.xyz = RL.xyz; pa.scaling_act = RL.scales; pa.rotation_act = RL.rots;
-    int rc;
-    if ((rc = gms_points_expand_forward(&pa, cuda_stream))) return rc;
-    gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
-    gms_raster_inputs in;
-    gms_raster_saved saved;
-    const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
-    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
-                                   &saved))) return rc;
-    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
-    return GMS_OK;
+    return render_frame("gms_points_render_frame", a, alloc, alloc_user, cuda_stream,
+        [&](int* P) {
+            if (!a->triangles || !a->features || !a->opacity_raw) return set_err(GMS_E_ARG, "gms_points_render_frame: model tensors required%s%s");
+            if (a->P < 0) return set_err(GMS_E_ARG, "gms_points_render_frame: P < 0%s%s");
+            *P = a->P;
+            return GMS_OK;
+        },
+        [&](int P, const RenderLayout& RL, const float**) {
+            // pseudo-mesh triangles -> xyz = v1, (eps, exp(log s2), exp(log s3)), normalised quaternion
+            gms_points_args pa;
+            memset(&pa, 0, sizeof(pa));
+            pa.P = P; pa.triangles = a->triangles; pa.eps = a->eps; pa.xyz = RL.xyz; pa.scaling_act = RL.scales; pa.rotation_act = RL.rots;
+            return gms_points_expand_forward(&pa, cuda_stream);
+        });
 }
 
 size_t gms_pseudomesh_bind_scratch_bytes(int32_t F) {
@@ -2188,7 +2222,7 @@ int gms_pseudomesh_bind(const gms_pseudomesh_bind_args* a, void* cuda_stream) {
         return set_err(GMS_E_ARG, "gms_pseudomesh_bind: null argument%s%s");
     if (a->P < 0 || a->F < 1 || a->V < 1) return set_err(GMS_E_ARG, "gms_pseudomesh_bind: need P >= 0, F >= 1, V >= 1%s%s");
     if (a->scratch_bytes < gms_pseudomesh_bind_scratch_bytes(a->F)) return set_err(GMS_E_ARG, "gms_pseudomesh_bind: scratch too small%s%s");
-    char* base = reinterpret_cast<char*>(aligned_base_c(a->scratch));
+    char* base = reinterpret_cast<char*>(aligned_base(a->scratch));
     float4* cent = carve<float4>(base, a->F);
     uint32_t* n_deg = carve<uint32_t>(base, 1);
     GMS_CUDA(cudaMemsetAsync(n_deg, 0, sizeof(uint32_t), st));
@@ -2229,37 +2263,29 @@ size_t gms_bound_points_render_workspace_bytes(int32_t P, int32_t W, int32_t H) 
 
 int gms_bound_points_render_frame(const gms_bound_points_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii)
-        return set_err(GMS_E_ARG, "gms_bound_points_render_frame: null argument%s%s");
-    if (!a->face || !a->coeffs || !a->vertices || !a->faces || !a->features || !a->opacity_raw || !a->settings.viewmatrix)
-        return set_err(GMS_E_ARG, "gms_bound_points_render_frame: model tensors required%s%s");
-    if (a->P < 0 || a->F < 1 || a->V < 1) return set_err(GMS_E_ARG, "gms_bound_points_render_frame: need P >= 0, F >= 1, V >= 1%s%s");
-    const int P = a->P, W = a->settings.image_width, H = a->settings.image_height;
-    if (a->workspace_bytes < gms_bound_points_render_workspace_bytes(P, W, H))
-        return set_err(GMS_E_ARG, "gms_bound_points_render_frame: workspace too small%s%s");
-    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
-    // binding + driving pose -> re-posed triangle -> xyz = v1, (eps, exp(log s2), exp(log s3)), normalised quaternion
-    if (P > 0) {
-        gms_pseudomesh_repose_args r;
-        memset(&r, 0, sizeof(r));
-        r.P = P; r.face = a->face; r.coeffs = a->coeffs; r.V = a->V; r.F = a->F; r.vertices = a->vertices; r.faces = a->faces;
-        gms_points_args pa;
-        memset(&pa, 0, sizeof(pa));
-        pa.P = P; pa.eps = a->eps; pa.xyz = RL.xyz; pa.scaling_act = RL.scales; pa.rotation_act = RL.rots;
-        span_begin(K_EXP_FWD, st);
-        k_points_bound_expand_fwd<<<(P + GMS_PM_BLOCK - 1) / GMS_PM_BLOCK, GMS_PM_BLOCK, 0, st>>>(r, pa, a->settings.viewmatrix);
-        GMS_AFTER_LAUNCH("points_bound_expand_fwd", 0, st);
-        span_end(st);
-    }
-    gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
-    gms_raster_inputs in;
-    gms_raster_saved saved;
-    const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
-    int rc;
-    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
-                                   &saved))) return rc;
-    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
-    return GMS_OK;
+    return render_frame("gms_bound_points_render_frame", a, alloc, alloc_user, cuda_stream,
+        [&](int* P) {
+            if (!a->face || !a->coeffs || !a->vertices || !a->faces || !a->features || !a->opacity_raw || !a->settings.viewmatrix)
+                return set_err(GMS_E_ARG, "gms_bound_points_render_frame: model tensors required%s%s");
+            if (a->P < 0 || a->F < 1 || a->V < 1) return set_err(GMS_E_ARG, "gms_bound_points_render_frame: need P >= 0, F >= 1, V >= 1%s%s");
+            *P = a->P;
+            return GMS_OK;
+        },
+        [&](int P, const RenderLayout& RL, const float**) {
+            // binding + driving pose -> re-posed triangle -> xyz = v1, (eps, exp(log s2), exp(log s3)), normalised quaternion
+            if (P == 0) return GMS_OK;
+            gms_pseudomesh_repose_args r;
+            memset(&r, 0, sizeof(r));
+            r.P = P; r.face = a->face; r.coeffs = a->coeffs; r.V = a->V; r.F = a->F; r.vertices = a->vertices; r.faces = a->faces;
+            gms_points_args pa;
+            memset(&pa, 0, sizeof(pa));
+            pa.P = P; pa.eps = a->eps; pa.xyz = RL.xyz; pa.scaling_act = RL.scales; pa.rotation_act = RL.rots;
+            span_begin(K_EXP_FWD, st);
+            k_points_bound_expand_fwd<<<(P + GMS_PM_BLOCK - 1) / GMS_PM_BLOCK, GMS_PM_BLOCK, 0, st>>>(r, pa, a->settings.viewmatrix);
+            GMS_AFTER_LAUNCH("points_bound_expand_fwd", 0, st);
+            span_end(st);
+            return GMS_OK;
+        });
 }
 
 int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
@@ -2277,35 +2303,18 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     if ((rc = frame_gaussian_count("gms_train_frame", m, &P))) return rc;
     const int W = a->settings.image_width, H = a->settings.image_height;
     if (a->workspace_bytes < gms_frame_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_train_frame: workspace too small%s%s");
-    FrameLayout FL = frame_layout(aligned_base_c(a->workspace), P, W, H);
+    FrameLayout FL = frame_layout(aligned_base(a->workspace), P, W, H);
     gms_raster_outputs out = {FL.image, FL.radii, FL.invdepth, 0};
     std::vector<gms_expand_args> ea;
     gms_raster_inputs in;
     gms_raster_saved saved;
-    if ((rc = mesh_expand_forward(m, FL.xyz, FL.scales, FL.rots, cuda_stream, &ea))) return rc;
-    const FrameGaussians g = {P, a->M, FL.xyz, FL.scales, FL.rots, a->features, a->opacity_raw, FL.opac};
+    if ((rc = mesh_expand_forward(m, FL.g.xyz, FL.g.scales, FL.g.rots, cuda_stream, &ea))) return rc;
+    const FrameGaussians g = {P, a->M, FL.g.xyz, FL.g.scales, FL.g.rots, a->features, a->opacity_raw, FL.g.opac};
     if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
                                    &saved))) return rc;
-    // loss + dL/dimage
-    gms_loss_args la;
-    memset(&la, 0, sizeof(la));
-    la.C = 3; la.H = H; la.W = W; la.img = FL.image; la.gt = a->gt; la.lambda_dssim = a->lambda_dssim; la.loss = a->loss;
-    la.dL_dimg = FL.dimage; la.scratch = FL.loss_scratch; la.scratch_bytes = FL.loss_bytes;
-    if ((rc = gms_l1_ssim_loss(&la, cuda_stream))) return rc;
-    if (a->event_loss_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_loss_ready), st));
-    // rasterizer backward: dL/dshs goes straight to the caller's gradient buffer
-    gms_raster_grads gr;
-    memset(&gr, 0, sizeof(gr));
-    gr.dL_dmeans3D = FL.d_xyz; gr.dL_dmeans2D = FL.d_m2d; gr.dL_dopacities = FL.d_opac;
-    if (a->d_color_sh) {    // factored SH gradient: colour gradient + this camera's centre (right behind it) for gms_adam_sh_factored
-        gr.dL_dcolors_sh = a->d_color_sh;
-        GMS_CUDA(cudaMemcpyAsync(a->d_color_sh + 3 * (size_t)P, a->settings.campos, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    } else if (!a->sh_adam) gr.dL_dshs = a->d_features;
-    gr.dL_dscales = FL.d_scales; gr.dL_drotations = FL.d_rots;
     // sh_adam: the preprocess backward updates `features` in place; it is the frame's last reader of them (the expansion
     // backward below does not read them)
-    if ((rc = raster_backward_impl(&a->settings, &in, FL.radii, &saved, FL.dimage, nullptr, &gr, cuda_stream, a->d_opacity_raw, a->sh_adam)))
-        return rc;
+    if ((rc = frame_loss_backward(a, FL, in, saved, FL.d_xyz, a->d_color_sh, cuda_stream))) return rc;
     if (a->event_sh_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_sh_ready), st));
     // expansion backward (vertex gradients are accumulated with atomics: the caller keeps d_vertices zeroed)
     if ((rc = mesh_expand_backward(ea, FL.d_xyz, FL.d_scales, FL.d_rots, a->d_vertices, a->d_alpha_raw, a->d_scale_raw, cuda_stream)))
@@ -2350,31 +2359,19 @@ int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void*
     const int W = a->settings.image_width, H = a->settings.image_height;
     if (W <= 0 || H <= 0) return set_err(GMS_E_ARG, "gms_free_train_frame: bad image size%s%s");
     if (a->workspace_bytes < gms_frame_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_free_train_frame: workspace too small%s%s");
-    FrameLayout FL = frame_layout(aligned_base_c(a->workspace), P, W, H);
+    FrameLayout FL = frame_layout(aligned_base(a->workspace), P, W, H);
     gms_raster_outputs out = {FL.image, FL.radii, FL.invdepth, 0};
     gms_raster_inputs in;
     gms_raster_saved saved;
     int rc;
-    if ((rc = free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, FL.scales, FL.rots, st))) return rc;
-    const FrameGaussians g = {P, a->M, a->xyz, FL.scales, FL.rots, a->features, a->opacity_raw, FL.opac};
+    if ((rc = free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, FL.g.scales, FL.g.rots, st))) return rc;
+    const FrameGaussians g = {P, a->M, a->xyz, FL.g.scales, FL.g.rots, a->features, a->opacity_raw, FL.g.opac};
     if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
                                    &saved))) return rc;
-    gms_loss_args la;
-    memset(&la, 0, sizeof(la));
-    la.C = 3; la.H = H; la.W = W; la.img = FL.image; la.gt = a->gt; la.lambda_dssim = a->lambda_dssim; la.loss = a->loss;
-    la.dL_dimg = FL.dimage; la.scratch = FL.loss_scratch; la.scratch_bytes = FL.loss_bytes;
-    if ((rc = gms_l1_ssim_loss(&la, cuda_stream))) return rc;
-    if (a->event_loss_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_loss_ready), st));
-    gms_raster_grads gr;
-    memset(&gr, 0, sizeof(gr));
-    gr.dL_dmeans3D = a->d_xyz; gr.dL_dmeans2D = FL.d_m2d; gr.dL_dopacities = FL.d_opac;
-    if (!a->sh_adam) gr.dL_dshs = a->d_features;
-    gr.dL_dscales = FL.d_scales; gr.dL_drotations = FL.d_rots;
-    if ((rc = raster_backward_impl(&a->settings, &in, FL.radii, &saved, FL.dimage, nullptr, &gr, cuda_stream, a->d_opacity_raw, a->sh_adam)))
-        return rc;
+    if ((rc = frame_loss_backward(a, FL, in, saved, a->d_xyz, nullptr, cuda_stream))) return rc;
     if (P > 0) {
         FreeActBwd b;
-        b.P = P; b.cols = a->scale_cols; b.rotation_raw = a->rotation_raw; b.scales = FL.scales;
+        b.P = P; b.cols = a->scale_cols; b.rotation_raw = a->rotation_raw; b.scales = FL.g.scales;
         b.d_scales = FL.d_scales; b.d_rots = FL.d_rots; b.d_m2d = FL.d_m2d; b.radii = FL.radii;
         b.d_scaling_raw = a->d_scaling_raw; b.d_rotation_raw = a->d_rotation_raw; b.accum = a->accum; b.denom = a->denom;
         b.counters = geom_layout(aligned_base(saved.geom), P).counters;
@@ -2389,24 +2386,18 @@ int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void*
 
 int gms_free_render_frame(const gms_free_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii)
-        return set_err(GMS_E_ARG, "gms_free_render_frame: null argument%s%s");
-    if (!free_model_ok(a->P, a->M, a->scale_cols, a->xyz, a->scaling_raw, a->rotation_raw, a->features, a->opacity_raw))
-        return set_err(GMS_E_ARG, "gms_free_render_frame: need P >= 0, 1 <= M <= 16, scale_cols 2 or 3 and every model tensor%s%s");
-    if (!aligned16(a->rotation_raw)) return set_err(GMS_E_ARG, "gms_free_render_frame: rotation_raw must be 16-byte aligned%s%s");
-    const int P = a->P, W = a->settings.image_width, H = a->settings.image_height;
-    if (a->workspace_bytes < gms_render_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_free_render_frame: workspace too small%s%s");
-    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
-    int rc;
-    if ((rc = free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, RL.scales, RL.rots, st))) return rc;
-    gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
-    gms_raster_inputs in;
-    gms_raster_saved saved;
-    const FrameGaussians g = {P, a->M, a->xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
-    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
-                                   &saved))) return rc;
-    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
-    return GMS_OK;
+    return render_frame("gms_free_render_frame", a, alloc, alloc_user, cuda_stream,
+        [&](int* P) {
+            if (!free_model_ok(a->P, a->M, a->scale_cols, a->xyz, a->scaling_raw, a->rotation_raw, a->features, a->opacity_raw))
+                return set_err(GMS_E_ARG, "gms_free_render_frame: need P >= 0, 1 <= M <= 16, scale_cols 2 or 3 and every model tensor%s%s");
+            if (!aligned16(a->rotation_raw)) return set_err(GMS_E_ARG, "gms_free_render_frame: rotation_raw must be 16-byte aligned%s%s");
+            *P = a->P;
+            return GMS_OK;
+        },
+        [&](int P, const RenderLayout& RL, const float** xyz) {
+            *xyz = a->xyz;
+            return free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, RL.scales, RL.rots, st);
+        });
 }
 
 // ------------------------------------------------------------------------------------------ gs_flame checkpoint render
@@ -2442,33 +2433,25 @@ size_t gms_flame_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { retur
 
 int gms_flame_render_frame(const gms_flame_render_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii)
-        return set_err(GMS_E_ARG, "gms_flame_render_frame: null argument%s%s");
-    if (!a->vertices || !a->faces || !a->alpha || !a->scaling_log || !a->rotation_raw || !a->features || !a->opacity_raw)
-        return set_err(GMS_E_ARG, "gms_flame_render_frame: model tensors required%s%s");
-    if (a->F < 0 || a->K < 1 || a->V < 1 || a->M < 1 || a->M > 16 || (int64_t)a->F * a->K > INT32_MAX)
-        return set_err(GMS_E_ARG, "gms_flame_render_frame: need F >= 0, K >= 1, V >= 1, 1 <= M <= 16 and F*K < 2^31%s%s");
-    if (!aligned16(a->rotation_raw)) return set_err(GMS_E_ARG, "gms_flame_render_frame: rotation_raw must be 16-byte aligned%s%s");
-    const int P = a->F * a->K, W = a->settings.image_width, H = a->settings.image_height;
-    if (a->workspace_bytes < gms_flame_render_workspace_bytes(P, W, H))
-        return set_err(GMS_E_ARG, "gms_flame_render_frame: workspace too small%s%s");
-    RenderLayout RL = render_layout(aligned_base_c(a->workspace), P);
-    if (P > 0) {
-        span_begin(K_EXP_FWD, st);
-        k_flame_act<<<(P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, st>>>(P, a->K, a->alpha, a->faces, a->vertices,
-                                                                                       a->scaling_log, a->rotation_raw, RL.xyz, RL.scales, RL.rots);
-        GMS_AFTER_LAUNCH("flame_act", 0, st);
-        span_end(st);
-    }
-    gms_raster_outputs out = {a->image, a->radii, a->invdepth, GMS_FORWARD_ONLY};
-    gms_raster_inputs in;
-    gms_raster_saved saved;
-    const FrameGaussians g = {P, a->M, RL.xyz, RL.scales, RL.rots, a->features, a->opacity_raw, RL.opac};
-    int rc;
-    if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
-                                   &saved))) return rc;
-    if (a->num_rendered) *a->num_rendered = saved.num_rendered;
-    return GMS_OK;
+    return render_frame("gms_flame_render_frame", a, alloc, alloc_user, cuda_stream,
+        [&](int* P) {
+            if (!a->vertices || !a->faces || !a->alpha || !a->scaling_log || !a->rotation_raw || !a->features || !a->opacity_raw)
+                return set_err(GMS_E_ARG, "gms_flame_render_frame: model tensors required%s%s");
+            if (a->F < 0 || a->K < 1 || a->V < 1 || a->M < 1 || a->M > 16 || (int64_t)a->F * a->K > INT32_MAX)
+                return set_err(GMS_E_ARG, "gms_flame_render_frame: need F >= 0, K >= 1, V >= 1, 1 <= M <= 16 and F*K < 2^31%s%s");
+            if (!aligned16(a->rotation_raw)) return set_err(GMS_E_ARG, "gms_flame_render_frame: rotation_raw must be 16-byte aligned%s%s");
+            *P = a->F * a->K;
+            return GMS_OK;
+        },
+        [&](int P, const RenderLayout& RL, const float**) {
+            if (P == 0) return GMS_OK;
+            span_begin(K_EXP_FWD, st);
+            k_flame_act<<<(P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, st>>>(P, a->K, a->alpha, a->faces, a->vertices,
+                                                                                           a->scaling_log, a->rotation_raw, RL.xyz, RL.scales, RL.rots);
+            GMS_AFTER_LAUNCH("flame_act", 0, st);
+            span_end(st);
+            return GMS_OK;
+        });
 }
 
 struct DensifyScratch { int4* flags; int4* incl; void* cub; size_t cub_bytes; size_t total; };
@@ -2498,7 +2481,7 @@ int gms_densify_plan(const gms_densify_plan_args* a, void* cuda_stream) {
     memset(a->result, 0, 5 * sizeof(int32_t));
     if (a->P == 0) return GMS_OK;
     const int P = a->P;
-    DensifyScratch S = densify_scratch(aligned_base_c(a->scratch), P);
+    DensifyScratch S = densify_scratch(aligned_base(a->scratch), P);
     DensifyPlanK k;
     k.P = P; k.cols = a->scale_cols; k.accum = a->accum; k.denom = a->denom; k.scaling_raw = a->scaling_raw; k.opacity_raw = a->opacity_raw;
     k.eps = a->eps; k.grad_threshold = a->grad_threshold; k.split_scale = a->split_scale; k.min_opacity = a->min_opacity;
@@ -2533,7 +2516,7 @@ int gms_densify_apply(const gms_densify_apply_args* a, void* cuda_stream) {
         if (!free_set_ok(a->src[t]) || (a->new_P > 0 && !free_set_ok(a->dst[t])))
             return set_err(GMS_E_ARG, "gms_densify_apply: every source and destination tensor is required%s%s");
     if (a->new_P == 0) return GMS_OK;
-    DensifyScratch S = densify_scratch(const_cast<void*>(aligned_base_c(const_cast<void*>(a->scratch))), a->P);
+    DensifyScratch S = densify_scratch(const_cast<void*>(aligned_base(const_cast<void*>(a->scratch))), a->P);
     DensifyApplyK k;
     k.P = a->P; k.cols = a->scale_cols; k.F = 3 * a->M; k.eps = a->eps; k.incl = S.incl;
     k.kept = r[1]; k.clones = r[2]; k.splits = r[3]; k.normals = a->normals;
@@ -2591,7 +2574,7 @@ int gms_knn_dist2(const gms_knn_args* a, void* cuda_stream) {
     if (!a->points || !a->dist2 || !a->scratch) return set_err(GMS_E_ARG, "gms_knn_dist2: null argument%s%s");
     if (a->scratch_bytes < gms_knn_scratch_bytes(a->P)) return set_err(GMS_E_ARG, "gms_knn_dist2: scratch too small%s%s");
     const int P = a->P, nbox = (P + GMS_KNN_BOX - 1) / GMS_KNN_BOX;
-    KnnLayout L = knn_layout(aligned_base_c(a->scratch), P);
+    KnnLayout L = knn_layout(aligned_base(a->scratch), P);
     span_begin(K_MISC, st);
     k_knn_bounds<<<GMS_KNN_BOUNDS_BLOCKS, 256, 0, st>>>(P, a->points, L.part);
     GMS_AFTER_LAUNCH("knn_bounds", 0, st);
@@ -2656,7 +2639,7 @@ int gms_flame_lbs_forward(const gms_flame_lbs_args* a, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     const int V = a->V;
     const int nsb = (V + GMS_FLAME_SB - 1) / GMS_FLAME_SB, nvb = (V + GMS_FLAME_VB - 1) / GMS_FLAME_VB;
-    GmsFlameWs w = gms_flame_ws(reinterpret_cast<float*>(aligned_base_c(a->workspace)), V);
+    GmsFlameWs w = gms_flame_ws(reinterpret_cast<float*>(aligned_base(a->workspace)), V);
     GmsFlameParents par;
     for (int j = 0; j < GMS_FLAME_NJ; j++) par.p[j] = a->parents[j];
     span_begin(K_MISC, st);
@@ -2678,7 +2661,7 @@ int gms_flame_lbs_backward(const gms_flame_lbs_args* a, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     const int V = a->V, B = a->n_shape + a->n_exp;
     const int nvb = (V + GMS_FLAME_VB - 1) / GMS_FLAME_VB;
-    GmsFlameWs w = gms_flame_ws(reinterpret_cast<float*>(aligned_base_c(a->workspace)), V);
+    GmsFlameWs w = gms_flame_ws(reinterpret_cast<float*>(aligned_base(a->workspace)), V);
     GmsFlameParents par;
     for (int j = 0; j < GMS_FLAME_NJ; j++) par.p[j] = a->parents[j];
     span_begin(K_MISC, st);

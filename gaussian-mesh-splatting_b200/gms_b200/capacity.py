@@ -1,4 +1,5 @@
-"""Per-view binning capacity of the sync-free frames (NativeFrame for training, NativeRenderer for rendering).
+"""Per-view binning capacity of the sync-free frames (NativeFrame for training, NativeRenderer for rendering), and the
+host side every one-call frame shares: its argument checks and its launch.
 
 A sync-free frame does not read N (the number of tile duplicates) back before it bins: the binning region is sized for a
 PREDICTED capacity, N stays on the device and the range kernel mirrors (N, overflow flag) into a ring of mapped pinned host
@@ -12,6 +13,20 @@ import collections
 import ctypes as C
 
 import torch
+
+
+def check_float32(t: torch.Tensor, what: str, dev) -> None:
+    """Raw pointers go straight to CUDA kernels: refuse a tensor that is not a contiguous float32 one on `dev`."""
+    if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == dev):
+        raise RuntimeError(f"{what} must be a contiguous float32 CUDA tensor on {dev}")
+
+
+def recorded_event(ev, dev) -> torch.cuda.Event:
+    """`ev`, or (when None) a new event recorded once on the current stream of `dev`, which creates its cudaEvent_t."""
+    if ev is None:
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(dev))
+    return ev
 
 
 def grow_only_alloc(dev):
@@ -109,3 +124,44 @@ class SyncFreeCapacity:
         n = max(int(self.n_rendered.value), 0)
         self._note(key, n)
         self.capacity = n
+
+    def _check_view(self, cam, bg, where: str = None, gt=None, gt_fits: bool = True) -> None:
+        """The camera, background (and ground truth) of a frame are float32 on the frame's device, at its image size;
+        `where` names the caller in the messages (default: the class)."""
+        owner = type(self).__name__
+        where = where or owner
+        for t, what in (() if gt is None else ((gt, "gt"),)) + ((bg, "bg"), (cam.world_view_transform, "camera matrices"),
+                                                               (cam.full_proj_transform, "camera matrices"), (cam.camera_center, "camera centre")):
+            if not t.is_cuda or t.device != self.dev or t.dtype != torch.float32:
+                raise RuntimeError(f"{where}: {what} must be float32 on {self.dev}")
+        if int(cam.image_width) != self.W or int(cam.image_height) != self.H or not gt_fits:
+            raise ValueError(f"{owner} was sized for {self.W}x{self.H}; got a {cam.image_width}x{cam.image_height} camera")
+
+    def _launch(self, fn: str, a, cam, bg, scale_modifier: float = 1.0, antialiasing: bool = False, capacity: int = None,
+                n_host: int = None, relearn: bool = False) -> bool:
+        """Fills the settings, workspace, num_rendered and capacity fields every one-call frame's args struct shares and
+        calls `fn` on the current stream.  With `capacity` (and the mapped (N, flag) address `n_host`) the frame is sync-free
+        at that capacity.  Otherwise the frame is synchronising when it has to learn N (the first frame, or `relearn`) or
+        the frames are not sync-free, and sync-free on the next ring slot at the view's predicted capacity else.  Returns
+        whether the frame learned N."""
+        from . import _lib
+        s = a.settings
+        s.image_height, s.image_width, s.tanfovx, s.tanfovy = self.H, self.W, cam.tanfovx, cam.tanfovy
+        s.bg, s.scale_modifier = bg.data_ptr(), float(scale_modifier)
+        s.viewmatrix, s.projmatrix, s.campos = cam.world_view_transform.data_ptr(), cam.full_proj_transform.data_ptr(), cam.camera_center.data_ptr()
+        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = self.model.active_sh_degree, 0, 0, int(bool(antialiasing))
+        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
+        a.num_rendered = C.pointer(self.n_rendered)
+        learn = False
+        if capacity is None:
+            key = self._view_key(cam)
+            learn = self.sync_free and (self.capacity == 0 or relearn)
+            if self.sync_free and not learn:
+                n_host = self._sync_free_slot(key, self.dev)
+                capacity = self.capacity
+        a.binning_capacity, a.n_host_mapped = int(capacity or 0), n_host
+        with torch.cuda.device(self.dev):
+            _lib.check(getattr(_lib.lib(), fn)(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream), fn)
+        if learn:           # the synchronising frame told us N
+            self._learned_first(key)
+        return learn

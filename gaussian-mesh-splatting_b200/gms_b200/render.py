@@ -19,14 +19,13 @@ per view (SyncFreeCapacity).  An overflowed render (N above its capacity) gives 
 re-renders those views before it reads its results."""
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import dataclass
 from typing import List, Sequence
 
 import torch
 
 from . import _lib, io_image
-from .capacity import SyncFreeCapacity, grow_only_alloc
+from .capacity import SyncFreeCapacity, check_float32, grow_only_alloc
 from .metrics import METRIC_NAMES, image_metrics, scratch_bytes
 
 
@@ -73,26 +72,16 @@ class NativeRenderer(SyncFreeCapacity):
     def _check(self, cam, bg) -> None:
         m = self.model
         for name in ("vertices", "_alpha", "_scale", "_opacity"):
-            t = getattr(m, name)
-            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
-                raise RuntimeError(f"NativeRenderer: model.{name} must be a contiguous float32 CUDA tensor on {self.dev}")
+            check_float32(getattr(m, name), f"NativeRenderer: model.{name}", self.dev)
         if m.faces.device != self.dev:
             raise RuntimeError("NativeRenderer: model.faces must live on the model's device")
         if m._scale.shape[0] != self.radii.shape[0]:
             raise RuntimeError("NativeRenderer: the model's Gaussian count changed; make a new renderer")
         self._check_view(cam, bg)
 
-    def _check_view(self, cam, bg) -> None:
-        for t, what in ((bg, "bg"), (cam.world_view_transform, "camera matrices"), (cam.full_proj_transform, "camera matrices"),
-                        (cam.camera_center, "camera centre")):
-            if not t.is_cuda or t.device != self.dev or t.dtype != torch.float32:
-                raise RuntimeError(f"{type(self).__name__}: {what} must be float32 on {self.dev}")
-        if int(cam.image_width) != self.W or int(cam.image_height) != self.H:
-            raise ValueError(f"{type(self).__name__} was sized for {self.W}x{self.H}; got a {cam.image_width}x{cam.image_height} camera")
-
-    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
-        """One gms_render_frame into the renderer's buffers: capacity 0 = synchronising, else sync-free with (N, flag) at
-        the mapped address n_host."""
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int = None, n_host: int = None) -> None:
+        """One gms_render_frame into the renderer's buffers: sync-free at `capacity` with (N, flag) at the mapped address
+        `n_host` when given, else as SyncFreeCapacity._launch decides."""
         self._check(cam, bg)
         m = self.model
         feats = self._features()
@@ -107,29 +96,14 @@ class NativeRenderer(SyncFreeCapacity):
         self._call("gms_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
 
     def _call(self, fn: str, a, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
-        """Fills the settings, outputs, workspace and capacity fields shared by every render-args struct and calls `fn`."""
-        s = a.settings
-        s.image_height, s.image_width, s.tanfovx, s.tanfovy = self.H, self.W, cam.tanfovx, cam.tanfovy
-        s.bg, s.scale_modifier = bg.data_ptr(), float(scale_modifier)
-        s.viewmatrix, s.projmatrix, s.campos = cam.world_view_transform.data_ptr(), cam.full_proj_transform.data_ptr(), cam.camera_center.data_ptr()
-        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = self.model.active_sh_degree, 0, 0, int(bool(antialiasing))
+        """Points `a`'s outputs at the renderer's buffers and issues `fn`."""
         a.image, a.invdepth, a.radii = self.image.data_ptr(), self.invdepth.data_ptr(), self.radii.data_ptr()
-        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
-        a.num_rendered = C.pointer(self.n_rendered)
-        a.binning_capacity, a.n_host_mapped = int(capacity), n_host
-        with torch.cuda.device(self.dev):
-            _lib.check(getattr(_lib.lib(), fn)(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream), fn)
+        self._launch(fn, a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
 
     def render(self, cam, bg: torch.Tensor, scale_modifier: float = 1.0, antialiasing: bool = False):
         """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view, the reference's render(...)["render"], ["radii"],
         ["depth"]."""
-        key = self._view_key(cam)
-        if self.capacity == 0:
-            self._render(cam, bg, scale_modifier, antialiasing, 0, None)
-            self._learned_first(key)
-        else:
-            n_host = self._sync_free_slot(key, self.dev)
-            self._render(cam, bg, scale_modifier, antialiasing, self.capacity, n_host)
+        self._render(cam, bg, scale_modifier, antialiasing)
         return self.image, self.radii, self.invdepth
 
     def _gt_float(self, gt: torch.Tensor) -> torch.Tensor:
@@ -195,15 +169,14 @@ class PointsRenderer(NativeRenderer):
     def _check(self, cam, bg) -> None:
         m = self.model
         for name, t in (("triangles", self._triangles), ("_features", m._features), ("_opacity", m._opacity)):
-            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
-                raise RuntimeError(f"PointsRenderer: {name} must be a contiguous float32 CUDA tensor on {self.dev}")
+            check_float32(t, f"PointsRenderer: {name}", self.dev)
         P = self.radii.shape[0]
         if tuple(self._triangles.shape) != (P, 3, 3) or m._features.shape[0] != P or tuple(m._opacity.shape) != (P, 1):
             raise RuntimeError(f"PointsRenderer: sized for {P} Gaussians: triangles must be [{P},3,3], features [{P},M,3], "
                                f"opacity [{P},1]; got {tuple(self._triangles.shape)}")
         self._check_view(cam, bg)
 
-    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int = None, n_host: int = None) -> None:
         m = self.model
         self._check(cam, bg)
         a = _lib.PointsRenderArgs()
@@ -245,8 +218,7 @@ class MeshBoundPointsRenderer(NativeRenderer):
         m, b = self.model, self.model.binding
         P = self.radii.shape[0]
         for name, t in (("_features", m._features), ("_opacity", m._opacity), ("binding.coeffs", b.coeffs)):
-            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
-                raise RuntimeError(f"MeshBoundPointsRenderer: {name} must be a contiguous float32 CUDA tensor on {self.dev}")
+            check_float32(t, f"MeshBoundPointsRenderer: {name}", self.dev)
         if b.P != P or m._features.shape[0] != P or tuple(m._opacity.shape) != (P, 1):
             raise RuntimeError(f"MeshBoundPointsRenderer: sized for {P} Gaussians: features must be [{P},M,3], opacity [{P},1]")
         v = m.vertices if self._frame_vertices is None else self._frame_vertices
@@ -259,7 +231,7 @@ class MeshBoundPointsRenderer(NativeRenderer):
                 raise RuntimeError(f"MeshBoundPointsRenderer: {name} must be a contiguous CUDA tensor on {self.dev}")
         self._check_view(cam, bg)
 
-    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int = None, n_host: int = None) -> None:
         m, b = self.model, self.model.binding
         self._check(cam, bg)
         v = m.vertices if self._frame_vertices is None else self._frame_vertices
@@ -279,6 +251,15 @@ class MeshBoundPointsRenderer(NativeRenderer):
             return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing)
         finally:
             self._frame_vertices = None
+
+
+def renderer_for(r, cls, model, cams: Sequence, P: int):
+    """The evaluate() renderer of a trainer: `r` while it fits the cameras' image size and the model's Gaussian count P,
+    else a new cls(model, W, H)."""
+    W, H = int(cams[0].image_width), int(cams[0].image_height)
+    if r is None or (r.W, r.H) != (W, H) or r.radii.shape[0] != P:
+        r = cls(model, W, H)
+    return r
 
 
 def render_points_frame(model, cam, bg: torch.Tensor, triangles: torch.Tensor = None, scale_modifier: float = 1.0,
@@ -308,14 +289,12 @@ class NativeFreeRenderer(NativeRenderer):
     def _check(self, cam, bg) -> None:
         m = self.model
         for name in m.NAMES:
-            t = getattr(m, name)
-            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
-                raise RuntimeError(f"NativeFreeRenderer: model.{name} must be a contiguous float32 CUDA tensor on {self.dev}")
+            check_float32(getattr(m, name), f"NativeFreeRenderer: model.{name}", self.dev)
         if m.P != self.radii.shape[0]:
             raise RuntimeError("NativeFreeRenderer: the model's Gaussian count changed; make a new renderer")
         self._check_view(cam, bg)
 
-    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int = None, n_host: int = None) -> None:
         m = self.model
         self._check(cam, bg)
         a = _lib.FreeRenderArgs()
@@ -347,14 +326,12 @@ class FlameRenderer(NativeRenderer):
                 and tuple(v.shape) == (V, 3)):
             raise RuntimeError(f"FlameRenderer: the pose `vertices` must be a contiguous float32 [{V},3] CUDA tensor on {self.dev}")
         for name in ("alpha", "_scaling", "_rotation", "_features", "_opacity"):
-            t = getattr(m, name)
-            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
-                raise RuntimeError(f"FlameRenderer: {name} must be a contiguous float32 CUDA tensor on {self.dev}")
+            check_float32(getattr(m, name), f"FlameRenderer: {name}", self.dev)
         if m.P != self.radii.shape[0]:
             raise RuntimeError("FlameRenderer: the checkpoint's Gaussian count changed; make a new renderer")
         self._check_view(cam, bg)
 
-    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
+    def _render(self, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int = None, n_host: int = None) -> None:
         m = self.model
         self._check(cam, bg)
         v = m.vertices if self._frame_vertices is None else self._frame_vertices

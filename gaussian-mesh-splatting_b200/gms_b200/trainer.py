@@ -21,7 +21,7 @@ import torch.distributed as dist
 
 import diff_gaussian_rasterization as dgr
 
-from .capacity import SyncFreeCapacity, grow_only_alloc
+from .capacity import SyncFreeCapacity, check_float32, grow_only_alloc, recorded_event
 from .flame import NativeFlame
 from .io_image import GroundTruthBuffer
 from .losses import fused_training_loss
@@ -93,8 +93,7 @@ class NativeFrame(SyncFreeCapacity):
             m.faces = m.faces.long().contiguous()
         for name in ("vertices", "_alpha", "_scale", "_features", "_opacity"):
             t = getattr(m, name)
-            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
-                raise RuntimeError(f"NativeFrame: model.{name} must be a contiguous float32 CUDA tensor on {self.dev}")
+            check_float32(t, f"NativeFrame: model.{name}", self.dev)
             if t.grad is None or not t.grad.is_contiguous() or t.grad.device != self.dev:
                 raise RuntimeError(f"NativeFrame: model.{name}.grad must be a preallocated contiguous buffer (FlatAdam provides it)")
         if m.faces.device != self.dev:
@@ -130,12 +129,7 @@ class NativeFrame(SyncFreeCapacity):
         from . import _lib
         if gt.dtype == torch.uint8:
             gt = self._gt_u8(gt, "NativeFrame.run")
-        for t, what in ((gt, "gt"), (bg, "bg"), (cam.world_view_transform, "camera matrices"), (cam.full_proj_transform, "camera matrices"),
-                        (cam.camera_center, "camera centre")):
-            if not t.is_cuda or t.device != self.dev or t.dtype != torch.float32:
-                raise RuntimeError(f"NativeFrame.run: {what} must be float32 on {self.dev}")
-        if int(cam.image_width) != self.W or int(cam.image_height) != self.H or tuple(gt.shape[-2:]) != (self.H, self.W):
-            raise ValueError(f"NativeFrame was sized for {self.W}x{self.H}; got a {cam.image_width}x{cam.image_height} camera")
+        self._check_view(cam, bg, "NativeFrame.run", gt=gt, gt_fits=tuple(gt.shape[-2:]) == (self.H, self.W))
         if not gt.is_contiguous() or gt.dtype != torch.float32:
             gt = gt.contiguous().float()
         m = self.model
@@ -154,38 +148,18 @@ class NativeFrame(SyncFreeCapacity):
                 self.exchange = torch.zeros(self.world, self.slot, dtype=torch.float32, device=self.dev)
             a.d_features, a.d_color_sh = None, self.exchange[self.rank].data_ptr()
             if self.world > 1:
-                if self.ev_sh is None:
-                    self.ev_sh = torch.cuda.Event()
-                    self.ev_sh.record(torch.cuda.current_stream(self.dev))      # (creates the underlying cudaEvent_t)
+                self.ev_sh = recorded_event(self.ev_sh, self.dev)
                 a.event_sh_ready = self.ev_sh.cuda_event
         if sh_adam is not None:
             a.d_features = None
             a.sh_adam = C.pointer(sh_adam)
-        if self.ev_loss is None:
-            self.ev_loss = torch.cuda.Event()
-            self.ev_loss.record(torch.cuda.current_stream(self.dev))            # (creates the underlying cudaEvent_t)
+        self.ev_loss = recorded_event(self.ev_loss, self.dev)
         a.event_loss_ready = self.ev_loss.cuda_event
         if self._loss_read is not None:         # an asynchronous read-back of the previous frame's loss (read_loss_async) must be
             torch.cuda.current_stream(self.dev).wait_event(self._loss_read)     # done before this frame's loss kernels overwrite it
             self._loss_read = None
-        s = a.settings
-        s.image_height, s.image_width, s.tanfovx, s.tanfovy = self.H, self.W, cam.tanfovx, cam.tanfovy
-        s.bg, s.scale_modifier = bg.data_ptr(), 1.0
-        s.viewmatrix, s.projmatrix, s.campos = cam.world_view_transform.data_ptr(), cam.full_proj_transform.data_ptr(), cam.camera_center.data_ptr()
-        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = m.active_sh_degree, 0, 0, 0
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
-        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
-        a.num_rendered = C.pointer(self.n_rendered)
-        key = self._view_key(cam)
-        first = self.capacity == 0
-        if self.sync_free and not first:
-            a.n_host_mapped = self._sync_free_slot(key, self.dev)
-            a.binning_capacity = self.capacity
-        with torch.cuda.device(self.dev):
-            _lib.check(_lib.lib().gms_train_frame(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream),
-                       "gms_train_frame")
-        if self.sync_free and first:           # the one synchronising frame told us N
-            self._learned_first(key)
+        self._launch("gms_train_frame", a, cam, bg)
         return self.loss[0]
 
 
@@ -303,12 +277,9 @@ class MeshTrainer:
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model on held-out views with the trainer's background, the test half of
         training_report (train.py:183-218): NativeRenderer.evaluate, one host synchronisation for the whole set."""
-        from .render import NativeRenderer
-        W, H = int(cams[0].image_width), int(cams[0].image_height)
-        r = self._renderer
-        if r is None or (r.W, r.H) != (W, H) or r.radii.shape[0] != self.model._scale.shape[0]:
-            r = self._renderer = NativeRenderer(self.model, W, H)
-        return r.evaluate(cams, gts, self.bg, protocol=protocol)
+        from .render import NativeRenderer, renderer_for
+        self._renderer = renderer_for(self._renderer, NativeRenderer, self.model, cams, self.model._scale.shape[0])
+        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol)
 
     def state_dict(self) -> dict:
         """What resuming needs (single GPU, fast=True): FlatAdam's flat parameters, moments and step counts, and the active
@@ -395,18 +366,12 @@ class NativeFreeFrame(SyncFreeCapacity):
         m = self.model
         for n in m.NAMES:
             t = getattr(m, n)
-            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.device == self.dev):
-                raise RuntimeError(f"NativeFreeFrame: model.{n} must be a contiguous float32 CUDA tensor on {self.dev}")
+            check_float32(t, f"NativeFreeFrame: model.{n}", self.dev)
             if t.grad is None or not t.grad.is_contiguous() or t.grad.shape != t.shape:
                 raise RuntimeError(f"NativeFreeFrame: model.{n}.grad must be a preallocated contiguous buffer (FlatAdam provides it)")
         if self.accum.shape[0] != m.P:
             raise RuntimeError("NativeFreeFrame: the model's Gaussian count changed; call resize()")
-        for t, what in ((gt, "gt"), (bg, "bg"), (cam.world_view_transform, "camera matrices"), (cam.full_proj_transform, "camera matrices"),
-                        (cam.camera_center, "camera centre")):
-            if not t.is_cuda or t.device != self.dev or t.dtype != torch.float32:
-                raise RuntimeError(f"NativeFreeFrame.run: {what} must be float32 on {self.dev}")
-        if int(cam.image_width) != self.W or int(cam.image_height) != self.H or tuple(gt.shape) != (3, self.H, self.W):
-            raise ValueError(f"NativeFreeFrame was sized for {self.W}x{self.H}; got a {cam.image_width}x{cam.image_height} camera")
+        self._check_view(cam, bg, "NativeFreeFrame.run", gt=gt, gt_fits=tuple(gt.shape) == (3, self.H, self.W))
 
     def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, stats: bool = True, sh_adam=None) -> torch.Tensor:
         """stats: add this frame's densification statistics to `accum` / `denom`.  sh_adam (FlatAdam.begin_fused_sh_step()):
@@ -429,28 +394,11 @@ class NativeFreeFrame(SyncFreeCapacity):
             a.d_features, a.sh_adam = None, C.pointer(sh_adam)
         if stats:
             a.accum, a.denom = self.accum.data_ptr(), self.denom.data_ptr()
-        if self.ev_loss is None:
-            self.ev_loss = torch.cuda.Event()
-            self.ev_loss.record(torch.cuda.current_stream(self.dev))
+        self.ev_loss = recorded_event(self.ev_loss, self.dev)
         a.event_loss_ready = self.ev_loss.cuda_event
-        s = a.settings
-        s.image_height, s.image_width, s.tanfovx, s.tanfovy = self.H, self.W, cam.tanfovx, cam.tanfovy
-        s.bg, s.scale_modifier = bg.data_ptr(), 1.0
-        s.viewmatrix, s.projmatrix, s.campos = cam.world_view_transform.data_ptr(), cam.full_proj_transform.data_ptr(), cam.camera_center.data_ptr()
-        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = m.active_sh_degree, 0, 0, 0
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
-        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
-        a.num_rendered = C.pointer(self.n_rendered)
         key = self._view_key(cam)
-        learn = self.capacity == 0 or self._view_epoch.get(key) != self._epoch
-        if self.sync_free and not learn:
-            a.n_host_mapped = self._sync_free_slot(key, self.dev)
-            a.binning_capacity = self.capacity
-        with torch.cuda.device(self.dev):
-            _lib.check(_lib.lib().gms_free_train_frame(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream),
-                       "gms_free_train_frame")
-        if self.sync_free and learn:
-            self._learned_first(key)
+        if self._launch("gms_free_train_frame", a, cam, bg, relearn=self._view_epoch.get(key) != self._epoch):
             self._view_epoch[key] = self._epoch
         return self.loss[0]
 
@@ -645,12 +593,9 @@ class FreeTrainer:
 
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model on held-out views (NativeFreeRenderer.evaluate)."""
-        from .render import NativeFreeRenderer
-        W, H = int(cams[0].image_width), int(cams[0].image_height)
-        r = self._renderer
-        if r is None or (r.W, r.H) != (W, H) or r.radii.shape[0] != self.model.P:
-            r = self._renderer = NativeFreeRenderer(self.model, W, H)
-        return r.evaluate(cams, gts, self.bg, protocol=protocol)
+        from .render import NativeFreeRenderer, renderer_for
+        self._renderer = renderer_for(self._renderer, NativeFreeRenderer, self.model, cams, self.model.P)
+        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol)
 
 
 # ---------------------------------------------------------------------------------------------- gs_flame
@@ -749,10 +694,7 @@ class FlameTrainer:
 
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model (at its current pose) on held-out views (NativeRenderer.evaluate)."""
-        from .render import NativeRenderer
+        from .render import NativeRenderer, renderer_for
         self.model.refresh_vertices()
-        W, H = int(cams[0].image_width), int(cams[0].image_height)
-        r = self._renderer
-        if r is None or (r.W, r.H) != (W, H):
-            r = self._renderer = NativeRenderer(self.model, W, H)
-        return r.evaluate(cams, gts, self.bg, protocol=protocol)
+        self._renderer = renderer_for(self._renderer, NativeRenderer, self.model, cams, self.model.P)
+        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol)
