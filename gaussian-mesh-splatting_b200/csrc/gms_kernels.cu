@@ -2123,10 +2123,18 @@ static int frame_raster_forward(const FrameGaussians& g, const gms_raster_settin
 
 size_t gms_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { (void)W; (void)H; return render_layout(nullptr, P).total + 512; }
 
+// The active SH degree against the model's coefficient rows, checked by every frame with its model, before its first launch
+// (raster_forward_impl repeats it for the plain rasterizer ABI, after a frame's expansion step has already run).
+static int frame_sh_check(const char* fn, int sh_degree, int M) {
+    if (sh_degree < 0 || sh_degree > 3) return set_err(GMS_E_ARG, "%s: sh_degree must be 0..3%s", fn);
+    if ((sh_degree + 1) * (sh_degree + 1) > M) return set_err(GMS_E_ARG, "%s: sh_degree needs more coefficients than M%s", fn);
+    return GMS_OK;
+}
+
 extern "C++" {      // templates need C++ linkage
 
 // A forward-only frame around the model's own checks and expansion step: the output checks; check_model(&P), which checks
-// the model and gives its Gaussian count; the workspace check; expand(P, RL, &xyz) into the render layout (free Gaussians
+// the model and gives its Gaussian count; the SH degree check; the workspace check; expand(P, RL, &xyz) into the render layout (free Gaussians
 // point xyz at the model's own centres); one rasterizer forward; num_rendered.  Every gms_*_render_args names its
 // settings, output, workspace and capacity fields alike.
 template <typename Args, typename CheckModel, typename Expand>
@@ -2135,6 +2143,7 @@ static int render_frame(const char* fn, const Args* a, gms_alloc_fn alloc, void*
     if (!a || !alloc || !a->workspace || !a->image || !a->invdepth || !a->radii) return set_err(GMS_E_ARG, "%s: null argument%s", fn);
     int P, rc;
     if ((rc = check_model(&P))) return rc;
+    if ((rc = frame_sh_check(fn, a->settings.sh_degree, a->M))) return rc;
     if (a->workspace_bytes < gms_render_workspace_bytes(P, a->settings.image_width, a->settings.image_height))
         return set_err(GMS_E_ARG, "%s: workspace too small%s", fn);
     const RenderLayout RL = render_layout(aligned_base(a->workspace), P);
@@ -2301,6 +2310,7 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
                           a->segments, a->n_segments, a->alpha_activation};
     int P, rc;
     if ((rc = frame_gaussian_count("gms_train_frame", m, &P))) return rc;
+    if ((rc = frame_sh_check("gms_train_frame", a->settings.sh_degree, a->M))) return rc;
     const int W = a->settings.image_width, H = a->settings.image_height;
     if (a->workspace_bytes < gms_frame_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_train_frame: workspace too small%s%s");
     FrameLayout FL = frame_layout(aligned_base(a->workspace), P, W, H);
@@ -2356,6 +2366,8 @@ int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void*
     if (a->sh_adam && (!a->sh_adam->m || !a->sh_adam->v || a->sh_adam->step < 1 || a->M != 16 || a->settings.sh_degree < 0 ||
                        a->settings.sh_degree > 3))
         return set_err(GMS_E_ARG, "gms_free_train_frame: bad sh_adam%s%s");
+    int rc;
+    if ((rc = frame_sh_check("gms_free_train_frame", a->settings.sh_degree, a->M))) return rc;
     const int W = a->settings.image_width, H = a->settings.image_height;
     if (W <= 0 || H <= 0) return set_err(GMS_E_ARG, "gms_free_train_frame: bad image size%s%s");
     if (a->workspace_bytes < gms_frame_workspace_bytes(P, W, H)) return set_err(GMS_E_ARG, "gms_free_train_frame: workspace too small%s%s");
@@ -2363,7 +2375,6 @@ int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void*
     gms_raster_outputs out = {FL.image, FL.radii, FL.invdepth, 0};
     gms_raster_inputs in;
     gms_raster_saved saved;
-    int rc;
     if ((rc = free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, FL.g.scales, FL.g.rots, st))) return rc;
     const FrameGaussians g = {P, a->M, a->xyz, FL.g.scales, FL.g.rots, a->features, a->opacity_raw, FL.g.opac};
     if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,

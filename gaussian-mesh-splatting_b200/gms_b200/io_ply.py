@@ -63,6 +63,9 @@ def read_ply_vertices(path: str) -> Tuple[np.ndarray, List[str]]:
     return data, [n for n, _ in props]
 
 
+_F_REST_COUNTS = {3 * ((d + 1) ** 2 - 1) for d in range(4)}      # 0, 9, 24, 45
+
+
 def _sorted_cols(data, names, prefix):
     cols = sorted([n for n in names if n.startswith(prefix)], key=lambda x: int(x.split("_")[-1]))
     return np.stack([np.asarray(data[n], np.float32) for n in cols], axis=1) if cols else np.zeros((data.shape[0], 0), np.float32)
@@ -74,9 +77,15 @@ def load_gaussian_ply(path: str) -> Dict[str, torch.Tensor]:
     data, names = read_ply_vertices(path)
     P = data.shape[0]
     xyz = np.stack([data["x"], data["y"], data["z"]], axis=1).astype(np.float32)
-    fdc = _sorted_cols(data, names, "f_dc_").reshape(P, 3, 1)
+    fdc = _sorted_cols(data, names, "f_dc_")
     frest = _sorted_cols(data, names, "f_rest_")
-    frest = frest.reshape(P, 3, frest.shape[1] // 3) if frest.shape[1] else frest.reshape(P, 3, 0)
+    # the reference asserts 3 * ((max_sh_degree + 1)^2 - 1) f_rest properties (scene/gaussian_model.py:238-241); any other
+    # count has no SH degree the rasterizer could evaluate
+    if fdc.shape[1] != 3 or frest.shape[1] not in _F_REST_COUNTS:
+        raise ValueError(f"{path}: {fdc.shape[1]} f_dc_* and {frest.shape[1]} f_rest_* properties; a Gaussian PLY has 3 f_dc_* and "
+                         f"3 * ((d + 1)^2 - 1) f_rest_* for an SH degree d in 0..3, i.e. one of {sorted(_F_REST_COUNTS)}")
+    fdc = fdc.reshape(P, 3, 1)
+    frest = frest.reshape(P, 3, frest.shape[1] // 3)
     out = dict(_xyz=torch.tensor(xyz), _features_dc=torch.tensor(fdc).transpose(1, 2).contiguous(),
                _features_rest=torch.tensor(frest).transpose(1, 2).contiguous(),
                _opacity=torch.tensor(np.asarray(data["opacity"], np.float32)[:, None]),

@@ -299,6 +299,35 @@ CASES += [
      "bad image size"),
 ]
 
+# The active SH degree is checked against the model's M with the model, ahead of the workspace check: a frame whose
+# degree needs more coefficients than its rows hold never reaches its expansion or activation launches.
+SH_RANGE = "sh_degree must be 0..3"
+SH_M = "sh_degree needs more coefficients than M"
+_MODEL_NULL = {"gms_render_frame": "vertices", "gms_points_render_frame": "triangles", "gms_bound_points_render_frame": "face",
+               "gms_free_render_frame": "xyz", "gms_flame_render_frame": "alpha", "gms_train_frame": "vertices",
+               "gms_free_train_frame": "xyz"}
+_MODEL_MSG = {"gms_free_render_frame": FREE_MODEL, "gms_free_train_frame": FREE_MODEL}
+for _entry in ENTRIES:
+    CASES += [
+        (_entry, "sh_degree_neg", _set_settings(sh_degree=-1), SH_RANGE),
+        (_entry, "sh_degree_4", _set_settings(sh_degree=4), SH_RANGE),
+        (_entry, "sh_degree_2_M4", lambda a: (_set(M=4)(a), _set_settings(sh_degree=2)(a)), SH_M),
+        (_entry, "sh_degree_3_M15", lambda a: (_set(M=15)(a), _set_settings(sh_degree=3)(a)), SH_M),
+        (_entry, "sh_degree_1_M1", lambda a: (_set(M=1)(a), _set_settings(sh_degree=1)(a)), SH_M),
+        (_entry, "sh_degree_0_M1", lambda a: (_set(M=1)(a), _set_settings(sh_degree=0)(a)), WS),
+        (_entry, "sh_degree_1_M4", lambda a: (_set(M=4)(a), _set_settings(sh_degree=1)(a)), WS),
+        (_entry, "sh_degree_2_M9", lambda a: (_set(M=9)(a), _set_settings(sh_degree=2)(a)), WS),
+        # two faults: the model check runs first, the SH degree check before the workspace check
+        (_entry, "model_and_sh_degree", lambda a, t=_MODEL_NULL[_entry]: (_set(**{t: None})(a), _set_settings(sh_degree=4)(a)),
+         _MODEL_MSG.get(_entry, MESH_MODEL)),
+        (_entry, "sh_degree_and_workspace", lambda a: (_set(M=4, workspace_bytes=0)(a), _set_settings(sh_degree=3)(a)), SH_M),
+    ]
+CASES += [
+    # with sh_adam the SH Adam check owns the degree range, as before
+    ("gms_train_frame", "sh_adam_and_sh_degree_M", lambda a: (_sh_adam(a, step=0), _set(M=4)(a)), "bad sh_adam"),
+    ("gms_free_train_frame", "sh_degree_M_and_W", lambda a: (_set(M=4)(a), _set_settings(image_width=0)(a)), SH_M),
+]
+
 
 def _noop_alloc():
     return _lib.ALLOC_FN(lambda user, which, n: 0)

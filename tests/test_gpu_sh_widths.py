@@ -1,0 +1,763 @@
+"""-m gpu: models with fewer than 16 SH coefficients (--sh_degree 0, 1 and 2: M = 1, 4, 9) through every kernel that treats
+them differently from M = 16.
+
+At M != 16 the preprocess kernels read the SH rows and write the dL/dshs rows at a stride of 3M floats, as float4 when 3M is
+a multiple of 4 (M = 4, 8, 12) and element by element otherwise (M = 1, 2, 9); the staged shared-memory tile is used at
+M = 16 only.  The packed SH segment of FlatAdam takes its DC / rest learning rate with period M; the trainers drop the
+fused SH Adam step; densification copies rows of 3M floats.  Here each of those paths is checked against a float64
+reference, against the same model zero-padded to M = 16 (bit for bit where no float atomics are involved), or against
+torch.optim.Adam."""
+import copy
+import ctypes as C
+import os
+
+import numpy as np
+import pytest
+import torch
+
+import aten_reference
+import densify_oracle as D
+import diff_gaussian_rasterization as dgr
+import flame_driver
+import flame_reference as fr
+from gms_b200 import _lib, rasterizer, scenes
+from gms_b200.model import FlameCheckpoint, FlameGaussianModel, FreeGaussianModel, MeshGaussianModel, PointsModel
+from gms_b200.optim import FlatAdam, free_model_groups, mesh_model_groups
+from gms_b200.render import FlameRenderer, MeshBoundPointsRenderer, NativeFreeRenderer, NativeRenderer, PointsRenderer
+from gms_b200.trainer import FlameTrainer, FreeOptimizationParams, FreeTrainer, MeshTrainer, NativeFreeFrame, render_frame
+from gpu_helpers import (GRAD_TOL, assert_forward_parity, assert_grad_parity, assert_image_parity, gpu_settings, oracle_chain,
+                         run_gpu, run_oracle)
+from helpers import random_gaussians, settings_from_camera
+from test_gpu_free_train import (RAW_TOL, SYNC_NOISE, _compare_densified, _native_state, _Options, _oracle_raw, _trainer_from_state,
+                                 _views)
+from test_gpu_native_frame import _frame_outputs
+
+pytestmark = pytest.mark.gpu
+
+W_R, H_R = 333, 201             # ragged: 21 x 13 tiles, neither side a multiple of 16
+P_R = 3000
+N_CULLED = 300                  # behind the camera: radii 0
+LAMBDA = 0.2
+BG = (0.2, 0.5, 0.9)
+
+
+def _pad16(f):
+    """[P, M, 3] -> [P, 16, 3] with zero rows above M."""
+    return torch.cat([f, torch.zeros(f.shape[0], 16 - f.shape[1], 3, dtype=f.dtype, device=f.device)], 1).contiguous()
+
+
+def _raster_case(M, D, aa=False, seed=0):
+    cam = scenes.look_at_camera((2.8, 0.6, 1.1), (0, 0, 0), W_R, H_R)
+    S = settings_from_camera(cam, sh_degree=D, bg=(0.1, 0.4, 0.8), antialiasing=aa)
+    # the same Gaussians for every M (the rows are cut from the same 16): the cases differ only in the SH width.  No flat
+    # splats: their near-singular covariances amplify the float-atomic noise of the end-to-end gradients (DESIGN.md 2.2),
+    # which test_gpu_parity pins; here the SH rows are under test
+    g = random_gaussians(P_R, seed=100 + seed, extent=1.2, flat_frac=0.0)
+    # a share of the Gaussians behind the camera: culled, their gradient rows must be exact zeros
+    campos = torch.tensor(np.asarray(S.campos, np.float32))
+    g["means3D"][:N_CULLED] = 1.4 * campos + 0.1 * torch.randn(N_CULLED, 3, generator=torch.Generator().manual_seed(seed))
+    g["shs"] = g["shs"][:, :M].contiguous()
+    rs = np.random.RandomState(7 + M)
+    return S, g, rs.randn(3, H_R, W_R).astype(np.float32), rs.randn(H_R, W_R).astype(np.float32)
+
+
+# real SH basis of degree <= 3 (the rasterizer's constants, to double precision)
+_C0 = 0.28209479177387814
+_C1 = 0.4886025119029199
+_C2 = (1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396)
+_C3 = (-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154, -0.4570457994644658, 1.445305721320277,
+       -0.5900435899266435)
+
+
+def _sh_basis64(means, campos):
+    """B_k(dir) for k < 16 in float64, dir = normalize(mean - campos): [P, 16]."""
+    d = means.astype(np.float64) - np.asarray(campos, np.float64)
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    x, y, z = d[:, 0], d[:, 1], d[:, 2]
+    xx, yy, zz = x * x, y * y, z * z
+    return np.stack([np.full_like(x, _C0), -_C1 * y, _C1 * z, -_C1 * x,
+                     _C2[0] * x * y, _C2[1] * y * z, _C2[2] * (2 * zz - xx - yy), _C2[3] * x * z, _C2[4] * (xx - yy),
+                     _C3[0] * y * (3 * xx - yy), _C3[1] * x * y * z, _C3[2] * y * (4 * zz - xx - yy),
+                     _C3[3] * z * (2 * zz - 3 * xx - 3 * yy), _C3[4] * x * (4 * zz - xx - yy), _C3[5] * z * (xx - yy),
+                     _C3[6] * x * (xx - 3 * yy)], 1)
+
+
+# dL/dshs[i,k,c] = B_k(dir_i) * g_c with g the clamp-masked colour gradient.  The kernel evaluates B_k in fp32 from an fp32
+# direction: a few ulp of max(|B_k|, 1) (|B_k| <= 1.1 up to degree 2), plus one rounding of the product.  2^-20 |g_c| is
+# 8 ulp of |g_c|: derived from that error budget, not measured.
+SH_ELEMENT_BOUND = 2.0 ** -20
+
+
+def _check_sh_elements(S, means, dsh, dgeom, clamped, radii, D):
+    """Every dL/dshs[i, k, c] of a visible Gaussian within 2^-20 |g_c| of B_k(dir_i) g_c; returns max err / bound."""
+    vis = radii > 0
+    nD = (D + 1) ** 2
+    g = dgeom[:, 6:9].astype(np.float64) * (clamped == 0)
+    want = _sh_basis64(means, S.campos)[:, :nD, None] * g[:, None, :]
+    err = np.abs(dsh[:, :nD].astype(np.float64) - want)[vis]
+    bound = (SH_ELEMENT_BOUND * np.abs(g)[:, None, :] * np.ones((1, nD, 1)))[vis]
+    bad = err > bound
+    assert not bad.any(), (f"{int(bad.sum())} SH gradient elements off B_k(dir) g_c by more than 2^-20 |g_c|; worst "
+                           f"{float(err[bad].max()):.3e} at bound {float(bound[bad][np.argmax(err[bad])]):.3e}")
+    return float((err / np.maximum(bound, 1e-300)).max()) if err.size else 0.0
+
+
+def _rel(a, b):
+    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
+    return float(np.abs(a - b).max()) / max(float(np.abs(b).max()), 1e-30)
+
+
+# ------------------------------------------------------------------------------------- a. rasterizer against the oracle
+
+RASTER_CASES = [(1, 0, False), (2, 0, True), (4, 0, False), (4, 1, False), (8, 1, False), (9, 1, True), (9, 2, False),
+                (12, 2, False), (16, 2, False)]
+
+
+@pytest.mark.parametrize("M,D,aa", RASTER_CASES, ids=[f"M{m}-D{d}{'-aa' if a else ''}" for m, d, a in RASTER_CASES])
+def test_rasterizer_matches_oracle(M, D, aa):
+    """Forward and backward at M coefficients per row (the float4 row path at M = 4, 8, 12, the per-element one at M = 1,
+    2, 9; M = 16 is the control) against the oracle; dL/dshs [P, M, 3] with zero columns above the active degree, zero rows
+    for culled Gaussians, and every element against B_k(dir) g_c in float64."""
+    S, g, dC, dI = _raster_case(M, D, aa)
+    color, radii, invd, state, grads = run_gpu(S, g, dC, dI)
+    st, gref = run_oracle(S, g, dC, dI)
+    assert_forward_parity(st, color, radii, invd, state)
+    assert_grad_parity(grads, gref, st=st)
+    dsh = grads["shs"]
+    assert dsh.shape == (P_R, M, 3)
+    assert (dsh[:, (D + 1) ** 2:] == 0).all()
+    culled = radii == 0
+    assert culled[:N_CULLED].all() and (dsh[culled] == 0).all()
+    worst = _check_sh_elements(S, g["means3D"].numpy(), dsh, grads["_dgeom"], state["clamped"], radii, D)
+    ok = st.ambiguous == 0
+    print(f"[sh widths] M={M} D={D} aa={aa}: max|image-oracle| {float(np.abs(color - st.color)[:, ok].max()):.2e}, "
+          f"dL/dshs err/max {_rel(dsh, gref['dL_dsh']):.2e}, worst SH element err / bound {worst:.3f}")
+
+
+# ------------------------------------------------------------------------------- b. equivalence with zero padding to 16
+
+@pytest.mark.parametrize("M,D", [(1, 0), (2, 0), (4, 1), (9, 2), (12, 2)])
+def test_zero_padded_rows_render_the_same_bits(M, D):
+    """The same Gaussians with their rows zero-padded to M = 16 at the same degree: image, inverse depth, radii, point list
+    and tile ranges bit-identical; dL/dshs[:, :M] within SYNC_NOISE["_features"], test_gpu_free_train's bound on the
+    run-to-run spread of the composite backward's float atomics -- the spread of two runs of the padded model is measured
+    here too and must stay under the same bound; sh_staged 0, 1 and 2 (all of which fall back at M != 16) render the same
+    bits."""
+    S, g, dC, dI = _raster_case(M, D, seed=1)
+    gp = dict(g, shs=_pad16(g["shs"]))
+    a = run_gpu(S, g, dC, dI)
+    b = run_gpu(S, gp, dC, dI)
+    b2 = run_gpu(S, gp, dC, dI)
+    for i in range(3):
+        np.testing.assert_array_equal(a[i], b[i])
+    for k in ("point_list", "ranges", "tile_keys"):
+        np.testing.assert_array_equal(a[3][k], b[3][k])
+    spread = _rel(b2[4]["shs"], b[4]["shs"])
+    diff = _rel(a[4]["shs"], b[4]["shs"][:, :M])
+    print(f"[sh widths] M={M} D={D} vs zero-padded: dL/dshs |diff|/max {diff:.2e}, padded run-to-run {spread:.2e}")
+    assert spread <= SYNC_NOISE["_features"] and diff <= SYNC_NOISE["_features"]
+    assert (b[4]["shs"][:, M:] == 0).all()
+    for staged in (0, 1, 2):
+        with _Options({"sh_staged": staged}):
+            c = run_gpu(S, g, dC, dI)
+        for i in range(3):
+            np.testing.assert_array_equal(a[i], c[i])
+        assert _rel(c[4]["shs"], a[4]["shs"]) <= SYNC_NOISE["_features"]
+        _check_sh_elements(S, g["means3D"].numpy(), c[4]["shs"], c[4]["_dgeom"], c[3]["clamped"], c[1], D)
+
+
+# ------------------------------------------------------------------------------------------- c. DIRECT_SH_GRAD at M < 16
+
+def _shim_backward(S, g, dC, dI, sink=None):
+    """Forward + backward through the shim; with `sink`, `shs` is a leaf whose .grad is that view and DIRECT_SH_GRAD is on."""
+    t = {k: v.cuda() for k, v in g.items()}
+    sh = torch.nn.Parameter(t["shs"].clone())
+    if sink is not None:
+        sh.grad = sink
+    r = dgr.GaussianRasterizer(raster_settings=gpu_settings(S))
+    old = rasterizer.DIRECT_SH_GRAD
+    rasterizer.DIRECT_SH_GRAD = sink is not None
+    try:
+        color, radii, invd = r(means3D=t["means3D"], means2D=torch.zeros_like(t["means3D"], requires_grad=True), opacities=t["opacities"],
+                               shs=sh, scales=t["scales"], rotations=t["rotations"])
+        ((color * torch.tensor(dC, device="cuda")).sum() + (invd[0] * torch.tensor(dI, device="cuda")).sum()).backward()
+    finally:
+        rasterizer.DIRECT_SH_GRAD = old
+    torch.cuda.synchronize()
+    return sh, radii.cpu().numpy()
+
+
+@pytest.mark.parametrize("M,D", [(1, 0), (4, 1), (9, 2)])
+def test_direct_sh_grad_sink_at_fewer_coefficients(M, D):
+    """The in-place SH gradient (a contiguous, 16-byte-aligned view into a larger buffer, pre-filled with NaN): every row
+    overwritten (culled rows with zeros), the canary after it untouched, and the result the autograd path's."""
+    S, g, dC, dI = _raster_case(M, D, seed=2)
+    n = P_R * M * 3
+    buf = torch.full((n + 64,), float("nan"), device="cuda")
+    buf[n:] = 1234.5
+    sink = buf[:n].view(P_R, M, 3)
+    assert sink.data_ptr() % 16 == 0 and sink.is_contiguous()
+    sh, radii = _shim_backward(S, g, dC, dI, sink)
+    assert sh.grad.data_ptr() == buf.data_ptr()
+    got = buf[:n].view(P_R, M, 3).cpu().numpy()
+    assert np.isfinite(got).all()
+    assert (buf[n:] == 1234.5).all()
+    assert (got[radii == 0] == 0).all() and (radii == 0).sum() >= N_CULLED
+    ref, radii2 = _shim_backward(S, g, dC, dI)
+    np.testing.assert_array_equal(radii, radii2)
+    ref = ref.grad.cpu().numpy()
+    assert _rel(got, ref) <= SYNC_NOISE["_features"]
+    np.testing.assert_array_equal(got[radii == 0], ref[radii == 0])
+
+
+# --------------------------------------------------------------------------------------------- d. Adam, period != 16
+
+@pytest.mark.parametrize("period", [1, 4, 9])
+def test_adam_abi_packed_segment_period(period):
+    """gms_adam_step through the raw C ABI with a packed segment of inner 3 and period 1, 4 or 9, segment ends that are not
+    multiples of 4, and a shard offset, against a float64 restatement of torch.optim.Adam's update."""
+    gen = torch.Generator().manual_seed(period)
+    n_total = 64 * 37
+    ends = [103, 103 + 3 * period * 23 + 2, n_total]
+    lr0, lr1, inner, per = [1e-2, 3e-3, 5e-2], [1e-2, 2e-4, 5e-2], [1, 3, 1], [0, period, 0]
+    p0 = torch.randn(n_total, generator=gen); g0 = torch.randn(n_total, generator=gen) * 0.1
+    m0 = torch.randn(n_total, generator=gen) * 0.01; v0 = torch.rand(n_total, generator=gen) * 1e-3
+    idx = torch.arange(n_total)
+    lr = torch.full((n_total,), lr0[2], dtype=torch.float64)
+    seg = (idx >= ends[0]) & (idx < ends[1])
+    lr[seg] = torch.where(((idx[seg] - ends[0]) // 3) % period == 0, lr0[1], lr1[1]).double()
+    lr[idx < ends[0]] = lr0[0]
+    step, b1, b2, eps = 5, 0.9, 0.999, 1e-15
+    m_ref = b1 * m0.double() + (1 - b1) * g0.double()
+    v_ref = b2 * v0.double() + (1 - b2) * g0.double() ** 2
+    p_ref = p0.double() - lr / (1 - b1 ** step) * m_ref / (v_ref.sqrt() / (1 - b2 ** step) ** 0.5 + eps)
+    for off, n in ((0, n_total), (64 * 3, 64 * 21), (8, n_total - 8 - 5)):
+        p, g, m, v = (t.clone().cuda() for t in (p0, g0, m0, v0))
+        a = _lib.AdamArgs()
+        a.n, a.offset = n, off
+        a.p, a.g, a.m, a.v = (t[off:].data_ptr() for t in (p, g, m, v))
+        a.nseg = 3
+        for i in range(3):
+            a.seg_end[i], a.lr0[i], a.lr1[i], a.inner[i], a.period[i] = ends[i], lr0[i], lr1[i], inner[i], per[i]
+        a.beta1, a.beta2, a.eps, a.step, a.zero_grad, a.zero_end = b1, b2, eps, step, 0, 0
+        _lib.check(_lib.lib().gms_adam_step(C.byref(a), torch.cuda.current_stream().cuda_stream), "gms_adam_step")
+        sl = slice(off, off + n)
+        np.testing.assert_allclose(p.cpu()[sl].numpy(), p_ref[sl].float().numpy(), rtol=2e-5, atol=1e-7)
+        np.testing.assert_allclose(m.cpu()[sl].numpy(), m_ref[sl].float().numpy(), rtol=2e-6, atol=2e-8)
+        np.testing.assert_allclose(v.cpu()[sl].numpy(), v_ref[sl].float().numpy(), rtol=2e-6, atol=1e-12)
+        untouched = torch.ones(n_total, dtype=torch.bool); untouched[sl] = False
+        assert torch.equal(p.cpu()[untouched], p0[untouched])
+
+
+def _torch_adam_like(opt):
+    """torch.optim.Adam over copies of FlatAdam's parameters, the packed SH group split into f_dc and f_rest groups."""
+    groups, copies = [], []
+    for gr in opt.groups:
+        p = gr["param"].detach()
+        if "period" in gr:
+            dc, rest = torch.nn.Parameter(p[:, :1].clone()), torch.nn.Parameter(p[:, 1:].clone())
+            groups += [dict(params=[dc], lr=gr["lr0"]), dict(params=[rest], lr=gr["lr1"])]
+            copies.append((gr["param"], (dc, rest)))
+        else:
+            c = torch.nn.Parameter(p.clone())
+            groups.append(dict(params=[c], lr=gr["lr"]))
+            copies.append((gr["param"], (c,)))
+    return torch.optim.Adam(groups, lr=0.0, eps=1e-15), copies
+
+
+def _flat_adam_five_steps(opt):
+    adam, copies = _torch_adam_like(opt)
+    gen = torch.Generator(device="cuda").manual_seed(11)
+    for it in range(5):
+        for p, cs in copies:
+            gr = 1e-2 * torch.randn(p.shape, device="cuda", generator=gen)
+            p.grad.copy_(gr)
+            if len(cs) == 2:
+                cs[0].grad, cs[1].grad = gr[:, :1].clone(), gr[:, 1:].clone()
+            else:
+                cs[0].grad = gr.clone()
+        opt.step()
+        adam.step()
+    for p, cs in copies:
+        want = torch.cat([c.detach() for c in cs], 1) if len(cs) == 2 else cs[0].detach()
+        torch.testing.assert_close(p.detach(), want, rtol=1e-5, atol=1e-7)
+
+
+def _free_raw(P, M, kind="gs", seed=3):
+    g = random_gaussians(P, seed=seed, extent=0.8, flat_frac=0.0)
+    gen = torch.Generator().manual_seed(seed + 1)
+    s = torch.log(g["scales"])
+    if kind == "gs_flat":
+        s = s[:, 1:]
+    rot = g["rotations"] * (0.5 + torch.rand(P, 1, generator=gen))
+    return dict(xyz=g["means3D"], scaling=s.contiguous(), rotation=rot, features=g["shs"][:, :M].contiguous(),
+                opacity=torch.logit(g["opacities"]))
+
+
+def _free_model(raw, kind, degree):
+    return FreeGaussianModel(raw["xyz"], raw["scaling"], raw["rotation"], raw["features"], raw["opacity"], kind, "cuda", degree)
+
+
+@pytest.mark.parametrize("M", [1, 4, 9])
+def test_flat_adam_groups_match_torch_adam(M):
+    """FlatAdam over free_model_groups and mesh_model_groups at M = 1, 4, 9 (the SH segment's DC / rest phase has period M)
+    against torch.optim.Adam with separate f_dc / f_rest groups (f_rest empty at M = 1), 5 steps."""
+    m = _free_model(_free_raw(501, M), "gs", 3)
+    _flat_adam_five_steps(FlatAdam(free_model_groups(m, 1e-3)))
+    p = scenes.init_mesh_gaussians(*scenes.icosphere(2), K=3, seed=3, sh_coeffs=M)
+    mm = MeshGaussianModel.from_params(p, "cuda", packed_features=True)
+    assert mm._features.shape[1] == M
+    _flat_adam_five_steps(FlatAdam(mesh_model_groups(mm)))
+
+
+# --------------------------------------------------------------------------------------------- e. one-call frames
+
+def _degrees(M):
+    top = int(round(M ** 0.5)) - 1
+    return [top] if top == 0 else [top, top - 1]
+
+
+FRAME_CASES = [(M, d) for M in (1, 4, 9) for d in _degrees(M)]
+
+
+@pytest.mark.parametrize("kind", ["gs", "gs_flat"])
+@pytest.mark.parametrize("M,degree", FRAME_CASES)
+def test_free_train_frame_matches_oracle(kind, M, degree):
+    """gms_free_train_frame at M coefficients: the sync-free frame against the float64 oracle chain (radii and N bit-exact,
+    image, loss, raw gradients within RAW_TOL), its image bit-identical to the synchronising first frame's, and
+    gms_free_render_frame giving the same image and radii."""
+    W, H = 272, 208
+    raw = _free_raw(3000, M, kind)
+    cam = scenes.ring_cameras(8, 2.5, W, H)[1]
+    cam_d, gt, bg = cam.to("cuda"), torch.rand(3, H, W, generator=torch.Generator().manual_seed(M)).cuda(), torch.tensor(BG, device="cuda")
+    m = _free_model(raw, kind, degree)
+    assert m.active_sh_degree == degree
+    opt = FlatAdam(free_model_groups(m, 1e-3))
+    fr = NativeFreeFrame(m, W, H, LAMBDA)
+    fr.run(cam_d, gt, bg, stats=False)
+    torch.cuda.synchronize()
+    first = _views(fr, m.P)
+    loss = float(fr.run(cam_d, gt, bg, stats=False))
+    torch.cuda.synchronize()
+    assert fr.overflows == 0 and fr.capacity > fr.last_num_rendered > 0
+    out = _views(fr, m.P)
+    assert torch.equal(first["image"], out["image"]) and torch.equal(first["radii"], out["radii"])
+    image, radii, _ = NativeFreeRenderer(m, W, H).render(cam_d, bg)
+    torch.cuda.synchronize()
+    assert torch.equal(image, out["image"]) and torch.equal(radii, out["radii"])
+    img = out["image"].cpu().double().requires_grad_(True)
+    aten_reference.training_loss(img, gt.cpu().double(), LAMBDA).backward()
+    S = settings_from_camera(cam, sh_degree=degree, bg=BG)
+    st, og = _oracle_raw(raw, kind, out, img.grad.float().numpy(), S)
+    np.testing.assert_array_equal(out["radii"].cpu().numpy(), st.radii)
+    assert fr.last_num_rendered == st.N
+    assert_image_parity(st, out["image"].cpu().numpy())
+    ref_loss = float(aten_reference.training_loss(torch.tensor(st.color, dtype=torch.float64), gt.cpu().double(), LAMBDA))
+    assert abs(loss - ref_loss) <= 1e-5 * max(1.0, abs(ref_loss))
+    assert m._features.grad.shape == (m.P, M, 3)
+    errs = {k: _rel(getattr(m, k).grad.detach().cpu().double().reshape(ref.shape), ref) for k, ref in og.items()}
+    print(f"[sh widths free frame {kind} M={M} D={degree}] grad err/max: " + ", ".join(f"{k} {e:.2e}" for k, e in errs.items()))
+    for k, e in errs.items():
+        assert e <= RAW_TOL[k], (k, e)
+
+
+@pytest.mark.parametrize("M,degree", FRAME_CASES)
+def test_mesh_train_frame_matches_oracle(M, degree):
+    """gms_train_frame through MeshTrainer(native=True) at M coefficients (no factored / fused SH path) against the oracle
+    chain: radii and N bit-exact, image, loss and every raw gradient within GRAD_TOL."""
+    W, H = 256, 240
+    p = scenes.init_mesh_gaussians(*scenes.icosphere(3), K=3, seed=21, trained_like=True, sh_coeffs=M)
+    cam = scenes.look_at_camera((2.2, 0.7, 1.0), (0, 0, 0), W, H)
+    gt = torch.rand(3, H, W, generator=torch.Generator().manual_seed(M))
+    model = MeshGaussianModel.from_params(p, "cuda", sh_degree=degree, active_sh_degree=degree, packed_features=True)
+    tr = MeshTrainer(model, torch.tensor(BG, device="cuda"), LAMBDA, native=True, optimizer_step=False)
+    assert tr.sh_factored is False
+    cam_d, gt_d = cam.to("cuda"), gt.cuda()
+    tr.step(cam_d, gt_d)                    # the first (synchronising) frame; the second is sync-free
+    model.vertices.grad.zero_()
+    loss = float(tr._frame.run(cam_d, gt_d, tr.bg))
+    torch.cuda.synchronize()
+    fr = tr._frame
+    P = model._scale.shape[0]
+    out = _frame_outputs(fr, P)
+    img = out["image"].double().requires_grad_(True)
+    aten_reference.training_loss(img, gt.double(), LAMBDA).backward()
+    S = settings_from_camera(cam, sh_degree=degree, bg=BG)
+    st, og = oracle_chain(p, S, img.grad.float().numpy(), (out["xyz"], out["scales"], out["rotations"]))
+    np.testing.assert_array_equal(out["radii"].numpy(), st.radii)
+    assert fr.last_num_rendered == st.N
+    assert_image_parity(st, out["image"].numpy())
+    ref_loss = float(aten_reference.training_loss(torch.tensor(st.color, dtype=torch.float64), gt.double(), LAMBDA))
+    assert abs(loss - ref_loss) <= 1e-5 * max(1.0, abs(ref_loss))
+    fg = model._features.grad.detach().cpu()
+    assert fg.shape == (P, M, 3)
+    got = dict(vertices=model.vertices.grad, _alpha=model._alpha.grad, _scale=model._scale.grad, _opacity=model._opacity.grad,
+               _features_dc=fg[:, :1], _features_rest=fg[:, 1:])
+    errs = {k: _rel(got[k].detach().cpu().reshape(r.shape), r) if r.numel() else 0.0 for k, r in og.items()}
+    print(f"[sh widths mesh frame M={M} D={degree}] grad err/max: " + ", ".join(f"{k} {e:.2e}" for k, e in errs.items()))
+    for k, e in errs.items():
+        assert e <= GRAD_TOL.get(k, 2e-4), (k, e)
+
+
+@pytest.mark.parametrize("M,degree", FRAME_CASES)
+def test_render_frames_equal_the_zero_padded_model(M, degree):
+    """gms_render_frame (one mesh and a segmented multi-mesh model), gms_free_render_frame, gms_points_render_frame,
+    gms_bound_points_render_frame (the pseudo-mesh bound to a driving mesh, drawn at a moved pose) and
+    gms_flame_render_frame (a gs_flame checkpoint) at M coefficients render the same image and radii, bit for bit, as the
+    same model zero-padded to M = 16."""
+    from gms_b200.model import MultiMeshGaussianModel
+    W, H = 240, 176
+    cam, bg = scenes.look_at_camera((2.2, 0.7, 1.0), (0, 0, 0), W, H).to("cuda"), torch.tensor(BG, device="cuda")
+
+    def same(render_a, render_b, tag):
+        a = [t.clone() for t in render_a()]
+        b = [t.clone() for t in render_b()]
+        torch.cuda.synchronize()
+        assert torch.equal(a[0], b[0]) and torch.equal(a[1], b[1]), tag
+        assert (a[1] > 0).any(), tag
+
+    p = scenes.init_mesh_gaussians(*scenes.icosphere(3), K=3, seed=4, trained_like=True, sh_coeffs=M)
+    q = copy.copy(p)
+    q._features_rest = _pad16(torch.cat((p._features_dc, p._features_rest), 1))[:, 1:]
+    mk = lambda x: MeshGaussianModel.from_params(x, "cuda", sh_degree=degree, active_sh_degree=degree, packed_features=True)
+    ma, mb = mk(p), mk(q)
+    same(lambda: NativeRenderer(ma, W, H).render(cam, bg), lambda: NativeRenderer(mb, W, H).render(cam, bg), "mesh")
+    plists = []
+    for feats in (M, 16):
+        pl = []
+        for k, (K, lvl) in enumerate(((2, 2), (5, 1))):
+            v, f = scenes.icosphere(lvl, radius=0.4)
+            x = scenes.init_mesh_gaussians(v + np.float32([0.7 * k - 0.35, 0.1 * k, 0]), f, K=K, seed=9 + k, sh_coeffs=M)
+            if feats == 16:
+                x._features_rest = _pad16(torch.cat((x._features_dc, x._features_rest), 1))[:, 1:]
+            pl.append(x)
+        plists.append(MultiMeshGaussianModel.from_mesh_params(pl, "cuda", sh_degree=degree, active_sh_degree=degree,
+                                                              packed_features=True, segmented=True))
+    assert plists[0].segments is not None
+    same(lambda: NativeRenderer(plists[0], W, H).render(cam, bg), lambda: NativeRenderer(plists[1], W, H).render(cam, bg), "segments")
+    raw = _free_raw(2000, M, "gs_flat", seed=M)
+    fa = _free_model(raw, "gs_flat", degree)
+    fb = _free_model(dict(raw, features=_pad16(raw["features"])), "gs_flat", degree)
+    same(lambda: NativeFreeRenderer(fa, W, H).render(cam, bg), lambda: NativeFreeRenderer(fb, W, H).render(cam, bg), "free")
+    args = (raw["xyz"], raw["scaling"], raw["rotation"])
+    pa = PointsModel.from_gaussians(*args, raw["features"][:, :1], raw["features"][:, 1:], raw["opacity"], "cuda", degree)
+    pf = _pad16(raw["features"])
+    pb = PointsModel.from_gaussians(*args, pf[:, :1], pf[:, 1:], raw["opacity"], "cuda", degree)
+    same(lambda: PointsRenderer(pa, W, H).render(cam, bg), lambda: PointsRenderer(pb, W, H).render(cam, bg), "points")
+    v, f = scenes.icosphere(2, radius=0.8)
+    v, f = torch.from_numpy(v).cuda(), torch.from_numpy(f).cuda()
+    ba, bb = pa.bind_to_mesh(v, f), pb.bind_to_mesh(v, f)
+    moved = v * torch.tensor([1.1, 0.95, 1.0], device="cuda")
+    same(lambda: MeshBoundPointsRenderer(ba, W, H).render(cam, bg, vertices=moved),
+         lambda: MeshBoundPointsRenderer(bb, W, H).render(cam, bg, vertices=moved), "bound points")
+    ck = _flame_checkpoints(M, degree)
+    fcam = scenes.look_at_camera((0.3, 0.1, 0.2), (0, 0, 0), W, H).to("cuda")
+    same(lambda: FlameRenderer(ck[0], W, H).render(fcam, bg), lambda: FlameRenderer(ck[1], W, H).render(fcam, bg), "flame")
+
+
+def _flame_scene(sh_degree, K=10, W=256, H=256):
+    """test_gpu_flame's synthetic FLAME scene with a model of (sh_degree + 1)^2 coefficients whose rows are all non-zero."""
+    torch.manual_seed(0)
+    drv = flame_driver.SyntheticFlame(rings=23, segments=24).cuda()
+    m = FlameGaussianModel.create(drv, torch.from_numpy(drv.faces).cuda(), K=K, seed=3, sh_degree=sh_degree)
+    with torch.no_grad():
+        m._features[:, 1:] = 0.2 * torch.randn(m._features[:, 1:].shape, device="cuda", generator=torch.Generator(device="cuda").manual_seed(5))
+    m.active_sh_degree = sh_degree
+    cams = [scenes.look_at_camera((0.35 * np.cos(a), 0.1, 0.35 * np.sin(a)), (0, 0, 0), W, H).to("cuda")
+            for a in np.linspace(0, 2 * np.pi, 4, endpoint=False)]
+    g = torch.Generator(device="cuda").manual_seed(1)
+    return m, cams, [torch.rand(3, H, W, device="cuda", generator=g) for _ in cams], torch.ones(3, device="cuda")
+
+
+def _flame_checkpoints(M, degree):
+    """A gs_flame checkpoint of M coefficients as io_ply.save_flame_model writes it, and the same zero-padded to 16, both
+    posed by the driver."""
+    import tempfile
+    from gms_b200 import io_ply
+    m, _, _, _ = _flame_scene(int(round(M ** 0.5)) - 1)
+    with tempfile.TemporaryDirectory() as d:
+        ply = f"{d}/point_cloud.ply"
+        io_ply.save_flame_model(ply, m)
+        data = io_ply.load_flame_model(ply)
+    assert data["_features_rest"].shape[1] == M - 1
+    padded = dict(data, _features_rest=_pad16(torch.cat((data["_features_dc"], data["_features_rest"]), 1))[:, 1:])
+    out = [FlameCheckpoint(c, "cuda", active_sh_degree=degree) for c in (data, padded)]
+    for c in out:
+        c.vertices = c.driver_vertices(m.driver)
+    assert out[0].active_sh_degree == out[1].active_sh_degree == degree
+    return out
+
+
+@pytest.mark.parametrize("M", [1, 4, 9])
+def test_densify_copies_rows_of_3M_floats(M):
+    """gms_densify_plan / gms_densify_apply with F = 3M floats per feature row and P not a multiple of the block size,
+    against the restated reference densification: kept and cloned rows (features included) exact, split children within a
+    few ulp, every moment exact (appended rows start at zero)."""
+    P = 50_001
+    gen = torch.Generator(device="cuda").manual_seed(M)
+    r = lambda *s: torch.randn(*s, device="cuda", generator=gen)
+    st = dict(xyz=r(P, 3), scaling=float(np.log(0.05)) + 1.2 * r(P, 3), rotation=r(P, 4), opacity=2 * r(P, 1), features=r(P, M, 3))
+    for n in D.NAMES:
+        st["m_" + n], st["v_" + n] = 1e-3 * r(*st[n].shape), 1e-6 * r(*st[n].shape).abs()
+    denom = torch.randint(0, 5, (P,), device="cuda", generator=gen).float()
+    accum = 3e-4 * r(P).abs() * 4
+    accum[denom == 0] = 0
+    normals = r(P, 2, 3)
+    for size_prune in (False, True):
+        tr = _trainer_from_state({k: v.cpu() for k, v in st.items()}, "gs", accum, denom, 3.0)
+        counts = tr.densify(size_prune=size_prune, normals=normals)
+        ref, _, rcounts = D.densify(st, accum, denom, normals, 3.0, size_prune=size_prune)
+        assert counts == rcounts and min(counts[1:4]) > 0
+        got = _native_state(tr)
+        assert got["features"].shape == (counts[0], M, 3)
+        _compare_densified(got, {k: v.cpu() for k, v in ref.items()}, counts, f"M={M} size_prune={size_prune}")
+
+
+# --------------------------------------------------------------------------------------------- f. trainers
+
+def _close_up_to_adam_sign_flips(a, b, lr, tag, steps=3):
+    """Within rtol 1e-3 / atol 2e-3 (test_gpu_step's bound for the two arms), except that Adam (eps 1e-15) moves an element
+    whose gradient is at the level of the float-atomic noise by about +/- lr whatever its size, so the two arms may step a
+    few such elements in opposite directions: at most max(2, 1e-4 of the elements) outside the bound, none by more than
+    2 lr per step."""
+    a, b = a.detach().double().cpu(), b.detach().double().cpu()
+    d = (a - b).abs()
+    over = int((d > 2e-3 + 1e-3 * b.abs()).sum())
+    print(f"[sh widths] {tag}: max|native - reference| {float(d.max()) if d.numel() else 0.0:.2e}, {over} of {d.numel()} over the bound")
+    assert over <= max(2, 1e-4 * d.numel()), (tag, over)
+    assert d.numel() == 0 or float(d.max()) <= 2 * steps * lr, tag
+
+
+@pytest.mark.parametrize("degree", [0, 1, 2])
+def test_mesh_trainer_tracks_the_reference_arm(degree):
+    """MeshTrainer(native=True) at M = (degree + 1)^2 against the reference-ordered arm (two-step expansion, ATen loss,
+    torch.optim.Adam with f_dc / f_rest groups) for three steps; oneupSHdegree stops at the model's degree."""
+    M = (degree + 1) ** 2
+    W, H = 320, 240
+    p = scenes.init_mesh_gaussians(*scenes.icosphere(4), K=3, seed=5, sh_coeffs=M)
+    cam = scenes.look_at_camera((2.4, 0.5, 0.9), (0, 0, 0), W, H).to("cuda")
+    bg = torch.ones(3, device="cuda")
+    gt_model = MeshGaussianModel.from_params(scenes.init_mesh_gaussians(*scenes.icosphere(4), K=3, seed=77), "cuda")
+    with torch.no_grad():
+        gt = render_frame(gt_model, cam, bg)[0].clamp(0, 1).contiguous()
+    ma = MeshGaussianModel.from_params(p, "cuda", sh_degree=degree, active_sh_degree=0, packed_features=True)
+    mb = MeshGaussianModel.from_params(p, "cuda", sh_degree=degree, active_sh_degree=0, packed_features=False)
+    for m in (ma, mb):
+        for _ in range(5):
+            m.oneupSHdegree()
+        assert m.active_sh_degree == degree
+    ta = MeshTrainer(ma, bg, native=True)
+    tb = MeshTrainer(mb, bg, fast=False, loss_fn=aten_reference.training_loss)
+    assert ta.sh_factored is False
+    la = [ta.step(cam, gt).item() for _ in range(3)]
+    lb = [tb.step(cam, gt).item() for _ in range(3)]
+    print(f"[sh widths mesh trainer M={M}] losses native {la}, reference {lb}")
+    np.testing.assert_allclose(la, lb, rtol=2e-4)
+    assert la[2] < la[0]
+    lrs = {g["name"]: g["lr"] for g in tb.opt.param_groups}
+    for n, lr in (("_opacity", lrs["opacity"]), ("_features_dc", lrs["f_dc"]), ("_features_rest", lrs["f_rest"])):
+        _close_up_to_adam_sign_flips(getattr(ma, n), getattr(mb, n), lr, n)
+    # resume: state_dict -> load_state_dict into a new trainer of a fresh model restores every parameter, moment, step count
+    # and the active degree bit for bit
+    state = ta.state_dict()
+    mc = MeshGaussianModel.from_params(p, "cuda", sh_degree=degree, active_sh_degree=0, packed_features=True)
+    tc = MeshTrainer(mc, bg, native=True)
+    tc.load_state_dict(state)
+    assert mc.active_sh_degree == degree and tc.opt.steps == ta.opt.steps
+    for n in ("p", "m", "v"):
+        assert torch.equal(getattr(tc.opt, n), getattr(ta.opt, n)), n
+    for n in ("vertices", "_alpha", "_scale", "_opacity", "_features"):
+        assert getattr(mc, n).shape[1:] == getattr(ma, n).shape[1:] and torch.equal(getattr(mc, n), getattr(ma, n)), n
+
+
+@pytest.mark.parametrize("degree", [0, 1, 2])
+def test_free_trainer_at_fewer_coefficients(degree):
+    """FreeTrainer at M = (degree + 1)^2 (dense SH gradient rows and FlatAdam.step instead of the fused SH step), against
+    the reference-ordered arm: steps 1 and 2 against torch.optim.Adam with f_dc / f_rest groups fed each frame's own
+    gradients, the densification of step 3 against the restated reference densification on the same state and draws.
+    oneupSHdegree stops at the model's degree; the densification leaves the features and their Adam group at [P', M, 3];
+    state_dict resumes bit for bit."""
+    M = (degree + 1) ** 2
+    W, H = 256, 256
+    raw = _free_raw(4000, M, "gs_flat", seed=30 + degree)
+    cams = [c.to("cuda") for c in scenes.ring_cameras(4, 2.5, W, H)]
+    bg = torch.tensor(BG, device="cuda")
+    gts = [torch.rand(3, H, W, generator=torch.Generator().manual_seed(i)).cuda() for i in range(4)]
+    m = _free_model(raw, "gs_flat", 0)
+    for _ in range(5):
+        m.oneupSHdegree()
+    assert m.active_sh_degree == m.max_sh_degree == degree
+    draws = torch.Generator(device="cuda").manual_seed(degree)
+
+    class Checked(FreeTrainer):
+        def densify(self, size_prune, normals=None):
+            st = {n: getattr(self.model, "_" + n).detach().clone() for n in D.NAMES}
+            nat = _native_state(self)
+            for n in D.NAMES:
+                st["m_" + n], st["v_" + n] = nat["m_" + n].cuda(), nat["v_" + n].cuda()
+            acc, den = self.frame.accum.clone(), self.frame.denom.clone()
+            normals = torch.randn(max(self.model.P, 1), 2, 3, device="cuda", generator=draws)
+            counts = super().densify(size_prune, normals)
+            ref, _, rc = D.densify(st, acc, den, normals, self.extent, size_prune=size_prune)
+            assert counts == rc
+            _compare_densified(_native_state(self), {k: v.cpu() for k, v in ref.items()}, counts, f"FreeTrainer M={M}")
+            return counts
+
+    tr = Checked(m, bg, 3.0, FreeOptimizationParams(densify_from_iter=2, densification_interval=3, densify_until_iter=100))
+    assert tr.fused_sh is False
+    # steps 1 and 2: torch.optim.Adam with f_dc / f_rest groups on copies of the parameters, fed the frames' own gradients
+    adam, copies = _torch_adam_like(tr.adam)
+    for it in (1, 2):
+        adam.param_groups[0]["lr"] = tr._xyz_lr(it)
+        seen = {}
+        tr.step(cams[it - 1], gts[it - 1], before_update=lambda: seen.update({n: getattr(m, n).grad.detach().clone() for n in m.NAMES}))
+        for (p_, cs), n in zip(copies, ("_xyz", "_scaling", "_rotation", "_opacity", "_features")):
+            assert p_ is getattr(m, n)
+            if len(cs) == 2:
+                cs[0].grad, cs[1].grad = seen[n][:, :1].clone(), seen[n][:, 1:].clone()
+            else:
+                cs[0].grad = seen[n].clone()
+        adam.step()
+        torch.cuda.synchronize()
+        assert seen["_features"].shape == (4000, M, 3) and seen["_features"].abs().max() > 0
+        for p_, cs in copies:
+            want = torch.cat([c.detach() for c in cs], 1) if len(cs) == 2 else cs[0].detach()
+            torch.testing.assert_close(p_.detach(), want, rtol=1e-5, atol=1e-7)
+    # step 3: the densification (checked in Checked.densify) changes P, the features stay [P', M, 3]
+    tr.step(cams[2], gts[2])
+    assert len(tr.densifications) == 1 and m.P != 4000
+    fi = tr.adam.group_index("features")
+    assert m._features.shape == (m.P, M, 3) and tuple(tr.adam.groups[fi]["param"].shape) == (m.P, M, 3)
+    assert m._features.grad.shape == (m.P, M, 3)
+    tr.step(cams[3], gts[3])
+    torch.cuda.synchronize()
+    # resume: a new trainer of a model with the current shapes restores the optimizer, the statistics and the degree bit for bit
+    state = tr.state_dict()
+    snap = {n: getattr(m, n).detach().clone() for n in m.NAMES}
+    m2 = FreeGaussianModel(snap["_xyz"], torch.zeros_like(snap["_scaling"]), snap["_rotation"], torch.zeros_like(snap["_features"]),
+                           snap["_opacity"], "gs_flat", "cuda", 0)
+    tr2 = FreeTrainer(m2, bg, 3.0, tr.opt)
+    tr2.load_state_dict(state)
+    assert m2.active_sh_degree == degree and tr2.iteration == tr.iteration and tr2.adam.steps == tr.adam.steps
+    for n in ("p", "m", "v"):
+        assert torch.equal(getattr(tr2.adam, n), getattr(tr.adam, n)), n
+    for n in m.NAMES:
+        assert torch.equal(getattr(m2, n), snap[n]), n
+    st2 = tr2.state_dict()
+    assert torch.equal(st2["accum"], state["accum"]) and torch.equal(st2["denom"], state["denom"])
+
+
+@pytest.mark.parametrize("degree", [0, 1, 2])
+def test_flame_trainer_tracks_the_reference_arm(degree):
+    """FlameTrainer at M = (degree + 1)^2 (flame_model_groups' packed SH segment with period M, FlatAdam.step instead of the
+    fused SH step) against the reference arm for three steps, with test_gpu_flame's bound: 10x the run-to-run spread of two
+    native runs or 1 % of the group's learning rate, at most max(2, 1e-4 of the elements) over it, none over 6 lr.
+    oneupSHdegree stops at the model's degree."""
+    M = (degree + 1) ** 2
+    runs = []
+    for arm in (True, False):
+        m, cams, gts, bg = _flame_scene(degree)
+        m.active_sh_degree = 0
+        for _ in range(5):
+            m.oneupSHdegree()
+        assert m.active_sh_degree == m.max_sh_degree == degree and m._features.shape[1] == M
+        a = fr.AtenFlameArm(m, bg) if arm else None
+        t = FlameTrainer(m, bg)
+        assert t.fused_sh is False
+        fi = t.adam.group_index("features")
+        assert t.adam.groups[fi]["period"] == M
+        losses = []
+        for i in range(3):
+            ln = float(t.step(cams[i % 4], gts[i % 4]))
+            losses.append((ln, float(a.step(cams[i % 4], gts[i % 4])) if arm else None))
+        torch.cuda.synchronize()
+        runs.append((m, a, losses))
+    (m, arm, losses), (m2, _, _) = runs
+    print(f"[sh widths flame M={M}] losses (native, reference) {losses}")
+    for ln, lr in losses:
+        assert abs(ln - lr) <= 1e-4 * abs(lr)
+    lrs = {g["name"]: g["lr"] for g in arm.adam.param_groups}
+    mine = lambda mm, n: mm._features[:, :1] if n == "_features_dc" else mm._features[:, 1:] if n == "_features_rest" else getattr(mm, n)
+    for n in fr.AtenFlameArm.NAMES + ("_alpha", "_scales", "_opacity", "_features_dc", "_features_rest"):
+        p, r, p2 = mine(m, n).detach(), arm.p[n].detach(), mine(m2, n).detach()
+        if p.numel() == 0:
+            continue
+        d, noise = float((p - r).abs().max()), float((p - p2).abs().max())
+        bound = max(10 * noise, 1e-2 * lrs[n])
+        over = int(((p - r).abs() > bound).sum())
+        print(f"[sh widths flame M={M}] after 3 steps {n}: max|native - reference| {d:.3e}, run-to-run {noise:.3e}, {over} of {p.numel()} over {bound:.3e}")
+        assert over <= max(2, 1e-4 * p.numel()) and d <= 6 * lrs[n], n
+
+
+# --------------------------------------------------------------------------------------------- g. command line
+
+@pytest.fixture(scope="module")
+def cli_scene(tmp_path_factory):
+    from test_gpu_dataset import _write_rendered_blender
+    root = str(tmp_path_factory.mktemp("sh_cli_scene") / "scene")
+    _write_rendered_blender(root)
+    return root
+
+
+def _api_loop(root, argv, hooks):
+    """The library loop the command line stands for, at the argv's --sh_degree: load_scene's view order, the trainer,
+    before_update at the same iterations.  Returns the final parameters."""
+    from gms_b200 import dataset
+    from gms_b200.cli import train as cli_train
+    args = cli_train.parse_args(["-s", root] + argv)
+    if args.gs_type == "gs_mesh":
+        sc = dataset.load_scene(root, "gs_mesh", eval=True, num_splats=2)
+        m = MeshGaussianModel.from_params(cli_train._mesh_params(sc.mesh, args.sh_degree), "cuda", sh_degree=args.sh_degree,
+                                          active_sh_degree=0, packed_features=True)
+        tr = MeshTrainer(m, torch.zeros(3, device="cuda"), native=True)
+        for it, v in enumerate(sc.view_order(args.iterations), 1):
+            tr.optimizer_step = it < args.iterations
+            tr.step(sc.train_cameras[v], sc.train_images[v], before_update=(lambda: None) if it in hooks else None)
+        names = ("vertices", "_alpha", "_scale", "_features", "_opacity")
+    else:
+        sc = dataset.load_scene(root, args.gs_type, eval=True)
+        m = FreeGaussianModel.from_point_cloud(*sc.point_cloud[:2], args.gs_type, args.sh_degree)
+        tr = FreeTrainer(m, torch.zeros(3, device="cuda"), sc.cameras_extent, cli_train.free_params(args), white_background=False,
+                         generator=torch.Generator(device="cuda").manual_seed(0))
+        for it, v in enumerate(sc.view_order(args.iterations), 1):
+            tr.step(sc.train_cameras[v], sc.train_images[v], before_update=(lambda: None) if it in hooks else None)
+        names = FreeGaussianModel.NAMES
+    torch.cuda.synchronize()
+    return {n: getattr(m, n).detach().clone() for n in names}
+
+
+@pytest.mark.parametrize("gs_type,degree", [("gs_mesh", 0), ("gs_flat", 1)])
+def test_command_line_trains_and_renders_at_a_low_degree(cli_scene, gs_type, degree, tmp_path):
+    """train.py --sh_degree 0 (gs_mesh) and 1 (gs_flat): the saved point_cloud.ply holds 3((d + 1)^2 - 1) f_rest_*
+    properties (0 and 9), render.py draws what the library's renderer draws of the loaded model, and the final parameters
+    stay within the run-to-run spread of the library loop."""
+    from gms_b200 import dataset, io_ply
+    from gms_b200.cli import render as cli_render
+    from gms_b200.cli import train as cli_train
+    from test_gpu_cli import FLAT_ARGV, HOOKS_FLAT, HOOKS_MESH, MESH_ARGV, _expected_renders, _within_spread
+    M = (degree + 1) ** 2
+    argv = (MESH_ARGV if gs_type == "gs_mesh" else FLAT_ARGV) + ["--sh_degree", str(degree)]
+    hooks = HOOKS_MESH if gs_type == "gs_mesh" else HOOKS_FLAT
+    out = str(tmp_path / "out")
+    run = cli_train.Training(cli_train.parse_args(["-s", cli_scene, "-m", out] + argv)).prepare().run()
+    assert run.model._features.shape[1:] == (M, 3)
+    ply = str(tmp_path / "out" / "point_cloud" / "iteration_30" / "point_cloud.ply")
+    _, names = io_ply.read_ply_vertices(ply)
+    assert sum(n.startswith("f_rest_") for n in names) == 3 * (M - 1)
+    # render.py against the library's renderer of the loaded model (the checkpoint's degree, as load_ply sets it)
+    cli_render.main(["-m", out, "--gs_type", gs_type, "--quiet"])
+    model, cls = cli_render.load_model(gs_type, ply, degree, torch.device("cuda"))
+    assert model._features.shape[1] == M and model.active_sh_degree == degree
+    sc = dataset.load_scene(cli_scene, "gs_flat", eval=True, shuffle=False)
+    bg = torch.zeros(3, device="cuda")
+    for split, cams in (("train", sc.train_cameras), ("test", sc.test_cameras)):
+        want = tmp_path / split
+        _expected_renders(model, cls, cams, bg, str(want))
+        for i in range(len(cams)):
+            with open(os.path.join(out, split, "ours_30", f"renders_{gs_type}", f"{i:05d}.png"), "rb") as f, \
+                    open(want / f"{i:05d}.png", "rb") as g:
+                assert f.read() == g.read(), f"{split} {i}"
+    names_ = ("vertices", "_alpha", "_scale", "_features", "_opacity") if gs_type == "gs_mesh" else FreeGaussianModel.NAMES
+    final = {n: getattr(run.model, n).detach().clone() for n in names_}
+    a, b = _api_loop(cli_scene, argv, hooks), _api_loop(cli_scene, argv, hooks)
+    _within_spread(final, a, b, f"{gs_type} --sh_degree {degree} CLI vs API")

@@ -2,6 +2,7 @@
 import os
 
 import numpy as np
+import pytest
 import torch
 
 from gms_b200 import io_ply, scenes
@@ -79,3 +80,57 @@ def test_two_column_scaling_gets_the_s0_column_like_the_reference(tmp_path):
     assert [n for n in names if n.startswith("scale_")] == ["scale_0", "scale_1", "scale_2"]       # scene/gaussian_model.py:179-180
     np.testing.assert_allclose(np.asarray(data["scale_0"]), np.log(np.float32(1e-8)), rtol=1e-6)
     np.testing.assert_array_equal(np.asarray(data["scale_2"]), sc[:, 1].numpy())
+
+
+@pytest.mark.parametrize("M", [1, 4, 9])
+def test_round_trip_below_sixteen_coefficients(tmp_path, M):
+    """--sh_degree 0, 1, 2: 3 * (M - 1) f_rest properties (none at degree 0), channel-major, and [P, M - 1, 3] on load."""
+    xyz, fdc, frest, op, sc, rot = _random_model(P=13, M=M, seed=M)
+    p = str(tmp_path / "point_cloud.ply")
+    io_ply.save_gaussian_ply(p, xyz, fdc, frest, op, sc, rot)
+    data, names = io_ply.read_ply_vertices(p)
+    n_rest = 3 * (M - 1)
+    assert names == ["x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2"] + [f"f_rest_{i}" for i in range(n_rest)] + \
+        ["opacity", "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3"]
+    for k in range(n_rest):        # f_rest_k holds coefficient (k % (M - 1)) + 1 of channel k // (M - 1)
+        np.testing.assert_array_equal(np.asarray(data[f"f_rest_{k}"]), frest[:, k % (M - 1), k // (M - 1)].numpy())
+    g = io_ply.load_gaussian_ply(p)
+    assert g["_features_rest"].shape == (13, M - 1, 3)
+    for k, v in dict(_xyz=xyz, _features_dc=fdc, _features_rest=frest, _opacity=op, _scaling=sc, _rotation=rot).items():
+        assert g[k].shape == v.shape and torch.equal(g[k], v), k
+    back = torch.cat((g["_features_dc"], g["_features_rest"]), 1)
+    assert back.shape == (13, M, 3) and torch.equal(back, torch.cat((fdc, frest), 1))
+
+
+def _write_ply(path, names, rows):
+    with open(path, "wb") as f:
+        f.write(("ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % rows.shape[0]).encode())
+        for n in names:
+            f.write(f"property float {n}\n".encode())
+        f.write(b"end_header\n")
+        np.ascontiguousarray(rows, "<f4").tofile(f)
+
+
+@pytest.mark.parametrize("n_rest,n_dc", [(3, 3), (6, 3), (12, 3), (44, 3), (48, 3), (9, 2), (0, 0)])
+def test_refuses_sh_property_counts_of_no_degree(tmp_path, n_rest, n_dc):
+    """f_rest counts other than 0, 9, 24 and 45 (or f_dc counts other than 3) name no SH degree 0..3: refused by name."""
+    names = ["x", "y", "z", "nx", "ny", "nz"] + [f"f_dc_{i}" for i in range(n_dc)] + [f"f_rest_{i}" for i in range(n_rest)] + \
+        ["opacity", "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3"]
+    p = str(tmp_path / "bad.ply")
+    _write_ply(p, names, np.random.RandomState(0).randn(4, len(names)))
+    with pytest.raises(ValueError, match=rf"{n_dc} f_dc_\* and {n_rest} f_rest_\* properties"):
+        io_ply.load_gaussian_ply(p)
+
+
+@pytest.mark.parametrize("M", [1, 4, 9, 16])
+def test_free_model_checkpoint_keeps_its_coefficient_count(tmp_path, M):
+    """FreeGaussianModel.save -> from_checkpoint (on the CPU): features [P, M, 3] and max_sh_degree from M."""
+    from gms_b200.model import FreeGaussianModel
+    xyz, fdc, frest, op, sc, rot = _random_model(P=9, M=M, S=2, seed=20 + M)
+    m = FreeGaussianModel(xyz, sc, rot, torch.cat((fdc, frest), 1), op, "gs_flat", "cpu", active_sh_degree=3)
+    assert m.max_sh_degree == m.active_sh_degree == int(round(M ** 0.5)) - 1
+    p = str(tmp_path / "point_cloud.ply")
+    m.save(p)
+    back = FreeGaussianModel.from_checkpoint(p, "gs_flat", "cpu")
+    assert back._features.shape == (9, M, 3) and torch.equal(back._features, m._features.detach())
+    assert back.max_sh_degree == m.max_sh_degree
