@@ -2,14 +2,14 @@
 
     python gaussian-mesh-splatting_b200/build.py [--force] [--verbose]
 """
+import glob
 import os
 import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "gms_kernels.cu")
-DEPS = [os.path.join(HERE, "csrc", f) for f in ("gms_kernels.cu", "gms_common.cuh", "gms_preprocess.cuh",
-                                                "gms_expand.cuh", "gms_composite_common.cuh", "gms_composite_fwd.cuh", "gms_composite_bwd.cuh", "gms_loss.cuh", "gms_sort.cuh", "gms_binning.cuh", "gms_image.cuh", "gms_free.cuh", "gms_knn.cuh", "gms_flame.cuh")] + \
+DEPS = [SRC] + sorted(glob.glob(os.path.join(HERE, "csrc", "*.cuh"))) + \
        [os.path.join(HERE, "..", "include", "gms_b200.h"), os.path.abspath(__file__)]    # this file: FLAGS (the target arch) live here
 OUT = os.path.join(HERE, "gms_b200", "libgms_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

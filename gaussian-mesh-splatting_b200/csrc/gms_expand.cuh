@@ -700,3 +700,292 @@ GMS_HD void gms_points_vertices_fwd(const gms_points_vertices_args& a, int i) {
 #pragma unroll
     for (int k = 0; k < 3; k++) { t[k] = c[k]; t[3 + k] = keep ? p2[k] : p3[k]; t[6 + k] = keep ? p3[k] : p2[k]; }
 }
+
+#if defined(__CUDACC__)
+
+// ------------------------------------------------------------------------------------------ expansion kernels
+// One thread per face.  The per-Gaussian streams (K rows per face: 36-48 B per thread, i.e. a 36-48 B stride between
+// lanes) are staged through shared memory: the block copies its contiguous slice of every stream with fully coalesced
+// accesses, the per-face maths then reads / writes shared memory (gms_expand_face_* with fl = slot in the block).
+// STAGED = false is the direct variant (option "expand_staged" = 0, and whenever K makes the staging exceed 48 KB).
+constexpr int GMS_EXP_BLOCK = 128;
+
+__device__ __forceinline__ const float* exp_stage_in(const float* src, int width, size_t g0, int ng, int cap, float*& sm) {
+    if (!src) return nullptr;
+    float* dst = sm; sm += (size_t)cap * width;
+    const float* s0 = src + g0 * width;
+    for (int i = threadIdx.x; i < ng * width; i += GMS_EXP_BLOCK) dst[i] = s0[i];
+    return dst;
+}
+__device__ __forceinline__ float* exp_stage_out(float* dst, int width, int cap, float*& sm) {
+    if (!dst) return nullptr;
+    float* b = sm; sm += (size_t)cap * width;
+    return b;
+}
+__device__ __forceinline__ void exp_stage_flush(float* dst, const float* buf, int width, size_t g0, int ng) {
+    if (!dst) return;
+    float* d0 = dst + g0 * width;
+    for (int i = threadIdx.x; i < ng * width; i += GMS_EXP_BLOCK) d0[i] = buf[i];
+}
+
+template <int ACT>
+__device__ __forceinline__ void expand_face_fwd(const gms_expand_args& a, int f, int fl) {
+    if constexpr (ACT == GMS_ALPHA_RELU) gms_expand_face_fwd_relu(a, f, fl);
+    else gms_expand_face_fwd_act<ACT>(a, f, fl);
+}
+template <int ACT>
+__device__ __forceinline__ void expand_face_bwd(const gms_expand_args& a, const gms_expand_grads& g, int f, int fl) {
+    if constexpr (ACT == GMS_ALPHA_RELU) gms_expand_face_bwd_relu(a, g, f, fl);
+    else gms_expand_face_bwd_act<ACT>(a, g, f, fl);
+}
+
+template <bool STAGED, int ACT>
+__device__ __forceinline__ void expand_fwd_block(const gms_expand_args& a) {
+    const int f0 = blockIdx.x * GMS_EXP_BLOCK, f = f0 + threadIdx.x;
+    if (!STAGED) {
+        if (f < a.F) expand_face_fwd<ACT>(a, f, f);
+        return;
+    }
+    extern __shared__ float4 exp_smem4[];
+    float* sm = reinterpret_cast<float*>(exp_smem4);
+    const int nf = min(GMS_EXP_BLOCK, a.F - f0), ng = nf * a.K, cap = GMS_EXP_BLOCK * a.K;
+    const size_t g0 = (size_t)f0 * a.K;
+    gms_expand_args l = a;
+    l.alpha_raw = exp_stage_in(a.alpha_raw, 3, g0, ng, cap, sm);
+    l.scale_raw = exp_stage_in(a.scale_raw, 1, g0, ng, cap, sm);
+    l.alpha = exp_stage_out(a.alpha, 3, cap, sm);
+    l.xyz = exp_stage_out(a.xyz, 3, cap, sm);
+    l.scaling_log = exp_stage_out(a.scaling_log, 3, cap, sm);
+    l.scaling_act = exp_stage_out(a.scaling_act, 3, cap, sm);
+    l.rotation_raw = exp_stage_out(a.rotation_raw, 4, cap, sm);
+    l.rotation_act = exp_stage_out(a.rotation_act, 4, cap, sm);
+    __syncthreads();
+    if (f < a.F) expand_face_fwd<ACT>(l, f, threadIdx.x);
+    __syncthreads();
+    exp_stage_flush(a.alpha, l.alpha, 3, g0, ng);
+    exp_stage_flush(a.xyz, l.xyz, 3, g0, ng);
+    exp_stage_flush(a.scaling_log, l.scaling_log, 3, g0, ng);
+    exp_stage_flush(a.scaling_act, l.scaling_act, 3, g0, ng);
+    exp_stage_flush(a.rotation_raw, l.rotation_raw, 4, g0, ng);
+    exp_stage_flush(a.rotation_act, l.rotation_act, 4, g0, ng);
+}
+
+template <bool STAGED>
+__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_fwd(gms_expand_args a) { expand_fwd_block<STAGED, GMS_ALPHA_RELU>(a); }
+template <bool STAGED>
+__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_softmax_fwd(gms_expand_args a) { expand_fwd_block<STAGED, GMS_ALPHA_SOFTMAX>(a); }
+
+template <bool STAGED, int ACT>
+__device__ __forceinline__ void expand_bwd_block(const gms_expand_args& a, const gms_expand_grads& g) {
+    const int f0 = blockIdx.x * GMS_EXP_BLOCK, f = f0 + threadIdx.x;
+    if (!STAGED) {
+        if (f < a.F) expand_face_bwd<ACT>(a, g, f, f);
+        return;
+    }
+    extern __shared__ float4 exp_smem4[];
+    float* sm = reinterpret_cast<float*>(exp_smem4);
+    const int nf = min(GMS_EXP_BLOCK, a.F - f0), ng = nf * a.K, cap = GMS_EXP_BLOCK * a.K;
+    const size_t g0 = (size_t)f0 * a.K;
+    gms_expand_args l = a;
+    gms_expand_grads lg = g;
+    l.alpha_raw = exp_stage_in(a.alpha_raw, 3, g0, ng, cap, sm);
+    l.scale_raw = exp_stage_in(a.scale_raw, 1, g0, ng, cap, sm);
+    lg.dL_dxyz = exp_stage_in(g.dL_dxyz, 3, g0, ng, cap, sm);
+    lg.dL_dscaling_log = exp_stage_in(g.dL_dscaling_log, 3, g0, ng, cap, sm);
+    lg.dL_dscaling_act = exp_stage_in(g.dL_dscaling_act, 3, g0, ng, cap, sm);
+    lg.dL_drotation_raw = exp_stage_in(g.dL_drotation_raw, 4, g0, ng, cap, sm);
+    lg.dL_drotation_act = exp_stage_in(g.dL_drotation_act, 4, g0, ng, cap, sm);
+    lg.dL_dalpha_raw = exp_stage_out(g.dL_dalpha_raw, 3, cap, sm);
+    lg.dL_dscale_raw = exp_stage_out(g.dL_dscale_raw, 1, cap, sm);
+    __syncthreads();
+    if (f < a.F) expand_face_bwd<ACT>(l, lg, f, threadIdx.x);     // per-face outputs (dL_dtriangles, vertex atomics) stay global
+    __syncthreads();
+    exp_stage_flush(g.dL_dalpha_raw, lg.dL_dalpha_raw, 3, g0, ng);
+    exp_stage_flush(g.dL_dscale_raw, lg.dL_dscale_raw, 1, g0, ng);
+}
+
+template <bool STAGED>
+__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_bwd(gms_expand_args a, gms_expand_grads g) {
+    expand_bwd_block<STAGED, GMS_ALPHA_RELU>(a, g);
+}
+template <bool STAGED>
+__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_softmax_bwd(gms_expand_args a, gms_expand_grads g) {
+    expand_bwd_block<STAGED, GMS_ALPHA_SOFTMAX>(a, g);
+}
+
+// Splat-parallel expansion for many splats per face (gs_flame: K = 100 on ~10k faces).  One warp per face: every lane reads
+// the face and evaluates its frame and quaternion in lockstep (one instruction stream per face, as cheap as one lane
+// computing them and broadcasting the result, without the shuffles), then lane j handles splats j, j + 32, ...: consecutive
+// lanes touch consecutive rows, so every per-Gaussian stream is read and written coalesced without staging.  Each splat is
+// the per-thread kernel's gms_expand_splat_* call, so the forward is bit-identical to it.  The backward sums each lane's
+// dt / dq / ds1 / ds2 partials over its splats, reduces them across the warp (butterfly), and lane 0 finishes the face: one
+// set of vertex atomics per face, as in the per-thread kernel.  Only the order of the sum over K differs.
+constexpr int GMS_EXP_WIDE_BLOCK = 128;                     // 4 faces per block
+constexpr int GMS_EXP_WIDE_MIN_K = 16;                      // expand_wide = 1: softmax weights with K >= this (DESIGN.md 4.5)
+
+template <int ACT>
+__global__ void __launch_bounds__(GMS_EXP_WIDE_BLOCK) k_expand_wide_fwd(gms_expand_args a) {
+    const int f = blockIdx.x * (GMS_EXP_WIDE_BLOCK / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (f >= a.F) return;
+    GmsFaceState s;
+    gms_expand_face_load(a, f, s);
+    if (a.triangles && lane == 0) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) a.triangles[9 * (size_t)f + k] = s.t[k];
+    }
+    gms_expand_face_frame(a, s);
+    for (int k = lane; k < a.K; k += 32) gms_expand_splat_fwd<ACT>(a, s, (size_t)f * a.K + k);
+}
+
+template <int ACT>
+__global__ void __launch_bounds__(GMS_EXP_WIDE_BLOCK) k_expand_wide_bwd(gms_expand_args a, gms_expand_grads g) {
+    const int f = blockIdx.x * (GMS_EXP_WIDE_BLOCK / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (f >= a.F) return;                                   // whole warps: f is uniform across the warp
+    GmsFaceState s;
+    gms_expand_face_load(a, f, s);
+    gms_expand_face_frame(a, s);
+    float acc[15];                                          // dt[9], dq[4], ds1, ds2
+#pragma unroll
+    for (int i = 0; i < 15; i++) acc[i] = 0.f;
+    for (int k = lane; k < a.K; k += 32) gms_expand_splat_bwd<ACT>(a, g, s, (size_t)f * a.K + k, acc, acc + 9, acc[13], acc[14]);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+#pragma unroll
+        for (int i = 0; i < 15; i++) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
+    }
+    if (lane == 0) gms_expand_face_bwd_tail(a, g, s, f, acc, acc + 9, acc[13], acc[14]);
+}
+
+__global__ void __launch_bounds__(128) k_points_expand_fwd(gms_points_args a) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.P) return;
+    gms_points_face_fwd(a, i);
+}
+
+__global__ void __launch_bounds__(128) k_points_vertices(gms_points_vertices_args a) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.P) return;
+    gms_points_vertices_fwd(a, i);
+}
+
+// ------------------------------------------------------------------------------------------ mesh-driven pseudo-mesh
+// scripts/edit_pseudomesh_based_on_estimated_mesh.py:14-94: bind every pseudo-triangle to the nearest face of a driving mesh
+// (nearest centroid, brute force), then re-pose it from any pose of that mesh (gms_expand.cuh: gms_pm_*).
+#define GMS_PM_BLOCK 128
+#define GMS_PM_TILE 512        // face centroids staged through shared memory per pass
+
+__device__ __forceinline__ void pm_load_face(const float* __restrict__ vertices, const int64_t* __restrict__ faces, int f, float* v) {
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const int64_t vi = faces[3 * (size_t)f + c];
+        v[3 * c] = vertices[3 * vi]; v[3 * c + 1] = vertices[3 * vi + 1]; v[3 * c + 2] = vertices[3 * vi + 2];
+    }
+}
+
+// Per face: (centroid, 1 if degenerate else 0), and the number of degenerate faces.
+__global__ void __launch_bounds__(GMS_PM_BLOCK) k_pseudomesh_faces(int F, const float* __restrict__ vertices,
+                                                                    const int64_t* __restrict__ faces, float4* __restrict__ cent,
+                                                                    uint32_t* __restrict__ n_degenerate) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= F) return;
+    float v[9], m[3];
+    pm_load_face(vertices, faces, f, v);
+    GmsPmFrame fr;
+    const bool deg = gms_pm_frame(v, v + 3, v + 6, fr);
+    gms_pm_centroid(v, v + 3, v + 6, m);
+    cent[f] = make_float4(m[0], m[1], m[2], deg ? 1.f : 0.f);
+    if (deg) atomicAdd(n_degenerate, 1u);
+}
+
+// One thread per pseudo-triangle: nearest non-degenerate face centroid (double distance, lowest index on a tie; the first
+// non-degenerate face is taken whatever its distance, so a non-finite query still binds in range), then the 9 coefficients.
+__global__ void __launch_bounds__(GMS_PM_BLOCK) k_pseudomesh_bind(int P, int F, const float* __restrict__ triangles,
+                                                                   const float* __restrict__ vertices, const int64_t* __restrict__ faces,
+                                                                   const float4* __restrict__ cent, int32_t* __restrict__ face_out,
+                                                                   float* __restrict__ coeffs) {
+    __shared__ double sx[GMS_PM_TILE], sy[GMS_PM_TILE], sz[GMS_PM_TILE];
+    __shared__ uint8_t sdeg[GMS_PM_TILE];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    float w[9], q[3] = {0.f, 0.f, 0.f};
+    if (i < P) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) w[k] = triangles[9 * (size_t)i + k];
+        gms_pm_centroid(w, w + 3, w + 6, q);
+    }
+    const double qx = q[0], qy = q[1], qz = q[2];
+    double best = 0.0;
+    int bi = -1;
+    for (int t0 = 0; t0 < F; t0 += GMS_PM_TILE) {
+        const int n = min(GMS_PM_TILE, F - t0);
+        __syncthreads();
+        for (int j = threadIdx.x; j < n; j += blockDim.x) {
+            const float4 c = cent[t0 + j];
+            sx[j] = c.x; sy[j] = c.y; sz[j] = c.z; sdeg[j] = c.w != 0.f;
+        }
+        __syncthreads();
+        for (int j = 0; j < n; j++) {
+            if (sdeg[j]) continue;
+            const double d = gms_pm_dist2(qx, qy, qz, sx[j], sy[j], sz[j]);
+            if (d < best || bi < 0) { best = d; bi = t0 + j; }
+        }
+    }
+    if (i >= P) return;
+    float v[9], c[9];
+    pm_load_face(vertices, faces, bi, v);
+    GmsPmFrame fr;
+    gms_pm_frame(v, v + 3, v + 6, fr);
+    gms_pm_coeffs(fr, v, w, c);
+    face_out[i] = bi;
+#pragma unroll
+    for (int k = 0; k < 9; k++) coeffs[9 * (size_t)i + k] = c[k];
+}
+
+// The pseudo-triangle of binding i in the driving pose (vertices, faces).
+__device__ __forceinline__ void pm_reposed(const gms_pseudomesh_repose_args& a, int i, float* w) {
+    float v[9], c[9];
+    pm_load_face(a.vertices, a.faces, a.face[i], v);
+#pragma unroll
+    for (int k = 0; k < 9; k++) c[k] = a.coeffs[9 * (size_t)i + k];
+    GmsPmFrame fr;
+    gms_pm_frame(v, v + 3, v + 6, fr);
+    gms_pm_repose(fr, v, c, w);
+}
+
+__global__ void __launch_bounds__(GMS_PM_BLOCK) k_pseudomesh_repose(gms_pseudomesh_repose_args a) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.P) return;
+    float w[9];
+    pm_reposed(a, i, w);
+#pragma unroll
+    for (int k = 0; k < 9; k++) a.triangles[9 * (size_t)i + k] = w[k];
+}
+
+// Re-pose + the gs_points expansion in one pass (the triangles never reach global memory).  The core reads the re-posed
+// triangle from a per-thread slot in shared memory, as k_points_expand_fwd reads it from the triangles array: the core's
+// fp32 expressions leave contraction to the compiler, and reading the vertices from memory in both kernels keeps its
+// choices, and so the Gaussians, bit-identical to the triangles path.  A Gaussian whose re-posed triangle is not finite (its
+// driving face is degenerate in this pose) is placed at the camera centre, -R^T t of the view matrix: its view-space depth
+// is ~0 <= the near plane, so the preprocess's first test culls it (radius 0, no tile) before it reads anything else of it.
+__global__ void __launch_bounds__(GMS_PM_BLOCK) k_points_bound_expand_fwd(gms_pseudomesh_repose_args r, gms_points_args a,
+                                                                           const float* __restrict__ view) {
+    __shared__ float tri[GMS_PM_BLOCK * 9];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= r.P) return;
+    float w[9];
+    pm_reposed(r, i, w);
+    float* t = tri + 9 * threadIdx.x;
+#pragma unroll
+    for (int k = 0; k < 9; k++) t[k] = w[k];
+    asm volatile("" ::: "memory");      // no store-to-load forwarding: the core loads its vertices, as in the triangles path
+    gms_points_core_fwd(a, i, t, t + 3, t + 6);
+    bool finite = true;
+#pragma unroll
+    for (int k = 0; k < 9; k++) finite = finite && isfinite(w[k]);
+    if (!finite) {
+#pragma unroll
+        for (int j = 0; j < 3; j++)
+            a.xyz[3 * (size_t)i + j] = -(view[4 * j] * view[12] + view[4 * j + 1] * view[13] + view[4 * j + 2] * view[14]);
+    }
+}
+
+#endif  // __CUDACC__

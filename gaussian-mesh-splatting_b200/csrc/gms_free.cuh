@@ -43,6 +43,34 @@ __global__ void __launch_bounds__(GMS_FREE_BLOCK) k_free_act_fwd(int P, int cols
     reinterpret_cast<float4*>(rots)[i] = make_float4(q[0] / n, q[1] / n, q[2] / n, q[3] / n);
 }
 
+// xyz from the checkpoint's activated weights and the driving pose (the product of the expansion forward, same operation
+// order), scales and rotations from the checkpoint's rows as k_free_act_fwd activates them.  C linkage: its symbol, and
+// the name profiler traces give it, is the plain `k_flame_act`.
+extern "C" __global__ void __launch_bounds__(GMS_FREE_BLOCK) k_flame_act(int P, int K, const float* __restrict__ alpha, const int64_t* __restrict__ faces,
+                                                              const float* __restrict__ vertices, const float* __restrict__ scaling_log,
+                                                              const float* __restrict__ rotation_raw, float* __restrict__ xyz,
+                                                              float* __restrict__ scales, float* __restrict__ rots) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P) return;
+    const size_t f = (size_t)(i / K);
+    float t[9];
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const int64_t vi = faces[3 * f + c];
+        t[3 * c] = vertices[3 * vi]; t[3 * c + 1] = vertices[3 * vi + 1]; t[3 * c + 2] = vertices[3 * vi + 2];
+    }
+    const float al0 = alpha[3 * (size_t)i], al1 = alpha[3 * (size_t)i + 1], al2 = alpha[3 * (size_t)i + 2];
+#pragma unroll
+    for (int c = 0; c < 3; c++) xyz[3 * (size_t)i + c] = al0 * t[c] + al1 * t[3 + c] + al2 * t[6 + c];
+    const float* s = scaling_log + 3 * (size_t)i;
+    float* so = scales + 3 * (size_t)i;
+    so[0] = expf(s[0]); so[1] = expf(s[1]); so[2] = expf(s[2]);
+    const float4 r = reinterpret_cast<const float4*>(rotation_raw)[i];
+    const float q[4] = {r.x, r.y, r.z, r.w};
+    const float n = gms_quat_norm(q);
+    reinterpret_cast<float4*>(rots)[i] = make_float4(q[0] / n, q[1] / n, q[2] / n, q[3] / n);
+}
+
 __global__ void __launch_bounds__(GMS_FREE_BLOCK) k_free_act_bwd(FreeActBwd b) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= b.P) return;
