@@ -623,6 +623,263 @@ int gmso_composite_backward(const gmso_settings* s, const int32_t* ranges, const
 }
 
 /* =====================================================================
+ * A.3 in float64, with a per-element error budget.
+ *
+ * ref64[P,10]: the per-Gaussian sums of gmso_composite_backward (same order: mean2D x/y NDC-scaled, conic xx/xy(half)/yy,
+ * opacity, rgb, inverse depth), every per-pair quantity evaluated in double.  The blend decisions (which splats blend at a
+ * pixel, n_contrib) are the fp32 forward's, and G = exp() in double of the canonical fp32 power (quad_power) -- the
+ * operation is defined by the fp32 forward, whose decisions the kernels reproduce bit for bit outside threshold-ambiguous
+ * pixels; a float64 power would weigh other pixels for edge-on slivers.  dx, dy are the fp32 differences both sides form.
+ * alpha = min(0.99f, op * G); T is the double front-to-back product over the blended splats (not recovered by division from
+ * the fp32 final_T), the background term uses the double final T, and dL/dalpha, the colour-behind recurrence and the
+ * moment terms are double.  Like the two functions above, it covers only the tiles gmso_set_tile_stride selects.
+ *
+ * budget[P,10]: a first-order bound, derived from the operation sequence of the fp32 kernels (gms_bwd_pair, gms_red_flush,
+ * gms_bwd_commit), on |any correct fp32 implementation - ref64|.  u = 2^-24.  Every term is bounded through its absolute
+ * value, per blended (pixel, splat) pair:
+ *     cd   = |c . dL/dC| summed per channel (+ |invd * dL/dD|),   bgd = sum_ch |bg_ch * dL/dC_ch|,
+ *     Babs = the colour-behind recurrence on absolute values:  Babs <- alpha * cd + (1 - alpha) * Babs,
+ *     |q|  = G * (T * (cd + Babs) + T_final * bgd / (1 - alpha)),
+ *     mean2D x: op * W/2 * |q| * (|conx dx| + |cony dy|),   mean2D y: op * H/2 * |q| * (|conz dy| + |cony dx|),
+ *     conic:    op/2 * |q| * (dx^2, |dx dy|, dy^2),          opacity: |q|,    rgb / inverse depth: alpha * T * |dL/dC|, |dL/dD|.
+ * With m = that magnitude, the pair's share is u * (C0 + K_p) * m and each Gaussian adds u * (CSUM + n_quads_i) * sum m:
+ *   C0 = 24, the longest chain of one pair's own roundings:  G = ex2.approx(power * log2e):  <= 2^-22 (4 u) for ex2, and
+ *        |power| * (1 + 0.23) u <= 6.8 u for the argument (blending needs G >= 1/255, |power| <= ln 255; 0.23 u is the
+ *        rounding of log2e), alpha = op * G: 1 -> alpha within 12 u;  c . dL/dC: 4 (three / four FMAs);  c - Bdot, * T, the
+ *        FMA with the background term: 3;  * G: 1 (+ G's 12);  the moment products before the sum (q dy, + of the lane's two
+ *        pixels, dx * (dx * sq)): 3;  w = alpha * T and the dL/dC products: alpha's 12 + 2.  12 + 1 + 4 + 3 + 3 + 1 = 24.
+ *   K_p  = sum over the pixel's blended splats l of (CSTEP + CALPHA * a_l):  the transmittance in front of splat j is
+ *        recovered as final_T * prod_{l >= j} rcp(1 - alpha_l), with final_T the fp32 forward product: per splat 2 u in the
+ *        forward (1 - alpha, *) and 4 u in the recovery (1 - alpha, rcp.approx <= 1 ulp = 2 u, *); the alpha of a splat in
+ *        FRONT of j enters T_j with its own error (12 u) times alpha / (1 - alpha) (behind j it cancels between the forward
+ *        product and the recovery).  Bdot for a splat behind j costs 2 u (FMA, *) plus alpha's 12 u times
+ *        max(1, alpha / (1 - alpha)).  T_j's and Bdot_j's splat sets are disjoint (in front / behind), so
+ *        CSTEP = 6 + 14 = 20 and CALPHA = 12, with a_l = alpha_l / (1 - alpha_l) (0 where alpha is clamped to 0.99f:
+ *        the same constant on both sides).  Unlike a plain count k this keeps the 1 / (1 - alpha) amplification of nearly
+ *        opaque splats.
+ *   CSUM = 22, the summation:  each quad adds its 64 pixels as two pixels per lane (1) and a serial 32-term row sum in two
+ *        16-chains joined at the end (15 + 1) in its shared-memory panel, then the commit's products (<= 5: conx * s, the
+ *        FMA with cony * s, * op, * W/2).  n_quads_i = the number of 8x8 quads in which Gaussian i blends at any pixel: the
+ *        float atomics add one partial sum per (quad, splat) pair in any order, a chain of at most n_quads_i.
+ * Threshold-ambiguous pixels (ambiguous[px], see gmso_composite_forward) get an ALLOWANCE: an fp32 implementation with
+ * another exp() may take the other decision for a splat f whose alpha lies in the band around 1/255 (blended or not), or
+ * not stop at the splat f that ended the pixel.  Each such f is a flip candidate; for each one, to first order:
+ *   - f itself gains or loses its whole term: its full magnitude m_f;
+ *   - a blended splat j behind f sees T_j, and every blended j sees T_final, scaled by (1 - alpha_f) or its inverse, a
+ *     relative change <= r_f = alpha_f / (1 - alpha_f) (alpha_f for a candidate that does not blend in the forward):
+ *     r_f * m_j for j behind f (its T-terms, colour terms included), r_f * G_j T_final bgd / (1 - alpha_j) for j in front;
+ *   - a blended splat j in front of f sees its colour behind change by the product of (1 - alpha) between them times
+ *     alpha_f (c_f - B_f) . dL/dC, so T_j Bdot_j moves by <= alpha_f (cd_f + cmax) T_f / (1 - alpha_j), T_f the
+ *     transmittance in front of f and cmax the largest cd at the pixel (|B| <= cmax for any set of decisions),
+ * each carried through the moment factors of the magnitude above.  These are added to the budgets (nothing is exempted).
+ * A candidate that does not blend in the forward is a pair the other implementation adds, with its own roundings: its
+ * magnitude also enters the rounding shares above, at C0 + K_p + CSTEP + CALPHA * a_f (the pixel's chain one splat
+ * longer), and the summation share through n_quads_i, which counts the quads of candidates too.
+ * amb_share[i] = the largest share of any component's budget of Gaussian i that comes from such allowances.
+ * A Gaussian that blends at no pixel and decides at no ambiguous pixel has ref64 = budget = 0: exactly zero is required.
+ * ===================================================================== */
+#define GMSO_U (1.0 / 16777216.0)
+#define GMSO_C0 24.0
+#define GMSO_CSTEP 20.0
+#define GMSO_CALPHA 12.0
+#define GMSO_CSUM 22.0
+#define GMSO_NACC 41    /* per Gaussian and thread: ref 10, (C0+K)*m 10, m 10, allowance 10, n_quads 1 */
+
+typedef struct {
+    uint32_t g;
+    int blend;          /* blends in the fp32 forward; 0: a decision candidate at an ambiguous pixel */
+    int flip;           /* a decision another exp() may take the other way (ambiguous pixels only) */
+    double dx, dy, G, alpha, T, cd, Babs;
+} gmso_e64;
+
+/* the ten term magnitudes of a pair whose |dL/dalpha * G| is qa and whose colour weight alpha * T is w */
+static inline void gmso_mag64(const float* co, const gmso_e64* x, double qa, double w, const double* dpx, double dinv,
+                              double hW, double hH, double* m) {
+    const double cx = co[0], cy = co[1], cz = co[2], op = co[3], dx = x->dx, dy = x->dy;
+    m[0] = op * hW * qa * (fabs(cx * dx) + fabs(cy * dy));
+    m[1] = op * hH * qa * (fabs(cz * dy) + fabs(cy * dx));
+    m[2] = 0.5 * op * qa * dx * dx;
+    m[3] = 0.5 * op * qa * fabs(dx * dy);
+    m[4] = 0.5 * op * qa * dy * dy;
+    m[5] = qa;
+    for (int ch = 0; ch < 3; ch++) m[6 + ch] = w * fabs(dpx[ch]);
+    m[9] = w * fabs(dinv);
+}
+
+int gmso_composite_backward64(const gmso_settings* s, const int32_t* ranges, const uint32_t* point_list,
+                              const float* means2D, const float* rgb, const float* conic_opacity,
+                              const float* depths, const int32_t* n_contrib, const uint8_t* ambiguous,
+                              const float* dL_dpix /*[3,H,W]*/, const float* dL_dinvdepth_pix /*[H,W] or NULL*/,
+                              double* ref64 /*[P,10]*/, double* budget /*[P,10]*/, double* amb_share /*[P]*/) {
+    const int W = s->W, H = s->H, P = s->P;
+    const int gx = (W + GMSO_BLOCK - 1) / GMSO_BLOCK, gy = (H + GMSO_BLOCK - 1) / GMSO_BLOCK;
+    const double hW = (double)(0.5f * W), hH = (double)(0.5f * H);
+    const double amax = (double)0.99f;
+    const double bgc[3] = {s->bg[0], s->bg[1], s->bg[2]};
+    int maxlen = 1;
+    for (int t = 0; t < gx * gy; t++) maxlen = imax(maxlen, ranges[2 * t + 1] - ranges[2 * t]);
+    double* tot = (double*)calloc((size_t)P * GMSO_NACC, sizeof(double));
+    if (!tot) return -1;
+#pragma omp parallel
+    {
+        double* l = (double*)calloc((size_t)P * GMSO_NACC, sizeof(double));
+        gmso_e64* e = (gmso_e64*)malloc(sizeof(gmso_e64) * (size_t)maxlen);
+        uint8_t* qhit = (uint8_t*)malloc((size_t)maxlen);
+#pragma omp for schedule(dynamic, 1)
+        for (int tile = 0; tile < gx * gy; tile++) {
+            if (tile % g_tile_stride) continue;
+            const int tx0 = (tile % gx) * GMSO_BLOCK, ty0 = (tile / gx) * GMSO_BLOCK;
+            const int r0 = ranges[2 * tile], r1 = ranges[2 * tile + 1];
+            memset(qhit, 0, (size_t)maxlen);
+            for (int py = ty0; py < ty0 + GMSO_BLOCK && py < H; py++)
+                for (int px = tx0; px < tx0 + GMSO_BLOCK && px < W; px++) {
+                    const size_t pix = (size_t)py * W + px;
+                    const int quad = ((py - ty0) >> 3) * 2 + ((px - tx0) >> 3);
+                    const int last = n_contrib[pix], amb = ambiguous[pix] != 0;
+                    const float pfx = (float)px, pfy = (float)py;
+                    /* the fp32 forward's decisions; at an ambiguous pixel also the band candidates and the stopping splat */
+                    int n = 0;
+                    const int lim = amb ? r1 - r0 : last;
+                    float T32 = 1.0f;
+                    for (int jj = 0; jj < lim; jj++) {
+                        const uint32_t g = point_list[r0 + jj];
+                        const float dx = means2D[2 * g] - pfx, dy = means2D[2 * g + 1] - pfy;
+                        const float* co = conic_opacity + 4 * g;
+                        const float power = quad_power(co, dx, dy);
+                        if (power > 0.0f) continue;
+                        const float a32 = fminf(0.99f, co[3] * expf(power));
+                        /* the forward's ambiguity tests, decision by decision */
+                        const int aband = amb && fabsf(a32 - 1.0f / 255.0f) < 4e-6f * (1.0f / 255.0f) + 1e-9f;
+                        const int blend = a32 >= 1.0f / 255.0f && jj < last;
+                        const int stop = a32 >= 1.0f / 255.0f && jj >= last;     /* the splat the forward stopped at */
+                        const float test_T = T32 * (1.f - a32);
+                        const int tband = amb && a32 >= 1.0f / 255.0f && fabsf(test_T - 0.0001f) < 1e-9f;
+                        if (blend) T32 = test_T;
+                        if (!blend && !((aband || tband) && (stop || a32 < 1.0f / 255.0f))) {
+                            if (stop) break;
+                            continue;
+                        }
+                        gmso_e64* x = e + n++;
+                        x->g = g; x->blend = blend;
+                        x->flip = aband | (tband && blend ? 2 : 0) | (tband && stop ? 4 : 0);
+                        x->dx = dx; x->dy = dy;
+                        x->G = exp((double)power);
+                        x->alpha = fmin(amax, (double)co[3] * x->G);
+                        qhit[jj] |= (uint8_t)(1u << quad);
+                        if (stop) break;
+                    }
+                    if (n == 0) continue;
+                    double T = 1.0, K = 0.0;
+                    for (int k = 0; k < n; k++) {
+                        e[k].T = T;
+                        if (!e[k].blend) continue;
+                        const double a = e[k].alpha;
+                        K += GMSO_CSTEP + (a < amax ? GMSO_CALPHA * a / (1.0 - a) : 0.0);
+                        T *= 1.0 - a;
+                    }
+                    const double Tfin = T;
+                    double dpx[3], bgdot = 0.0, bgabs = 0.0;
+                    for (int ch = 0; ch < 3; ch++) {
+                        dpx[ch] = dL_dpix[(size_t)ch * H * W + pix];
+                        bgdot += bgc[ch] * dpx[ch];
+                        bgabs += fabs(bgc[ch] * dpx[ch]);
+                    }
+                    const double dinv = dL_dinvdepth_pix ? dL_dinvdepth_pix[pix] : 0.0;
+                    double B = 0.0, Babs = 0.0, cmax = 0.0;
+                    for (int k = n - 1; k >= 0; k--) {
+                        const uint32_t g = e[k].g;
+                        const float* co = conic_opacity + 4 * g;
+                        const double cx = co[0], cy = co[1], cz = co[2], op = co[3];
+                        const double dx = e[k].dx, dy = e[k].dy, G = e[k].G, a = e[k].alpha, Tk = e[k].T;
+                        const double invd = 1.0 / (double)depths[g];
+                        double cdp = invd * dinv, cd = fabs(invd * dinv);
+                        for (int ch = 0; ch < 3; ch++) {
+                            cdp += (double)rgb[3 * g + ch] * dpx[ch];
+                            cd += fabs((double)rgb[3 * g + ch] * dpx[ch]);
+                        }
+                        e[k].cd = cd; e[k].Babs = Babs;
+                        cmax = fmax(cmax, cd);
+                        if (!e[k].blend) continue;
+                        const double dLa = Tk * (cdp - B) - Tfin * bgdot / (1.0 - a);
+                        const double q = dLa * G;
+                        const double t[10] = {op * hW * q * (-cx * dx - cy * dy), op * hH * q * (-cz * dy - cy * dx),
+                                              -0.5 * op * q * dx * dx, -0.5 * op * q * dx * dy, -0.5 * op * q * dy * dy, q,
+                                              a * Tk * dpx[0], a * Tk * dpx[1], a * Tk * dpx[2], a * Tk * dinv};
+                        double m[10];
+                        gmso_mag64(co, e + k, G * (Tk * (cd + Babs) + Tfin * bgabs / (1.0 - a)), a * Tk, dpx, dinv, hW, hH, m);
+                        double* acc = l + (size_t)g * GMSO_NACC;
+                        for (int c = 0; c < 10; c++) {
+                            acc[c] += t[c];
+                            acc[10 + c] += (GMSO_C0 + K) * m[c];
+                            acc[20 + c] += m[c];
+                        }
+                        B = a * cdp + (1.0 - a) * B;
+                        Babs = a * cd + (1.0 - a) * Babs;
+                    }
+                    /* allowances for the flip candidates of an ambiguous pixel */
+                    for (int f = 0; f < n; f++) {
+                        if (!e[f].flip) continue;
+                        const double af = e[f].alpha, Tf = e[f].T;
+                        const double rf = e[f].blend ? af / (1.0 - af) : af;
+                        for (int k = 0; k < n; k++) {
+                            const gmso_e64* x = e + k;
+                            if (k != f && !x->blend) continue;
+                            const double a = x->alpha, G = x->G, Tk = x->T;
+                            const double full = G * (Tk * (x->cd + x->Babs) + Tfin * bgabs / (1.0 - a));
+                            double qa = 0.0, w = 0.0;
+                            if (e[f].flip & 5) {          /* f alone blends or not */
+                                if (k == f) { qa = full; w = a * Tk; }
+                                else if (k > f) { qa = rf * full; w = rf * a * Tk; }
+                                else qa = G * (af * (e[f].cd + cmax) * Tf + rf * Tfin * bgabs) / (1.0 - a);
+                            }
+                            if (e[f].flip & 2) {          /* the pixel stops at f: f and everything behind it drop out */
+                                if (k >= f) { qa += full; w += a * Tk; }
+                                else qa += G * Tf * (cmax + bgabs) / (1.0 - a);
+                            }
+                            double m[10];
+                            gmso_mag64(conic_opacity + 4 * x->g, x, qa, w, dpx, dinv, hW, hH, m);
+                            double* acc = l + (size_t)x->g * GMSO_NACC;
+                            for (int c = 0; c < 10; c++) acc[30 + c] += m[c];
+                            if (k == f && !x->blend) {
+                                /* the pair another implementation adds carries its own roundings and enters the sums */
+                                double mo[10];
+                                gmso_mag64(conic_opacity + 4 * x->g, x, full, a * Tk, dpx, dinv, hW, hH, mo);
+                                const double Kf = K + GMSO_CSTEP + (a < amax ? GMSO_CALPHA * a / (1.0 - a) : 0.0);
+                                for (int c = 0; c < 10; c++) {
+                                    acc[10 + c] += (GMSO_C0 + Kf) * mo[c];
+                                    acc[20 + c] += mo[c];
+                                }
+                            }
+                        }
+                    }
+                }
+            for (int jj = 0; jj < r1 - r0; jj++) {
+                const uint8_t h = qhit[jj];
+                if (h) l[(size_t)point_list[r0 + jj] * GMSO_NACC + 40] += (h & 1) + ((h >> 1) & 1) + ((h >> 2) & 1) + ((h >> 3) & 1);
+            }
+        }
+#pragma omp critical
+        {
+            for (size_t k = 0; k < (size_t)P * GMSO_NACC; k++) tot[k] += l[k];
+        }
+        free(l); free(e); free(qhit);
+    }
+    for (int i = 0; i < P; i++) {
+        const double* a = tot + (size_t)i * GMSO_NACC;
+        double share = 0.0;
+        for (int c = 0; c < 10; c++) {
+            const double b = GMSO_U * (a[10 + c] + (GMSO_CSUM + a[40]) * a[20 + c]) + a[30 + c];
+            ref64[10 * i + c] = a[c];
+            budget[10 * i + c] = b;
+            if (b > 0.0) share = fmax(share, a[30 + c] / b);
+        }
+        amb_share[i] = share;
+    }
+    free(tot);
+    return 0;
+}
+
+/* =====================================================================
  * A.4 preprocess backward (computeCov2D backward + projection + SH + cov3D).
  * Inputs are the per-Gaussian gradients from the composite backward (float).
  * ===================================================================== */

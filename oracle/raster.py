@@ -252,6 +252,28 @@ def composite_backward(st: ForwardState, dL_dcolor, dL_dinvdepth=None) -> dict:
     return g
 
 
+def composite_backward64(st: ForwardState, dL_dcolor, dL_dinvdepth=None) -> dict:
+    """The composite backward evaluated in float64 on the fp32 forward's blend decisions, with a per-element error budget
+    (gmso_composite_backward64 in gms_oracle.c derives it).  Returns ref64 [P,10] and budget [P,10] in the order of the
+    kernels' per-Gaussian record (mean2D x/y, conic xx/xy/yy, opacity, rgb, inverse depth) and amb_share [P]: the largest
+    share of a Gaussian's budget that comes from the allowance at threshold-ambiguous pixels."""
+    P = st.radii.shape[0]
+    H, W = st.settings.image_height, st.settings.image_width
+    dL_dcolor = _f32(dL_dcolor).reshape(3, H, W)
+    dinv = _f32(dL_dinvdepth)
+    if dinv is not None:
+        dinv = dinv.reshape(H, W)
+    out = dict(ref64=np.zeros((P, 10), np.float64), budget=np.zeros((P, 10), np.float64), amb_share=np.zeros(P, np.float64))
+    pl = st.point_list if st.N > 0 else np.zeros(1, np.uint32)
+    amb = np.ascontiguousarray(st.ambiguous, dtype=np.uint8)
+    rc = lib().gmso_composite_backward64(ctypes.byref(st.cs), _p(st.ranges), _p(pl), _p(st.means2D), _p(st.rgb),
+                                         _p(st.conic_opacity), _p(st.depths), _p(st.n_contrib), _p(amb), _p(dL_dcolor),
+                                         _p(dinv), _p(out["ref64"]), _p(out["budget"]), _p(out["amb_share"]))
+    if rc != 0:
+        raise RuntimeError(f"gmso_composite_backward64 failed rc={rc}")
+    return out
+
+
 def preprocess_backward(st: ForwardState, g: dict) -> dict:
     P = st.radii.shape[0]
     inp = st.inputs
@@ -284,6 +306,8 @@ def backward(st: ForwardState, dL_dcolor, dL_dinvdepth=None) -> dict:
     g = composite_backward(st, dL_dcolor, dL_dinvdepth)
     out = preprocess_backward(st, g)
     out["_composite"] = g
+    # the upstream gradients, for checks that re-evaluate the composite backward (composite_backward64)
+    out["_upstream"] = (dL_dcolor, dL_dinvdepth)
     return out
 
 

@@ -90,8 +90,9 @@ def oracle_chain(p, S, dC, gpu, triangles=None):
     return st, grads
 
 
-def assert_forward_parity(st, color, radii, invd, state, tol=1e-5):
-    """Bit-exact indices, <= tol per pixel (threshold-ambiguous pixels get a bounded looser check)."""
+def assert_forward_parity(st, color, radii, invd, state, tol=1e-5, max_ambiguous=5e-4):
+    """Bit-exact indices, <= tol per pixel (threshold-ambiguous pixels get a bounded looser check; at most `max_ambiguous` of
+    the image may be threshold-ambiguous)."""
     np.testing.assert_array_equal(radii, st.radii)
     assert state["num_rendered"] == st.N
     if st.radii.shape[0]:
@@ -106,13 +107,13 @@ def assert_forward_parity(st, color, radii, invd, state, tol=1e-5):
     np.testing.assert_array_equal(state["point_list"].astype(np.uint32), st.point_list)
     np.testing.assert_array_equal(state["tile_keys"].astype(np.uint64), st.keys_sorted >> np.uint64(32))
     np.testing.assert_array_equal(state["ranges"], st.ranges)
-    ok = assert_image_parity(st, color, tol)
+    ok = assert_image_parity(st, color, tol, max_ambiguous)
     np.testing.assert_array_equal(state["n_contrib"][ok], st.n_contrib[ok])
     assert np.abs(invd - st.invdepth)[:, ok].max() <= tol
     assert np.abs(state["final_T"] - st.final_T)[ok].max() <= tol
 
 
-def assert_image_parity(st, color, tol=1e-5):
+def assert_image_parity(st, color, tol=1e-5, max_ambiguous=5e-4):
     """<= tol per pixel outside the threshold-ambiguous pixels; returns the mask of those other pixels.
     Threshold-ambiguous pixels: the oracle flags a pixel when one of its skip / stop decisions (alpha < 1/255,
     T(1-alpha) < 1e-4) lies within the +-1e-6 relative band in which exp() (GPU: ex2.approx.ftz) may fall on the other side.
@@ -126,7 +127,7 @@ def assert_image_parity(st, color, tol=1e-5):
     cmax = float(max(1.0, np.abs(st.rgb).max())) if st.radii.shape[0] else 1.0
     print(f"[parity] {st.settings.image_width}x{st.settings.image_height} P={st.radii.shape[0]} N={st.N}: max|image-oracle| = {err_ok:.2e}; "
           f"threshold-ambiguous pixels = {n_amb} ({n_amb / ok.size:.1e} of the image), worst there = {err_amb:.2e} (bound {cmax / 255:.1e})")
-    assert n_amb <= max(4, 5e-4 * ok.size), f"too many threshold-ambiguous pixels: {n_amb}"
+    assert n_amb <= max(4, max_ambiguous * ok.size), f"too many threshold-ambiguous pixels: {n_amb}"
     assert err_ok <= tol, err_ok
     assert err_amb <= 2.0 * cmax / 255.0, err_amb
     return ok
@@ -150,20 +151,71 @@ ILL_CONDITIONED = {"scales": 25.0, "rotations": 25.0, "cov3D_precomp": 25.0, "me
 STAGE2_TOL = {"scales": 5e-3, "rotations": 5e-3, "cov3D_precomp": 5e-3, "means3D": 5e-4}   # means3D: the J*W chain of near-edge-on splats, measured <= 9e-5
 
 
+COMPOSITE_GROUPS = {"dL_dmean2D": slice(0, 2), "dL_dconic": slice(2, 5), "dL_dopacity": slice(5, 6), "dL_dcolor": slice(6, 9),
+                    "dL_dinvdepth": slice(9, 10)}
+COMPONENTS = ("mean2D.x", "mean2D.y", "conic.xx", "conic.xy", "conic.yy", "opacity", "rgb.r", "rgb.g", "rgb.b", "invdepth")
+
+
+def composite_floor_errors(st, dg, comp):
+    """The global stage-1 measure: per group, max over the visible Gaussians of |gpu - oracle| / max |oracle|."""
+    vis = st.radii > 0
+    out = {}
+    for k, sl in COMPOSITE_GROUPS.items():
+        got = dg[:, sl].astype(np.float64)
+        ref = np.asarray(comp[k], np.float64).reshape(got.shape)
+        scale = max(np.abs(ref).max(), 1e-30)
+        out[k] = float(np.abs(got - ref)[vis].max() / scale) if vis.any() else 0.0
+    return out
+
+
+def composite_budget_ratios(dg, ref64, budget):
+    """|gpu - ref64| / budget per Gaussian and component (0 where both are exactly equal, inf where the budget is 0 and the
+    value is not, NaN where the value is NaN)."""
+    err = np.abs(np.asarray(dg, np.float64)[:, :10] - ref64)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.where(err == 0, 0.0, err / budget)
+
+
+# Gaussians whose budget is mostly the allowance of threshold-ambiguous pixels (amb_share > 0.5), as a share of those with any
+# gradient: measured <= 6.5 % on the random parity scenes, whose few ambiguous pixels are mostly the T < 1e-4 stop deep in a
+# list; 10 % keeps the allowance from quietly taking over a scene.
+AMB_MOSTLY_MAX = 0.10
+
+
+def assert_composite_per_gaussian(st, dgeom, ref64, budget, amb_share=None, label=""):
+    """Every Gaussian and every component of the composite backward's per-Gaussian record: |gpu - ref64| <= budget, the float64
+    reference and the a-priori budget of oracle.raster.composite_backward64.  A Gaussian that blends nowhere has budget 0
+    and must come out exactly zero.  Prints the worst ratio per component."""
+    assert np.isfinite(ref64).all() and np.isfinite(budget).all(), "non-finite float64 reference or budget"
+    finite = np.isfinite(np.asarray(dgeom)[:, :10])
+    assert finite.all(), f"non-finite composite backward at {int((~finite).sum())} elements, e.g. {np.argwhere(~finite)[0].tolist()}"
+    r = composite_budget_ratios(dgeom, ref64, budget)
+    worst = r.max(0) if r.shape[0] else np.zeros(10)
+    has = (budget > 0).any(1)
+    mostly = int((amb_share > 0.5).sum()) if amb_share is not None else 0
+    print(f"[per-Gaussian{(' ' + label) if label else ''}] worst |gpu - ref64| / budget: "
+          + ", ".join(f"{c} {w:.3g}" for c, w in zip(COMPONENTS, worst))
+          + f"; {int(has.sum())} Gaussians with a gradient, {mostly} of them mostly ambiguous-pixel allowance")
+    bad = np.argwhere(~(r <= 1))
+    assert bad.shape[0] == 0, (f"composite backward outside its budget at {bad.shape[0]} elements, e.g. Gaussian {bad[0][0]} "
+                               f"{COMPONENTS[bad[0][1]]}: gpu {float(dgeom[bad[0][0], bad[0][1]]):.9g} ref64 "
+                               f"{ref64[bad[0][0], bad[0][1]]:.9g} budget {budget[bad[0][0], bad[0][1]]:.3g}")
+    assert mostly <= AMB_MOSTLY_MAX * max(int(has.sum()), 1), f"{mostly} of {int(has.sum())} budgets are mostly allowance"
+    return worst
+
+
 def assert_backward_stages(st, g_gpu, g_ref, tol_composite=2e-5, tol_pre=5e-5):
     dg = g_gpu.get("_dgeom")
     comp = g_ref.get("_composite")
     if dg is None or comp is None:
         return False
-    vis = st.radii > 0
-    groups = {"dL_dmean2D": dg[:, 0:2], "dL_dconic": dg[:, 2:5], "dL_dopacity": dg[:, 5], "dL_dcolor": dg[:, 6:9], "dL_dinvdepth": dg[:, 9]}
     msg = []
-    for k, got in groups.items():
-        ref = np.asarray(comp[k], np.float64).reshape(got.shape)
-        scale = max(np.abs(ref).max(), 1e-30)
-        e = np.abs(got.astype(np.float64) - ref)[vis].max() / scale if vis.any() else 0.0
+    for k, e in composite_floor_errors(st, dg, comp).items():
         msg.append(f"{k} {e:.1e}")
         assert e <= tol_composite, f"composite backward {k}: {e:.3e} > {tol_composite}"
+    assert "_upstream" in g_ref, "the oracle gradients carry no upstream gradients (_upstream): the per-Gaussian check needs them"
+    r = raster.composite_backward64(st, *g_ref["_upstream"])
+    assert_composite_per_gaussian(st, dg, r["ref64"], r["budget"], r["amb_share"])
     # stage 2: the oracle's preprocess backward on the GPU's own sums
     fed = dict(dL_dmean2D=dg[:, 0:2].astype(np.float64), dL_dconic=dg[:, 2:5].astype(np.float64), dL_dopacity=dg[:, 5].astype(np.float64),
                dL_dcolor=dg[:, 6:9].astype(np.float64), dL_dinvdepth=dg[:, 9].astype(np.float64))
@@ -180,7 +232,7 @@ def assert_backward_stages(st, g_gpu, g_ref, tol_composite=2e-5, tol_pre=5e-5):
     return True
 
 
-def assert_grad_parity(g_gpu, g_ref, tol=2e-4, st=None):
+def assert_grad_parity(g_gpu, g_ref, tol=2e-4, st=None, tol_composite=2e-5):
     pairs = [("means3D", "dL_dmeans3D"), ("means2D", "dL_dmeans2D"), ("opacities", "dL_dopacity"), ("shs", "dL_dsh"),
              ("colors_precomp", "dL_dcolors_precomp"), ("scales", "dL_dscales"), ("rotations", "dL_drotations"),
              ("cov3D_precomp", "dL_dcov3D")]
@@ -195,4 +247,4 @@ def assert_grad_parity(g_gpu, g_ref, tol=2e-4, st=None):
             checked += 1
     assert checked >= 5
     if st is not None:
-        assert_backward_stages(st, g_gpu, g_ref)
+        assert_backward_stages(st, g_gpu, g_ref, tol_composite=tol_composite)

@@ -56,6 +56,7 @@ def test_config3_sampled_tile_backward_matches_oracle_at_full_size():
         raster.set_tile_stride(1)
     go = raster.preprocess_backward(st, gc)
     go["_composite"] = gc
+    go["_upstream"] = (dC, None)       # zero outside the sampled tiles, where n_contrib is 0 as well
     # forward on the sampled tiles
     worst, amb = 0.0, 0
     for tile in range(0, T, stride):

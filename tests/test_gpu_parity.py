@@ -8,7 +8,8 @@ import torch
 
 from gms_b200 import _lib, scenes
 from helpers import settings_from_camera, random_gaussians
-from gpu_helpers import run_gpu, run_oracle, assert_forward_parity, assert_grad_parity
+from gpu_helpers import run_gpu, run_oracle, assert_composite_per_gaussian, assert_forward_parity, assert_grad_parity
+from oracle import raster
 
 pytestmark = pytest.mark.gpu
 
@@ -85,7 +86,9 @@ def test_saturating_scene_early_termination_and_long_lists():
     st, gref = run_oracle(S, g, dC, dI)
     assert (st.ranges[:, 1] - st.ranges[:, 0]).max() > 1000 and (st.final_T < 2e-4).mean() > 0.2
     assert_forward_parity(st, color, radii, invd, state)
-    assert_grad_parity(grads, gref, tol=5e-4)
+    # the global stage-1 floor at the end-to-end tolerance (measured 1.0e-4 on an H100): the per-element budget of
+    # assert_backward_stages is the sharp check for the deep lists
+    assert_grad_parity(grads, gref, tol=5e-4, st=st, tol_composite=5e-4)
 
 
 def test_flat_mesh_gaussians_edge_on_slivers():
@@ -101,7 +104,7 @@ def test_flat_mesh_gaussians_edge_on_slivers():
     color, radii, invd, state, grads = run_gpu(S, g, dC, dI)
     st, gref = run_oracle(S, g, dC, dI)
     assert_forward_parity(st, color, radii, invd, state)
-    assert_grad_parity(grads, gref, tol=5e-4)
+    assert_grad_parity(grads, gref, tol=5e-4, st=st)
 
 
 @pytest.mark.parametrize("fwd,bwd,tile_order,minb", [(2, 5, 1, 6), (2, 5, 0, 4), (2, 5, 1, 8), (2, 3, 1, 6), (3, 3, 0, 6), (3, 5, 1, 6)])
@@ -348,6 +351,10 @@ def test_sh_tile_staging_equals_direct_access(P, deg):
     # extent 2.5 puts splats next to the camera: screen-filling footprints whose gradients are fp32 atomic sums over
     # ~1e4 pixels with cancellation (the oracle sums in double) -- 5x the usual tolerance for this scene
     assert_grad_parity(a[4], gref, tol=1e-3)
+    # the composite backward per Gaussian (the preprocess backward of these splats, 6.4e-4 of max for means3D on an H100, is
+    # left to the end-to-end tolerance above)
+    r = raster.composite_backward64(st, dC, dI)
+    assert_composite_per_gaussian(st, a[4]["_dgeom"], r["ref64"], r["budget"], r["amb_share"])
 
 
 def test_empty_and_invisible_inputs():
