@@ -27,6 +27,7 @@
 #include "gms_free.cuh"
 #include "gms_knn.cuh"
 #include "gms_flame.cuh"
+#include "gms_lpips.cuh"
 
 // ------------------------------------------------------------------------------------------ host state
 static thread_local char g_err[512] = "";
@@ -70,11 +71,12 @@ static int sm_count() {
 
 // Optional per-kernel timing with CUDA events recorded on the launching stream (bench.py's roofline numbers).
 enum { K_PRE_FWD = 0, K_SORT_P, K_SCAN, K_EMIT, K_SORT_N, K_RANGES, K_COMP_FWD, K_COMP_BWD, K_PRE_BWD, K_EXP_FWD, K_EXP_BWD, K_LOSS_STATS, K_LOSS_GRAD, K_ADAM, K_MISC,
-       K_METRICS, K_METRICS_FIN, K_COUNT };
+       K_METRICS, K_METRICS_FIN, K_LPIPS_CONV, K_LPIPS_POOL, K_LPIPS_HEAD, K_COUNT };
 static const char* const g_kernel_names[K_COUNT] = {"preprocess_fwd", "cub_sort_depth", "cub_scan_tiles", "emit_dups", "cub_sort_tiles",
                                                     "tile_ranges", "composite_fwd", "composite_bwd", "preprocess_bwd", "expand_fwd",
                                                     "expand_bwd", "ssim_stats", "ssim_grad", "adam", "misc",
-                                                    "image_metrics", "metrics_finalize"};
+                                                    "image_metrics", "metrics_finalize", "lpips_conv", "lpips_pool",
+                                                    "lpips_head"};
 static int g_opt_time = 0;
 struct TimedSpan { int id; cudaEvent_t a, b; };
 static TimedSpan g_spans[1 << 15];
@@ -361,6 +363,75 @@ int gms_image_metrics(const gms_metrics_args* a, void* cuda_stream) {
                      a->img, a->gt, win, part))) return rc;
     return launch("metrics_finalize", K_METRICS_FIN, 0, st, 1, 256, 0, k_metrics_finalize, C, metric_tiles(H, W),
                   1.0 / ((double)H * (double)W), part, a->out);
+}
+
+// VGG16 up to relu5_3 (torchvision's vgg16().features): conv l reads Cin[l] channels and writes Cout[l]; the target maps are
+// the outputs of convs 1, 3, 6, 9 and 12 (features' 1-based layers 4, 9, 16, 23, 30), each followed by a 2x2 max-pool but
+// the last.
+static const int kLpipsCin[13] = {3, 64, 64, 128, 128, 256, 256, 256, 512, 512, 512, 512, 512};
+static const int kLpipsCout[13] = {64, 64, 128, 128, 256, 256, 256, 512, 512, 512, 512, 512, 512};
+static const int kLpipsTarget[5] = {1, 3, 6, 9, 12};
+static int lpips_kp(int l) { return l == 0 ? 32 : 9 * kLpipsCin[l]; }
+
+struct LpipsLayout {
+    float* act[2];      // ping-pong [2,H,W,64] (every later level holds at most as many floats)
+    double* part[5];    // per target layer: one partial per head block
+    int blocks[5];
+    size_t total;
+};
+static LpipsLayout lpips_layout(void* base, int H, int W) {
+    LpipsLayout L;
+    char* p = reinterpret_cast<char*>(base);
+    for (int i = 0; i < 2; i++) L.act[i] = carve<float>(p, (size_t)2 * H * W * 64);
+    for (int l = 0; l < 5; l++) {
+        const size_t hw = (size_t)(H >> l) * (W >> l);
+        L.blocks[l] = (int)((hw + GMS_LPIPS_HEAD_PIX - 1) / GMS_LPIPS_HEAD_PIX);
+        L.part[l] = carve<double>(p, L.blocks[l]);
+    }
+    L.total = (size_t)(p - reinterpret_cast<char*>(base));
+    return L;
+}
+
+size_t gms_lpips_scratch_bytes(int32_t H, int32_t W) {
+    if (H < 16 || W < 16) return 0;
+    return lpips_layout(nullptr, H, W).total + 256;
+}
+
+int gms_lpips_vgg(const gms_lpips_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !a->img || !a->gt || !a->weights || !a->out || !a->scratch) return set_err(GMS_E_ARG, "gms_lpips_vgg: null argument%s%s");
+    if (a->H < 16 || a->W < 16) return set_err(GMS_E_ARG, "gms_lpips_vgg: H and W must be at least 16%s%s");
+    if (a->scratch_bytes < gms_lpips_scratch_bytes(a->H, a->W)) return set_err(GMS_E_ARG, "gms_lpips_vgg: scratch too small%s%s");
+    const LpipsLayout L = lpips_layout(aligned_base(a->scratch), a->H, a->W);
+    const float* w = a->weights;
+    const float* lin = a->weights;
+    for (int l = 0; l < 13; l++) lin += (size_t)kLpipsCout[l] * (lpips_kp(l) + 1);
+    LpipsFinal fin;
+    int H = a->H, W = a->W, cur = 0, target = 0, rc;
+    const float* in = nullptr;
+    for (int l = 0; l < 13; l++) {
+        LpipsConv c;
+        c.in = in; c.img = a->img; c.gt = a->gt; c.w = w; c.bias = w + (size_t)kLpipsCout[l] * lpips_kp(l);
+        c.out = L.act[cur]; c.H = H; c.W = W; c.Cin = kLpipsCin[l]; c.Cout = kLpipsCout[l]; c.Kp = lpips_kp(l);
+        w = c.bias + kLpipsCout[l];
+        const dim3 grid((unsigned)((2 * (size_t)H * W + GMS_LPIPS_BM - 1) / GMS_LPIPS_BM), (unsigned)(c.Cout / GMS_LPIPS_BN));
+        if ((rc = launch("lpips_conv", K_LPIPS_CONV, 0, st, grid, 128, 0, l == 0 ? k_lpips_conv<true> : k_lpips_conv<false>, c))) return rc;
+        in = c.out;
+        if (l != kLpipsTarget[target]) { cur ^= 1; continue; }
+        const int C = c.Cout, hw = H * W;
+        void (*head)(const float*, int, const float*, double*) =
+            C == 64 ? k_lpips_head<2> : C == 128 ? k_lpips_head<4> : C == 256 ? k_lpips_head<8> : k_lpips_head<16>;
+        if ((rc = launch("lpips_head", K_LPIPS_HEAD, 0, st, L.blocks[target], 256, 0, head, c.out, hw, lin, L.part[target]))) return rc;
+        fin.part[target] = L.part[target]; fin.blocks[target] = L.blocks[target]; fin.inv_hw[target] = 1.0 / (double)hw;
+        lin += C;
+        if (++target == 5) break;
+        const size_t n4 = (size_t)2 * (H / 2) * (W / 2) * (C / 4);
+        if ((rc = launch("lpips_pool", K_LPIPS_POOL, 0, st, (unsigned)((n4 + 255) / 256), 256, 0, k_lpips_pool, c.out, H, W, C,
+                         L.act[cur ^ 1]))) return rc;
+        in = L.act[cur ^ 1];
+        H /= 2; W /= 2;
+    }
+    return launch("lpips_finalize", -1, 0, st, 1, 256, 0, k_lpips_finalize, fin, a->out);
 }
 
 int gms_adam_step(const gms_adam_args* a, void* cuda_stream) {

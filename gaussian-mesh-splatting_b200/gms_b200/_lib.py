@@ -241,6 +241,15 @@ class MetricsArgs(C.Structure):
                 ("quantize", C.c_int32), ("out", C.c_void_p), ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t)]
 
 
+LPIPS_WEIGHT_FLOATS = 14716480    # GMS_LPIPS_WEIGHT_FLOATS
+
+
+class LpipsArgs(C.Structure):
+    """struct gms_lpips_args"""
+    _fields_ = [("H", C.c_int32), ("W", C.c_int32), ("img", C.c_void_p), ("gt", C.c_void_p), ("weights", C.c_void_p),
+                ("out", C.c_void_p), ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t)]
+
+
 class AdamShArgs(C.Structure):
     _fields_ = [("P", C.c_int32), ("M", C.c_int32), ("sh_degree", C.c_int32), ("R", C.c_int32), ("xyz", C.c_void_p),
                 ("exchange", C.c_void_p), ("slot_floats", C.c_int64), ("grad_scale", C.c_float), ("p", C.c_void_p),
@@ -292,7 +301,8 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_bound_points_render_frame", "gms_free_train_frame", "gms_free_render_frame", "gms_densify_scratch_bytes",
                "gms_densify_plan", "gms_densify_apply", "gms_knn_scratch_bytes", "gms_knn_dist2",
                "gms_flame_render_workspace_bytes", "gms_flame_render_frame", "gms_image_composite_rgba", "gms_image_resize_u8",
-               "gms_flame_lbs_workspace_bytes", "gms_flame_lbs_forward", "gms_flame_lbs_backward"]
+               "gms_flame_lbs_workspace_bytes", "gms_flame_lbs_forward", "gms_flame_lbs_backward", "gms_lpips_scratch_bytes",
+               "gms_lpips_vgg"]
 
 _lib = None
 
@@ -376,6 +386,9 @@ def lib():
     L.gms_flame_lbs_backward.argtypes = [C.POINTER(FlameLbsArgs), C.c_void_p]
     L.gms_metrics_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]
     L.gms_image_metrics.argtypes = [C.POINTER(MetricsArgs), C.c_void_p]
+    L.gms_lpips_scratch_bytes.restype = C.c_size_t
+    L.gms_lpips_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
+    L.gms_lpips_vgg.argtypes = [C.POINTER(LpipsArgs), C.c_void_p]
     _lib = L
     # GMS_OPTIONS="key=value,key=value": tuning knobs applied at load (A/B runs of whole test suites / benches)
     for kv in filter(None, os.environ.get("GMS_OPTIONS", "").split(",")):

@@ -20,7 +20,7 @@ re-renders those views before it reads its results."""
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import List, Sequence
+from typing import List, Optional, Sequence
 
 import torch
 
@@ -34,6 +34,7 @@ class Evaluation:
     per_view: torch.Tensor      # float64 [n,4] on the host, columns METRIC_NAMES
     mean: torch.Tensor          # float64 [4]: the mean of the per-view values (PSNR too, as both reference scripts average it)
     rerun: List[int]            # views whose first render overflowed its capacity and was re-rendered before scoring
+    lpips: Optional[torch.Tensor] = None    # float32 [n] on the host: per-view LPIPS when evaluate() was given an Lpips
 
 
 class NativeRenderer(SyncFreeCapacity):
@@ -115,15 +116,19 @@ class NativeRenderer(SyncFreeCapacity):
         return gt.to(self.dev, non_blocking=True)
 
     def evaluate(self, cams: Sequence, gts: Sequence[torch.Tensor], bg: torch.Tensor, protocol: str = "training_report",
-                 scale_modifier: float = 1.0, antialiasing: bool = False) -> Evaluation:
+                 scale_modifier: float = 1.0, antialiasing: bool = False, lpips=None) -> Evaluation:
         """Renders every view and scores it against its ground truth (metrics.METRIC_NAMES under `protocol`, "training_report"
         or "metrics"), all on the current stream into one device array; the host synchronises once, at the end.  Views whose
         render overflowed its predicted capacity are then re-rendered, sized from their true N, and re-scored before the
-        array is read."""
+        array is read.  Given an lpips.Lpips (protocol "metrics" only, as metrics.py alone reports LPIPS), each view's LPIPS
+        is scored in the same pass on the 8-bit round trip of the render and of the ground truth, into Evaluation.lpips."""
         if len(cams) != len(gts):
             raise ValueError(f"evaluate: {len(cams)} cameras but {len(gts)} ground-truth images")
+        if lpips is not None and protocol != "metrics":
+            raise ValueError(f"evaluate: LPIPS is scored under protocol 'metrics' only (metrics.py); got {protocol!r}")
         n = len(cams)
         out = torch.empty(n, len(METRIC_NAMES), dtype=torch.float64, device=self.dev)
+        lp = torch.empty(n, 6, dtype=torch.float32, device=self.dev) if lpips is not None else None
         slots = torch.full((max(n, 1), 2), -1, dtype=torch.int32).pin_memory()     # per view: (N, overflow flag), mapped
         slots_np = slots.numpy()
         keys = [self._view_key(c) for c in cams]
@@ -131,7 +136,10 @@ class NativeRenderer(SyncFreeCapacity):
 
         def one(v, capacity):
             self._render(cams[v], bg, scale_modifier, antialiasing, capacity, slots.data_ptr() + 8 * v)
-            image_metrics(self.image, self._gt_float(gts[v]), protocol, out=out[v], scratch=self._metric_scratch)
+            gt = self._gt_float(gts[v])
+            image_metrics(self.image, gt, protocol, out=out[v], scratch=self._metric_scratch)
+            if lp is not None:
+                lpips.lpips(self._round_trip(self.image, 0), self._round_trip(gt, 1), out=lp[v])
 
         for v in range(n):
             caps.append(self._predict_capacity(keys[v]))
@@ -148,9 +156,23 @@ class NativeRenderer(SyncFreeCapacity):
             one(v, max(int(slots_np[v, 0]), 1))
         if n:
             self.capacity = max(caps)
+        lp_host = None
+        if lp is not None:          # ordered before the read-back below, which waits for it
+            lp_host = torch.empty(n, dtype=torch.float32).pin_memory()
+            lp_host.copy_(lp[:, 5], non_blocking=True)
         per_view = out.cpu()        # (waits for the re-runs, if any)
         mean = per_view.mean(0) if n else torch.full((len(METRIC_NAMES),), float("nan"), dtype=torch.float64)
-        return Evaluation(per_view=per_view, mean=mean, rerun=rerun)
+        return Evaluation(per_view=per_view, mean=mean, rerun=rerun, lpips=lp_host)
+
+    def _round_trip(self, image: torch.Tensor, slot: int) -> torch.Tensor:
+        """save_image's 8-bit rounding of float [3,H,W] and back to byte / 255 (what metrics.py reads from the PNG), into one
+        of two reused device buffers."""
+        if getattr(self, "_rt", None) is None:
+            self._rt = (torch.empty(self.H, 3 * self.W, dtype=torch.uint8, device=self.dev),
+                        [torch.empty(3, self.H, self.W, dtype=torch.float32, device=self.dev) for _ in range(2)])
+        u8, f = self._rt
+        io_image.quantize(image, out=u8)
+        return io_image.to_device_float(u8.view(self.H, self.W, 3), out=f[slot])
 
 
 class PointsRenderer(NativeRenderer):

@@ -731,6 +731,31 @@ typedef struct gms_metrics_args {
 int gms_metrics_scratch_bytes(int32_t C, int32_t H, int32_t W, size_t* bytes);
 int gms_image_metrics(const gms_metrics_args* a, void* cuda_stream);
 
+/* LPIPS of an image against its ground truth: lpips(render, gt, net_type='vgg') (lpipsPyTorch, metrics.py:74), version 0.1,
+ * forward only, deterministically (per-block partial sums added in a fixed order in double, no atomics).  Both images are
+ * float [3,H,W] as the reference's tensors hold them (to_tensor of the PNG: byte / 255); they are not mapped to [-1,1].
+ * out (device, float [6]): the five layer terms (relu1_2, relu2_2, relu3_3, relu4_3, relu5_3), then their sum, LPIPS.
+ * Packed weights (float, GMS_LPIPS_WEIGHT_FLOATS), in this order:
+ *   for each of the 13 convs of torchvision's vgg16().features (Cin -> Cout: 3->64, 64->64, 64->128, 128->128, 128->256,
+ *   256->256 twice, 256->512, 512->512 five times): the weight [Cout][Kp] with K ordered (ky, kx, ci), i.e.
+ *   weight.permute(0, 2, 3, 1) flattened, Kp = 9 * Cin, except conv1_1's Kp = 32 (27 values, then 5 zeros); then the bias
+ *   [Cout].  Then the lin weights lin0..lin4 (vgg.pth's lin{l}.model.1.weight), 64 + 128 + 256 + 512 + 512 floats.
+ * H or W < 16 (relu5_3 would be empty), a null pointer or scratch smaller than gms_lpips_scratch_bytes(H, W) is
+ * GMS_E_ARG, returned without a launch.  Caller's stream, no host synchronisation. */
+#define GMS_LPIPS_WEIGHT_FLOATS 14716480
+typedef struct gms_lpips_args {
+    int32_t H, W;               /* >= 16 */
+    const float* img;           /* [3,H,W] */
+    const float* gt;            /* [3,H,W] */
+    const float* weights;       /* packed, see above */
+    float* out;                 /* device [6] */
+    void* scratch;              /* gms_lpips_scratch_bytes(H, W) bytes */
+    size_t scratch_bytes;
+} gms_lpips_args;
+/* Scratch of gms_lpips_vgg at H x W (two [2,H,W,64] activation buffers and the partial sums); 0 when H or W < 16. */
+size_t gms_lpips_scratch_bytes(int32_t H, int32_t W);
+int gms_lpips_vgg(const gms_lpips_args* a, void* cuda_stream);
+
 /* ---- image sink / source (SURVEY.md section 8(f) rank 4) ---------------------------------------- */
 
 /* float [C,H,W] -> 8-bit interleaved rows, byte = clamp(x * 255 + 0.5, 0, 255) truncated: the device half of
