@@ -70,10 +70,17 @@ class NativeRenderer(SyncFreeCapacity):
         f = m._features if m._features is not None else m.get_features      # packed SH: zero-copy
         return f.detach().contiguous()
 
+    _sweep_vertices = None      # set by render(vertices=...) for that one frame
+
     def _check(self, cam, bg) -> None:
         m = self.model
         for name in ("vertices", "_alpha", "_scale", "_opacity"):
             check_float32(getattr(m, name), f"NativeRenderer: model.{name}", self.dev)
+        v = self._sweep_vertices
+        if v is not None:
+            check_float32(v, "NativeRenderer: the frame's vertices", self.dev)
+            if v.shape != m.vertices.shape:
+                raise RuntimeError(f"NativeRenderer: the frame's vertices must be {list(m.vertices.shape)}; got {list(v.shape)}")
         if m.faces.device != self.dev:
             raise RuntimeError("NativeRenderer: model.faces must live on the model's device")
         if m._scale.shape[0] != self.radii.shape[0]:
@@ -87,11 +94,12 @@ class NativeRenderer(SyncFreeCapacity):
         m = self.model
         feats = self._features()
         a = _lib.RenderArgs()
-        a.V, a.M = m.vertices.shape[0], feats.shape[1]
+        v = m.vertices if self._sweep_vertices is None else self._sweep_vertices
+        a.V, a.M = v.shape[0], feats.shape[1]
         a.F, a.K, seg = m.frame_sizes()
         if seg is not None:
             a.segments, a.n_segments = seg, len(seg)
-        a.vertices, a.faces, a.alpha_raw, a.scale_raw = m.vertices.data_ptr(), m.faces.data_ptr(), m._alpha.data_ptr(), m._scale.data_ptr()
+        a.vertices, a.faces, a.alpha_raw, a.scale_raw = v.data_ptr(), m.faces.data_ptr(), m._alpha.data_ptr(), m._scale.data_ptr()
         a.features, a.opacity_raw, a.eps = feats.data_ptr(), m._opacity.data_ptr(), m.eps_s0
         a.alpha_activation = getattr(m, "alpha_activation", _lib.ALPHA_RELU)
         self._call("gms_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
@@ -101,10 +109,17 @@ class NativeRenderer(SyncFreeCapacity):
         a.image, a.invdepth, a.radii = self.image.data_ptr(), self.invdepth.data_ptr(), self.radii.data_ptr()
         self._launch(fn, a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
 
-    def render(self, cam, bg: torch.Tensor, scale_modifier: float = 1.0, antialiasing: bool = False):
+    def render(self, cam, bg: torch.Tensor, scale_modifier: float = 1.0, antialiasing: bool = False,
+               vertices: torch.Tensor = None):
         """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view, the reference's render(...)["render"], ["radii"],
-        ["depth"]."""
-        self._render(cam, bg, scale_modifier, antialiasing)
+        ["depth"].  `vertices` (float32, model.vertices' shape), when given, is this frame's mesh in place of the model's
+        (one frame of an animated sweep, renderer/gaussian_animated_renderer's `triangles` as vertices[faces]); the model
+        is never modified."""
+        self._sweep_vertices = None if vertices is None else vertices.detach()
+        try:
+            self._render(cam, bg, scale_modifier, antialiasing)
+        finally:
+            self._sweep_vertices = None
         return self.image, self.radii, self.invdepth
 
     def _gt_float(self, gt: torch.Tensor) -> torch.Tensor:
