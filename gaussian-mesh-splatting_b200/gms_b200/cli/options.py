@@ -24,6 +24,11 @@ OPT_PARAMS_FREE = (("iterations", 30_000), ("position_lr_init", 0.00016), ("posi
 OPT_PARAMS_MESH = (("iterations", 30_000), ("vertices_lr", 0.0), ("alpha_lr", 0.001), ("feature_lr", 0.0025), ("opacity_lr", 0.05),
                    ("scaling_lr", 0.005), ("rotation_lr", 0.001), ("random_background", False), ("use_mesh", True),
                    ("lambda_dssim", 0.2))
+# OptimizationParamsFlame (gs_flame)
+OPT_PARAMS_FLAME = (("iterations", 30_000), ("alpha_lr", 0.001), ("feature_lr", 0.0025), ("opacity_lr", 0.05), ("scaling_lr", 0.005),
+                    ("rotation_lr", 0.001), ("flame_shape_lr", 0.01), ("flame_exp_lr", 0.001), ("flame_pose_lr", 0.001),
+                    ("flame_neck_pose_lr", 0.001), ("flame_trans_lr", 0.001), ("vertices_enlargement_lr", 0.0002),
+                    ("random_background", False), ("use_mesh", True), ("lambda_dssim", 0.2))
 
 # what train.py's ModelParams.extract keeps (the group's own keys plus the three train.py sets on it) -> cfg_args
 MODEL_KEYS = tuple(n for n, _, _ in MODEL_PARAMS) + ("num_splats", "meshes", "gs_type")

@@ -1,8 +1,11 @@
-"""python -m gms_b200.cli.train -s <scene> [-m <output>] [--gs_type gs_mesh|gs_flat|gs] ...: the reference's train.py on the
-native trainers.
+"""python -m gms_b200.cli.train -s <scene> [-m <output>] [--gs_type gs_mesh|gs_multi_mesh|gs_flame|gs_flat|gs] ...: the
+reference's train.py on the native trainers.
 
-Flags, defaults and the output directory are the reference's (cfg_args, cameras.json, input.ply,
-point_cloud/iteration_N/point_cloud.ply [+ model_params.pt], chkpnt<N>.pth).  One iteration, in train.py's order
+Flags, defaults and the output directory are the reference's (cfg_args, cameras.json, input.ply -- input_<i>.ply per mesh
+for gs_multi_mesh --, point_cloud/iteration_N/point_cloud.ply [+ model_params.pt or flame_params.pt], chkpnt<N>.pth).
+gs_multi_mesh trains on a COLMAP scene with --meshes a b ... (sparse/0/<name>.obj) and one --num_splats per mesh
+(MultiMeshGaussianModel, MeshTrainer); gs_flame on a NeRF-synthetic scene with the FLAME model file --flame_model
+(NativeFlame, FlameTrainer).  One iteration, in train.py's order
 (train.py:61-157):
 
     SH degree up every 1000 -> the view from the Scene's view order -> background (torch.rand(3) on the device under
@@ -19,7 +22,12 @@ Deliberate differences:
     background generator), not the reference's capture() tuple; a resumed run continues the uninterrupted run's sequence of
     views and backgrounds, where the reference re-shuffles.
   * --seed (default 0) seeds what safe_state seeds: the view shuffle and order, the initial model and the backgrounds.
-  * Not built, refused by name: gs_flame, gs_multi_mesh, --antialiasing, --debug, --debug_from, --detect_anomaly,
+  * gs_multi_mesh without --meshes, or with a --num_splats count other than the --meshes count, is refused (the reference's
+    zip would drop the unmatched meshes); so are gs_multi_mesh on a NeRF-synthetic scene and gs_flame on a COLMAP scene, on
+    which the reference crashes, and gs_flame without its model file.
+  * flame_params.pt carries the FLAME buffers as NativeFlame.to_point_cloud()'s dict, not the reference's pickled
+    FLAMEPointCloud: cli.render and cli.render_flame rebuild the model from the checkpoint alone.
+  * Not built, refused by name: --antialiasing, --debug, --debug_from, --detect_anomaly,
     --convert_SHs_python, --compute_cov3D_python, --save_xyz, --data_device other than cuda.  --ip / --port are accepted and
     ignored (the reference does not start its viewer either)."""
 from __future__ import annotations
@@ -39,13 +47,14 @@ import numpy as np
 import torch
 
 from .. import dataset, io_ply
-from ..model import FreeGaussianModel, MeshGaussianModel
+from ..model import FlameGaussianModel, FreeGaussianModel, MeshGaussianModel, MultiMeshGaussianModel
 from ..scenes import MeshGaussianParams
-from ..trainer import FreeOptimizationParams, FreeTrainer, MeshTrainer
+from ..trainer import FlameOptimizationParams, FlameTrainer, FreeOptimizationParams, FreeTrainer, MeshTrainer
 from . import options
 
-GS_TYPES = ("gs_mesh", "gs_flat", "gs")
+GS_TYPES = ("gs_mesh", "gs_multi_mesh", "gs_flame", "gs_flat", "gs")
 FREE_TYPES = ("gs", "gs_flat")
+MESH_TYPES = ("gs_mesh", "gs_multi_mesh")       # MeshTrainer: OptimizationParamsMesh, SH degree up in the loop
 # flags of the reference that the native training frames do not implement: (name, default)
 REFUSED = (("debug_from", -1), ("detect_anomaly", False), ("save_xyz", False), ("convert_SHs_python", False),
            ("compute_cov3D_python", False), ("debug", False), ("antialiasing", False))
@@ -68,10 +77,22 @@ def build_parser(gs_type: str) -> ArgumentParser:
     p.add_argument("--start_checkpoint", type=str, default=None)
     p.add_argument("--save_xyz", action="store_true")
     options.add_group(p, "Loading Parameters", options.MODEL_PARAMS)
-    options.add_group(p, "Optimization Parameters", options.OPT_PARAMS_MESH if gs_type == "gs_mesh" else options.OPT_PARAMS_FREE)
+    opt = options.OPT_PARAMS_MESH if gs_type in MESH_TYPES else options.OPT_PARAMS_FLAME if gs_type == "gs_flame" else options.OPT_PARAMS_FREE
+    options.add_group(p, "Optimization Parameters", opt)
     options.add_group(p, "Pipeline Parameters", options.PIPELINE_PARAMS)
     p.add_argument("--seed", type=int, default=0, help="seeds the view shuffle and order, the initial model and the backgrounds")
+    p.add_argument("--flame_model", type=str, default=dataset.DEFAULT_FLAME_MODEL,
+                   help="gs_flame: FLAME's model file (FlameConfig's path, relative to the working directory)")
     return p
+
+
+def scene_kind(source_path: str):
+    """"colmap" (sparse/), "blender" (transforms_train.json) or None, as Scene.__init__ tells them apart."""
+    if os.path.exists(os.path.join(source_path, "sparse")):
+        return "colmap"
+    if os.path.exists(os.path.join(source_path, "transforms_train.json")):
+        return "blender"
+    return None
 
 
 def parse_args(argv) -> Namespace:
@@ -83,14 +104,26 @@ def parse_args(argv) -> Namespace:
     gs_type = pre.parse_known_args(argv)[0].gs_type
     parser = build_parser(gs_type if gs_type in GS_TYPES else "gs_mesh")
     if gs_type not in GS_TYPES:
-        parser.error(f"--gs_type {gs_type} is not supported (supported: {', '.join(GS_TYPES)}); gs_flame needs the FLAME model "
-                     f"files and gs_multi_mesh a COLMAP mesh reader")
+        parser.error(f"--gs_type {gs_type} is not supported (supported: {', '.join(GS_TYPES)})")
     args = parser.parse_args(argv)
     for name, default in REFUSED:
         if getattr(args, name) != default:
             parser.error(f"--{name} is not supported by the native training frames")
     if args.data_device != "cuda":
         parser.error(f"--data_device {args.data_device} is not supported: images stay resident on the GPU (--data_device cuda)")
+    if gs_type == "gs_multi_mesh":
+        if not args.meshes:
+            parser.error("--gs_type gs_multi_mesh needs --meshes (the names of sparse/0/<name>.obj) and one --num_splats per mesh")
+        if len(args.num_splats) != len(args.meshes):
+            parser.error(f"--gs_type gs_multi_mesh needs one --num_splats per --meshes entry; got {len(args.num_splats)} "
+                         f"--num_splats for {len(args.meshes)} --meshes")
+    if gs_type == "gs_flame" and not os.path.isfile(args.flame_model):
+        parser.error(f"--gs_type gs_flame needs FLAME's model file: --flame_model {args.flame_model} does not exist")
+    kind = scene_kind(args.source_path)
+    need = {"gs_multi_mesh": "colmap", "gs_flame": "blender"}.get(gs_type)
+    if need is not None and kind is not None and kind != need:
+        parser.error(f"--gs_type {gs_type} trains on {'COLMAP' if need == 'colmap' else 'NeRF-synthetic'} scenes; "
+                     f"--source_path {args.source_path} is a {'COLMAP' if kind == 'colmap' else 'NeRF-synthetic'} scene")
     args.save_iterations.append(args.iterations)
     return args
 
@@ -122,6 +155,10 @@ def iteration_events(it: int, args: Namespace) -> List[str]:
 
 def free_params(args: Namespace) -> FreeOptimizationParams:
     return FreeOptimizationParams(**{k: getattr(args, k) for k in FreeOptimizationParams.__dataclass_fields__ if k != "min_opacity"})
+
+
+def flame_params(args: Namespace) -> FlameOptimizationParams:
+    return FlameOptimizationParams(**{k: getattr(args, k) for k in FlameOptimizationParams.__dataclass_fields__})
 
 
 class ViewOrder:
@@ -184,7 +221,12 @@ def write_cameras_json(path: str, scene: dataset.Scene, seed: int) -> None:
 
 def write_input_ply(path: str, scene: dataset.Scene, source_path: str, gs_type: str, seed: int) -> None:
     """Scene.__init__'s input.ply: a byte copy of the dataset's own cloud file where it has one, else the cloud the
-    reference's reader would have stored (the random NeRF-synthetic cloud, the converted COLMAP points, the gs_mesh cloud)."""
+    reference's reader would have stored (the random NeRF-synthetic cloud, the converted COLMAP points, the gs_mesh cloud).
+    gs_multi_mesh writes input_<i>.ply per mesh next to `path` instead; gs_flame's cloud needs the model (Training.prepare)."""
+    if gs_type == "gs_multi_mesh":
+        for i, cloud in enumerate(scene.mesh_clouds):
+            io_ply.save_point_cloud(os.path.join(os.path.dirname(path), f"input_{i}.ply"), *cloud)
+        return
     if gs_type == "gs_mesh":
         io_ply.save_point_cloud(path, *dataset.mesh_input_cloud(scene.mesh, seed))
         return
@@ -251,18 +293,24 @@ class Training:
             f.write(options.cfg_args_string(a))
         if self.scene is None:
             self.scene = dataset.load_scene(a.source_path, a.gs_type, a.white_background, a.eval, a.resolution, a.images,
-                                            a.num_splats[0], a.seed, device=self.dev)
+                                            a.num_splats if a.gs_type == "gs_multi_mesh" else a.num_splats[0], a.seed,
+                                            device=self.dev, meshes=a.meshes, flame_model=a.flame_model)
         sc = self.scene
-        write_input_ply(os.path.join(a.model_path, "input.ply"), sc, a.source_path, a.gs_type, a.seed)
+        if a.gs_type != "gs_flame":
+            write_input_ply(os.path.join(a.model_path, "input.ply"), sc, a.source_path, a.gs_type, a.seed)
         write_cameras_json(os.path.join(a.model_path, "cameras.json"), sc, a.seed)
         sizes = {(c.image_width, c.image_height) for c in sc.train_cameras + sc.test_cameras}
         if len(sizes) > 1:
             raise ValueError(f"training needs every view at one size; this scene has {sorted(sizes)} (-r sets a common width)")
         self.bg = torch.tensor([1.0, 1.0, 1.0] if a.white_background else [0.0, 0.0, 0.0], dtype=torch.float32, device=self.dev)
         self.bg_gen = torch.Generator(device=self.dev).manual_seed(a.seed) if a.random_background else None
-        if a.gs_type == "gs_mesh":
-            self.model = MeshGaussianModel.from_params(_mesh_params(sc.mesh, a.sh_degree), self.dev, sh_degree=a.sh_degree,
-                                                       active_sh_degree=0, packed_features=True)
+        if a.gs_type in MESH_TYPES:
+            if a.gs_type == "gs_mesh":
+                self.model = MeshGaussianModel.from_params(_mesh_params(sc.mesh, a.sh_degree), self.dev, sh_degree=a.sh_degree,
+                                                           active_sh_degree=0, packed_features=True)
+            else:
+                self.model = MultiMeshGaussianModel.from_mesh_params([_mesh_params(p, a.sh_degree) for p in sc.meshes], self.dev,
+                                                                     sh_degree=a.sh_degree, active_sh_degree=0, packed_features=True)
             tr = self.trainer = MeshTrainer(self.model, self.bg, a.lambda_dssim, native=True)
             lrs = {"vertices": a.vertices_lr, "alpha": a.alpha_lr, "opacity": a.opacity_lr, "scaling": a.scaling_lr}
             for g in tr.opt.groups:         # OptimizationParamsMesh's learning rates (mesh_model_groups' f_rest = f_dc / 20)
@@ -270,6 +318,13 @@ class Training:
                     g["lr0"], g["lr1"] = a.feature_lr, a.feature_lr / 20.0
                 else:
                     g["lr"] = lrs[g["name"]]
+        elif a.gs_type == "gs_flame":
+            from ..flame import NativeFlame
+            self.driver = NativeFlame.from_model_file(a.flame_model, device=self.dev)
+            self.model = FlameGaussianModel.create(self.driver, sc.flame.faces, K=dataset.FLAME_K, sh_degree=a.sh_degree, seed=a.seed,
+                                                   device=self.dev)
+            io_ply.save_point_cloud(os.path.join(a.model_path, "input.ply"), *dataset.flame_input_cloud(self.model, sc.flame))
+            self.trainer = FlameTrainer(self.model, self.bg, flame_params(a))
         else:
             points, colors, _ = sc.point_cloud
             self.model = FreeGaussianModel.from_point_cloud(points, colors, a.gs_type, a.sh_degree, self.dev)
@@ -314,6 +369,10 @@ class Training:
         path = os.path.join(self.args.model_path, "point_cloud", f"iteration_{it}", "point_cloud.ply")
         if self.args.gs_type == "gs_mesh":
             io_ply.save_mesh_model(path, self.model)
+        elif self.args.gs_type == "gs_multi_mesh":
+            io_ply.save_multi_mesh_model(path, self.model)
+        elif self.args.gs_type == "gs_flame":
+            io_ply.save_flame_model(path, self.model, point_cloud=self.driver.to_point_cloud())
         else:
             self.model.save(path)
 
@@ -339,7 +398,7 @@ class Training:
         events = [torch.cuda.Event() for _ in range(self.LOSS_SLOTS)]
         self._pending, self._ema = collections.deque(), 0.0
         self._progress = _Progress(self.first_iter, a.iterations, a.quiet)
-        mesh = a.gs_type == "gs_mesh"
+        mesh = a.gs_type in MESH_TYPES
         for it in range(self.first_iter + 1, a.iterations + 1):
             ev = iteration_events(it, a)
             self.events.append((it, ev))

@@ -6,6 +6,9 @@ Restates the reference's scene loading (no reference code is imported):
     and the sparse-model readers                                         scene/colmap_loader.py
   * gs_mesh scenes: readNerfSyntheticMeshInfo                            games/mesh_splatting/scene/dataset_readers.py:40-105
     with GaussianMeshModel.create_from_pcd                               games/mesh_splatting/scene/gaussian_mesh_model.py:49-84
+  * gs_multi_mesh scenes: readColmapMeshSceneInfo                        games/multi_mesh_splatting/scene/dataset_readers.py:38-114
+    with GaussianMultiMeshModel.create_from_pcd                          games/multi_mesh_splatting/scene/gaussian_multi_mesh_model.py:35-77
+  * gs_flame scenes: readNerfSyntheticFlameInfo                          games/flame_splatting/scene/dataset_readers.py:48-130
   * resolution: loadCam                                                  utils/camera_utils.py:19-52
   * cameras_extent: getNerfppNorm                                        scene/dataset_readers.py:45-66
   * the shuffle and the training loop's view order                       scene/__init__.py:84-86, train.py:90-92
@@ -15,9 +18,10 @@ prepared on the GPU: gms_image_composite_rgba puts Blender's RGBA over the backg
 gms_image_resize_u8 is PILtoTorch's Image.resize bit for bit.  Every view stays resident as uint8 [H,W,3] (a quarter of the
 float32 [3,H,W] the reference keeps); the trainers dequantize it per step.
 
-Unlike the reference, nothing is written into the source directory: the reference stores points3d.ply / points3D.ply there
-and reads it back; here the same float32 / byte round trip (io_ply.point_cloud_elements -> point_cloud_arrays) happens in
-memory.
+Unlike the reference, nothing is written into the source directory: the reference stores points3d.ply / points3D.ply (and
+points3d_<i>.ply for gs_multi_mesh) there and reads it back; here the same float32 / byte round trip
+(io_ply.point_cloud_elements -> point_cloud_arrays) happens in memory, and the clouds a gs_mesh, gs_multi_mesh or gs_flame
+run stores as its input ply are rebuilt from the initial parameters (mesh_input_cloud, Scene.mesh_clouds, flame_input_cloud).
 """
 from __future__ import annotations
 
@@ -434,6 +438,9 @@ class Scene:
     cameras_extent: float
     point_cloud: Optional[Tuple[np.ndarray, np.ndarray, np.ndarray]] = None    # (points, colors, normals) as fetchPly
     mesh: Optional[MeshGaussianParams] = None                                   # gs_mesh initial parameters
+    meshes: Optional[List[MeshGaussianParams]] = None                           # gs_multi_mesh: per mesh, in --meshes order
+    mesh_clouds: Optional[List[Tuple[np.ndarray, np.ndarray]]] = None           # gs_multi_mesh: per mesh, points3d_<i>.ply's cloud
+    flame: Optional["FlameInit"] = None                                         # gs_flame
     train_images: List[torch.Tensor] = field(default_factory=list)            # resident uint8 [H,W,3] (load_scene)
     test_images: List[torch.Tensor] = field(default_factory=list)
     mode: str = "RGB"                   # what the files decode to: "RGBA" (NeRF-synthetic, composited) or "RGB" (COLMAP)
@@ -501,13 +508,84 @@ def mesh_input_cloud(mesh: MeshGaussianParams, seed: int = 0) -> Tuple[np.ndarra
     return xyz.numpy(), (shs * SH_C0 + 0.5) * 255
 
 
-SUPPORTED = {"blender": ("gs", "gs_flat", "gs_mesh"), "colmap": ("gs", "gs_flat")}
+def mesh_draws(F: int, K: int, gen: torch.Generator, rs: np.random.RandomState) -> Tuple[torch.Tensor, np.ndarray]:
+    """One mesh's random initialisation in the reference readers' order: alpha = torch.rand(F, K, 3) from `gen`, then
+    shs = random((F*K, 3)) / 255 from `rs` (float64)."""
+    alpha = torch.rand(F, int(K), 3, generator=gen)
+    shs = rs.random_sample((F * int(K), 3)) / 255.0
+    return alpha, shs
+
+
+def multi_mesh_gaussians(source_path: str, meshes: List[str], num_splats: List[int], seed: int = 0):
+    """readColmapMeshSceneInfo + GaussianMultiMeshModel.create_from_pcd: mesh i is sparse/0/<meshes[i]>.obj as written (no
+    transform_vertices), its alpha and colours drawn mesh by mesh from one torch CPU generator and one RandomState, both
+    seeded `seed` (the reference's global streams after safe_state); DC = RGB2SH of SH2RGB(shs) in float32, rest 0, _scale 1,
+    opacity inverse_sigmoid(0.1).  -> (per-mesh MeshGaussianParams, per-mesh (points float32 [F*K,3], colours float64
+    [F*K,3]): the cloud storePly writes as points3d_<i>.ply, alpha @ the float32 triangles and SH2RGB(shs) * 255)."""
+    if len(meshes) != len(num_splats):
+        raise ValueError(f"gs_multi_mesh needs one --num_splats per --meshes entry; got {len(num_splats)} for {len(meshes)} meshes")
+    gen, rs = torch.Generator().manual_seed(int(seed)), np.random.RandomState(seed)
+    params, clouds = [], []
+    for name, K in zip(meshes, num_splats):
+        verts, faces = io_obj.read_obj(os.path.join(source_path, "sparse", "0", f"{name}.obj"))
+        F, P = faces.shape[0], faces.shape[0] * int(K)
+        alpha, shs = mesh_draws(F, K, gen, rs)
+        triangles = verts[faces]
+        clouds.append((torch.matmul(alpha, triangles).reshape(P, 3).numpy(), (shs * SH_C0 + 0.5) * 255))
+        fdc = ((torch.tensor(shs * SH_C0 + 0.5).float() - 0.5) / SH_C0).reshape(P, 1, 3).contiguous()
+        x = 0.1 * torch.ones(P, 1)
+        params.append(MeshGaussianParams(verts.contiguous(), faces, alpha, torch.ones(P, 1), fdc, torch.zeros(P, 15, 3),
+                                         torch.log(x / (1 - x))))
+    return params, clouds
+
+
+FLAME_K = 100       # readNerfSyntheticFlameInfo's num_pts_each_triangle
+DEFAULT_FLAME_MODEL = os.path.join("games", "flame_splatting", "FLAME", "model", "flame2023.pkl")   # FlameConfig's path
+
+
+@dataclass
+class FlameInit:
+    """What readNerfSyntheticFlameInfo draws on the host: the FLAME model file, its faces (int64 [F,3]), alpha =
+    torch.rand(F, 100, 3) and SH2RGB(shs) (float64 [F*100,3]) from generators seeded `seed` -- the draws
+    FlameGaussianModel.create(driver, faces, K=100, seed=seed) makes.  The mesh itself needs the driver
+    (flame_input_cloud)."""
+    model_path: str
+    faces: torch.Tensor
+    alpha: torch.Tensor
+    colors: np.ndarray
+    seed: int = 0
+
+
+def flame_init(model_path: str, seed: int = 0) -> FlameInit:
+    from . import flame as _flame
+    faces = torch.tensor(np.asarray(_flame.read_model_file(model_path)["f"]).astype(np.int64))
+    alpha, shs = mesh_draws(faces.shape[0], FLAME_K, torch.Generator().manual_seed(int(seed)), np.random.RandomState(seed))
+    return FlameInit(model_path, faces, alpha, shs * SH_C0 + 0.5, int(seed))
+
+
+def flame_input_cloud(model, init: FlameInit) -> Tuple[np.ndarray, np.ndarray]:
+    """readNerfSyntheticFlameInfo's points3d.ply (the `input.ply` of a gs_flame run) for the FlameGaussianModel built from
+    `init`: alpha (the raw torch.rand draws, not the softmax) @ the triangles of the mesh at the model's current parameters
+    (zero and enlargement 8.35 for a new model), colours SH2RGB(shs) * 255 (float64; save_point_cloud truncates them to
+    bytes).  -> (points float32 [F*K,3], colours float64 [F*K,3])."""
+    verts = model.refresh_vertices().detach()
+    alpha = model._alpha.detach()
+    F, K = alpha.shape[0], alpha.shape[1]
+    xyz = torch.matmul(alpha, verts[model.faces]).reshape(F * K, 3)
+    return xyz.cpu().numpy(), init.colors * 255
+
+
+SUPPORTED = {"blender": ("gs", "gs_flat", "gs_mesh", "gs_flame"), "colmap": ("gs", "gs_flat", "gs_multi_mesh")}
 
 
 def read_scene(source_path: str, gs_type: str, white_background: bool = False, eval: bool = False, resolution: int = -1,
-               images: str = "images", num_splats: int = 2, seed: int = 0, shuffle: bool = True) -> Scene:
+               images: str = "images", num_splats=2, seed: int = 0, shuffle: bool = True, meshes: Optional[List[str]] = None,
+               flame_model: str = DEFAULT_FLAME_MODEL) -> Scene:
     """Everything of load_scene but the images, on the host: cameras (CPU tensors), names, extent, point cloud or mesh
-    parameters and the view-order stream.  Image files are only opened for their size."""
+    parameters and the view-order stream.  Image files are only opened for their size.
+
+    num_splats: K of a gs_mesh scene (an int), or a list with one K per entry of `meshes` for gs_multi_mesh.  flame_model:
+    the FLAME model file of a gs_flame scene (the reference's default path, relative to the working directory)."""
     if os.path.exists(os.path.join(source_path, "sparse")):
         kind = "colmap"
     elif os.path.exists(os.path.join(source_path, "transforms_train.json")):
@@ -545,8 +623,12 @@ def read_scene(source_path: str, gs_type: str, white_background: bool = False, e
             out.append(make_camera(v.R, v.T, v.FovX, v.FovY, w, h, uid))
         return out
 
-    pcd, mesh = None, None
-    if kind == "blender":
+    pcd, mesh, multi, clouds, flame = None, None, None, None, None
+    if gs_type == "gs_multi_mesh":
+        multi, clouds = multi_mesh_gaussians(source_path, list(meshes or []), list(num_splats), seed)
+    elif gs_type == "gs_flame":
+        flame = flame_init(flame_model, seed)
+    elif kind == "blender":
         if gs_type == "gs_mesh":
             mesh = mesh_gaussians_from_obj(os.path.join(source_path, "mesh.obj"), num_splats, seed)
         elif os.path.exists(os.path.join(source_path, "points3d.ply")):
@@ -559,18 +641,19 @@ def read_scene(source_path: str, gs_type: str, white_background: bool = False, e
             pcd = io_ply.load_point_cloud(os.path.join(sparse, "points3D.ply"))
         else:
             pcd = io_ply.point_cloud_arrays(io_ply.point_cloud_elements(*read_colmap_points(sparse)))
-    return Scene(cams(train), cams(test), train, test, extent, pcd, mesh, mode="RGBA" if kind == "blender" else "RGB",
-                 white_background=bool(white_background), _rng_state=rng.getstate())
+    return Scene(cams(train), cams(test), train, test, extent, pcd, mesh, multi, clouds, flame,
+                 mode="RGBA" if kind == "blender" else "RGB", white_background=bool(white_background), _rng_state=rng.getstate())
 
 
 def load_scene(source_path: str, gs_type: str, white_background: bool = False, eval: bool = False, resolution: int = -1,
-               images: str = "images", num_splats: int = 2, seed: int = 0, shuffle: bool = True, device="cuda",
-               workers: Optional[int] = None) -> Scene:
+               images: str = "images", num_splats=2, seed: int = 0, shuffle: bool = True, device="cuda",
+               workers: Optional[int] = None, meshes: Optional[List[str]] = None, flame_model: str = DEFAULT_FLAME_MODEL) -> Scene:
     """A COLMAP (`sparse/` present) or NeRF-synthetic (`transforms_train.json`) scene as the reference's Scene(args) builds
     it for `gs_type`, with every ground-truth image prepared on `device` (uint8 [H,W,3], resident) and the cameras moved
     there.  `seed` plays safe_state's role: it seeds the shuffle / view-order stream, the random point cloud and the gs_mesh
-    initialisation.  Images are decoded on `workers` host threads (default: up to 8); the result does not depend on it."""
-    sc = read_scene(source_path, gs_type, white_background, eval, resolution, images, num_splats, seed, shuffle)
+    initialisation.  Images are decoded on `workers` host threads (default: up to 8); the result does not depend on it.
+    meshes / flame_model: as read_scene."""
+    sc = read_scene(source_path, gs_type, white_background, eval, resolution, images, num_splats, seed, shuffle, meshes, flame_model)
     if workers is None:
         workers = min(8, os.cpu_count() or 1)
     prep = GroundTruthPreparer(device)

@@ -78,15 +78,7 @@ class NativeFlame:
         """FLAME's model pickle -> the buffers exactly as FLAME.__init__ casts and reshapes them (FLAME.py:93-121): keys
         v_template, f, shapedirs, posedirs, J_regressor (dense, or a pickled scipy sparse matrix), kintree_table, weights;
         chumpy arrays are read from their pickled state."""
-        with open(path, "rb") as fh:
-            d = _ModelUnpickler(fh, encoding="latin1").load()
-        if not isinstance(d, dict):
-            raise ValueError(f"{path}: not a FLAME model file (a pickled dict)")
-        arr = {}
-        for k in ("v_template", "f", "shapedirs", "posedirs", "J_regressor", "kintree_table", "weights"):
-            if k not in d:
-                raise ValueError(f"{path}: FLAME model file has no {k!r}")
-            arr[k] = _to_array(d[k], k)
+        arr = read_model_file(path)
         f32 = lambda a: torch.tensor(np.array(a, dtype=np.float32))         # smplx.utils.to_np / to_tensor
         posedirs = np.reshape(arr["posedirs"], [-1, arr["posedirs"].shape[-1]]).T
         parents = f32(arr["kintree_table"][0]).long()
@@ -171,6 +163,21 @@ class NativeFlame:
         """The forward into model.vertices (zeroing model.vertices.grad) and the backward from model.vertices.grad into the
         six FLAME tensors' .grad, with the argument blocks built once (FlameTrainer's sync-free path)."""
         return BoundFlame(self, model)
+
+
+def read_model_file(path: str) -> dict:
+    """FLAME's model pickle on the host: {v_template, f, shapedirs, posedirs, J_regressor, kintree_table, weights} as numpy
+    arrays (chumpy arrays from their pickled state, a scipy sparse J_regressor densified)."""
+    with open(path, "rb") as fh:
+        d = _ModelUnpickler(fh, encoding="latin1").load()
+    if not isinstance(d, dict):
+        raise ValueError(f"{path}: not a FLAME model file (a pickled dict)")
+    arr = {}
+    for k in ("v_template", "f", "shapedirs", "posedirs", "J_regressor", "kintree_table", "weights"):
+        if k not in d:
+            raise ValueError(f"{path}: FLAME model file has no {k!r}")
+        arr[k] = _to_array(d[k], k)
+    return arr
 
 
 class BoundFlame:

@@ -659,7 +659,11 @@ class FlameTrainer:
         self._renderer = None
         self._lbs = None
 
-    def step(self, cam: Camera, gt: torch.Tensor) -> torch.Tensor:
+    def step(self, cam: Camera, gt: torch.Tensor, bg: Optional[torch.Tensor] = None, before_update=None) -> torch.Tensor:
+        """One iteration.  bg: this step's background instead of the trainer's (train.py's --random_background).
+        before_update: called after the frame and the driver's backward, before any parameter changes (train.py's
+        training_report and Scene.save see the parameters before the iteration's Adam step); the step then does not fuse the
+        SH Adam update into the frame."""
         it = self.iteration + 1
         m = self.model
         if it % 1000 == 0:
@@ -677,20 +681,35 @@ class FlameTrainer:
         if self.frame is None:
             self.frame = NativeFrame(m, cam.image_width, cam.image_height, self.opt.lambda_dssim, sync_free=self.sync_free)
         take_step = it < self.opt.iterations         # train.py steps the optimizer on every iteration but the last
-        sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and take_step else None
-        loss = self.frame.run(cam, gt, self.bg, sh_adam=sh_adam)
+        fused = self.fused_sh and take_step and before_update is None
+        sh_adam = self.adam.begin_fused_sh_step() if fused else None
+        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, sh_adam=sh_adam)
         if native:
             self._lbs.backward()                 # writes the FLAME tensors' flat .grad views
         else:
             torch.autograd.backward(verts, m.vertices.grad)      # accumulates into the FLAME tensors' flat .grad views
+        if before_update is not None:
+            before_update()
         if not take_step:
             self.adam.zero_grad()
-        elif self.fused_sh:
+        elif fused:
             self.adam.step_rest()
+        elif self.fused_sh:
+            self.adam.step_dense()
         else:
             self.adam.step()
         self.iteration = it
         return loss
+
+    def state_dict(self) -> dict:
+        """What resuming needs: FlatAdam's flat parameters (the FLAME tensors among them), moments and step counts, the active
+        SH degree and the iteration.  Copies on the device."""
+        return {"adam": self.adam.state_dict(), "active_sh_degree": int(self.model.active_sh_degree), "iteration": int(self.iteration)}
+
+    def load_state_dict(self, state: dict) -> None:
+        self.adam.load_state_dict(state["adam"])
+        self.model.active_sh_degree = int(state["active_sh_degree"])
+        self.iteration = int(state["iteration"])
 
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model (at its current pose) on held-out views (NativeRenderer.evaluate)."""
