@@ -28,6 +28,7 @@
 #include "gms_knn.cuh"
 #include "gms_flame.cuh"
 #include "gms_lpips.cuh"
+#include "gms_alpha.cuh"
 
 // ------------------------------------------------------------------------------------------ host state
 static thread_local char g_err[512] = "";
@@ -1539,6 +1540,176 @@ int gms_knn_dist2(const gms_knn_args* a, void* cuda_stream) {
     if ((rc = launch("knn_gather", -1, 0, st, (P + 255) / 256, 256, 0, k_knn_gather, P, a->points, L.idx_s, L.sorted))) return rc;
     if ((rc = launch("knn_box_bounds", -1, 0, st, (nbox + 7) / 8, 256, 0, k_knn_box_bounds, P, nbox, L.sorted, L.blo, L.bhi))) return rc;
     if ((rc = launch("knn_search", -1, 0, st, nbox, GMS_KNN_BOX, 0, k_knn_search, P, nbox, L.sorted, L.blo, L.bhi, a->dist2))) return rc;
+    span_end(st);
+    return GMS_OK;
+}
+
+// ---- alpha shape and normals (gms_alpha.cuh)
+
+struct GridLayout {
+    GmsGridStats* part;                 // [GMS_GRID_STAT_BLOCKS] partial bounds and sums
+    GmsGrid* grid;                      // [1] origin, 1 / cell size, mean
+    uint64_t* key; uint64_t* key_s;     // [P] cell keys, unsorted / sorted
+    uint32_t* idx; uint32_t* idx_s;     // [P] point indices, unsorted / sorted
+    float4* p4;                         // [P] points in index order, w = index
+    float4* sorted;                     // [P] points in key order, w = index
+    void* cub; size_t cub_bytes;
+};
+
+static GridLayout grid_layout(char*& p, int Pn) {
+    GridLayout L;
+    L.part = carve<GmsGridStats>(p, GMS_GRID_STAT_BLOCKS);
+    L.grid = carve<GmsGrid>(p, 1);
+    L.key = carve<uint64_t>(p, Pn); L.key_s = carve<uint64_t>(p, Pn);
+    L.idx = carve<uint32_t>(p, Pn); L.idx_s = carve<uint32_t>(p, Pn);
+    L.p4 = carve<float4>(p, Pn); L.sorted = carve<float4>(p, Pn);
+    L.cub_bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, L.cub_bytes, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr,
+                                    Pn, 0, 3 * GMS_GRID_BITS);
+    return L;
+}
+
+// bounds, mean, cell keys and the key-sorted points; the cub temp storage is L.cub
+static int grid_build(const GridLayout& L, int P, const float* pts, double hmin, cudaStream_t st) {
+    int rc;
+    if ((rc = launch("grid_stats", -1, 0, st, GMS_GRID_STAT_BLOCKS, 256, 0, k_grid_stats, P, pts, L.part))) return rc;
+    if ((rc = launch("grid_fold", -1, 0, st, 1, 256, 0, k_grid_fold, P, L.part, hmin, L.grid))) return rc;
+    if ((rc = launch("grid_keys", -1, 0, st, (P + 255) / 256, 256, 0, k_grid_keys, P, pts, L.grid, L.key, L.idx, L.p4))) return rc;
+    size_t tb = L.cub_bytes;
+    GMS_CUDA(cub::DeviceRadixSort::SortPairs(L.cub, tb, L.key, L.key_s, L.idx, L.idx_s, P, 0, 3 * GMS_GRID_BITS, st));
+    return launch("grid_gather", -1, 0, st, (P + 255) / 256, 256, 0, k_grid_gather, P, L.p4, L.idx_s, L.sorted);
+}
+
+struct AlphaLayout {
+    GridLayout g;
+    int32_t* alive;                     // [P] 0 for a duplicate of a lower index
+    int64_t* n_all; int64_t* off_all;   // [P+1] 3-alpha list lengths / offsets
+    int64_t* n_up; int64_t* off_up;     // [P+1] 2-alpha higher-index list lengths / offsets
+    int64_t* fcount; int64_t* foff;     // [P+1] faces per lowest vertex / offsets
+    int32_t* ref; int32_t* voff;        // [P+1] referenced flags / vertex rows
+    size_t total;
+};
+
+static AlphaLayout alpha_layout(void* base, int P) {
+    AlphaLayout L;
+    char* p = reinterpret_cast<char*>(base);
+    const int Pn = P > 0 ? P : 1;
+    L.alive = carve<int32_t>(p, Pn);
+    L.n_all = carve<int64_t>(p, Pn + 1); L.off_all = carve<int64_t>(p, Pn + 1);
+    L.n_up = carve<int64_t>(p, Pn + 1); L.off_up = carve<int64_t>(p, Pn + 1);
+    L.fcount = carve<int64_t>(p, Pn + 1); L.foff = carve<int64_t>(p, Pn + 1);
+    L.ref = carve<int32_t>(p, Pn + 1); L.voff = carve<int32_t>(p, Pn + 1);
+    L.g = grid_layout(p, Pn);
+    size_t scan64 = 0, scan32 = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, scan64, (int64_t*)nullptr, (int64_t*)nullptr, Pn + 1);
+    cub::DeviceScan::ExclusiveSum(nullptr, scan32, (int32_t*)nullptr, (int32_t*)nullptr, Pn + 1);
+    L.g.cub_bytes = std::max(L.g.cub_bytes, std::max(scan64, scan32));
+    L.g.cub = p;
+    p += align_up(L.g.cub_bytes);
+    L.total = (size_t)(p - reinterpret_cast<char*>(base));
+    return L;
+}
+
+int gms_alpha_shape(const gms_alpha_shape_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !alloc || !a->n_faces || !a->n_vertices || a->P < 0 || a->P == INT32_MAX || !(a->alpha > 0.0) || !isfinite(a->alpha) ||
+        (a->P > 0 && !a->points))
+        return set_err(GMS_E_ARG, "gms_alpha_shape: need non-null arguments, 0 <= P < INT32_MAX and a finite alpha > 0%s%s");
+    *a->n_faces = 0; *a->n_vertices = 0;
+    if (a->P == 0) return GMS_OK;
+    const int P = a->P, nb = (P + 255) / 256;
+    const double alpha = a->alpha, alpha2 = alpha * alpha;
+    void* sbase = alloc(alloc_user, GMS_ALPHA_BUF_SCRATCH, alpha_layout(nullptr, P).total + 256);
+    if (!sbase) return set_err(GMS_E_ALLOC, "gms_alpha_shape: scratch allocation failed%s%s");
+    AlphaLayout L = alpha_layout(aligned_base(sbase), P);
+    int rc;
+    span_begin(K_MISC, st);
+    if ((rc = grid_build(L.g, P, a->points, 3.0 * alpha * (1.0 + 1e-6), st))) return rc;
+    if ((rc = launch("alpha_dedup", -1, 0, st, nb, 256, 0, k_alpha_dedup, P, L.g.key_s, L.g.sorted, L.alive))) return rc;
+    const double r_all2 = 9.0 * alpha2 * (1.0 + 1e-9), r_up2 = 4.0 * alpha2 * (1.0 + 1e-9);
+    GMS_CUDA(cudaMemsetAsync(L.n_all + P, 0, sizeof(int64_t), st));
+    GMS_CUDA(cudaMemsetAsync(L.n_up + P, 0, sizeof(int64_t), st));
+    if ((rc = launch("alpha_lists_count", -1, 0, st, nb, 256, 0, k_alpha_lists<true>, P, L.g.key_s, L.g.sorted, L.alive, r_all2, r_up2,
+                     L.n_all, L.n_up, (const int64_t*)nullptr, (const int64_t*)nullptr, (int32_t*)nullptr, (int32_t*)nullptr))) return rc;
+    size_t tb = L.g.cub_bytes;
+    GMS_CUDA(cub::DeviceScan::ExclusiveSum(L.g.cub, tb, L.n_all, L.off_all, P + 1, st));
+    tb = L.g.cub_bytes;
+    GMS_CUDA(cub::DeviceScan::ExclusiveSum(L.g.cub, tb, L.n_up, L.off_up, P + 1, st));
+    int64_t tot[2];
+    GMS_CUDA(cudaMemcpyAsync(&tot[0], L.off_all + P, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    GMS_CUDA(cudaMemcpyAsync(&tot[1], L.off_up + P, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    GMS_CUDA(cudaStreamSynchronize(st));                // host synchronisation 1: the list lengths
+    if (tot[1] >= INT32_MAX) return set_err(GMS_E_ARG, "gms_alpha_shape: the 2-alpha neighbour lists exceed 2^31 entries%s%s");
+    const size_t n_all = (size_t)std::max<int64_t>(tot[0], 1), n_up = (size_t)std::max<int64_t>(tot[1], 1);
+    size_t seg_bytes = 0;
+    cub::DeviceSegmentedSort::SortKeys(nullptr, seg_bytes, (const int32_t*)nullptr, (int32_t*)nullptr, (int)n_up, P, L.off_up, L.off_up + 1);
+    const size_t lists_bytes = align_up(n_all * 4) + 2 * align_up(n_up * 4) + align_up(seg_bytes) + 256;
+    void* lbase = alloc(alloc_user, GMS_ALPHA_BUF_LISTS, lists_bytes);
+    if (!lbase) return set_err(GMS_E_ALLOC, "gms_alpha_shape: neighbour list allocation failed%s%s");
+    char* lp = reinterpret_cast<char*>(aligned_base(lbase));
+    int32_t* all = carve<int32_t>(lp, n_all);
+    int32_t* up = carve<int32_t>(lp, n_up);
+    int32_t* up_s = carve<int32_t>(lp, n_up);
+    void* seg_tmp = lp;
+    if ((rc = launch("alpha_lists_fill", -1, 0, st, nb, 256, 0, k_alpha_lists<false>, P, L.g.key_s, L.g.sorted, L.alive, r_all2, r_up2,
+                     (int64_t*)nullptr, (int64_t*)nullptr, (const int64_t*)L.off_all, (const int64_t*)L.off_up, all, up))) return rc;
+    if (tot[1] > 0) GMS_CUDA(cub::DeviceSegmentedSort::SortKeys(seg_tmp, seg_bytes, (const int32_t*)up, up_s, (int)tot[1], P, L.off_up,
+                                                                L.off_up + 1, st));
+    GMS_CUDA(cudaMemsetAsync(L.ref, 0, sizeof(int32_t) * (P + 1), st));
+    GMS_CUDA(cudaMemsetAsync(L.fcount + P, 0, sizeof(int64_t), st));
+    const int fb = (P + GMS_ALPHA_WARPS - 1) / GMS_ALPHA_WARPS;
+    if ((rc = launch("alpha_faces_count", -1, 0, st, fb, GMS_ALPHA_WARPS * 32, 0, k_alpha_faces<true>, P, (const float4*)L.g.p4,
+                     (const int64_t*)L.off_all, (const int32_t*)all, (const int64_t*)L.off_up, (const int32_t*)up_s, alpha2, L.fcount, L.ref,
+                     (const int64_t*)nullptr, (const int32_t*)nullptr, (int64_t*)nullptr))) return rc;
+    tb = L.g.cub_bytes;
+    GMS_CUDA(cub::DeviceScan::ExclusiveSum(L.g.cub, tb, L.fcount, L.foff, P + 1, st));
+    tb = L.g.cub_bytes;
+    GMS_CUDA(cub::DeviceScan::ExclusiveSum(L.g.cub, tb, L.ref, L.voff, P + 1, st));
+    int64_t F = 0;
+    int32_t V = 0;
+    GMS_CUDA(cudaMemcpyAsync(&F, L.foff + P, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    GMS_CUDA(cudaMemcpyAsync(&V, L.voff + P, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    GMS_CUDA(cudaStreamSynchronize(st));                // host synchronisation 2: the output sizes
+    *a->n_faces = F; *a->n_vertices = V;
+    if (F > 0) {
+        int64_t* faces = reinterpret_cast<int64_t*>(alloc(alloc_user, GMS_ALPHA_BUF_FACES, sizeof(int64_t) * 3 * (size_t)F));
+        int64_t* index = reinterpret_cast<int64_t*>(alloc(alloc_user, GMS_ALPHA_BUF_INDEX, sizeof(int64_t) * (size_t)V));
+        if (!faces || !index) return set_err(GMS_E_ALLOC, "gms_alpha_shape: output allocation failed%s%s");
+        if ((rc = launch("alpha_faces_emit", -1, 0, st, fb, GMS_ALPHA_WARPS * 32, 0, k_alpha_faces<false>, P, (const float4*)L.g.p4,
+                         (const int64_t*)L.off_all, (const int32_t*)all, (const int64_t*)L.off_up, (const int32_t*)up_s, alpha2,
+                         (int64_t*)nullptr, (int32_t*)nullptr, (const int64_t*)L.foff, (const int32_t*)L.voff, faces))) return rc;
+        if ((rc = launch("alpha_index", -1, 0, st, nb, 256, 0, k_alpha_index, P, (const int32_t*)L.ref, (const int32_t*)L.voff, index))) return rc;
+    }
+    span_end(st);
+    return GMS_OK;
+}
+
+static size_t normals_layout(void* base, int P, GridLayout* out) {
+    char* p = reinterpret_cast<char*>(base);
+    GridLayout L = grid_layout(p, P > 0 ? P : 1);
+    L.cub = p;
+    p += align_up(L.cub_bytes);
+    if (out) *out = L;
+    return (size_t)(p - reinterpret_cast<char*>(base));
+}
+
+size_t gms_normals_scratch_bytes(int32_t P) { return normals_layout(nullptr, P, nullptr) + 512; }
+
+int gms_estimate_normals(const gms_normals_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || a->P < 0 || !(a->radius > 0.0) || !isfinite(a->radius) || a->max_nn < 1 || a->max_nn > GMS_NORMALS_MAX_NN)
+        return set_err(GMS_E_ARG, "gms_estimate_normals: need P >= 0, a finite radius > 0 and 1 <= max_nn <= GMS_NORMALS_MAX_NN%s%s");
+    if (a->P == 0) return GMS_OK;
+    if (!a->points || !a->normals || !a->scratch) return set_err(GMS_E_ARG, "gms_estimate_normals: null argument%s%s");
+    if (a->scratch_bytes < gms_normals_scratch_bytes(a->P)) return set_err(GMS_E_ARG, "gms_estimate_normals: scratch too small%s%s");
+    const int P = a->P;
+    GridLayout L;
+    normals_layout(aligned_base(a->scratch), P, &L);
+    int rc;
+    span_begin(K_MISC, st);
+    if ((rc = grid_build(L, P, a->points, a->radius * (1.0 + 1e-6), st))) return rc;
+    if ((rc = launch("normals", -1, 0, st, (P + 127) / 128, 128, 0, k_normals, P, (const uint64_t*)L.key_s, (const float4*)L.sorted,
+                     (const float4*)L.p4, (const GmsGrid*)L.grid, a->radius * a->radius, (int)a->max_nn, a->normals))) return rc;
     span_end(st);
     return GMS_OK;
 }

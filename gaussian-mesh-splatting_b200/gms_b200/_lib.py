@@ -273,6 +273,23 @@ class KnnArgs(C.Structure):
     _fields_ = [("P", C.c_int32), ("points", C.c_void_p), ("dist2", C.c_void_p), ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t)]
 
 
+ALPHA_BUF_SCRATCH, ALPHA_BUF_LISTS, ALPHA_BUF_FACES, ALPHA_BUF_INDEX = 0, 1, 2, 3     # GMS_ALPHA_BUF_*: gms_alpha_shape's allocations
+ALPHA_LIST_CAP = 256        # GMS_ALPHA_LIST_CAP: 3-alpha list entries staged in shared memory per point
+NORMALS_MAX_NN = 64         # GMS_NORMALS_MAX_NN
+
+
+class AlphaShapeArgs(C.Structure):
+    """struct gms_alpha_shape_args"""
+    _fields_ = [("P", C.c_int32), ("points", C.c_void_p), ("alpha", C.c_double), ("n_faces", C.POINTER(C.c_int64)),
+                ("n_vertices", C.POINTER(C.c_int64))]
+
+
+class NormalsArgs(C.Structure):
+    """struct gms_normals_args"""
+    _fields_ = [("P", C.c_int32), ("points", C.c_void_p), ("radius", C.c_double), ("max_nn", C.c_int32), ("normals", C.c_void_p),
+                ("scratch", C.c_void_p), ("scratch_bytes", C.c_size_t)]
+
+
 FLAME_JOINTS = 5    # GMS_FLAME_JOINTS
 
 
@@ -302,7 +319,7 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_densify_plan", "gms_densify_apply", "gms_knn_scratch_bytes", "gms_knn_dist2",
                "gms_flame_render_workspace_bytes", "gms_flame_render_frame", "gms_image_composite_rgba", "gms_image_resize_u8",
                "gms_flame_lbs_workspace_bytes", "gms_flame_lbs_forward", "gms_flame_lbs_backward", "gms_lpips_scratch_bytes",
-               "gms_lpips_vgg"]
+               "gms_lpips_vgg", "gms_alpha_shape", "gms_normals_scratch_bytes", "gms_estimate_normals"]
 
 _lib = None
 
@@ -389,6 +406,10 @@ def lib():
     L.gms_lpips_scratch_bytes.restype = C.c_size_t
     L.gms_lpips_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
     L.gms_lpips_vgg.argtypes = [C.POINTER(LpipsArgs), C.c_void_p]
+    L.gms_alpha_shape.argtypes = [C.POINTER(AlphaShapeArgs), ALLOC_FN, C.c_void_p, C.c_void_p]
+    L.gms_normals_scratch_bytes.restype = C.c_size_t
+    L.gms_normals_scratch_bytes.argtypes = [C.c_int32]
+    L.gms_estimate_normals.argtypes = [C.POINTER(NormalsArgs), C.c_void_p]
     _lib = L
     # GMS_OPTIONS="key=value,key=value": tuning knobs applied at load (A/B runs of whole test suites / benches)
     for kv in filter(None, os.environ.get("GMS_OPTIONS", "").split(",")):

@@ -13,6 +13,7 @@ and the reference's scripts/ for trained models (gs_multi_mesh and gs_flame rend
     python -m gms_b200.cli.render_multi_mesh           -m <output>                       scripts/render_multi_mesh.py
     python -m gms_b200.cli.render_from_mesh_to_mesh    -m <output> --target_mesh <obj>   scripts/render_from_mesh_to_mesh.py
     python -m gms_b200.cli.save_pseudomesh             --model_path <output>             scripts/save_pseudomesh.py
+    python -m gms_b200.cli.create_dummy_mesh           --pseudomesh_path <triangles.pt>  scripts/create_dummy_mesh.py
     python -m gms_b200.cli.edit_pseudomesh             --triangle_soup_path ... --save_dir ...
                                                                           scripts/edit_pseudomesh_based_on_estimated_mesh.py
 

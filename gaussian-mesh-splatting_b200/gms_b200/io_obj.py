@@ -2,7 +2,8 @@
 Soup and modifications"): the driving mesh read in, its edited pose read back, and edited pseudo-meshes written out.
 
     read_obj(path)  -> vertices float32 [V,3], faces int64 [F,3]   (`v` and `f` records only)
-    write_obj(path, vertices, faces)                              (scripts/save_pseudomesh.py:52-59, write_simple_obj)
+    write_obj(path, vertices, faces[, normals])                   (scripts/save_pseudomesh.py:52-59, write_simple_obj;
+                                                                   with normals, the dummy mesh of cli.create_dummy_mesh)
 """
 from __future__ import annotations
 
@@ -43,15 +44,26 @@ def read_obj(path: str):
     return v, f
 
 
-def write_obj(path: str, vertices, faces) -> None:
-    """write_simple_obj's format: `v %f %f %f` per vertex, then `f %d %d %d` per face, 1-based."""
+def write_obj(path: str, vertices, faces, normals=None) -> None:
+    """write_simple_obj's format: `v %f %f %f` per vertex, then `f %d %d %d` per face, 1-based.  With per-vertex normals
+    [V,3]: `v %f %f %f`, then `vn %f %f %f` per vertex, then `f a//a b//b c//c` per face."""
     v = vertices.detach().cpu().numpy() if torch.is_tensor(vertices) else np.asarray(vertices)
     f = faces.detach().cpu().numpy() if torch.is_tensor(faces) else np.asarray(faces)
+    if normals is not None:
+        n = normals.detach().cpu().numpy() if torch.is_tensor(normals) else np.asarray(normals)
+        if n.reshape(-1, 3).shape[0] != v.reshape(-1, 3).shape[0]:
+            raise ValueError(f"write_obj: {n.reshape(-1, 3).shape[0]} normals for {v.reshape(-1, 3).shape[0]} vertices")
     with open(path, "w") as fp:
         for x in v.reshape(-1, 3):
             fp.write("v %f %f %f\n" % (x[0], x[1], x[2]))
+        if normals is None:
+            for t in f.reshape(-1, 3).astype(np.int64) + 1:
+                fp.write("f %d %d %d\n" % (t[0], t[1], t[2]))
+            return
+        for x in n.reshape(-1, 3):
+            fp.write("vn %f %f %f\n" % (x[0], x[1], x[2]))
         for t in f.reshape(-1, 3).astype(np.int64) + 1:
-            fp.write("f %d %d %d\n" % (t[0], t[1], t[2]))
+            fp.write("f %d//%d %d//%d %d//%d\n" % (t[0], t[0], t[1], t[1], t[2], t[2]))
 
 
 def triangle_soup(triangles: torch.Tensor):

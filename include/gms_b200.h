@@ -663,6 +663,56 @@ typedef struct gms_knn_args {
 size_t gms_knn_scratch_bytes(int32_t P);
 int gms_knn_dist2(const gms_knn_args* a, void* cuda_stream);
 
+/* ---- the editing mesh of a pseudo-mesh (scripts/create_dummy_mesh.py) ----------------------------- */
+
+/* open3d's CreateFromPointCloudAlphaShape for finite float32 points [P,3], every geometric quantity in float64 (DESIGN.md 4.11).
+ *   Exact duplicates: a point equal to a point of lower index takes no part (the written positions are the same either way).
+ *   Triangle (a < b < c) is output iff it is a face of the Delaunay tetrahedralization of the remaining points and exactly
+ *   one of its (one or two) incident tetrahedra has circumradius <= alpha.  For points in general position this is open3d's
+ *   triangle set.  Tie rule under degeneracy: with w = (b-a) x (c-a), circumcentre c_f and tau_p = (|p-c_f|^2 - r_f^2) /
+ *   (2 w.(p-c_f)), T+ = min tau over w.(p-c_f) > 0 and T- = max over < 0, the face is Delaunay iff T- < T+ strictly and no
+ *   point with w.(p-c_f) == 0 lies strictly inside the circumcircle; a side is kept iff r_f^2 + |w|^2 tau^2 <= alpha^2.
+ *   Collinear triples are never output.  This need not match Qhull's choice for cospherical or coplanar points.
+ *   Order: vertices are the referenced points in ascending original index (index[V], int64); faces[F,3] (int64, rows of the
+ *   vertex list) have ascending vertex indices and are in lexicographic order.
+ * The call sizes its memory through alloc(user, which, bytes) with which = GMS_ALPHA_BUF_*: SCRATCH (P-sized), LISTS (the
+ * neighbour lists, known after the first of two host synchronisations), FACES ([F,3] int64) and INDEX ([V] int64), the last
+ * two after the second and only when non-empty.  The caller owns what it returned and reads faces / index from it.
+ * GMS_E_ARG before any launch: a null pointer, P < 0, P = INT32_MAX, alpha <= 0 or not finite; after the first
+ * synchronisation when the 2-alpha lists hold 2^31 entries or more.  GMS_E_ALLOC when alloc returns NULL.  P = 0 gives
+ * F = V = 0 without a launch.  Runs on the caller's stream and returns after the last launch is enqueued. */
+#define GMS_ALPHA_BUF_SCRATCH 0
+#define GMS_ALPHA_BUF_LISTS 1
+#define GMS_ALPHA_BUF_FACES 2
+#define GMS_ALPHA_BUF_INDEX 3
+#define GMS_ALPHA_LIST_CAP 256     /* 3-alpha list entries staged in shared memory per point; longer lists are read from global */
+typedef struct gms_alpha_shape_args {
+    int32_t P;
+    const float* points;        /* [P,3] device, every coordinate finite (not checked here) */
+    double alpha;
+    int64_t* n_faces;           /* out, host: F */
+    int64_t* n_vertices;        /* out, host: V */
+} gms_alpha_shape_args;
+int gms_alpha_shape(const gms_alpha_shape_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
+
+/* open3d's EstimateNormals(KDTreeSearchParamHybrid(radius, max_nn)) with a stated sign.  For every point: the min(max_nn, k)
+ * nearest points by (float64 squared distance, index) with distance <= radius, the point itself and its duplicates
+ * included; the unit eigenvector of the smallest eigenvalue of their mean-centred float64 covariance (cyclic Jacobi), or
+ * (0,0,1) when k < 3.  Sign: n.(x - mean of all P points) >= 0; when that is exactly 0 the largest-magnitude component (the
+ * first of equals) is positive.  GMS_E_ARG before any launch: a null pointer, P < 0, radius <= 0 or not finite,
+ * max_nn outside 1..GMS_NORMALS_MAX_NN, too little scratch.  P = 0 is a no-op.  Caller's stream, no host synchronisation. */
+#define GMS_NORMALS_MAX_NN 64
+typedef struct gms_normals_args {
+    int32_t P;
+    const float* points;                   /* [P,3] device, finite */
+    double radius;
+    int32_t max_nn;
+    float* normals;                        /* out [P,3] */
+    void* scratch; size_t scratch_bytes;   /* gms_normals_scratch_bytes(P) */
+} gms_normals_args;
+size_t gms_normals_scratch_bytes(int32_t P);
+int gms_estimate_normals(const gms_normals_args* a, void* cuda_stream);
+
 /* ---- FLAME's vertex model (gs_flame) ----------------------------------------------------------- */
 
 /* FLAME.forward's vertices (games/flame_splatting/FLAME/FLAME.py:204-248 with smplx.lbs.lbs, landmarks left out) followed by
