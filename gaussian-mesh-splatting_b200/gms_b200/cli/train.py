@@ -17,6 +17,15 @@ The report and the save run inside the trainer's `before_update` callback, so th
 as the reference's do.  The loop itself never synchronises with the host: the loss reaches the progress display's moving
 average through pinned host slots and CUDA events that are polled, not waited on.
 
+TensorBoard, as prepare_output_and_logger / training_report (train.py:174-223): when torch.utils.tensorboard imports, a
+SummaryWriter(model_path) gets every iteration's train_loss_patches/l1_loss, train_loss_patches/total_loss and iter_time
+(ms), and at each --test_iterations entry the first five renders of each split (and their ground truth at the first listed
+test iteration), the split's loss_viewpoint - l1_loss / - psnr, scene/opacity_histogram and total_points; else it prints
+"Tensorboard not available: not logging progress".  The three per-iteration values travel through the same pinned slots
+(loss and L1, elements 0 and 1 of the frame's loss vector) with a pair of timing events per slot, and are written, as ONE
+event per iteration, once the slot's events have completed.  TensorBoard's writer spends its host time per event (a
+protobuf, a checksum in Python, a file append), so one event for the three values costs a third of three add_scalar calls.
+
 Deliberate differences:
   * chkpnt<N>.pth holds (state, N) with the library's own state (the trainer's state_dict(), the view-order stream and the
     background generator), not the reference's capture() tuple; a resumed run continues the uninterrupted run's sequence of
@@ -27,6 +36,11 @@ Deliberate differences:
     which the reference crashes, and gs_flame without its model file.
   * flame_params.pt carries the FLAME buffers as NativeFlame.to_point_cloud()'s dict, not the reference's pickled
     FLAMEPointCloud: cli.render and cli.render_flame rebuild the model from the checkpoint alone.
+  * TensorBoard: the per-iteration scalars are written when their slot is consumed, as one event per iteration holding
+    all three (the reference writes one event per tag), so the order of events across tags in the file differs from the
+    reference's (per tag, steps increase as there).  iter_time brackets the frame's launches, which on one GPU include
+    the SH Adam step the frame fuses into the preprocess backward (and for gs_flame the FLAME forward and backward); the
+    reference's window holds render, loss and backward only.  The writer is closed when run() returns or raises.
   * Not built, refused by name: --antialiasing, --debug, --debug_from, --detect_anomaly,
     --convert_SHs_python, --compute_cov3D_python, --save_xyz, --data_device other than cuda.  --ip / --port are accepted and
     ignored (the reference does not start its viewer either)."""
@@ -238,6 +252,34 @@ def write_input_ply(path: str, scene: dataset.Scene, source_path: str, gs_type: 
     io_ply.save_point_cloud(path, points, np.round(colors * 255.0))      # colors are bytes / 255: the round trip is exact
 
 
+def open_summary_writer(model_path: str, log):
+    """prepare_output_and_logger's writer: SummaryWriter(model_path) when torch.utils.tensorboard imports, else None after
+    the reference's message through `log`."""
+    try:
+        from torch.utils.tensorboard import SummaryWriter
+    except ImportError:
+        log("Tensorboard not available: not logging progress")
+        return None
+    return SummaryWriter(model_path)
+
+
+def add_scalars_event(writer, step: int, pairs) -> None:
+    """What add_scalar writes for each (tag, value) of `pairs` (a simple_value summary), in ONE event at `step`: one record,
+    one checksum pass and one file append in TensorBoard's writer instead of one per tag."""
+    from tensorboard.compat.proto.summary_pb2 import Summary
+    writer.file_writer.add_summary(Summary(value=[Summary.Value(tag=t, simple_value=float(v)) for t, v in pairs]), step)
+
+
+def report_configs(scene: dataset.Scene):
+    """training_report's validation configs: (name, cameras, resident images, image names) of the test views and of train
+    views 5, 10, ..., 25 taken mod n."""
+    n = len(scene.train_cameras)
+    idx = [i % n for i in range(5, 30, 5)]
+    names = scene.train_names
+    return (("test", scene.test_cameras, scene.test_images, scene.test_names),
+            ("train", [scene.train_cameras[i] for i in idx], [scene.train_images[i] for i in idx], [names[i] for i in idx]))
+
+
 def _mesh_params(p: MeshGaussianParams, sh_degree: int) -> MeshGaussianParams:
     """create_from_pcd's features for max_sh_degree `sh_degree` (the loader builds degree 3: the rest is zero anyway)."""
     M = (int(sh_degree) + 1) ** 2
@@ -266,9 +308,10 @@ class _Progress:
 
 
 class Training:
-    """One train.py run: prepare() builds the output directory, scene, model and trainer (and restores --start_checkpoint);
-    run() iterates.  Attributes the tests read: trainer, model, scene, order (ViewOrder), ema (per consumed iteration:
-    (iteration, loss, moving average)), reports ((iteration, split, L1, PSNR)), events (per iteration: iteration_events)."""
+    """One train.py run: prepare() builds the output directory, the TensorBoard writer, scene, model and trainer (and
+    restores --start_checkpoint); run() iterates.  Attributes the tests read: trainer, model, scene, order (ViewOrder), ema
+    (per consumed iteration: (iteration, loss, moving average)), reports ((iteration, split, L1, PSNR)), events (per
+    iteration: iteration_events), tb_writer (None without TensorBoard; closed once run() ends)."""
 
     LOSS_SLOTS = 64
 
@@ -278,6 +321,7 @@ class Training:
         self.ema, self.reports, self.events = [], [], []
         self.first_iter = 0
         self.scene = scene
+        self.tb_writer = None
 
     def log(self, msg: str) -> None:
         if not self.args.quiet:
@@ -291,6 +335,15 @@ class Training:
         os.makedirs(a.model_path, exist_ok=True)
         with open(os.path.join(a.model_path, "cfg_args"), "w") as f:
             f.write(options.cfg_args_string(a))
+        self.tb_writer = open_summary_writer(a.model_path, self.log)
+        try:
+            return self._setup()
+        except BaseException:
+            self.close_writer()
+            raise
+
+    def _setup(self) -> "Training":
+        a = self.args
         if self.scene is None:
             self.scene = dataset.load_scene(a.source_path, a.gs_type, a.white_background, a.eval, a.resolution, a.images,
                                             a.num_splats if a.gs_type == "gs_multi_mesh" else a.num_splats[0], a.seed,
@@ -349,20 +402,47 @@ class Training:
         if self.bg_gen is not None and state["bg_generator"] is not None:
             self.bg_gen.set_state(state["bg_generator"])
 
+    def close_writer(self) -> None:
+        if self.tb_writer is not None:
+            self.tb_writer.close()
+
     # ---- what happens at an iteration besides the frame
     def report(self, it: int) -> None:
         """training_report at a test iteration: the test views and train views 5, 10, ..., 25 (mod n) with the fixed
-        background; mean L1 and mean per-channel PSNR, as the reference prints them."""
-        sc = self.scene
-        n = len(sc.train_cameras)
-        configs = (("test", sc.test_cameras, sc.test_images),
-                   ("train", [sc.train_cameras[i % n] for i in range(5, 30, 5)], [sc.train_images[i % n] for i in range(5, 30, 5)]))
-        for name, cams, gts in configs:
+        background; mean L1 and mean per-channel PSNR, as the reference prints them.  With TensorBoard, also its images,
+        split scalars, opacity histogram and point count."""
+        w = self.tb_writer
+        for name, cams, gts, names in report_configs(self.scene):
             if cams:
                 r = self.trainer.evaluate(cams, gts)
                 l1, psnr = float(r.mean[0]), float(r.mean[3])
                 self.reports.append((it, name, l1, psnr))
                 self.log(f"\n[ITER {it}] Evaluating {name}: L1 {l1} PSNR {psnr}")
+                if w is not None:
+                    self._report_images(it, name, cams[:5], gts[:5], names[:5])
+                    w.add_scalar(f"{name}/loss_viewpoint - l1_loss", l1, it)
+                    w.add_scalar(f"{name}/loss_viewpoint - psnr", psnr, it)
+        if w is not None:
+            opacity = self.model.get_opacity.detach().cpu()
+            w.add_histogram("scene/opacity_histogram", opacity, it)
+            w.add_scalar("total_points", int(opacity.shape[0]), it)
+
+    def _report_images(self, it: int, name: str, cams, gts, names) -> None:
+        """The renders (and, at the first listed test iteration, the ground truth) of up to five views as the float tensors
+        the reference hands add_images: TensorBoard's own (x * 255) truncation then gives the reference's PNGs.  The renders
+        come from the renderer evaluate() just built and sized for these views, so none can overflow its capacity."""
+        w, r = self.tb_writer, self.trainer.renderer
+        for cam, gt, image_name in zip(cams, gts, names):
+            image = torch.clamp(r.render(cam, self.trainer.bg)[0], 0.0, 1.0)
+            w.add_images(f"{name}_view_{image_name}/render", image[None].cpu(), global_step=it)
+            if it == self.args.test_iterations[0]:
+                gt_image = torch.clamp(gt.cpu().permute(2, 0, 1).float() / 255.0, 0.0, 1.0)
+                w.add_images(f"{name}_view_{image_name}/ground_truth", gt_image[None], global_step=it)
+
+    def log_iteration(self, it: int, loss: float, l1: float, ms: float) -> None:
+        """training_report's per-iteration scalars, in one event."""
+        add_scalars_event(self.tb_writer, it, (("train_loss_patches/l1_loss", l1), ("train_loss_patches/total_loss", loss),
+                                               ("iter_time", ms)))
 
     def save(self, it: int) -> None:
         self.log(f"\n[ITER {it}] Saving Gaussians")
@@ -380,25 +460,44 @@ class Training:
         self.log(f"\n[ITER {it}] Saving Checkpoint")
         torch.save((self.state_dict(), it), os.path.join(self.args.model_path, f"chkpnt{it}.pth"))
 
-    # ---- the loss, read without synchronising
+    # ---- the loss, L1 and frame time, read without synchronising
+    def _slot_events(self, i: int):
+        """The events slot i's values wait for: the loss copy's, and with TensorBoard the frame's end."""
+        return (self._loss_ready[i],) + ((self._timing[i][1],) if self._timing else ())
+
     def _consume(self, block: bool = False) -> None:
-        while self._pending and (block or self._pending[0][2].query()):
-            it, i, ev = self._pending.popleft()
-            ev.synchronize()
-            loss = float(self._slots_np[i])
+        while self._pending and (block or all(e.query() for e in self._slot_events(self._pending[0][1]))):
+            it, i = self._pending.popleft()
+            for e in self._slot_events(i):
+                e.synchronize()
+            loss = float(self._slots_np[i, 0])
             self._ema = 0.4 * loss + 0.6 * self._ema
             self.ema.append((it, loss, self._ema))
+            if self._timing:
+                self.log_iteration(it, loss, float(self._slots_np[i, 1]), self._timing[i][0].elapsed_time(self._timing[i][1]))
             if it % 10 == 0:
                 self._progress.show(self._ema)
 
     def run(self) -> "Training":
+        try:
+            self._loop()
+        finally:
+            self.close_writer()
+        self.log("\nTraining complete.")
+        return self
+
+    def _loop(self) -> None:
         a, sc, dev = self.args, self.scene, self.dev
-        slots = torch.zeros(self.LOSS_SLOTS, dtype=torch.float32).pin_memory()
+        slots = torch.zeros(self.LOSS_SLOTS, 2, dtype=torch.float32).pin_memory()     # per slot: loss, L1
         self._slots_np = slots.numpy()
-        events = [torch.cuda.Event() for _ in range(self.LOSS_SLOTS)]
+        self._loss_ready = [torch.cuda.Event() for _ in range(self.LOSS_SLOTS)]
+        # train.py's iter_start / iter_end per slot; read only once the end event has completed
+        self._timing = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+                        for _ in range(self.LOSS_SLOTS)] if self.tb_writer is not None else None
         self._pending, self._ema = collections.deque(), 0.0
         self._progress = _Progress(self.first_iter, a.iterations, a.quiet)
         mesh = a.gs_type in MESH_TYPES
+        stream = torch.cuda.current_stream(dev)
         for it in range(self.first_iter + 1, a.iterations + 1):
             ev = iteration_events(it, a)
             self.events.append((it, ev))
@@ -410,25 +509,27 @@ class Training:
             # the last iteration takes no Adam step: never let the frame fuse one in
             before = (lambda: [f(it) for f in hooks]) if hooks or "step" not in ev else None
             if len(self._pending) == self.LOSS_SLOTS:
-                self._pending[0][2].synchronize()
+                for e in self._slot_events(self._pending[0][1]):
+                    e.synchronize()
                 self._consume()
             slot = it % self.LOSS_SLOTS
+            start, end = self._timing[slot] if self._timing else (None, None)
+            if start is not None:
+                start.record(stream)
             if mesh:
                 self.trainer.optimizer_step = "step" in ev
-                self.trainer.step(sc.train_cameras[v], sc.train_images[v], loss_host=slots[slot:slot + 1], loss_ready=events[slot],
-                                  bg=bg, before_update=before)
+                self.trainer.step(sc.train_cameras[v], sc.train_images[v], loss_host=slots[slot], loss_ready=self._loss_ready[slot],
+                                  bg=bg, before_update=before, frame_end=end)
             else:
-                loss = self.trainer.step(sc.train_cameras[v], sc.train_images[v], bg=bg, before_update=before)
-                slots[slot:slot + 1].copy_(loss.reshape(1), non_blocking=True)
-                events[slot].record(torch.cuda.current_stream(dev))
-            self._pending.append((it, slot, events[slot]))
+                self.trainer.step(sc.train_cameras[v], sc.train_images[v], bg=bg, before_update=before, frame_end=end)
+                slots[slot].copy_(self.trainer.loss_vector[:2], non_blocking=True)
+                self._loss_ready[slot].record(stream)
+            self._pending.append((it, slot))
             self._consume()
             if "checkpoint" in ev:
                 self.checkpoint(it)
         self._consume(block=True)
         self._progress.close()
-        self.log("\nTraining complete.")
-        return self
 
 
 def main(argv=None) -> Training:

@@ -102,12 +102,13 @@ class NativeFrame(SyncFreeCapacity):
     def read_loss_async(self, loss_host: torch.Tensor, loss_ready: Optional[torch.cuda.Event] = None) -> None:
         """Copy the last frame's loss into pinned host memory from a side stream as soon as the LOSS kernels are done (the
         event gms_train_frame records ~40 % into the frame), not after the whole frame: a caller that waits for `loss_ready`
-        gets the value while the backward pass is still running and has that time to queue its next step."""
+        gets the value while the backward pass is still running and has that time to queue its next step.  The leading
+        loss_host.numel() values of the frame's [loss, L1, SSIM] vector are copied (1: the loss; 2: the loss and L1)."""
         if self._side is None:
             self._side = torch.cuda.Stream(self.dev)
         self._side.wait_event(self.ev_loss)
         with torch.cuda.stream(self._side):
-            loss_host.copy_(self.loss[:1].reshape(loss_host.shape), non_blocking=True)
+            loss_host.copy_(self.loss[:loss_host.numel()].reshape(loss_host.shape), non_blocking=True)
             if loss_ready is not None:
                 loss_ready.record(self._side)
             self._loss_read = torch.cuda.Event()
@@ -209,14 +210,18 @@ class MeshTrainer:
                     p.grad.mul_(1.0 / self.world)
 
     def step(self, cam: Camera, gt: torch.Tensor, loss_host: Optional[torch.Tensor] = None,
-             loss_ready: Optional[torch.cuda.Event] = None, bg: Optional[torch.Tensor] = None, before_update=None) -> torch.Tensor:
+             loss_ready: Optional[torch.cuda.Event] = None, bg: Optional[torch.Tensor] = None, before_update=None,
+             frame_end: Optional[torch.cuda.Event] = None) -> torch.Tensor:
         """One optimisation step.  If `loss_host` (pinned) / `loss_ready` are given, the loss is copied to the host from a side
         stream as soon as the loss kernels have run (native frames: NativeFrame.read_loss_async; otherwise right after the
         backward pass, before the optimizer kernels are queued): a caller that logs the loss every step gets it while the
         backward pass is still running and queues its next step in that time.  gt: float32 [3,H,W] or uint8 [H,W,3].
         bg: this step's background instead of the trainer's (train.py's --random_background).  before_update: called after
         the frame and before any parameter changes (train.py's training_report and Scene.save see the parameters before the
-        iteration's Adam step); the step then does not fuse the SH Adam update into the frame."""
+        iteration's Adam step); the step then does not fuse the SH Adam update into the frame.  frame_end: recorded on the
+        current stream right after the frame's launches (render, loss and backward, and on one GPU the SH Adam step the
+        frame fuses in), before before_update and any other optimizer work: with an event recorded just before step(), it
+        brackets train.py's iter_start / iter_end window."""
         bg = self.bg if bg is None else bg
         if self.native:
             if self._frame is None:
@@ -228,6 +233,8 @@ class MeshTrainer:
             fused = factored and self.world == 1 and before_update is None
             sh_adam = self.opt.begin_fused_sh_step() if fused else None
             loss = self._frame.run(cam, gt, bg, factored=factored and not fused, sh_adam=sh_adam)
+            if frame_end is not None:
+                frame_end.record(torch.cuda.current_stream(self._frame.dev))
             from . import rasterizer as _r
             _r.last_num_rendered = self._frame.last_num_rendered
             if loss_host is not None:
@@ -256,6 +263,8 @@ class MeshTrainer:
             loss.backward()
         finally:
             _r.DIRECT_SH_GRAD = prev       # never leak the in-place mode to other users of the rasterizer
+        if frame_end is not None:
+            frame_end.record(torch.cuda.current_stream(loss.device))
         if loss_host is not None:
             loss_host.copy_(loss.detach().reshape(loss_host.shape), non_blocking=True)
             if loss_ready is not None:
@@ -273,6 +282,12 @@ class MeshTrainer:
             for p in self.model.parameters():
                 p.grad = None
         return loss.detach()
+
+    @property
+    def renderer(self):
+        """The renderer the last evaluate() built or reused, sized for its cameras and the model's current Gaussian count
+        (None before the first): it draws those views of the current model without a second copy of the model."""
+        return self._renderer
 
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model on held-out views with the trainer's background, the test half of
@@ -488,11 +503,19 @@ class FreeTrainer:
         reset = it % o.opacity_reset_interval == 0 or (self.white_background and it == o.densify_from_iter)
         return True, densify, reset
 
-    def step(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor = None, before_update=None) -> torch.Tensor:
+    @property
+    def loss_vector(self) -> Optional[torch.Tensor]:
+        """The frame's device [3] vector [loss, L1, SSIM] of the last step (None before the first): the next step overwrites
+        it in stream order."""
+        return None if self.frame is None else self.frame.loss
+
+    def step(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor = None, before_update=None,
+             frame_end: Optional[torch.cuda.Event] = None) -> torch.Tensor:
         """One iteration.  bg: this step's background instead of the trainer's (train.py's --random_background).
         before_update: called after the frame and before densify / opacity reset / Adam (train.py's training_report and
         Scene.save see the parameters before the iteration's update); the step then does not fuse the SH Adam update into
-        the frame."""
+        the frame.  frame_end: recorded on the current stream right after the frame's launches, before before_update,
+        densification and any Adam step outside the frame (MeshTrainer.step)."""
         it = self.iteration + 1
         self.adam.groups[0]["lr"] = self._xyz_lr(it)
         if it % 1000 == 0:
@@ -506,6 +529,8 @@ class FreeTrainer:
                 self._loaded_stats = None
         sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and not densify and before_update is None else None
         loss = self.frame.run(cam, gt, self.bg if bg is None else bg, stats=stats, sh_adam=sh_adam)
+        if frame_end is not None:
+            frame_end.record(torch.cuda.current_stream(self.frame.dev))
         if before_update is not None:
             before_update()
         if densify:
@@ -591,6 +616,11 @@ class FreeTrainer:
         self.adam.m[o0:o1].zero_()
         self.adam.v[o0:o1].zero_()
 
+    @property
+    def renderer(self):
+        """The renderer the last evaluate() built or reused (MeshTrainer.renderer)."""
+        return self._renderer
+
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model on held-out views (NativeFreeRenderer.evaluate)."""
         from .render import NativeFreeRenderer, renderer_for
@@ -659,11 +689,19 @@ class FlameTrainer:
         self._renderer = None
         self._lbs = None
 
-    def step(self, cam: Camera, gt: torch.Tensor, bg: Optional[torch.Tensor] = None, before_update=None) -> torch.Tensor:
+    @property
+    def loss_vector(self) -> Optional[torch.Tensor]:
+        """The frame's device [3] vector [loss, L1, SSIM] of the last step (None before the first): the next step overwrites
+        it in stream order."""
+        return None if self.frame is None else self.frame.loss
+
+    def step(self, cam: Camera, gt: torch.Tensor, bg: Optional[torch.Tensor] = None, before_update=None,
+             frame_end: Optional[torch.cuda.Event] = None) -> torch.Tensor:
         """One iteration.  bg: this step's background instead of the trainer's (train.py's --random_background).
         before_update: called after the frame and the driver's backward, before any parameter changes (train.py's
         training_report and Scene.save see the parameters before the iteration's Adam step); the step then does not fuse the
-        SH Adam update into the frame."""
+        SH Adam update into the frame.  frame_end: recorded on the current stream right after the frame's launches and the
+        driver's backward, before before_update and any Adam step outside the frame (MeshTrainer.step)."""
         it = self.iteration + 1
         m = self.model
         if it % 1000 == 0:
@@ -688,6 +726,8 @@ class FlameTrainer:
             self._lbs.backward()                 # writes the FLAME tensors' flat .grad views
         else:
             torch.autograd.backward(verts, m.vertices.grad)      # accumulates into the FLAME tensors' flat .grad views
+        if frame_end is not None:
+            frame_end.record(torch.cuda.current_stream(self.frame.dev))
         if before_update is not None:
             before_update()
         if not take_step:
@@ -710,6 +750,11 @@ class FlameTrainer:
         self.adam.load_state_dict(state["adam"])
         self.model.active_sh_degree = int(state["active_sh_degree"])
         self.iteration = int(state["iteration"])
+
+    @property
+    def renderer(self):
+        """The renderer the last evaluate() built or reused (MeshTrainer.renderer)."""
+        return self._renderer
 
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model (at its current pose) on held-out views (NativeRenderer.evaluate)."""

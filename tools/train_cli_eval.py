@@ -8,13 +8,15 @@ from a seeded scenes.object_mesh(200_000) gs_mesh model, written as RGBA PNGs (a
 mesh as mesh.obj: 1M mesh-Gaussians at --num_splats 5.
 Measurements, `--runs` alternating runs per arm, each a host clock around `--steps` iterations ending in a device
 synchronisation (the scene is loaded once, outside the clock):
-  gs_mesh   cli.train's loop (reports and saves off) against a bare MeshTrainer.step loop over the same view order
+  gs_mesh   cli.train's loop (reports and saves off, TensorBoard hidden from the import: its cost is
+            tools/train_cli_tb_eval.py's to measure) against a bare MeshTrainer.step loop over the same view order
   gs_flat   the same with densification on (from the random 100k cloud), FreeTrainer.step as the bare loop; the number of
             densification steps inside the window is printed beside the times
   render    cli.render over the test views: views per second (PNGs written)
   metrics   cli.metrics over the rendered test views: seconds
 The card's name and power limit are printed in the same run."""
 import argparse
+import contextlib
 import json
 import os
 import subprocess
@@ -69,6 +71,21 @@ def write_scene(root, views, faces, W=1920, H=1080):
         f.write("".join("f %d %d %d\n" % tuple(t) for t in fcs + 1))
 
 
+@contextlib.contextmanager
+def tensorboard_hidden():
+    """torch.utils.tensorboard fails to import inside the block, as when TensorBoard is not installed: a Training prepared
+    there writes no event file."""
+    saved = sys.modules.get("torch.utils.tensorboard")
+    sys.modules["torch.utils.tensorboard"] = None
+    try:
+        yield
+    finally:
+        if saved is not None:
+            sys.modules["torch.utils.tensorboard"] = saved
+        else:
+            sys.modules.pop("torch.utils.tensorboard", None)
+
+
 class _NoSave(cli_train.Training):
     def save(self, it):
         pass
@@ -92,7 +109,8 @@ def bench_train(root, out, gs_type, steps, runs, extra):
     order = scene.view_order(steps)
 
     def cli():
-        t = _NoSave(cli_train.parse_args(argv), scene=scene).prepare()
+        with tensorboard_hidden():
+            t = _NoSave(cli_train.parse_args(argv), scene=scene).prepare()
         dt, _ = _timed(t.run)
         return dt, len(getattr(t.trainer, "densifications", []))
 

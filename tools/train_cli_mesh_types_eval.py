@@ -11,7 +11,8 @@ Scenes (deterministic):
           faces dropped; random shape / expression / pose bases), and `--views` NeRF-synthetic views at 1920x1080 rendered
           from the model it starts training from (K = 100: 997,600 Gaussians), the last fifth held out.
 Measurements, `--runs` alternating runs per arm, each a host clock around `--steps` iterations ending in a device
-synchronisation (the scene is loaded once, outside the clock): cli.train's loop with reports and saves off against a bare
+synchronisation (the scene is loaded once, outside the clock): cli.train's loop with reports and saves off (and TensorBoard
+hidden from the import, as in tools/train_cli_eval.py) against a bare
 MeshTrainer.step / FlameTrainer.step loop over the same view order.  The card's name and power limit are printed in the
 same run."""
 import argparse
@@ -35,6 +36,9 @@ from gms_b200.flame import NativeFlame  # noqa: E402
 from gms_b200.model import FlameGaussianModel, MultiMeshGaussianModel  # noqa: E402
 from gms_b200.render import NativeRenderer  # noqa: E402
 from gms_b200.trainer import FlameTrainer, MeshTrainer  # noqa: E402
+
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+from train_cli_eval import tensorboard_hidden  # noqa: E402
 
 W, H = 1920, 1080
 NUM_SPLATS = [2, 4, 5, 9]
@@ -160,7 +164,8 @@ def bench_train(root, out, gs_type, steps, runs, extra):
     P = None
 
     def cli():
-        t = _NoSave(cli_train.parse_args(argv), scene=scene).prepare()
+        with tensorboard_hidden():
+            t = _NoSave(cli_train.parse_args(argv), scene=scene).prepare()
         dt, _ = _timed(t.run)
         return dt, int(t.model._opacity.shape[0])
 
