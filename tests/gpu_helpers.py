@@ -6,6 +6,7 @@ import diff_gaussian_rasterization as dgr
 from gms_b200 import rasterizer
 from oracle import expansion as oexp
 from oracle import raster
+from preprocess_budget_cases import assert_preprocess_per_element
 
 
 def gpu_settings(S: raster.Settings, dev="cuda"):
@@ -229,6 +230,11 @@ def assert_backward_stages(st, g_gpu, g_ref, tol_composite=2e-5, tol_pre=5e-5):
             msg.append(f"{kg} {e:.1e}")
             assert e <= STAGE2_TOL.get(kg, tol_pre), f"preprocess backward {kg}: {e:.3e} > {STAGE2_TOL.get(kg, tol_pre)}"
     print("[parity] backward stages (max err / max|ref|): " + ", ".join(msg))
+    # stage 2 per element: every parameter gradient within its budget around the float64 reference on the GPU's own record
+    # (oracle/preprocess64.py); dL/dmeans2D is the record's mean2D, bit for bit
+    got = {k: g_gpu[k] for k in ("means3D", "means2D", "opacities", "shs", "colors_precomp", "scales", "rotations", "cov3D_precomp")
+           if k in g_gpu}
+    assert_preprocess_per_element(st, got, dg)
     return True
 
 

@@ -726,15 +726,34 @@ def _api_loop(root, argv, hooks):
     return {n: getattr(m, n).detach().clone() for n in names}
 
 
+LIBRARY_RUNS = 6
+
+
+def _near_a_library_run(got, runs, what):
+    """Per tensor: the distance from `got` to the nearest of `runs` (runs of the library loop) is at most 10x the run-to-run
+    spread + 1e-7, the spread being the largest distance from one library run to its nearest other run (max |.| per tensor).
+    One pair of runs does not measure that spread: the frames accumulate with float atomics, and in a gs_flat run with
+    densification and an opacity reset the runs fall into a few discrete outcomes -- measured on an H100, two runs of the
+    library loop at --sh_degree 1 differ in _opacity by 6e-3-9e-3 or by 5.0e-2, the latter in 5 of the 6 pairs of 4 runs."""
+    for n in got:
+        for r in runs:
+            assert got[n].shape == r[n].shape, f"{what}: {n} shapes {tuple(got[n].shape)} vs {tuple(r[n].shape)}"
+        dist = lambda a, b: float((a[n] - b[n]).abs().max())
+        d_got = min(dist(got, r) for r in runs)
+        spread = max(min(dist(r, o) for j, o in enumerate(runs) if j != i) for i, r in enumerate(runs))
+        print(f"[{what}] {n}: to the nearest library run {d_got:.3e}, run-to-run spread {spread:.3e}")
+        assert d_got <= 10 * spread + 1e-7, f"{what}: {n} {d_got:.3e} against the run-to-run spread {spread:.3e}"
+
+
 @pytest.mark.parametrize("gs_type,degree", [("gs_mesh", 0), ("gs_flat", 1)])
-def test_command_line_trains_and_renders_at_a_low_degree(cli_scene, gs_type, degree, tmp_path):
+def test_command_line_low_degree_trains_renders_and_matches_a_library_run(cli_scene, gs_type, degree, tmp_path):
     """train.py --sh_degree 0 (gs_mesh) and 1 (gs_flat): the saved point_cloud.ply holds 3((d + 1)^2 - 1) f_rest_*
     properties (0 and 9), render.py draws what the library's renderer draws of the loaded model, and the final parameters
-    stay within the run-to-run spread of the library loop."""
+    are as close to a run of the library loop as its runs are to each other (_near_a_library_run)."""
     from gms_b200 import dataset, io_ply
     from gms_b200.cli import render as cli_render
     from gms_b200.cli import train as cli_train
-    from test_gpu_cli import FLAT_ARGV, HOOKS_FLAT, HOOKS_MESH, MESH_ARGV, _expected_renders, _within_spread
+    from test_gpu_cli import FLAT_ARGV, HOOKS_FLAT, HOOKS_MESH, MESH_ARGV, _expected_renders
     M = (degree + 1) ** 2
     argv = (MESH_ARGV if gs_type == "gs_mesh" else FLAT_ARGV) + ["--sh_degree", str(degree)]
     hooks = HOOKS_MESH if gs_type == "gs_mesh" else HOOKS_FLAT
@@ -759,5 +778,5 @@ def test_command_line_trains_and_renders_at_a_low_degree(cli_scene, gs_type, deg
                 assert f.read() == g.read(), f"{split} {i}"
     names_ = ("vertices", "_alpha", "_scale", "_features", "_opacity") if gs_type == "gs_mesh" else FreeGaussianModel.NAMES
     final = {n: getattr(run.model, n).detach().clone() for n in names_}
-    a, b = _api_loop(cli_scene, argv, hooks), _api_loop(cli_scene, argv, hooks)
-    _within_spread(final, a, b, f"{gs_type} --sh_degree {degree} CLI vs API")
+    runs = [_api_loop(cli_scene, argv, hooks) for _ in range(LIBRARY_RUNS)]
+    _near_a_library_run(final, runs, f"{gs_type} --sh_degree {degree} CLI vs API")

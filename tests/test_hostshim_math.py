@@ -10,7 +10,8 @@ import torch
 
 from gms_b200 import _lib, scenes
 from oracle import expansion as oexp
-from oracle import raster
+from oracle import preprocess64, raster
+from preprocess_budget_cases import check_per_element
 from helpers import settings_from_camera, random_gaussians
 from hostshim import build_shim
 
@@ -185,6 +186,12 @@ def test_preprocess_backward_vs_oracle(shim, aa):
     close(o["dm"], ref["dL_dmeans3D"], "means3D"); close(o["dcov"], ref["dL_dcov3D"], "cov3D")
     close(o["dsh"], ref["dL_dsh"], "sh"); close(o["dsc"], ref["dL_dscales"], "scales")
     close(o["drot"], ref["dL_drotations"], "rot"); close(o["dop"], ref["dL_dopacity"].reshape(-1), "opacity")
+    # per element: within the a-priori budget around the float64 reference on the same fp32 record (oracle/preprocess64.py)
+    r = preprocess64.preprocess_backward64(st, np.concatenate([d2, dc, dop[:, None], dcol, dinv[:, None]], 1))
+    worst = check_per_element(dict(means3D=o["dm"], cov3D_precomp=o["dcov"], shs=o["dsh"], scales=o["dsc"], rotations=o["drot"],
+                                   opacities=o["dop"]), r, st.radii > 0)
+    print("worst |shim - ref64| / budget: " + ", ".join(f"{k} {w:.3g}" for k, w in worst.items()))
+    assert all(w <= 1.0 for w in worst.values()), worst
 
 
 def test_points_pseudomesh_expansion_matches_reference_golden(shim, golden_dir):
