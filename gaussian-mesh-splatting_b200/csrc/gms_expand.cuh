@@ -195,7 +195,7 @@ GMS_HD void gms_face_frame_backward(const float* t, float eps, const GmsFrame& f
 
 // `f` indexes the per-FACE arrays (faces / triangles_in / triangles); `fl` indexes the per-GAUSSIAN streams (alpha_raw,
 // scale_raw and every output row): fl == f when they are the caller's arrays, fl == the face's slot in the block when the
-// kernel has redirected those pointers to its shared-memory staging buffers (k_expand_fwd / k_expand_bwd).
+// kernel has redirected those pointers to its shared-memory staging buffers (the staged k_expand_fwd).
 // A face is read, its frame and quaternion formed once (gms_expand_face_load / gms_expand_face_frame), then every splat is one call of
 // gms_expand_splat_fwd / gms_expand_splat_bwd: the per-thread kernels loop over the face's K splats, the wide kernels
 // (k_expand_wide_*) spread them over a warp's lanes.  Either way each splat's arithmetic is the same sequence of operations.
@@ -380,160 +380,16 @@ GMS_HD void gms_expand_face_bwd_act(const gms_expand_args& a, const gms_expand_g
     gms_expand_face_bwd_tail(a, g, s, f, dt, dq, ds1, ds2);
 }
 
-// The relu weights' whole-face functions as the per-thread gs_mesh kernels have always compiled them (k_expand_fwd /
-// k_expand_bwd): the same arithmetic as gms_expand_face_*_act<GMS_ALPHA_RELU>, written as one loop, kept as it is so those
-// kernels' machine code does not change.
-GMS_HD void gms_expand_face_fwd_relu(const gms_expand_args& a, int f, int fl) {
-    float t[9];
-    if (a.triangles_in) {
-#pragma unroll
-        for (int k = 0; k < 9; k++) t[k] = a.triangles_in[9 * (size_t)f + k];
-    } else {
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-            const int64_t vi = a.faces[3 * (size_t)f + c];
-            t[3 * c] = a.vertices[3 * vi]; t[3 * c + 1] = a.vertices[3 * vi + 1]; t[3 * c + 2] = a.vertices[3 * vi + 2];
-        }
-    }
-    if (a.triangles) {
-#pragma unroll
-        for (int k = 0; k < 9; k++) a.triangles[9 * (size_t)f + k] = t[k];
-    }
-    GmsFrame fr;
-    gms_face_frame(t, a.eps, fr);
-    float q[4];
-    GmsQuatAux ax;
-    gms_frame_quat(fr, q, ax);
-    const float qn = fmaxf(GMS_SQRTN(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
-    for (int k = 0; k < a.K; k++) {
-        const size_t p = (size_t)fl * a.K + k;
-        const float r0 = fmaxf(a.alpha_raw[3 * p], 0.f) + 1e-8f, r1 = fmaxf(a.alpha_raw[3 * p + 1], 0.f) + 1e-8f,
-                    r2 = fmaxf(a.alpha_raw[3 * p + 2], 0.f) + 1e-8f;
-        const float S = r0 + r1 + r2;
-        const float al0 = GMS_DIVN(r0, S), al1 = GMS_DIVN(r1, S), al2 = GMS_DIVN(r2, S);        // S >= 3e-8
-        if (a.alpha) { a.alpha[3 * p] = al0; a.alpha[3 * p + 1] = al1; a.alpha[3 * p + 2] = al2; }
-        if (a.xyz) {
-#pragma unroll
-            for (int c = 0; c < 3; c++) a.xyz[3 * p + c] = al0 * t[c] + al1 * t[3 + c] + al2 * t[6 + c];
-        }
-        const float cs = a.scale_raw[p];
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-            const float inner = fmaxf(cs * fr.s[c], 0.f) + a.eps;
-            if (a.scaling_log) a.scaling_log[3 * p + c] = logf(inner);
-            if (a.scaling_act) a.scaling_act[3 * p + c] = expf(logf(inner));
-        }
-        if (a.rotation_raw) { float* o = a.rotation_raw + 4 * p; o[0] = q[0]; o[1] = q[1]; o[2] = q[2]; o[3] = q[3]; }
-        if (a.rotation_act) { float* o = a.rotation_act + 4 * p; o[0] = GMS_DIVN(q[0], qn); o[1] = GMS_DIVN(q[1], qn); o[2] = GMS_DIVN(q[2], qn); o[3] = GMS_DIVN(q[3], qn); }
-    }
-}
-
-GMS_HD void gms_expand_face_bwd_relu(const gms_expand_args& a, const gms_expand_grads& g, int f, int fl) {
-    float t[9];
-    int64_t vi[3] = {0, 0, 0};
-    if (a.triangles_in) {
-#pragma unroll
-        for (int k = 0; k < 9; k++) t[k] = a.triangles_in[9 * (size_t)f + k];
-    } else {
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-            vi[c] = a.faces[3 * (size_t)f + c];
-            t[3 * c] = a.vertices[3 * vi[c]]; t[3 * c + 1] = a.vertices[3 * vi[c] + 1]; t[3 * c + 2] = a.vertices[3 * vi[c] + 2];
-        }
-    }
-    GmsFrame fr;
-    gms_face_frame(t, a.eps, fr);
-    float q[4];
-    GmsQuatAux ax;
-    gms_frame_quat(fr, q, ax);
-    const float qnorm = GMS_SQRTN(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    const float qn = fmaxf(qnorm, 1e-12f);
-    float dt[9];
-#pragma unroll
-    for (int k = 0; k < 9; k++) dt[k] = 0.f;
-    float dq[4] = {0.f, 0.f, 0.f, 0.f};
-    float ds1 = 0.f, ds2 = 0.f;
-    for (int k = 0; k < a.K; k++) {
-        const size_t p = (size_t)fl * a.K + k;
-        // --- xyz = alpha @ triangle
-        float dx[3] = {0.f, 0.f, 0.f};
-        if (g.dL_dxyz) { dx[0] = g.dL_dxyz[3 * p]; dx[1] = g.dL_dxyz[3 * p + 1]; dx[2] = g.dL_dxyz[3 * p + 2]; }
-        const float ar[3] = {a.alpha_raw[3 * p], a.alpha_raw[3 * p + 1], a.alpha_raw[3 * p + 2]};
-        const float r[3] = {fmaxf(ar[0], 0.f) + 1e-8f, fmaxf(ar[1], 0.f) + 1e-8f, fmaxf(ar[2], 0.f) + 1e-8f};
-        const float S = r[0] + r[1] + r[2];
-        const float al[3] = {GMS_DIVN(r[0], S), GMS_DIVN(r[1], S), GMS_DIVN(r[2], S)};
-        float dal[3];
-#pragma unroll
-        for (int j = 0; j < 3; j++) {
-            dal[j] = dx[0] * t[3 * j] + dx[1] * t[3 * j + 1] + dx[2] * t[3 * j + 2];
-#pragma unroll
-            for (int c = 0; c < 3; c++) dt[3 * j + c] += al[j] * dx[c];
-        }
-        const float dsum = dal[0] * al[0] + dal[1] * al[1] + dal[2] * al[2];
-        if (g.dL_dalpha_raw) {
-#pragma unroll
-            for (int j = 0; j < 3; j++) g.dL_dalpha_raw[3 * p + j] = ar[j] > 0.f ? GMS_DIVN(dal[j] - dsum, S) : 0.f;
-        }
-        // --- scaling
-        const float cs = a.scale_raw[p];
-        float dcs = 0.f;
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-            float gl = g.dL_dscaling_log ? g.dL_dscaling_log[3 * p + c] : 0.f;
-            const float prod = cs * fr.s[c];
-            const float inner = fmaxf(prod, 0.f) + a.eps;
-            if (g.dL_dscaling_act) gl += g.dL_dscaling_act[3 * p + c] * expf(logf(inner));
-            const float dprod = prod > 0.f ? GMS_DIVN(gl, inner) : 0.f;       // inner >= eps
-            dcs += dprod * fr.s[c];
-            if (c == 1) ds1 += dprod * cs;
-            if (c == 2) ds2 += dprod * cs;
-        }
-        if (g.dL_dscale_raw) g.dL_dscale_raw[p] = dcs;
-        // --- rotation (same quaternion for the K splats of the face: sum the incoming rows)
-        if (g.dL_drotation_raw) {
-            const float* d = g.dL_drotation_raw + 4 * p;
-            dq[0] += d[0]; dq[1] += d[1]; dq[2] += d[2]; dq[3] += d[3];
-        }
-        if (g.dL_drotation_act) {
-            const float* dp = g.dL_drotation_act + 4 * p;
-            const float d_x = dp[0], d_y = dp[1], d_z = dp[2], d_w = dp[3];
-            if (qnorm >= 1e-12f) {
-                const float u[4] = {GMS_DIVN(q[0], qn), GMS_DIVN(q[1], qn), GMS_DIVN(q[2], qn), GMS_DIVN(q[3], qn)};       // qn >= 1e-12
-                const float dd = d_x * u[0] + d_y * u[1] + d_z * u[2] + d_w * u[3];
-                dq[0] += GMS_DIVN(d_x - u[0] * dd, qn); dq[1] += GMS_DIVN(d_y - u[1] * dd, qn);
-                dq[2] += GMS_DIVN(d_z - u[2] * dd, qn); dq[3] += GMS_DIVN(d_w - u[3] * dd, qn);
-            } else {
-                dq[0] += GMS_DIVN(d_x, qn); dq[1] += GMS_DIVN(d_y, qn); dq[2] += GMS_DIVN(d_z, qn); dq[3] += GMS_DIVN(d_w, qn);
-            }
-        }
-    }
-    float dv0[3] = {0.f, 0.f, 0.f}, dv1[3] = {0.f, 0.f, 0.f}, dv2[3] = {0.f, 0.f, 0.f};
-    gms_frame_quat_backward(ax, dq, dv0, dv1, dv2);
-    gms_face_frame_backward(t, a.eps, fr, dv0, dv1, dv2, ds1, ds2, dt);
-    if (g.dL_dtriangles) {
-#pragma unroll
-        for (int k = 0; k < 9; k++) g.dL_dtriangles[9 * (size_t)f + k] = dt[k];
-    }
-    if (g.dL_dvertices && !a.triangles_in) {
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-            GMS_ATOMIC_ADD(&g.dL_dvertices[3 * vi[c]], dt[3 * c]);
-            GMS_ATOMIC_ADD(&g.dL_dvertices[3 * vi[c] + 1], dt[3 * c + 1]);
-            GMS_ATOMIC_ADD(&g.dL_dvertices[3 * vi[c] + 2], dt[3 * c + 2]);
-        }
-    }
-}
-
 // Whole face with the activation the arguments select (the host shim's entry points; the per-thread kernels call the
-// functions above directly).
+// templates above directly).
 GMS_HD void gms_expand_face_fwd(const gms_expand_args& a, int f, int fl) {
     if (a.alpha_activation == GMS_ALPHA_SOFTMAX) gms_expand_face_fwd_act<GMS_ALPHA_SOFTMAX>(a, f, fl);
-    else gms_expand_face_fwd_relu(a, f, fl);
+    else gms_expand_face_fwd_act<GMS_ALPHA_RELU>(a, f, fl);
 }
 
 GMS_HD void gms_expand_face_bwd(const gms_expand_args& a, const gms_expand_grads& g, int f, int fl) {
     if (a.alpha_activation == GMS_ALPHA_SOFTMAX) gms_expand_face_bwd_act<GMS_ALPHA_SOFTMAX>(a, g, f, fl);
-    else gms_expand_face_bwd_relu(a, g, f, fl);
+    else gms_expand_face_bwd_act<GMS_ALPHA_RELU>(a, g, f, fl);
 }
 
 
@@ -704,10 +560,11 @@ GMS_HD void gms_points_vertices_fwd(const gms_points_vertices_args& a, int i) {
 #if defined(__CUDACC__)
 
 // ------------------------------------------------------------------------------------------ expansion kernels
-// One thread per face.  The per-Gaussian streams (K rows per face: 36-48 B per thread, i.e. a 36-48 B stride between
-// lanes) are staged through shared memory: the block copies its contiguous slice of every stream with fully coalesced
-// accesses, the per-face maths then reads / writes shared memory (gms_expand_face_* with fl = slot in the block).
-// STAGED = false is the direct variant (option "expand_staged" = 0, and whenever K makes the staging exceed 48 KB).
+// One thread per face.  The forward's per-Gaussian streams (K rows per face: 36-48 B per thread, i.e. a 36-48 B stride
+// between lanes) are staged through shared memory: the block copies its contiguous slice of every stream with fully
+// coalesced accesses, the per-face maths then reads / writes shared memory (gms_expand_face_* with fl = slot in the block).
+// STAGED = false is the direct variant, for K whose staging would exceed 48 KB.  The backward reads and writes its rows
+// directly: staging them measured no faster (DESIGN.md 3.7).
 constexpr int GMS_EXP_BLOCK = 128;
 
 __device__ __forceinline__ const float* exp_stage_in(const float* src, int width, size_t g0, int ng, int cap, float*& sm) {
@@ -728,22 +585,11 @@ __device__ __forceinline__ void exp_stage_flush(float* dst, const float* buf, in
     for (int i = threadIdx.x; i < ng * width; i += GMS_EXP_BLOCK) d0[i] = buf[i];
 }
 
-template <int ACT>
-__device__ __forceinline__ void expand_face_fwd(const gms_expand_args& a, int f, int fl) {
-    if constexpr (ACT == GMS_ALPHA_RELU) gms_expand_face_fwd_relu(a, f, fl);
-    else gms_expand_face_fwd_act<ACT>(a, f, fl);
-}
-template <int ACT>
-__device__ __forceinline__ void expand_face_bwd(const gms_expand_args& a, const gms_expand_grads& g, int f, int fl) {
-    if constexpr (ACT == GMS_ALPHA_RELU) gms_expand_face_bwd_relu(a, g, f, fl);
-    else gms_expand_face_bwd_act<ACT>(a, g, f, fl);
-}
-
 template <bool STAGED, int ACT>
-__device__ __forceinline__ void expand_fwd_block(const gms_expand_args& a) {
+__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_fwd(gms_expand_args a) {
     const int f0 = blockIdx.x * GMS_EXP_BLOCK, f = f0 + threadIdx.x;
     if (!STAGED) {
-        if (f < a.F) expand_face_fwd<ACT>(a, f, f);
+        if (f < a.F) gms_expand_face_fwd_act<ACT>(a, f, f);
         return;
     }
     extern __shared__ float4 exp_smem4[];
@@ -760,7 +606,7 @@ __device__ __forceinline__ void expand_fwd_block(const gms_expand_args& a) {
     l.rotation_raw = exp_stage_out(a.rotation_raw, 4, cap, sm);
     l.rotation_act = exp_stage_out(a.rotation_act, 4, cap, sm);
     __syncthreads();
-    if (f < a.F) expand_face_fwd<ACT>(l, f, threadIdx.x);
+    if (f < a.F) gms_expand_face_fwd_act<ACT>(l, f, threadIdx.x);
     __syncthreads();
     exp_stage_flush(a.alpha, l.alpha, 3, g0, ng);
     exp_stage_flush(a.xyz, l.xyz, 3, g0, ng);
@@ -770,47 +616,10 @@ __device__ __forceinline__ void expand_fwd_block(const gms_expand_args& a) {
     exp_stage_flush(a.rotation_act, l.rotation_act, 4, g0, ng);
 }
 
-template <bool STAGED>
-__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_fwd(gms_expand_args a) { expand_fwd_block<STAGED, GMS_ALPHA_RELU>(a); }
-template <bool STAGED>
-__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_softmax_fwd(gms_expand_args a) { expand_fwd_block<STAGED, GMS_ALPHA_SOFTMAX>(a); }
-
-template <bool STAGED, int ACT>
-__device__ __forceinline__ void expand_bwd_block(const gms_expand_args& a, const gms_expand_grads& g) {
-    const int f0 = blockIdx.x * GMS_EXP_BLOCK, f = f0 + threadIdx.x;
-    if (!STAGED) {
-        if (f < a.F) expand_face_bwd<ACT>(a, g, f, f);
-        return;
-    }
-    extern __shared__ float4 exp_smem4[];
-    float* sm = reinterpret_cast<float*>(exp_smem4);
-    const int nf = min(GMS_EXP_BLOCK, a.F - f0), ng = nf * a.K, cap = GMS_EXP_BLOCK * a.K;
-    const size_t g0 = (size_t)f0 * a.K;
-    gms_expand_args l = a;
-    gms_expand_grads lg = g;
-    l.alpha_raw = exp_stage_in(a.alpha_raw, 3, g0, ng, cap, sm);
-    l.scale_raw = exp_stage_in(a.scale_raw, 1, g0, ng, cap, sm);
-    lg.dL_dxyz = exp_stage_in(g.dL_dxyz, 3, g0, ng, cap, sm);
-    lg.dL_dscaling_log = exp_stage_in(g.dL_dscaling_log, 3, g0, ng, cap, sm);
-    lg.dL_dscaling_act = exp_stage_in(g.dL_dscaling_act, 3, g0, ng, cap, sm);
-    lg.dL_drotation_raw = exp_stage_in(g.dL_drotation_raw, 4, g0, ng, cap, sm);
-    lg.dL_drotation_act = exp_stage_in(g.dL_drotation_act, 4, g0, ng, cap, sm);
-    lg.dL_dalpha_raw = exp_stage_out(g.dL_dalpha_raw, 3, cap, sm);
-    lg.dL_dscale_raw = exp_stage_out(g.dL_dscale_raw, 1, cap, sm);
-    __syncthreads();
-    if (f < a.F) expand_face_bwd<ACT>(l, lg, f, threadIdx.x);     // per-face outputs (dL_dtriangles, vertex atomics) stay global
-    __syncthreads();
-    exp_stage_flush(g.dL_dalpha_raw, lg.dL_dalpha_raw, 3, g0, ng);
-    exp_stage_flush(g.dL_dscale_raw, lg.dL_dscale_raw, 1, g0, ng);
-}
-
-template <bool STAGED>
+template <int ACT>
 __global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_bwd(gms_expand_args a, gms_expand_grads g) {
-    expand_bwd_block<STAGED, GMS_ALPHA_RELU>(a, g);
-}
-template <bool STAGED>
-__global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_softmax_bwd(gms_expand_args a, gms_expand_grads g) {
-    expand_bwd_block<STAGED, GMS_ALPHA_SOFTMAX>(a, g);
+    const int f = blockIdx.x * GMS_EXP_BLOCK + threadIdx.x;
+    if (f < a.F) gms_expand_face_bwd_act<ACT>(a, g, f, f);
 }
 
 // Splat-parallel expansion for many splats per face (gs_flame: K = 100 on ~10k faces).  One warp per face: every lane reads
@@ -820,10 +629,10 @@ __global__ void __launch_bounds__(GMS_EXP_BLOCK) k_expand_softmax_bwd(gms_expand
 // the per-thread kernel's gms_expand_splat_* call, so the forward is bit-identical to it.  The backward sums each lane's
 // dt / dq / ds1 / ds2 partials over its splats, reduces them across the warp (butterfly), and lane 0 finishes the face: one
 // set of vertex atomics per face, as in the per-thread kernel.  Only the order of the sum over K differs.
+// Softmax weights only: relu weights (gs_mesh) always run the per-thread kernels.
 constexpr int GMS_EXP_WIDE_BLOCK = 128;                     // 4 faces per block
-constexpr int GMS_EXP_WIDE_MIN_K = 16;                      // expand_wide = 1: softmax weights with K >= this (DESIGN.md 4.5)
+constexpr int GMS_EXP_WIDE_MIN_K = 16;                      // softmax weights with K >= this run these kernels (DESIGN.md 4.5)
 
-template <int ACT>
 __global__ void __launch_bounds__(GMS_EXP_WIDE_BLOCK) k_expand_wide_fwd(gms_expand_args a) {
     const int f = blockIdx.x * (GMS_EXP_WIDE_BLOCK / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (f >= a.F) return;
@@ -834,10 +643,9 @@ __global__ void __launch_bounds__(GMS_EXP_WIDE_BLOCK) k_expand_wide_fwd(gms_expa
         for (int k = 0; k < 9; k++) a.triangles[9 * (size_t)f + k] = s.t[k];
     }
     gms_expand_face_frame(a, s);
-    for (int k = lane; k < a.K; k += 32) gms_expand_splat_fwd<ACT>(a, s, (size_t)f * a.K + k);
+    for (int k = lane; k < a.K; k += 32) gms_expand_splat_fwd<GMS_ALPHA_SOFTMAX>(a, s, (size_t)f * a.K + k);
 }
 
-template <int ACT>
 __global__ void __launch_bounds__(GMS_EXP_WIDE_BLOCK) k_expand_wide_bwd(gms_expand_args a, gms_expand_grads g) {
     const int f = blockIdx.x * (GMS_EXP_WIDE_BLOCK / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (f >= a.F) return;                                   // whole warps: f is uniform across the warp
@@ -847,7 +655,8 @@ __global__ void __launch_bounds__(GMS_EXP_WIDE_BLOCK) k_expand_wide_bwd(gms_expa
     float acc[15];                                          // dt[9], dq[4], ds1, ds2
 #pragma unroll
     for (int i = 0; i < 15; i++) acc[i] = 0.f;
-    for (int k = lane; k < a.K; k += 32) gms_expand_splat_bwd<ACT>(a, g, s, (size_t)f * a.K + k, acc, acc + 9, acc[13], acc[14]);
+    for (int k = lane; k < a.K; k += 32)
+        gms_expand_splat_bwd<GMS_ALPHA_SOFTMAX>(a, g, s, (size_t)f * a.K + k, acc, acc + 9, acc[13], acc[14]);
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) {
 #pragma unroll

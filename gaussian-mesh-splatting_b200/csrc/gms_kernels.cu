@@ -46,10 +46,6 @@ static int g_opt_tile_order = 1;   // launch tiles longest list first (0: 2.79 m
 static int g_opt_sh_staged = 1;     // preprocess fwd/bwd: SH rows through a per-warp shared-memory tile (coalesced 128-bit accesses);
                                     // 0: direct (2.66 ms), 1: tile + register rows, 2: bwd in place in the tile (2.63 ms)
 static int g_opt_pre_bwd_minb = 4;  // k_preprocess_bwd min CTAs/SM (1: 2.67 ms, 3: 2.67 ms, 4: default)
-static int g_opt_expand_staged = 1; // expansion kernels, per-Gaussian streams staged through shared memory (coalesced): bit 0 forward
-                                    // (0: 2.74 ms), bit 1 backward (3: 2.67 ms, off)
-static int g_opt_expand_wide = 1;  // expansion kernels, one warp per face (k_expand_wide_*): 0 never, 1 softmax weights with K >=
-                                    // GMS_EXP_WIDE_MIN_K (default; relu meshes keep the per-thread kernels), 2 always (A/B runs, tests)
 static int g_opt_sort = 0;         // depth sort (and the emit + sort path's tile sort): 0 cub::DeviceRadixSort, 1 hand-written radix sort
                                    //    with device-side N clamped to the capacity (gms_sort.cuh; bit-identical order through the
                                    //    synchronising entry points and the sync-free frame; 2.67-2.70 ms against 2.40-2.42 ms
@@ -546,8 +542,6 @@ int gms_set_option(const char* key, int value) {
     else if (!strcmp(key, "tile_order")) p = &g_opt_tile_order;
     else if (!strcmp(key, "sort_impl")) p = &g_opt_sort;
     else if (!strcmp(key, "bin_impl")) p = &g_opt_bin;
-    else if (!strcmp(key, "expand_staged")) p = &g_opt_expand_staged;
-    else if (!strcmp(key, "expand_wide")) p = &g_opt_expand_wide;
     else if (!strcmp(key, "sh_staged")) p = &g_opt_sh_staged;
     else if (!strcmp(key, "pre_bwd_minblocks")) p = &g_opt_pre_bwd_minb;
     if (!p) return -1;
@@ -952,19 +946,15 @@ int gms_debug_unpack(const gms_raster_saved* saved, int32_t P, const int32_t* ra
                   conic_opacity, rgb, clamped);
 }
 
-// floats of shared memory per Gaussian row (host side: sizing the launch)
+// floats of shared memory per Gaussian row of the staged forward (host side: sizing the launch)
 static int exp_fwd_stage_width(const gms_expand_args& a) {
     return 3 + 1 + (a.alpha ? 3 : 0) + (a.xyz ? 3 : 0) + (a.scaling_log ? 3 : 0) + (a.scaling_act ? 3 : 0) +
            (a.rotation_raw ? 4 : 0) + (a.rotation_act ? 4 : 0);
 }
-static int exp_bwd_stage_width(const gms_expand_grads& g) {
-    return 3 + 1 + (g.dL_dxyz ? 3 : 0) + (g.dL_dscaling_log ? 3 : 0) + (g.dL_dscaling_act ? 3 : 0) +
-           (g.dL_drotation_raw ? 4 : 0) + (g.dL_drotation_act ? 4 : 0) + (g.dL_dalpha_raw ? 3 : 0) + (g.dL_dscale_raw ? 1 : 0);
-}
 
-// Which expansion kernels a call runs: the warp-per-face ones (option "expand_wide") or the per-thread ones.
+// Which expansion kernels a call runs: one warp per face for softmax weights with many splats per face, else one thread.
 static bool expand_wide(const gms_expand_args& a) {
-    return g_opt_expand_wide == 2 || (g_opt_expand_wide == 1 && a.alpha_activation == GMS_ALPHA_SOFTMAX && a.K >= GMS_EXP_WIDE_MIN_K);
+    return a.alpha_activation == GMS_ALPHA_SOFTMAX && a.K >= GMS_EXP_WIDE_MIN_K;
 }
 
 int gms_expand_forward(const gms_expand_args* a, void* cuda_stream) {
@@ -975,14 +965,14 @@ int gms_expand_forward(const gms_expand_args* a, void* cuda_stream) {
     if (a->alpha_activation != GMS_ALPHA_RELU && a->alpha_activation != GMS_ALPHA_SOFTMAX)
         return set_err(GMS_E_ARG, "alpha_activation must be 0 (relu) or 1 (softmax)%s%s");
     if (a->F == 0) return GMS_OK;
-    const bool softmax = a->alpha_activation == GMS_ALPHA_SOFTMAX;
     if (expand_wide(*a))
         return launch("expand_fwd", K_EXP_FWD, 0, st, (a->F + GMS_EXP_WIDE_BLOCK / 32 - 1) / (GMS_EXP_WIDE_BLOCK / 32), GMS_EXP_WIDE_BLOCK, 0,
-                      softmax ? k_expand_wide_fwd<GMS_ALPHA_SOFTMAX> : k_expand_wide_fwd<GMS_ALPHA_RELU>, *a);
+                      k_expand_wide_fwd, *a);
+    const bool softmax = a->alpha_activation == GMS_ALPHA_SOFTMAX;
     const size_t smem = (size_t)GMS_EXP_BLOCK * a->K * exp_fwd_stage_width(*a) * sizeof(float);
-    const bool staged = (g_opt_expand_staged & 1) && smem <= 48 * 1024;
-    void (*k)(gms_expand_args) = softmax ? (staged ? k_expand_softmax_fwd<true> : k_expand_softmax_fwd<false>)
-                                         : (staged ? k_expand_fwd<true> : k_expand_fwd<false>);
+    const bool staged = smem <= 48 * 1024;
+    void (*k)(gms_expand_args) = softmax ? (staged ? k_expand_fwd<true, GMS_ALPHA_SOFTMAX> : k_expand_fwd<false, GMS_ALPHA_SOFTMAX>)
+                                         : (staged ? k_expand_fwd<true, GMS_ALPHA_RELU> : k_expand_fwd<false, GMS_ALPHA_RELU>);
     return launch("expand_fwd", K_EXP_FWD, 0, st, (a->F + GMS_EXP_BLOCK - 1) / GMS_EXP_BLOCK, GMS_EXP_BLOCK, staged ? smem : 0, k, *a);
 }
 
@@ -1011,15 +1001,11 @@ int gms_expand_backward(const gms_expand_args* a, const gms_expand_grads* g, voi
     if (a->alpha_activation != GMS_ALPHA_RELU && a->alpha_activation != GMS_ALPHA_SOFTMAX)
         return set_err(GMS_E_ARG, "alpha_activation must be 0 (relu) or 1 (softmax)%s%s");
     if (a->F == 0) return GMS_OK;
-    const bool softmax = a->alpha_activation == GMS_ALPHA_SOFTMAX;
     if (expand_wide(*a))
         return launch("expand_bwd", K_EXP_BWD, 0, st, (a->F + GMS_EXP_WIDE_BLOCK / 32 - 1) / (GMS_EXP_WIDE_BLOCK / 32), GMS_EXP_WIDE_BLOCK, 0,
-                      softmax ? k_expand_wide_bwd<GMS_ALPHA_SOFTMAX> : k_expand_wide_bwd<GMS_ALPHA_RELU>, *a, *g);
-    const size_t smem = (size_t)GMS_EXP_BLOCK * a->K * exp_bwd_stage_width(*g) * sizeof(float);
-    const bool staged = (g_opt_expand_staged & 2) && smem <= 48 * 1024;
-    void (*k)(gms_expand_args, gms_expand_grads) = softmax ? (staged ? k_expand_softmax_bwd<true> : k_expand_softmax_bwd<false>)
-                                                           : (staged ? k_expand_bwd<true> : k_expand_bwd<false>);
-    return launch("expand_bwd", K_EXP_BWD, 0, st, (a->F + GMS_EXP_BLOCK - 1) / GMS_EXP_BLOCK, GMS_EXP_BLOCK, staged ? smem : 0, k, *a, *g);
+                      k_expand_wide_bwd, *a, *g);
+    return launch("expand_bwd", K_EXP_BWD, 0, st, (a->F + GMS_EXP_BLOCK - 1) / GMS_EXP_BLOCK, GMS_EXP_BLOCK, 0,
+                  a->alpha_activation == GMS_ALPHA_SOFTMAX ? k_expand_bwd<GMS_ALPHA_SOFTMAX> : k_expand_bwd<GMS_ALPHA_RELU>, *a, *g);
 }
 
 size_t gms_frame_workspace_bytes(int32_t P, int32_t W, int32_t H) { return frame_layout(nullptr, P, W, H).total + 512; }

@@ -859,9 +859,9 @@ int64_t gms_launch_count(int reset);
  * while option "time_kernels" is 1.  Fills up to max_kernels entries (accumulated ms, launch count, name) and
  * returns the number of kernel slots. */
 int gms_kernel_times(int reset, int max_kernels, double* ms_out, int64_t* count_out, const char** names_out);
-/* Tuning knobs (round-over-round experiments): "quad_masks", "warp_emit", "time_kernels", "composite_version",
- * "composite_fwd", "composite_bwd", "bwd_minblocks", "tile_order", "sort_impl", "expand_staged", "sh_staged",
- * "expand_wide" (DESIGN.md lists what each selects).  Returns the previous value; unknown keys return -1. */
+/* Tuning knobs (round-over-round experiments): "warp_emit", "time_kernels", "composite_fwd", "composite_bwd",
+ * "bwd_minblocks", "key16", "adam_sh_ieee", "tile_order", "sort_impl", "bin_impl", "sh_staged", "pre_bwd_minblocks"
+ * (DESIGN.md lists what each selects).  Returns the previous value; unknown keys return -1. */
 int gms_set_option(const char* key, int value);
 
 #ifdef __cplusplus

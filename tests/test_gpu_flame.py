@@ -1,8 +1,7 @@
 """-m gpu: gs_flame on the library's kernels.
 
-Expansion: the softmax weights through the per-thread kernels (staged and direct) and the warp-per-face kernels, on every
-mesh of tests/expansion_cases.py at K = 1, 3, 7, 40, 100, 128, per element against float64 (tests/softmax_expansion_cases.py);
-the wide forward bit for bit the per-thread one.
+Expansion: the softmax weights on every mesh of tests/expansion_cases.py at K = 1, 3, 7 (per-thread kernels) and K = 40,
+100, 128 (warp-per-face kernels), per element against float64 (tests/softmax_expansion_cases.py).
 Training: FlameGaussianModel + NativeFrame / FlameTrainer against the reference's op sequence (tests/flame_reference.AtenFlameArm)
 on the synthetic FLAME driver (tests/flame_driver.py): loss and gradients of the first step, three steps, launches per step."""
 import ctypes as C
@@ -33,7 +32,7 @@ def _tol(case):
     return TOL_SLIVER if case.name.startswith("sliver") else ec.TOL
 
 
-def _run(case, staged, wide, activation=_lib.ALPHA_SOFTMAX):
+def _run(case):
     stream = torch.cuda.current_stream().cuda_stream
 
     def put(arr):
@@ -41,42 +40,17 @@ def _run(case, staged, wide, activation=_lib.ALPHA_SOFTMAX):
         return t, t.data_ptr()
 
     def call(fn, *args):
-        args[0].alpha_activation = activation
+        args[0].alpha_activation = _lib.ALPHA_SOFTMAX
         _lib.check(fn(*[C.byref(x) for x in args], stream), fn.__name__)
 
     L = _lib.lib()
-    old_s, old_w = _lib.set_option("expand_staged", staged), _lib.set_option("expand_wide", wide)
-    try:
-        return ec.run_abi(case, put, lambda t: t.cpu().numpy(), lambda a: call(L.gms_expand_forward, a),
-                          lambda a, g: call(L.gms_expand_backward, a, g))
-    finally:
-        _lib.set_option("expand_staged", old_s)
-        _lib.set_option("expand_wide", old_w)
+    return ec.run_abi(case, put, lambda t: t.cpu().numpy(), lambda a: call(L.gms_expand_forward, a),
+                      lambda a, g: call(L.gms_expand_backward, a, g))
 
 
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
 def test_softmax_expansion_kernels_vs_float64(case):
-    ref = sc.Reference(case)
-    runs = {"staged": _run(case, 3, 0), "direct": _run(case, 0, 0), "wide": _run(case, 3, 2)}
-    for name, got in runs.items():
-        ec.check_case(ref, got, _tol(case), f"gpu softmax {name} {case.name}")
-    for k in ec.OUT_SHAPES:     # the wide forward is the per-thread forward, bit for bit
-        np.testing.assert_array_equal(runs["wide"][k], runs["staged"][k], err_msg=k)
-        np.testing.assert_array_equal(runs["direct"][k], runs["staged"][k], err_msg=k)
-
-
-RELU_CASES = ec.build_cases()
-
-
-@pytest.mark.parametrize("case", RELU_CASES, ids=lambda c: c.name)
-def test_forced_wide_kernels_with_relu_weights_vs_float64(case):
-    """expand_wide = 2 also sends relu weights (gs_mesh) through the warp-per-face kernels."""
-    ref = ec.Reference(case)
-    got = _run(case, 3, 2, _lib.ALPHA_RELU)
-    ec.check_case(ref, got, ec.TOL, f"gpu relu wide {case.name}")
-    per_thread = _run(case, 3, 0, _lib.ALPHA_RELU)
-    for k in ec.OUT_SHAPES:
-        np.testing.assert_allclose(got[k], per_thread[k], rtol=0, atol=0, err_msg=k)
+    ec.check_case(sc.Reference(case), _run(case), _tol(case), f"gpu softmax {case.name}")
 
 
 def test_softmax_expansion_vs_reference_golden():
@@ -89,25 +63,20 @@ def test_softmax_expansion_vs_reference_golden():
     cu = lambda k, g=True: torch.tensor(e[k], device="cuda").requires_grad_(g)
     raw, enl, al, sc = cu("raw_vertices"), cu("_vertices_enlargement"), cu("_alpha"), cu("_scales")
     faces = torch.tensor(e["faces"], device="cuda")
-    for wide in (0, 2):
-        old = _lib.set_option("expand_wide", wide)
-        try:
-            verts = flame_transform_vertices(raw[None], enl)
-            xyz, sl, rr, alpha, _ = expansion.expand(verts, faces, al, sc, activated=False, alpha_activation=_lib.ALPHA_SOFTMAX)
-            torch.cuda.synchronize()
-            for k, t in (("vertices", verts), ("alpha", alpha), ("_xyz", xyz), ("_scaling", sl), ("_rotation", rr)):
-                r = e[k]
-                err = float(np.abs(t.detach().cpu().numpy() - r).max() / np.abs(r).max())
-                assert err <= 2e-6, (wide, k, err)
-            g = torch.autograd.grad((xyz * cu("up_xyz", False)).sum() + (sl * cu("up_scaling", False)).sum() +
-                                    (rr * cu("up_rotation", False)).sum(), (al, sc, raw, enl))
-            for k, t in zip(("d_alpha", "d_scales", "d_raw_vertices", "d_vertices_enlargement"), g):
-                r = e[k]
-                err = float(np.abs(t.cpu().numpy() - r).max() / np.abs(r).max())
-                print(f"[flame] golden wide={wide} {k}: max|kernel - reference| / max|reference| {err:.2e}")
-                assert err <= 1e-4, (wide, k, err)
-        finally:
-            _lib.set_option("expand_wide", old)
+    verts = flame_transform_vertices(raw[None], enl)
+    xyz, sl, rr, alpha, _ = expansion.expand(verts, faces, al, sc, activated=False, alpha_activation=_lib.ALPHA_SOFTMAX)
+    torch.cuda.synchronize()
+    for k, t in (("vertices", verts), ("alpha", alpha), ("_xyz", xyz), ("_scaling", sl), ("_rotation", rr)):
+        r = e[k]
+        err = float(np.abs(t.detach().cpu().numpy() - r).max() / np.abs(r).max())
+        assert err <= 2e-6, (k, err)
+    g = torch.autograd.grad((xyz * cu("up_xyz", False)).sum() + (sl * cu("up_scaling", False)).sum() +
+                            (rr * cu("up_rotation", False)).sum(), (al, sc, raw, enl))
+    for k, t in zip(("d_alpha", "d_scales", "d_raw_vertices", "d_vertices_enlargement"), g):
+        r = e[k]
+        err = float(np.abs(t.cpu().numpy() - r).max() / np.abs(r).max())
+        print(f"[flame] golden {k}: max|kernel - reference| / max|reference| {err:.2e}")
+        assert err <= 1e-4, (k, err)
 
 
 def test_bad_alpha_activation_is_refused():
@@ -138,7 +107,7 @@ def _scene(K=10, rings=23, segments=24, W=256, H=256):
 
 @pytest.mark.parametrize("K", [10, 100])
 def test_first_step_loss_and_gradients_match_the_reference_arm(K):
-    """K = 100 runs the warp-per-face kernels inside gms_train_frame (expand_wide = 1, K >= 16); K = 10 the per-thread ones."""
+    """K = 100 runs the warp-per-face kernels inside gms_train_frame (softmax weights, K >= 16); K = 10 the per-thread ones."""
     m, cams, gts, bg = _scene(K=K)
     arm = fr.AtenFlameArm(m, bg)
     t = FlameTrainer(m, bg)

@@ -26,8 +26,7 @@ BG = (0.2, 0.5, 0.9)
 W = H = 256
 SIZES = [(240, 272), (256, 256), (400, 300)]      # T = 15 x 17 = 255, 16 x 16 = 256, 25 x 19 = 475 (300 = 18.75 tiles)
 OPTION_SETS = [{}, {"sort_impl": 1}, {"bin_impl": 1}, {"bin_impl": 1, "sort_impl": 1}, {"key16": 0}, {"key16": 0, "sort_impl": 1},
-               {"composite_fwd": 3}, {"composite_bwd": 3}, {"tile_order": 0}, {"sh_staged": 0}, {"sh_staged": 2},
-               {"expand_staged": 0}]
+               {"composite_fwd": 3}, {"composite_bwd": 3}, {"tile_order": 0}, {"sh_staged": 0}, {"sh_staged": 2}]
 # max err / max |ref| of the raw gradients; scales and rotations go through the near-singular 2D covariance (DESIGN.md 2.2)
 # run-to-run spread of the gradients between two frames of one camera, max |diff| / max |grad|: the composite backward adds
 # with float atomics; scales and rotations amplify it through the near-singular 2D covariance.  Largest spread measured over

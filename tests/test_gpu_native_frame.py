@@ -29,8 +29,7 @@ LAMBDA = 0.2
 BG = (0.2, 0.5, 0.9)
 SIZES = [(240, 272), (256, 256), (400, 300)]      # T = 15 x 17 = 255, 16 x 16 = 256, 25 x 19 = 475 (300 = 18.75 tiles)
 OPTION_SETS = [{}, {"sort_impl": 1}, {"bin_impl": 1}, {"bin_impl": 1, "sort_impl": 1}, {"key16": 0}, {"key16": 0, "sort_impl": 1},
-               {"composite_fwd": 3}, {"composite_bwd": 3}, {"tile_order": 0}, {"sh_staged": 0}, {"sh_staged": 2},
-               {"expand_staged": 0}]
+               {"composite_fwd": 3}, {"composite_bwd": 3}, {"tile_order": 0}, {"sh_staged": 0}, {"sh_staged": 2}]
 GRADS = ("vertices", "_alpha", "_scale", "_opacity", "_features")
 
 _scenes, _oracle = {}, {}

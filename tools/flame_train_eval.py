@@ -7,7 +7,7 @@ Arms, alternated round by round on the same model start and 16 ring cameras (ran
   autograd tests/flame_reference.AtenFlameArm: ATen softmax expansion, shim rasterizer, fused loss, torch.optim.Adam (11 groups).
 The driver is tests/flame_driver.SyntheticFlame (FLAME-shaped LBS).  Prints one JSON line: ms/step of both arms (median over
 rounds), library launches per native step, the driver's share of the native step (its forward + backward alone, timed
-with CUDA events), and the expand_fwd / expand_bwd spans inside the native step with expand_wide = 0 and 2."""
+with CUDA events), and the expand_fwd / expand_bwd spans inside the native step."""
 import argparse
 import json
 import os
@@ -78,15 +78,12 @@ def main():
     t.adam.zero_grad()
     spans = {}
     _lib.set_option("time_kernels", 1)
-    for wide in (0, 2):
-        old = _lib.set_option("expand_wide", wide)
-        timed(lambda i: t.step(cams[i % 16], gts[i % 16]), 3)
-        _lib.kernel_times(reset=True)
-        timed(lambda i: t.step(cams[i % 16], gts[i % 16]), a.steps)
-        kt = _lib.kernel_times(reset=True)
-        for k in ("expand_fwd", "expand_bwd"):
-            spans[f"{k}_ms_wide{wide}"] = round(kt[k][0] / kt[k][1], 4)
-        _lib.set_option("expand_wide", old)
+    timed(lambda i: t.step(cams[i % 16], gts[i % 16]), 3)
+    _lib.kernel_times(reset=True)
+    timed(lambda i: t.step(cams[i % 16], gts[i % 16]), a.steps)
+    kt = _lib.kernel_times(reset=True)
+    for k in ("expand_fwd", "expand_bwd"):
+        spans[f"{k}_ms"] = round(kt[k][0] / kt[k][1], 4)
     _lib.set_option("time_kernels", 0)
     nm = statistics.median(nat)
     print(json.dumps(dict(F=m.faces.shape[0], K=a.K, P=m.P, width=W, height=H, cameras=16, native_ms_per_step=round(nm, 3),
