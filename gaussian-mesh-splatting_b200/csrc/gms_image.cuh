@@ -34,6 +34,25 @@ k_image_quantize(const float* __restrict__ chw, uint8_t* __restrict__ out, int C
     for (int c = 0; c < C; c++) px[c] = gms_quantize_u8(chw[c * HW + pix]);
 }
 
+// The remote viewer's byte (train.py:72-74): `(torch.clamp(img, 0, 1) * 255).byte()` as ATen computes it on the device.
+// clamp keeps NaN (ATen's clamp kernel returns a NaN input as is), one rounded multiply, then c10's float -> uint8 cast,
+// which goes through int64: the conversion truncates toward zero and turns NaN into 0.  Unlike gms_quantize_u8 nothing is
+// rounded, so 0.999 gives 254, not 255.
+__device__ __forceinline__ uint8_t gms_clamp_u8(float x) {
+    const float c = isnan(x) ? x : fminf(fmaxf(x, 0.0f), 1.0f);
+    return (uint8_t)(long long)__fmul_rn(c, 255.0f);
+}
+
+// one thread per pixel: reads C coalesced planes, writes the pixel's C bytes of the packed [H,W,C] image
+__global__ void __launch_bounds__(256)
+k_image_clamp_u8(const float* __restrict__ chw, uint8_t* __restrict__ hwc, int C, int H, int W) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+    if (x >= W) return;
+    const size_t HW = (size_t)H * W, pix = (size_t)y * W + x;
+    uint8_t* px = hwc + pix * C;
+    for (int c = 0; c < C; c++) px[c] = gms_clamp_u8(chw[c * HW + pix]);
+}
+
 __global__ void __launch_bounds__(256)
 k_image_dequantize(const uint8_t* __restrict__ src, int src_is_hwc, float* __restrict__ chw, int C, int H, int W) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;

@@ -458,6 +458,12 @@ int gms_image_quantize(const float* chw, uint8_t* out, int32_t C, int32_t H, int
     return launch("image_quantize", -1, 0, st, dim3((W + 255) / 256, H), 256, 0, k_image_quantize, chw, out, C, H, W, row_prefix);
 }
 
+int gms_image_clamp_u8(const float* chw, uint8_t* hwc, int32_t C, int32_t H, int32_t W, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!chw || !hwc || C <= 0 || C > 4 || H <= 0 || H > 65535 || W <= 0) return set_err(GMS_E_ARG, "gms_image_clamp_u8: bad arguments%s%s");
+    return launch("image_clamp_u8", -1, 0, st, dim3((W + 255) / 256, H), 256, 0, k_image_clamp_u8, chw, hwc, C, H, W);
+}
+
 int gms_image_dequantize(const uint8_t* src, int32_t src_is_hwc, float* chw, int32_t C, int32_t H, int32_t W, void* cuda_stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (!src || !chw || C <= 0 || C > 4 || H <= 0 || W <= 0) return set_err(GMS_E_ARG, "gms_image_dequantize: bad arguments%s%s");

@@ -311,7 +311,7 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_expand_backward", "gms_last_error", "gms_version", "gms_launch_count", "gms_set_option",
                "gms_kernel_times", "gms_loss_scratch_bytes", "gms_l1_ssim_loss", "gms_adam_step",
                "gms_frame_workspace_bytes", "gms_train_frame", "gms_points_expand_forward",
-               "gms_points_prepare_vertices", "gms_image_quantize", "gms_image_dequantize", "gms_adam_sh_factored", "gms_frame_views",
+               "gms_points_prepare_vertices", "gms_image_quantize", "gms_image_clamp_u8", "gms_image_dequantize", "gms_adam_sh_factored", "gms_frame_views",
                "gms_render_workspace_bytes", "gms_render_frame", "gms_metrics_scratch_bytes", "gms_image_metrics",
                "gms_points_render_workspace_bytes", "gms_points_render_frame", "gms_pseudomesh_bind_scratch_bytes",
                "gms_pseudomesh_bind", "gms_pseudomesh_repose", "gms_bound_points_render_workspace_bytes",
@@ -364,6 +364,7 @@ def lib():
     L.gms_points_expand_forward.argtypes = [C.POINTER(PointsArgs), C.c_void_p]
     L.gms_points_prepare_vertices.argtypes = [C.POINTER(PointsVerticesArgs), C.c_void_p]
     L.gms_image_quantize.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+    L.gms_image_clamp_u8.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     L.gms_image_dequantize.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     L.gms_image_composite_rgba.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     L.gms_image_resize_u8.argtypes = [C.POINTER(ResizeArgs), C.c_void_p]

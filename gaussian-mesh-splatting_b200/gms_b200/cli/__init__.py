@@ -17,4 +17,8 @@ and the reference's scripts/ for trained models (gs_multi_mesh and gs_flame rend
     python -m gms_b200.cli.edit_pseudomesh             --triangle_soup_path ... --save_dir ...
                                                                           scripts/edit_pseudomesh_based_on_estimated_mesh.py
 
+and the server side of the SIBR remote viewer (renderer/gaussian_renderer/network_gui.py) for a trained model:
+
+    python -m gms_b200.cli.view                        -m <output> [--ip 127.0.0.1] [--port 6009]
+
 Each module has main(argv), which the tests call in-process."""

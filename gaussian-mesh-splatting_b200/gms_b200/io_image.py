@@ -109,6 +109,22 @@ def quantize(image: torch.Tensor, out: Optional[torch.Tensor] = None, row_prefix
     return out
 
 
+def clamp_u8(image: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """float32 [C,H,W] CUDA -> uint8 [H,W,C] = (clamp(image, 0, 1) * 255).byte().permute(1, 2, 0), bit for bit, in one
+    kernel on the current stream (gms_image_clamp_u8: truncates where quantize rounds)."""
+    if not (image.is_cuda and image.dtype == torch.float32 and image.is_contiguous() and image.dim() == 3):
+        raise RuntimeError("io_image.clamp_u8: contiguous float32 [C,H,W] CUDA tensor required")
+    Cn, H, W = image.shape
+    if out is None:
+        out = torch.empty((H, W, Cn), dtype=torch.uint8, device=image.device)
+    if not (out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (H, W, Cn) and out.device == image.device):
+        raise RuntimeError(f"io_image.clamp_u8: out must be a contiguous uint8 [{H},{W},{Cn}] tensor on {image.device}")
+    with torch.cuda.device(image.device):
+        _lib.check(_lib.lib().gms_image_clamp_u8(image.data_ptr(), out.data_ptr(), Cn, H, W,
+                                                 torch.cuda.current_stream(image.device).cuda_stream), "gms_image_clamp_u8")
+    return out
+
+
 def to_device_float(image_u8: torch.Tensor, out: Optional[torch.Tensor] = None, hwc: bool = True) -> torch.Tensor:
     """uint8 CUDA image ([H,W,C] if hwc else [C,H,W]) -> float [C,H,W] = byte / 255, one kernel on the current stream."""
     if not image_u8.is_cuda or image_u8.dtype != torch.uint8:

@@ -812,6 +812,11 @@ int gms_lpips_vgg(const gms_lpips_args* a, void* cuda_stream);
  * torchvision.utils.save_image (scripts/render_time_animated.py:86-87, scripts/render.py) in one pass.  Output row stride is
  * row_prefix + W*C bytes; row_prefix = 1 reserves PNG's filter byte (written 0), 0 gives plain HWC (PPM / raw video). */
 int gms_image_quantize(const float* chw, uint8_t* out, int32_t C, int32_t H, int32_t W, int32_t row_prefix, void* cuda_stream);
+/* float [C,H,W] -> uint8 [H,W,C], byte = (uint8)(int64)(clamp(x, 0, 1) * 255): the bytes of the remote viewer's
+ * `(torch.clamp(img, 0, 1) * 255).byte().permute(1, 2, 0).contiguous()` (train.py:72-74) on the device, bit for bit, NaN
+ * and +-inf included.  It truncates where gms_image_quantize rounds.  Bad sizes (C outside 1..4, H outside 1..65535,
+ * W < 1) or a null pointer are GMS_E_ARG, returned without a launch.  Caller's stream, no host synchronisation. */
+int gms_image_clamp_u8(const float* chw, uint8_t* hwc, int32_t C, int32_t H, int32_t W, void* cuda_stream);
 /* 8-bit image ([H,W,C] if src_is_hwc else [C,H,W]) -> float [C,H,W] = byte / 255 (ToTensor / PILtoTorch,
  * utils/general_utils.py:105-112): ground-truth images can stay 8-bit on the host and on the device. */
 int gms_image_dequantize(const uint8_t* src, int32_t src_is_hwc, float* chw, int32_t C, int32_t H, int32_t W, void* cuda_stream);
