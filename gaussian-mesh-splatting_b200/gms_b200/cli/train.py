@@ -8,14 +8,30 @@ gs_multi_mesh trains on a COLMAP scene with --meshes a b ... (sparse/0/<name>.ob
 (NativeFlame, FlameTrainer).  One iteration, in train.py's order
 (train.py:61-157):
 
-    SH degree up every 1000 -> the view from the Scene's view order -> background (torch.rand(3) on the device under
-    --random_background) -> the one-call training frame -> training_report at --test_iterations -> Scene.save at
+    [--viewer: the remote viewer's requests] -> SH degree up every 1000 -> the view from the Scene's view order ->
+    background (torch.rand(3) on the device under --random_background) -> the one-call training frame -> training_report at --test_iterations -> Scene.save at
     --save_iterations -> densify / opacity reset (gs, gs_flat) -> Adam on every iteration but the last -> checkpoint at
     --checkpoint_iterations.
 
 The report and the save run inside the trainer's `before_update` callback, so they see the parameters after N-1 updates,
 as the reference's do.  The loop itself never synchronises with the host: the loss reaches the progress display's moving
 average through pinned host slots and CUDA events that are polled, not waited on.
+
+Remote viewer, opt-in with --viewer (train.py:65-79 with network_gui.init, which the reference leaves commented out):
+--ip / --port are bound before the output folder is written (--port 0 binds a free port, printed and held in
+Training.viewer.address; an address that cannot be bound is an error naming it), and the listener and any connection are
+closed when run() returns or raises.  At the very top of every iteration a waiting SIBR viewer is accepted (one at a
+time) and its requests are answered (network_gui.serve_iteration) until one says `train` and (the iteration is not the
+last, or not `keep_alive`): a viewer that sends `train: false` pauses the run, and `keep_alive` holds the last iteration.
+A frame shows the parameters after N-1 updates at iteration N-1's active SH degree, with the fixed background (also
+under --random_background) and the request's scaling modifier; the verify string is the absolute source path.  A paused
+iteration draws no view, no background and no random number, so pausing does not change the run; iter_time and the loss
+display do not include viewer time.  A frame is cli.view's (view.Frames) on the trainer's live model: gs_mesh and
+gs_multi_mesh expanded from the raw parameters Adam updates in place; gs and gs_flat at the current Gaussian count (a
+renderer sized before a densification is replaced); gs_flame at its current FLAME parameters, one FLAME forward and one
+expansion per frame, drawn as cli.view draws a checkpoint saved at that moment.  Each frame costs one host
+synchronisation; a run with --viewer and no viewer connected synchronises no more than one without it.  Without
+--viewer no socket is opened.
 
 TensorBoard, as prepare_output_and_logger / training_report (train.py:174-223): when torch.utils.tensorboard imports, a
 SummaryWriter(model_path) gets every iteration's train_loss_patches/l1_loss, train_loss_patches/total_loss and iter_time
@@ -42,8 +58,8 @@ Deliberate differences:
     the SH Adam step the frame fuses into the preprocess backward (and for gs_flame the FLAME forward and backward); the
     reference's window holds render, loss and backward only.  The writer is closed when run() returns or raises.
   * Not built, refused by name: --antialiasing, --debug, --debug_from, --detect_anomaly,
-    --convert_SHs_python, --compute_cov3D_python, --save_xyz, --data_device other than cuda.  --ip / --port are accepted and
-    ignored (the reference does not start its viewer either)."""
+    --convert_SHs_python, --compute_cov3D_python, --save_xyz, --data_device other than cuda.  --ip / --port are only read
+    under --viewer (the reference does not start its viewer at all)."""
 from __future__ import annotations
 
 import collections
@@ -60,7 +76,7 @@ from typing import List
 import numpy as np
 import torch
 
-from .. import dataset, io_ply
+from .. import _lib, dataset, expansion, io_ply, network_gui
 from ..model import FlameGaussianModel, FreeGaussianModel, MeshGaussianModel, MultiMeshGaussianModel
 from ..scenes import MeshGaussianParams
 from ..trainer import FlameOptimizationParams, FlameTrainer, FreeOptimizationParams, FreeTrainer, MeshTrainer
@@ -97,6 +113,8 @@ def build_parser(gs_type: str) -> ArgumentParser:
     p.add_argument("--seed", type=int, default=0, help="seeds the view shuffle and order, the initial model and the backgrounds")
     p.add_argument("--flame_model", type=str, default=dataset.DEFAULT_FLAME_MODEL,
                    help="gs_flame: FLAME's model file (FlameConfig's path, relative to the working directory)")
+    p.add_argument("--viewer", action="store_true", default=False,
+                   help="serve the SIBR remote viewer on --ip / --port while training (train.py's network_gui loop)")
     return p
 
 
@@ -287,6 +305,41 @@ def _mesh_params(p: MeshGaussianParams, sh_degree: int) -> MeshGaussianParams:
     return MeshGaussianParams(p.vertices, p.faces, p._alpha, p._scale, p._features_dc, rest, p._opacity)
 
 
+class LiveFlame:
+    """What FlameRenderer draws of a FlameCheckpoint, at a gs_flame training model's current parameters.  refresh() does on
+    the device what save_flame_model does before it writes: the driver at the current FLAME tensors into model.vertices,
+    then the expansion's activated weights and raw scaling / rotation rows at that pose.  A frame drawn after it is the
+    frame cli.view draws from a checkpoint saved at that moment.  (The next FlameTrainer.step runs the driver again before
+    it reads model.vertices.)"""
+
+    def __init__(self, model):
+        self.model, self.faces, self._vertices_enlargement = model, model.faces, model._vertices_enlargement
+        self.vertices = self.alpha = self._scaling = self._rotation = None
+
+    @property
+    def active_sh_degree(self) -> int:
+        return self.model.active_sh_degree
+
+    @property
+    def P(self) -> int:
+        return self.model.P
+
+    @property
+    def _features(self) -> torch.Tensor:
+        return self.model._features.detach()
+
+    @property
+    def _opacity(self) -> torch.Tensor:
+        return self.model._opacity.detach()
+
+    def refresh(self) -> None:
+        m = self.model
+        self.vertices = m.refresh_vertices()
+        _, self._scaling, self._rotation, self.alpha, _ = expansion.expand(
+            self.vertices, m.faces, m._alpha.detach(), m._scales.detach(), m.eps_s0, activated=False,
+            alpha_activation=_lib.ALPHA_SOFTMAX)
+
+
 class _Progress:
     def __init__(self, first: int, last: int, quiet: bool):
         self.bar = None
@@ -311,7 +364,8 @@ class Training:
     """One train.py run: prepare() builds the output directory, the TensorBoard writer, scene, model and trainer (and
     restores --start_checkpoint); run() iterates.  Attributes the tests read: trainer, model, scene, order (ViewOrder), ema
     (per consumed iteration: (iteration, loss, moving average)), reports ((iteration, split, L1, PSNR)), events (per
-    iteration: iteration_events), tb_writer (None without TensorBoard; closed once run() ends)."""
+    iteration: iteration_events), tb_writer (None without TensorBoard; closed once run() ends), viewer
+    (network_gui.TrainingViewer under --viewer, else None; closed once run() ends)."""
 
     LOSS_SLOTS = 64
 
@@ -322,6 +376,7 @@ class Training:
         self.first_iter = 0
         self.scene = scene
         self.tb_writer = None
+        self.viewer = None
 
     def log(self, msg: str) -> None:
         if not self.args.quiet:
@@ -331,15 +386,23 @@ class Training:
     def prepare(self) -> "Training":
         a = self.args
         set_default_model_path(a)
-        self.log(f"Output folder: {a.model_path}")
-        os.makedirs(a.model_path, exist_ok=True)
-        with open(os.path.join(a.model_path, "cfg_args"), "w") as f:
-            f.write(options.cfg_args_string(a))
-        self.tb_writer = open_summary_writer(a.model_path, self.log)
+        if getattr(a, "viewer", False):         # network_gui.init comes before training() in train.py
+            self.viewer = network_gui.TrainingViewer(a.ip, a.port, os.path.abspath(a.source_path).encode("utf-8"), log=self.log)
+            ip, port = self.viewer.address
+            self.log(f"Serving the remote viewer on {ip}:{port}")
         try:
-            return self._setup()
+            self.log(f"Output folder: {a.model_path}")
+            os.makedirs(a.model_path, exist_ok=True)
+            with open(os.path.join(a.model_path, "cfg_args"), "w") as f:
+                f.write(options.cfg_args_string(a))
+            self.tb_writer = open_summary_writer(a.model_path, self.log)
+            self._setup()
+            if self.viewer is not None:
+                self.viewer.draw = self.viewer_frames()
+            return self
         except BaseException:
             self.close_writer()
+            self.close_viewer()
             raise
 
     def _setup(self) -> "Training":
@@ -405,6 +468,21 @@ class Training:
     def close_writer(self) -> None:
         if self.tb_writer is not None:
             self.tb_writer.close()
+
+    def close_viewer(self) -> None:
+        if self.viewer is not None:
+            self.viewer.close()
+
+    def viewer_frames(self):
+        """cli.view's Frames on the trainer's live model, with the fixed background."""
+        from ..render import FlameRenderer, NativeFreeRenderer, NativeRenderer
+        from .view import Frames
+        if self.args.gs_type in MESH_TYPES:
+            return Frames(self.model, NativeRenderer, self.bg)
+        if self.args.gs_type == "gs_flame":
+            live = LiveFlame(self.model)
+            return Frames(live, FlameRenderer, self.bg, refresh=live.refresh)
+        return Frames(self.model, NativeFreeRenderer, self.bg)
 
     # ---- what happens at an iteration besides the frame
     def report(self, it: int) -> None:
@@ -483,6 +561,7 @@ class Training:
             self._loop()
         finally:
             self.close_writer()
+            self.close_viewer()
         self.log("\nTraining complete.")
         return self
 
@@ -499,6 +578,9 @@ class Training:
         mesh = a.gs_type in MESH_TYPES
         stream = torch.cuda.current_stream(dev)
         for it in range(self.first_iter + 1, a.iterations + 1):
+            if self.viewer is not None:
+                with torch.no_grad():
+                    self.viewer.poll(it, a.iterations)
             ev = iteration_events(it, a)
             self.events.append((it, ev))
             if mesh and it % 1000 == 0:
@@ -536,7 +618,11 @@ def main(argv=None) -> Training:
     args = parse_args(sys.argv[1:] if argv is None else argv)
     if not torch.cuda.is_available():
         raise RuntimeError("gms_b200.cli.train needs a CUDA device")
-    return Training(args).prepare().run()
+    try:
+        run = Training(args).prepare()
+    except network_gui.AddressError as e:
+        sys.exit(f"gms_b200.cli.train: error: {e}")
+    return run.run()
 
 
 if __name__ == "__main__":

@@ -35,12 +35,18 @@ def build_parser() -> ArgumentParser:
 
 
 class Frames:
-    """draw(camera, scaling_modifier) for network_gui.serve: the frame's uint8 [H,W,3] bytes, in a pinned host buffer
-    that the next call at the same size overwrites."""
+    """draw(camera, scaling_modifier) for network_gui.serve and serve_iteration: the frame's uint8 [H,W,3] bytes, in a
+    pinned host buffer that the next call at the same size overwrites.
+
+    The renderers read the model's tensors at every frame, so a model that changes between frames (a training run's,
+    updated in place) is drawn as it is at the call.  A renderer sized for another Gaussian count than the model's (after
+    densification) is replaced before it draws.  `refresh`, when given, is called before each frame to bring the model
+    up to date (cli.train's gs_flame pose)."""
     SIZES = 4       # renderers kept, least recently used dropped first: resizing a viewer window asks for many sizes
 
-    def __init__(self, model, renderer_cls, bg: torch.Tensor, antialiasing: bool = False):
+    def __init__(self, model, renderer_cls, bg: torch.Tensor, antialiasing: bool = False, refresh=None):
         self.model, self.renderer_cls, self.bg, self.antialiasing = model, renderer_cls, bg, bool(antialiasing)
+        self.refresh = refresh
         self.dev = bg.device
         self.sizes = collections.OrderedDict()     # (W, H) -> (renderer, device bytes [H,W,3], pinned host bytes [H,W,3])
         self._cam_host = torch.empty(35, dtype=torch.float32).pin_memory()
@@ -49,7 +55,7 @@ class Frames:
     def _slot(self, width: int, height: int):
         key = (width, height)
         slot = self.sizes.get(key)
-        if slot is None:
+        if slot is None or slot[0].stale:
             slot = (self.renderer_cls(self.model, width, height),
                     torch.empty(height, width, 3, dtype=torch.uint8, device=self.dev),
                     torch.empty(height, width, 3, dtype=torch.uint8).pin_memory())
@@ -60,6 +66,8 @@ class Frames:
         return slot
 
     def __call__(self, cam: network_gui.MiniCam, scaling_modifier: float) -> memoryview:
+        if self.refresh is not None:
+            self.refresh()
         r, dev_u8, host_u8 = self._slot(int(cam.image_width), int(cam.image_height))
         self._cam_host.copy_(cam.packed())      # the previous frame's upload finished before its read-back
         self._cam_dev.copy_(self._cam_host, non_blocking=True)

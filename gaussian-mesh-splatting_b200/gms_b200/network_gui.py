@@ -14,6 +14,15 @@ both float32, plus `tanfovx` / `tanfovy` = tan(fov * 0.5) as render() computes t
 
 `serve` runs one session on an already-connected socket-like object; gms_b200.cli.view owns the listener and the frames.
 
+The training side (train.py:65-79, `cli.train --viewer`): `listen` binds the listener once, non-blocking as `init` leaves
+it; at the top of every iteration `TrainingViewer.poll` accepts a waiting viewer when none is connected (`try_connect`,
+at most one) and then runs `serve_iteration`, the reference's loop for that iteration: while the viewer stays connected,
+read a request, draw its camera when it has one, send the reply, and release the iteration only when the request says
+`train` and (iteration < iterations or not `keep_alive`).  A zero-resolution request gets the verify string and does not
+release the iteration (the reference's `do_training` is None there); so the last iteration is held for as long as the
+viewer asks to keep it alive.  Any error -- a malformed request, a dropped peer, a failed frame -- drops the connection,
+and training continues.
+
 Deliberate differences from the reference:
   * `read` waits for exactly the announced number of bytes; the reference calls recv once and can act on a short read
     of a large request.  A request longer than MAX_REQUEST bytes is refused.
@@ -22,7 +31,9 @@ Deliberate differences from the reference:
   * the verify string is sent as UTF-8 (the reference's ASCII for an ASCII path; the reference cannot answer at all when
     the path is not ASCII).
   * `shs_python` and `rot_scale_python` only move the same computation into Python in the reference, so they are parsed
-    and ignored; `train` and `keep_alive` steer a training loop and are parsed and ignored too.
+    and ignored; `train` and `keep_alive` steer a training loop (serve_iteration) and are ignored by `serve`.
+  * a dropped connection is closed at once; the reference drops its reference to it and leaves the close to the
+    garbage collector.
 A request that is not valid JSON, lacks a key the reference reads, or has a negative or non-integer resolution ends its
 session, as the reference's `conn = None` does, and so does a peer that goes away; the listener then waits for the next
 viewer."""
@@ -30,6 +41,7 @@ from __future__ import annotations
 
 import json
 import math
+import socket
 import traceback
 from dataclasses import dataclass
 from typing import Callable, Optional
@@ -175,3 +187,85 @@ def request(conn, message: dict) -> tuple:
     w, h = message["resolution_x"], message["resolution_y"]
     image = recv_exact(conn, w * h * 3) if w and h else None
     return image, recv_exact(conn, int.from_bytes(recv_exact(conn, 4), "little"))
+
+
+class AddressError(OSError):
+    """The listener's address cannot be bound."""
+
+
+def listen(ip: str, port: int) -> socket.socket:
+    """network_gui.init: a TCP listener bound to (ip, port) and listening, with settimeout(0) so that accept never waits.
+    Port 0 binds a free port (getsockname() names it).  An address that cannot be bound -- a busy port, an address of no
+    interface -- raises AddressError naming it."""
+    listener = socket.socket(socket.AF_INET, socket.SOCK_STREAM)
+    try:
+        listener.setsockopt(socket.SOL_SOCKET, socket.SO_REUSEADDR, 1)
+        listener.bind((ip, port))
+        listener.listen()
+        listener.settimeout(0)
+    except OSError as e:
+        listener.close()
+        raise AddressError(f"cannot listen for the remote viewer on {ip}:{port}: {e.strerror or e}") from None
+    return listener
+
+
+def try_connect(listener, log: Callable[[str], None] = print):
+    """network_gui.try_connect: the connection of a viewer waiting on `listener` (blocking from now on), or None when no
+    viewer waits."""
+    try:
+        conn, addr = listener.accept()
+    except OSError:         # BlockingIOError: nobody waits
+        return None
+    log(f"\nConnected by {addr}")
+    conn.settimeout(None)
+    return conn
+
+
+def serve_iteration(conn, draw: Callable[[MiniCam, float], object], verify: bytes, iteration: int, iterations: int,
+                    log: Callable[[str], None] = print) -> tuple:
+    """train.py:66-79 at one iteration: answers the viewer on `conn` (None: no viewer, return at once) until a request
+    releases the iteration -- `train` and (iteration < iterations or not `keep_alive`) -- or the connection drops, which
+    closes it.  draw(camera, scaling_modifier) returns a frame's bytes, as for `serve`.  Returns (conn, or None once
+    dropped; the number of frames sent)."""
+    frames = 0
+    while conn is not None:
+        try:
+            req = parse(read(conn))
+            image = None if req.camera is None else draw(req.camera, req.scaling_modifier)
+            send(conn, image, verify)
+            frames += req.camera is not None
+            if req.train and (iteration < iterations or not req.keep_alive):
+                break
+        except Exception as e:      # train.py:78-79: conn = None, and training goes on
+            if isinstance(e, OSError):
+                log(f"viewer disconnected at iteration {iteration}")
+            else:
+                log(f"closing the viewer's connection at iteration {iteration}:\n{traceback.format_exc()}")
+            conn.close()
+            conn = None
+    return conn, frames
+
+
+class TrainingViewer:
+    """The viewer of a training run: the listener `listen` binds, at most one connection, and poll() for the top of
+    every iteration.  `draw` (set once the model exists) and `verify` are serve_iteration's.  `frames` counts the frames
+    sent over the run."""
+
+    def __init__(self, ip: str, port: int, verify: bytes, log: Callable[[str], None] = print):
+        self.listener = listen(ip, port)
+        self.address = self.listener.getsockname()[:2]
+        self.verify, self.log = verify, log
+        self.conn, self.draw, self.frames = None, None, 0
+
+    def poll(self, iteration: int, iterations: int) -> None:
+        """train.py:65-79: try_connect when no viewer is connected, then serve_iteration."""
+        if self.conn is None:
+            self.conn = try_connect(self.listener, self.log)
+        self.conn, n = serve_iteration(self.conn, self.draw, self.verify, iteration, iterations, self.log)
+        self.frames += n
+
+    def close(self) -> None:
+        if self.conn is not None:
+            self.conn.close()
+            self.conn = None
+        self.listener.close()

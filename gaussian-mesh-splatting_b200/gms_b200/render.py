@@ -65,6 +65,12 @@ class NativeRenderer(SyncFreeCapacity):
     def _workspace_bytes(self, P: int) -> int:
         return _lib.lib().gms_render_workspace_bytes(P, self.W, self.H)
 
+    @property
+    def stale(self) -> bool:
+        """The model no longer has the Gaussian count this renderer was sized for (densification changed it): a new
+        renderer has to draw it."""
+        return self._adopt(self.model)[1] != self.radii.shape[0]
+
     def _features(self) -> torch.Tensor:
         m = self.model
         f = m._features if m._features is not None else m.get_features      # packed SH: zero-copy
