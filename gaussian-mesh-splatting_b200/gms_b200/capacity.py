@@ -64,6 +64,7 @@ class SyncFreeCapacity:
         self._view_n = {}                       # view key -> (N at the last visit, N at the visit before)
         self._n_max, self._n_last, self._frame_no = 0, 0, 0
         self.overflows = 0
+        self._epoch, self._view_epoch = 0, {}     # frames of a view learn N once per epoch after _forget_views (epoch > 0)
 
     @property
     def last_num_rendered(self) -> int:
@@ -125,28 +126,42 @@ class SyncFreeCapacity:
         self._note(key, n)
         self.capacity = n
 
-    def _check_view(self, cam, bg, where: str = None, gt=None, gt_fits: bool = True) -> None:
-        """The camera, background (and ground truth) of a frame are float32 on the frame's device, at its image size;
-        `where` names the caller in the messages (default: the class)."""
+    def _forget_views(self) -> None:
+        """The frame changed (its Gaussian count or its workspace size): every view's next frame learns its N with one
+        read-back."""
+        self._harvest()
+        self._epoch += 1
+        self._view_n.clear()
+        self._n_max = 0
+
+    up_to = False       # True: self.W x self.H is the largest view; smaller views run at their own size (training frames)
+
+    def _check_view(self, cam, bg, where: str = None, gt=None, gt_fits=None) -> None:
+        """The camera, background (and ground truth) of a frame are float32 on the frame's device, at its image size (up_to:
+        at most its image size); gt_fits(W, H), when given, tells whether the ground truth is the camera's W x H.  `where`
+        names the caller in the messages (default: the class)."""
         owner = type(self).__name__
         where = where or owner
         for t, what in (() if gt is None else ((gt, "gt"),)) + ((bg, "bg"), (cam.world_view_transform, "camera matrices"),
                                                                (cam.full_proj_transform, "camera matrices"), (cam.camera_center, "camera centre")):
             if not t.is_cuda or t.device != self.dev or t.dtype != torch.float32:
                 raise RuntimeError(f"{where}: {what} must be float32 on {self.dev}")
-        if int(cam.image_width) != self.W or int(cam.image_height) != self.H or not gt_fits:
-            raise ValueError(f"{owner} was sized for {self.W}x{self.H}; got a {cam.image_width}x{cam.image_height} camera")
+        W, H = int(cam.image_width), int(cam.image_height)
+        fits = W <= self.W and H <= self.H if self.up_to else (W, H) == (self.W, self.H)
+        if not fits or (gt_fits is not None and not gt_fits(W, H)):
+            sized = f"for views up to {self.W}x{self.H}" if self.up_to else f"for {self.W}x{self.H}"
+            raise ValueError(f"{owner} was sized {sized}; got a {cam.image_width}x{cam.image_height} camera")
 
     def _launch(self, fn: str, a, cam, bg, scale_modifier: float = 1.0, antialiasing: bool = False, capacity: int = None,
-                n_host: int = None, relearn: bool = False) -> bool:
+                n_host: int = None) -> bool:
         """Fills the settings, workspace, num_rendered and capacity fields every one-call frame's args struct shares and
         calls `fn` on the current stream.  With `capacity` (and the mapped (N, flag) address `n_host`) the frame is sync-free
-        at that capacity.  Otherwise the frame is synchronising when it has to learn N (the first frame, or `relearn`) or
-        the frames are not sync-free, and sync-free on the next ring slot at the view's predicted capacity else.  Returns
-        whether the frame learned N."""
+        at that capacity.  Otherwise the frame is synchronising when it has to learn N (the first frame, or the view's first
+        frame since _forget_views) or the frames are not sync-free, and sync-free on the next ring slot at the view's
+        predicted capacity else.  The image size is the camera's.  Returns whether the frame learned N."""
         from . import _lib
         s = a.settings
-        s.image_height, s.image_width, s.tanfovx, s.tanfovy = self.H, self.W, cam.tanfovx, cam.tanfovy
+        s.image_height, s.image_width, s.tanfovx, s.tanfovy = int(cam.image_height), int(cam.image_width), cam.tanfovx, cam.tanfovy
         s.bg, s.scale_modifier = bg.data_ptr(), float(scale_modifier)
         s.viewmatrix, s.projmatrix, s.campos = cam.world_view_transform.data_ptr(), cam.full_proj_transform.data_ptr(), cam.camera_center.data_ptr()
         s.sh_degree, s.prefiltered, s.debug, s.antialiasing = self.model.active_sh_degree, 0, 0, int(bool(antialiasing))
@@ -155,6 +170,7 @@ class SyncFreeCapacity:
         learn = False
         if capacity is None:
             key = self._view_key(cam)
+            relearn = self._epoch > 0 and self._view_epoch.get(key) != self._epoch
             learn = self.sync_free and (self.capacity == 0 or relearn)
             if self.sync_free and not learn:
                 n_host = self._sync_free_slot(key, self.dev)
@@ -164,4 +180,5 @@ class SyncFreeCapacity:
             _lib.check(getattr(_lib.lib(), fn)(C.byref(a), self._cb, None, torch.cuda.current_stream(self.dev).cuda_stream), fn)
         if learn:           # the synchronising frame told us N
             self._learned_first(key)
+            self._view_epoch[key] = self._epoch
         return learn

@@ -42,6 +42,11 @@ test iteration), the split's loss_viewpoint - l1_loss / - psnr, scene/opacity_hi
 event per iteration, once the slot's events have completed.  TensorBoard's writer spends its host time per event (a
 protobuf, a checksum in Python, a file append), so one event for the three values costs a third of three add_scalar calls.
 
+Views may differ in size, as the reference's cameras each carry their own (a COLMAP scene with several cameras, or source
+images of different sizes before -r rescales them): the trainer's one frame is sized for the largest training width and
+height and runs every view at the view's own size, training_report scores each size through its own renderer (the split
+means average the per-view values in float64) and its TensorBoard images are each at their view's size.
+
 Deliberate differences:
   * chkpnt<N>.pth holds (state, N) with the library's own state (the trainer's state_dict(), the view-order stream and the
     background generator), not the reference's capture() tuple; a resumed run continues the uninterrupted run's sequence of
@@ -288,6 +293,13 @@ def add_scalars_event(writer, step: int, pairs) -> None:
     writer.file_writer.add_summary(Summary(value=[Summary.Value(tag=t, simple_value=float(v)) for t, v in pairs]), step)
 
 
+def training_size(scene: dataset.Scene):
+    """(largest width, largest height) of the training views: the one frame of a run is sized for it and runs every
+    training view at the view's own size."""
+    cams = scene.train_cameras
+    return max(int(c.image_width) for c in cams), max(int(c.image_height) for c in cams)
+
+
 def report_configs(scene: dataset.Scene):
     """training_report's validation configs: (name, cameras, resident images, image names) of the test views and of train
     views 5, 10, ..., 25 taken mod n."""
@@ -415,9 +427,7 @@ class Training:
         if a.gs_type != "gs_flame":
             write_input_ply(os.path.join(a.model_path, "input.ply"), sc, a.source_path, a.gs_type, a.seed)
         write_cameras_json(os.path.join(a.model_path, "cameras.json"), sc, a.seed)
-        sizes = {(c.image_width, c.image_height) for c in sc.train_cameras + sc.test_cameras}
-        if len(sizes) > 1:
-            raise ValueError(f"training needs every view at one size; this scene has {sorted(sizes)} (-r sets a common width)")
+        max_size = training_size(sc)
         self.bg = torch.tensor([1.0, 1.0, 1.0] if a.white_background else [0.0, 0.0, 0.0], dtype=torch.float32, device=self.dev)
         self.bg_gen = torch.Generator(device=self.dev).manual_seed(a.seed) if a.random_background else None
         if a.gs_type in MESH_TYPES:
@@ -427,7 +437,7 @@ class Training:
             else:
                 self.model = MultiMeshGaussianModel.from_mesh_params([_mesh_params(p, a.sh_degree) for p in sc.meshes], self.dev,
                                                                      sh_degree=a.sh_degree, active_sh_degree=0, packed_features=True)
-            tr = self.trainer = MeshTrainer(self.model, self.bg, a.lambda_dssim, native=True)
+            tr = self.trainer = MeshTrainer(self.model, self.bg, a.lambda_dssim, native=True, max_size=max_size)
             lrs = {"vertices": a.vertices_lr, "alpha": a.alpha_lr, "opacity": a.opacity_lr, "scaling": a.scaling_lr}
             for g in tr.opt.groups:         # OptimizationParamsMesh's learning rates (mesh_model_groups' f_rest = f_dc / 20)
                 if g["name"] == "features":
@@ -440,13 +450,13 @@ class Training:
             self.model = FlameGaussianModel.create(self.driver, sc.flame.faces, K=dataset.FLAME_K, sh_degree=a.sh_degree, seed=a.seed,
                                                    device=self.dev)
             io_ply.save_point_cloud(os.path.join(a.model_path, "input.ply"), *dataset.flame_input_cloud(self.model, sc.flame))
-            self.trainer = FlameTrainer(self.model, self.bg, flame_params(a))
+            self.trainer = FlameTrainer(self.model, self.bg, flame_params(a), max_size=max_size)
         else:
             points, colors, _ = sc.point_cloud
             self.model = FreeGaussianModel.from_point_cloud(points, colors, a.gs_type, a.sh_degree, self.dev)
             gen = torch.Generator(device=self.dev).manual_seed(a.seed)
             self.trainer = FreeTrainer(self.model, self.bg, sc.cameras_extent, free_params(a), white_background=a.white_background,
-                                       generator=gen)
+                                       generator=gen, max_size=max_size)
         self.order = ViewOrder(sc)
         if a.start_checkpoint:
             state, self.first_iter = torch.load(a.start_checkpoint, map_location="cpu", weights_only=True)
@@ -508,7 +518,8 @@ class Training:
     def _report_images(self, it: int, name: str, cams, gts, names) -> None:
         """The renders (and, at the first listed test iteration, the ground truth) of up to five views as the float tensors
         the reference hands add_images: TensorBoard's own (x * 255) truncation then gives the reference's PNGs.  The renders
-        come from the renderer evaluate() just built and sized for these views, so none can overflow its capacity."""
+        come from the renderers evaluate() just built for these views (one per image size, each image at its view's size),
+        so none can overflow its capacity."""
         w, r = self.tb_writer, self.trainer.renderer
         for cam, gt, image_name in zip(cams, gts, names):
             image = torch.clamp(r.render(cam, self.trainer.bg)[0], 0.0, 1.0)

@@ -141,17 +141,26 @@ def to_device_float(image_u8: torch.Tensor, out: Optional[torch.Tensor] = None, 
 
 class GroundTruthBuffer:
     """The float [3,H,W] ground truth the loss and metric kernels read, from 8-bit [H,W,3] images (dataset.load_scene's
-    resident views): byte / 255 into ONE reused device buffer per frame or renderer, in stream order."""
+    resident views): byte / 255 into ONE reused device buffer per frame or renderer, in stream order.
 
-    def __init__(self, height: int, width: int, device):
-        self.H, self.W, self.dev = int(height), int(width), torch.device(device)
+    up_to: height x width is the largest image; a smaller [h,w,3] image lands in the buffer's first 3*h*w floats as a
+    contiguous [3,h,w] tensor.  `buf` is the last image's tensor."""
+
+    def __init__(self, height: int, width: int, device, up_to: bool = False):
+        self.H, self.W, self.dev, self.up_to = int(height), int(width), torch.device(device), bool(up_to)
         self.buf = None
+        self._store = None
 
     def __call__(self, gt_u8: torch.Tensor, who: str) -> torch.Tensor:
-        if tuple(gt_u8.shape) != (self.H, self.W, 3):
-            raise ValueError(f"{who}: uint8 ground truth must be [{self.H},{self.W},3]; got {tuple(gt_u8.shape)}")
-        if self.buf is None:
-            self.buf = torch.empty(3, self.H, self.W, dtype=torch.float32, device=self.dev)
+        shape = tuple(gt_u8.shape)
+        fits = len(shape) == 3 and shape[2] == 3 and (shape[0] <= self.H and shape[1] <= self.W if self.up_to
+                                                      else shape[:2] == (self.H, self.W))
+        if not fits:
+            want = f"at most [{self.H},{self.W},3]" if self.up_to else f"[{self.H},{self.W},3]"
+            raise ValueError(f"{who}: uint8 ground truth must be {want}; got {shape}")
+        if self._store is None:
+            self._store = torch.empty(3 * self.H * self.W, dtype=torch.float32, device=self.dev)
+        self.buf = self._store[:3 * shape[0] * shape[1]].view(3, shape[0], shape[1])
         return to_device_float(gt_u8.to(self.dev, non_blocking=True), out=self.buf, hwc=True)
 
 

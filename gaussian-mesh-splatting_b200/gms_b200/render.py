@@ -296,13 +296,46 @@ class MeshBoundPointsRenderer(NativeRenderer):
             self._frame_vertices = None
 
 
-def renderer_for(r, cls, model, cams: Sequence, P: int):
-    """The evaluate() renderer of a trainer: `r` while it fits the cameras' image size and the model's Gaussian count P,
-    else a new cls(model, W, H)."""
-    W, H = int(cams[0].image_width), int(cams[0].image_height)
-    if r is None or (r.W, r.H) != (W, H) or r.radii.shape[0] != P:
-        r = cls(model, W, H)
-    return r
+class RendererSet:
+    """The renderers of one model's views at any image sizes: one cls(model, W, H) per size, made when a view of that size
+    first needs one, all sized for the Gaussian count P they were made at (a trainer makes a new set when P changes)."""
+
+    def __init__(self, cls, model, P: int):
+        self.cls, self.model, self.P = cls, model, int(P)
+        self.by_size = {}
+
+    def for_view(self, cam):
+        """The renderer of `cam`'s image size."""
+        size = (int(cam.image_width), int(cam.image_height))
+        if size not in self.by_size:
+            self.by_size[size] = self.cls(self.model, *size)
+        return self.by_size[size]
+
+    def render(self, cam, bg: torch.Tensor, **kw):
+        """for_view(cam).render(cam, bg, **kw)."""
+        return self.for_view(cam).render(cam, bg, **kw)
+
+    def evaluate(self, cams: Sequence, gts: Sequence[torch.Tensor], bg: torch.Tensor, **kw) -> Evaluation:
+        """NativeRenderer.evaluate over views of any sizes: each size's views through that size's renderer (one host
+        synchronisation per size).  per_view, rerun and lpips are in view order; the mean is per_view's, in float64 on the
+        host."""
+        if len(cams) != len(gts):
+            raise ValueError(f"evaluate: {len(cams)} cameras but {len(gts)} ground-truth images")
+        groups = {}
+        for v, cam in enumerate(cams):
+            groups.setdefault((int(cam.image_width), int(cam.image_height)), []).append(v)
+        if len(groups) <= 1:
+            return self.for_view(cams[0]).evaluate(cams, gts, bg, **kw)
+        per_view = torch.empty(len(cams), len(METRIC_NAMES), dtype=torch.float64)
+        rerun, lpips = [], None
+        for views in groups.values():
+            e = self.for_view(cams[views[0]]).evaluate([cams[v] for v in views], [gts[v] for v in views], bg, **kw)
+            per_view[views] = e.per_view
+            rerun += [views[i] for i in e.rerun]
+            if e.lpips is not None:
+                lpips = torch.empty(len(cams), dtype=torch.float32) if lpips is None else lpips
+                lpips[views] = e.lpips
+        return Evaluation(per_view=per_view, mean=per_view.mean(0), rerun=sorted(rerun), lpips=lpips)
 
 
 def render_points_frame(model, cam, bg: torch.Tensor, triangles: torch.Tensor = None, scale_modifier: float = 1.0,

@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -27,6 +27,7 @@ from .io_image import GroundTruthBuffer
 from .losses import fused_training_loss
 from .model import MeshGaussianModel
 from .optim import FlatAdam, mesh_model_groups
+from .render import NativeFreeRenderer, NativeRenderer, RendererSet
 from .scenes import Camera
 
 
@@ -51,7 +52,38 @@ def render_frame(model: MeshGaussianModel, cam: Camera, bg: torch.Tensor, fused:
                                                       shs=model.get_features, scales=scales, rotations=rots)
 
 
-class NativeFrame(SyncFreeCapacity):
+class _FrameSize(SyncFreeCapacity):
+    """The image sizes a training frame runs.  An exact-size frame (up_to=False) runs W x H views only.  An up_to frame
+    runs every view of at most W x H at the view's own size, in ONE workspace of gms_frame_workspace_bytes(P, W, H):
+    gms_train_frame and gms_free_train_frame lay out the image-sized part of the workspace, the loss scratch and the
+    rasterizer's per-pixel scratch from the size in each call's settings, and each of those layouts for w x h <= W x H
+    fits in the one for W x H (their byte counts grow with w and with h).  The ground truth of a smaller view fills the
+    head of one W x H buffer.  The capacity prediction is per view, so views of different sizes keep their own N."""
+
+    def _init_size(self, width: int, height: int, up_to: bool) -> None:
+        self.W, self.H, self.up_to = int(width), int(height), bool(up_to)
+        self._gt_u8 = GroundTruthBuffer(self.H, self.W, self.dev, up_to=self.up_to)
+
+    def _fit_workspace(self) -> None:
+        """A workspace for the model's current Gaussian count at W x H (kept when it is large enough)."""
+        from . import _lib
+        need = int(_lib.lib().gms_frame_workspace_bytes(self._gaussians(), self.W, self.H))
+        if self.ws is None or self.ws.numel() < need:
+            self.ws = None
+            self.ws = torch.empty(need, dtype=torch.uint8, device=self.dev)
+
+    def grow(self, width: int, height: int) -> None:
+        """Run views of up to max(W, width) x max(H, height) from now on (an up_to frame).  When that is larger, the
+        workspace and the ground-truth buffer grow and every view's next frame learns its N with one read-back."""
+        W, H = max(self.W, int(width)), max(self.H, int(height))
+        larger = (W, H) != (self.W, self.H)
+        self._init_size(W, H, True)
+        if larger:
+            self._fit_workspace()
+            self._forget_views()
+
+
+class NativeFrame(_FrameSize):
     """One training frame through gms_train_frame: expansion, rasterizer, loss and both backward passes issued from ONE C
     call on the current stream -- no autograd graph, no per-op Python.  Gradients land in the parameters' preallocated
     .grad views (FlatAdam's flat buffer); intermediates live in a persistent workspace, rasterizer scratch in grow-only
@@ -59,17 +91,21 @@ class NativeFrame(SyncFreeCapacity):
 
     sync_free (default): only the FIRST frame learns N through the stock-style 4-byte read-back; from then on the binning
     region is sized per view by the capacity prediction of SyncFreeCapacity (gms_b200/capacity.py), and a frame whose N
-    exceeds its capacity renders the background with zero gradients and is counted in `overflows`."""
+    exceeds its capacity renders the background with zero gradients and is counted in `overflows`.
+
+    up_to: width x height is the largest view; smaller views run at their own size in the same workspace (_FrameSize)."""
 
     def __init__(self, model: MeshGaussianModel, width: int, height: int, lambda_dssim: float = 0.2, sync_free: bool = True,
-                 world: int = 1, rank: int = 0):
-        from . import _lib
+                 world: int = 1, rank: int = 0, up_to: bool = False):
         assert model._features is not None, "NativeFrame needs packed SH features"
-        self.model, self.W, self.H, self.lam = model, int(width), int(height), float(lambda_dssim)
+        self.model, self.lam = model, float(lambda_dssim)
         dev = model.vertices.device
         self.dev = dev
         P = model._scale.shape[0]
-        self.ws = torch.empty(int(_lib.lib().gms_frame_workspace_bytes(P, self.W, self.H)), dtype=torch.uint8, device=dev)
+        self._init_size(width, height, up_to)
+        self.ws = None
+        self._fit_workspace()
+        self.view_size = (self.W, self.H)       # W x H of the last frame
         self.loss = torch.zeros(3, dtype=torch.float32, device=dev)
         self._init_capacity(sync_free)
         # factored SH gradient (run(..., factored=True)): slot r of `exchange` = [3P colour gradients | camera centre | pad] of
@@ -83,7 +119,9 @@ class NativeFrame(SyncFreeCapacity):
                                     # colour gradients starts there, on the optimizer's communication stream)
         self._check_model()
         self._scratch, self._cb = grow_only_alloc(dev)
-        self._gt_u8 = GroundTruthBuffer(self.H, self.W, dev)
+
+    def _gaussians(self) -> int:
+        return self.model._scale.shape[0]
 
     def _check_model(self):
         """Raw pointers go straight to CUDA kernels: dtype / device / layout are checked here, once, instead of failing
@@ -119,7 +157,7 @@ class NativeFrame(SyncFreeCapacity):
         import ctypes as C
         from . import _lib
         v = _lib.FrameView()
-        _lib.check(_lib.lib().gms_frame_views(self.ws.data_ptr(), self.model._scale.shape[0], self.W, self.H, C.byref(v)), "gms_frame_views")
+        _lib.check(_lib.lib().gms_frame_views(self.ws.data_ptr(), self.model._scale.shape[0], *self.view_size, C.byref(v)), "gms_frame_views")
         return dict(xyz=v.xyz, exchange=self.exchange, degree=self.model.active_sh_degree, event=self.ev_sh)
 
     def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, factored: bool = False, sh_adam=None) -> torch.Tensor:
@@ -130,7 +168,8 @@ class NativeFrame(SyncFreeCapacity):
         from . import _lib
         if gt.dtype == torch.uint8:
             gt = self._gt_u8(gt, "NativeFrame.run")
-        self._check_view(cam, bg, "NativeFrame.run", gt=gt, gt_fits=tuple(gt.shape[-2:]) == (self.H, self.W))
+        self._check_view(cam, bg, "NativeFrame.run", gt=gt, gt_fits=lambda W, H: tuple(gt.shape[-2:]) == (H, W))
+        self.view_size = (int(cam.image_width), int(cam.image_height))
         if not gt.is_contiguous() or gt.dtype != torch.float32:
             gt = gt.contiguous().float()
         m = self.model
@@ -164,17 +203,37 @@ class NativeFrame(SyncFreeCapacity):
         return self.loss[0]
 
 
+def renderer_set(rs, cls, model, P: int):
+    """A trainer's evaluate() renderers: `rs` while it was made for the model's Gaussian count P, else a new set."""
+    return rs if rs is not None and rs.P == P else RendererSet(cls, model, P)
+
+
+def frame_for(frame, cam: Camera, max_size, make):
+    """A trainer's frame for `cam`: made by make(W, H) at the first step, for max_size (default: the first view's size),
+    and grown when a larger view arrives (_FrameSize.grow)."""
+    W, H = int(cam.image_width), int(cam.image_height)
+    if frame is None:
+        frame = make(*(max_size or (W, H)))
+    if W > frame.W or H > frame.H:
+        frame.grow(W, H)
+    return frame
+
+
 class MeshTrainer:
     """fwd + loss + bwd (+ gradient all-reduce) + Adam for one frame per rank.
 
     fast=True  : fused expansion launch, packed SH features (zero-copy get_features), fused L1+SSIM loss kernels,
                  FlatAdam (one launch, zeroes the gradient) -- everything on the library's kernels except sigmoid.
-    fast=False : the reference's op sequence (two-step expansion + getters, `loss_fn`, torch.optim.Adam) for A/B runs."""
+    fast=False : the reference's op sequence (two-step expansion + getters, `loss_fn`, torch.optim.Adam) for A/B runs.
+
+    Views may differ in size (one GPU): max_size (W, H), the largest view, sizes the one native frame (and the autograd
+    arm's ground-truth buffer) once; without it they are sized from the first view and grow when a larger one arrives."""
 
     def __init__(self, model: MeshGaussianModel, bg: torch.Tensor, lambda_dssim: float = 0.2, world: int = 1,
                  rank: int = 0, optimizer_step: bool = True, fast: bool = True, native: bool = False, sync_free: bool = True,
-                 loss_fn=None, sh_factored: bool = True):
+                 loss_fn=None, sh_factored: bool = True, max_size: Optional[Tuple[int, int]] = None):
         self.model, self.bg, self.lambda_dssim = model, bg, lambda_dssim
+        self.max_size = None if max_size is None else (int(max_size[0]), int(max_size[1]))
         self.world, self.rank = world, rank
         self.optimizer_step = optimizer_step
         self.fast = fast
@@ -224,9 +283,17 @@ class MeshTrainer:
         brackets train.py's iter_start / iter_end window."""
         bg = self.bg if bg is None else bg
         if self.native:
-            if self._frame is None:
-                self._frame = NativeFrame(self.model, cam.image_width, cam.image_height, self.lambda_dssim, sync_free=self.sync_free,
-                                          world=self.world, rank=self.rank)
+            if self.world > 1:
+                if self._frame is None:
+                    self._frame = NativeFrame(self.model, cam.image_width, cam.image_height, self.lambda_dssim, sync_free=self.sync_free,
+                                              world=self.world, rank=self.rank)
+                elif (int(cam.image_width), int(cam.image_height)) != (self._frame.W, self._frame.H):
+                    raise ValueError(f"MeshTrainer: data-parallel training (world {self.world}) needs every view at one size, "
+                                     f"{self._frame.W}x{self._frame.H}; got a {cam.image_width}x{cam.image_height} camera: "
+                                     f"views of mixed sizes are trained on one GPU only")
+            else:
+                self._frame = frame_for(self._frame, cam, self.max_size, lambda W, H: NativeFrame(
+                    self.model, W, H, self.lambda_dssim, sync_free=self.sync_free, up_to=True))
             factored = self.sh_factored and self.optimizer_step      # without an optimizer step the full gradient is materialised
             # one GPU: the frame applies the SH Adam step itself (no colour-gradient slot, no second read of the SH rows);
             # data parallel: the colour gradients are exchanged first and k_adam_sh consumes them
@@ -251,8 +318,12 @@ class MeshTrainer:
                 self.opt.zero_grad_partial(self.opt.ends[0])
             return loss
         if gt.dtype == torch.uint8:
-            if self._gt_u8 is None:
-                self._gt_u8 = GroundTruthBuffer(cam.image_height, cam.image_width, self.model.vertices.device)
+            H, W = int(gt.shape[0]), int(gt.shape[1])
+            b = self._gt_u8
+            if b is None or H > b.H or W > b.W:         # sized for max_size (and any earlier view), grown for a larger view
+                mW, mH = self.max_size or (0, 0)
+                self._gt_u8 = GroundTruthBuffer(max(H, mH, b.H if b else 0), max(W, mW, b.W if b else 0), self.model.vertices.device,
+                                                up_to=True)
             gt = self._gt_u8(gt, "MeshTrainer.step")
         from . import rasterizer as _r
         prev = _r.DIRECT_SH_GRAD
@@ -285,15 +356,15 @@ class MeshTrainer:
 
     @property
     def renderer(self):
-        """The renderer the last evaluate() built or reused, sized for its cameras and the model's current Gaussian count
-        (None before the first): it draws those views of the current model without a second copy of the model."""
+        """The renderers (render.RendererSet) the last evaluate() built or reused, one per image size, sized for the
+        model's current Gaussian count (None before the first): renderer.render(cam, bg) draws a view of the current model
+        at the view's size without a second copy of the model."""
         return self._renderer
 
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model on held-out views with the trainer's background, the test half of
-        training_report (train.py:183-218): NativeRenderer.evaluate, one host synchronisation for the whole set."""
-        from .render import NativeRenderer, renderer_for
-        self._renderer = renderer_for(self._renderer, NativeRenderer, self.model, cams, self.model._scale.shape[0])
+        training_report (train.py:183-218): NativeRenderer.evaluate, one host synchronisation per image size of the set."""
+        self._renderer = renderer_set(self._renderer, NativeRenderer, self.model, self.model._scale.shape[0])
         return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol)
 
     def state_dict(self) -> dict:
@@ -344,38 +415,37 @@ def expon_lr(step: int, lr_init: float, lr_final: float, lr_delay_steps: int = 0
     return float(delay * np.exp(np.log(lr_init) * (1 - t) + np.log(lr_final) * t))
 
 
-class NativeFreeFrame(SyncFreeCapacity):
+class NativeFreeFrame(_FrameSize):
     """One gs / gs_flat training frame through gms_free_train_frame: activation, rasterizer, loss, backward and (optionally)
     the densification statistics in ONE C call.  Gradients land in the parameters' .grad views (FlatAdam's flat buffer).
 
     Sync-free like NativeFrame, with one addition: after the model's Gaussian count changed (resize()), every view's next
-    frame learns its N with one read-back, so a growing model loses no frame to an overflowed capacity."""
+    frame learns its N with one read-back, so a growing model loses no frame to an overflowed capacity.
 
-    def __init__(self, model, width: int, height: int, lambda_dssim: float = 0.2, sync_free: bool = True):
-        self.model, self.W, self.H, self.lam = model, int(width), int(height), float(lambda_dssim)
+    up_to: width x height is the largest view; smaller views run at their own size in the same workspace (_FrameSize)."""
+
+    def __init__(self, model, width: int, height: int, lambda_dssim: float = 0.2, sync_free: bool = True, up_to: bool = False):
+        self.model, self.lam = model, float(lambda_dssim)
         self.dev = model._xyz.device
         self.loss = torch.zeros(3, dtype=torch.float32, device=self.dev)
         self._init_capacity(sync_free)
         self._scratch, self._cb = grow_only_alloc(self.dev)
         self.ws = None
-        self._epoch, self._view_epoch = 0, {}
         self.ev_loss = None
-        self._gt_u8 = GroundTruthBuffer(self.H, self.W, self.dev)
+        self._init_size(width, height, up_to)
         self.resize()
 
+    def _gaussians(self) -> int:
+        return self.model.P
+
     def resize(self) -> None:
-        """The model's P changed: grow the workspace, zero the statistics, forget every view's N."""
-        from . import _lib
+        """The model's P changed: grow the workspace (for the frame's largest view), zero the statistics, forget every
+        view's N."""
         P = self.model.P
-        need = int(_lib.lib().gms_frame_workspace_bytes(P, self.W, self.H))
-        if self.ws is None or self.ws.numel() < need:
-            self.ws = torch.empty(need, dtype=torch.uint8, device=self.dev)
+        self._fit_workspace()
         self.accum = torch.zeros(P, dtype=torch.float32, device=self.dev)
         self.denom = torch.zeros(P, dtype=torch.float32, device=self.dev)
-        self._harvest()
-        self._epoch += 1
-        self._view_n.clear()
-        self._n_max = 0
+        self._forget_views()
 
     def _check(self, gt, bg, cam):
         m = self.model
@@ -386,7 +456,7 @@ class NativeFreeFrame(SyncFreeCapacity):
                 raise RuntimeError(f"NativeFreeFrame: model.{n}.grad must be a preallocated contiguous buffer (FlatAdam provides it)")
         if self.accum.shape[0] != m.P:
             raise RuntimeError("NativeFreeFrame: the model's Gaussian count changed; call resize()")
-        self._check_view(cam, bg, "NativeFreeFrame.run", gt=gt, gt_fits=tuple(gt.shape) == (3, self.H, self.W))
+        self._check_view(cam, bg, "NativeFreeFrame.run", gt=gt, gt_fits=lambda W, H: tuple(gt.shape) == (3, H, W))
 
     def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, stats: bool = True, sh_adam=None) -> torch.Tensor:
         """stats: add this frame's densification statistics to `accum` / `denom`.  sh_adam (FlatAdam.begin_fused_sh_step()):
@@ -412,9 +482,7 @@ class NativeFreeFrame(SyncFreeCapacity):
         self.ev_loss = recorded_event(self.ev_loss, self.dev)
         a.event_loss_ready = self.ev_loss.cuda_event
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
-        key = self._view_key(cam)
-        if self._launch("gms_free_train_frame", a, cam, bg, relearn=self._view_epoch.get(key) != self._epoch):
-            self._view_epoch[key] = self._epoch
+        self._launch("gms_free_train_frame", a, cam, bg)
         return self.loss[0]
 
 
@@ -468,10 +536,12 @@ class FreeTrainer:
         nothing and no step count advances; the frame then runs without the fused SH step.  A lone opacity reset (white
         background at densify_from_iter) skips the opacity group only, whose bias correction lags by one from then on.
       - Appended rows start with zero Adam moments; reset_opacity zeroes the opacity moments.
-    The split samples come from torch.randn on the device (`generator`)."""
+    The split samples come from torch.randn on the device (`generator`).  Views may differ in size: max_size (W, H) as
+    MeshTrainer's; the frame keeps its size when densification changes P."""
 
     def __init__(self, model, bg: torch.Tensor, extent: float, opt: FreeOptimizationParams = None, white_background: bool = None,
-                 sync_free: bool = True, world: int = 1, generator: torch.Generator = None):
+                 sync_free: bool = True, world: int = 1, generator: torch.Generator = None,
+                 max_size: Optional[Tuple[int, int]] = None):
         if world != 1:
             raise ValueError("FreeTrainer trains on one GPU: data-parallel densification (all-reduced statistics) is not implemented")
         from .optim import free_model_groups
@@ -479,6 +549,7 @@ class FreeTrainer:
         self.opt = opt or FreeOptimizationParams()
         self.white_background = bool((bg == 1).all()) if white_background is None else bool(white_background)
         self.sync_free, self.generator = sync_free, generator
+        self.max_size = None if max_size is None else (int(max_size[0]), int(max_size[1]))
         o = self.opt
         self.fused_sh = model._features.shape[1] == 16
         self.adam = FlatAdam(free_model_groups(model, self._xyz_lr(0), o.feature_lr, o.opacity_lr, o.scaling_lr, o.rotation_lr),
@@ -521,12 +592,12 @@ class FreeTrainer:
         if it % 1000 == 0:
             self.model.oneupSHdegree()
         stats, densify, reset = self.schedule(it)
-        if self.frame is None:
-            self.frame = NativeFreeFrame(self.model, cam.image_width, cam.image_height, self.opt.lambda_dssim, sync_free=self.sync_free)
-            if self._loaded_stats is not None:      # load_state_dict before the first frame existed
-                self.frame.accum.copy_(self._loaded_stats[0])
-                self.frame.denom.copy_(self._loaded_stats[1])
-                self._loaded_stats = None
+        self.frame = frame_for(self.frame, cam, self.max_size, lambda W, H: NativeFreeFrame(
+            self.model, W, H, self.opt.lambda_dssim, sync_free=self.sync_free, up_to=True))
+        if self._loaded_stats is not None:      # load_state_dict before the first frame existed
+            self.frame.accum.copy_(self._loaded_stats[0])
+            self.frame.denom.copy_(self._loaded_stats[1])
+            self._loaded_stats = None
         sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and not densify and before_update is None else None
         loss = self.frame.run(cam, gt, self.bg if bg is None else bg, stats=stats, sh_adam=sh_adam)
         if frame_end is not None:
@@ -622,9 +693,8 @@ class FreeTrainer:
         return self._renderer
 
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
-        """L1 / SSIM / PSNR of the current model on held-out views (NativeFreeRenderer.evaluate)."""
-        from .render import NativeFreeRenderer, renderer_for
-        self._renderer = renderer_for(self._renderer, NativeFreeRenderer, self.model, cams, self.model.P)
+        """L1 / SSIM / PSNR of the current model on held-out views (NativeFreeRenderer.evaluate, MeshTrainer.evaluate)."""
+        self._renderer = renderer_set(self._renderer, NativeFreeRenderer, self.model, self.model.P)
         return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol)
 
 
@@ -676,10 +746,13 @@ class FlameTrainer:
 
     No densification (train.py densifies gs / gs_flat only), a constant learning rate per group (update_learning_rate is a
     no-op, gaussian_flame_model.py:226-228), and no optimizer step at the last iteration.  After step(), model.vertices
-    holds the pose the step rendered, not the updated parameters' (model.refresh_vertices() moves it; evaluate() does)."""
+    holds the pose the step rendered, not the updated parameters' (model.refresh_vertices() moves it; evaluate() does).
+    Views may differ in size: max_size (W, H) as MeshTrainer's."""
 
-    def __init__(self, model, bg: torch.Tensor, opt: FlameOptimizationParams = None, sync_free: bool = True):
+    def __init__(self, model, bg: torch.Tensor, opt: FlameOptimizationParams = None, sync_free: bool = True,
+                 max_size: Optional[Tuple[int, int]] = None):
         self.model, self.bg = model, bg
+        self.max_size = None if max_size is None else (int(max_size[0]), int(max_size[1]))
         self.opt = opt or FlameOptimizationParams()
         self.sync_free = sync_free
         self.fused_sh = model._features.shape[1] == 16
@@ -716,8 +789,8 @@ class FlameTrainer:
             with torch.no_grad():
                 m.vertices.copy_(verts)
             m.vertices.grad.zero_()
-        if self.frame is None:
-            self.frame = NativeFrame(m, cam.image_width, cam.image_height, self.opt.lambda_dssim, sync_free=self.sync_free)
+        self.frame = frame_for(self.frame, cam, self.max_size, lambda W, H: NativeFrame(
+            m, W, H, self.opt.lambda_dssim, sync_free=self.sync_free, up_to=True))
         take_step = it < self.opt.iterations         # train.py steps the optimizer on every iteration but the last
         fused = self.fused_sh and take_step and before_update is None
         sh_adam = self.adam.begin_fused_sh_step() if fused else None
@@ -757,8 +830,7 @@ class FlameTrainer:
         return self._renderer
 
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
-        """L1 / SSIM / PSNR of the current model (at its current pose) on held-out views (NativeRenderer.evaluate)."""
-        from .render import NativeRenderer, renderer_for
+        """L1 / SSIM / PSNR of the current model (at its current pose) on held-out views (MeshTrainer.evaluate)."""
         self.model.refresh_vertices()
-        self._renderer = renderer_for(self._renderer, NativeRenderer, self.model, cams, self.model.P)
+        self._renderer = renderer_set(self._renderer, NativeRenderer, self.model, self.model.P)
         return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol)
