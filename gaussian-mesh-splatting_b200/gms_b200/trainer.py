@@ -160,10 +160,12 @@ class NativeFrame(_FrameSize):
         _lib.check(_lib.lib().gms_frame_views(self.ws.data_ptr(), self.model._scale.shape[0], *self.view_size, C.byref(v)), "gms_frame_views")
         return dict(xyz=v.xyz, exchange=self.exchange, degree=self.model.active_sh_degree, event=self.ev_sh)
 
-    def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, factored: bool = False, sh_adam=None) -> torch.Tensor:
+    def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, factored: bool = False, sh_adam=None,
+            antialiasing: bool = False) -> torch.Tensor:
         """sh_adam (FlatAdam.begin_fused_sh_step()): the frame also applies the SH parameters' Adam step, and writes no SH
         gradient (unless `factored` asks for the colour gradient as well).  gt: float32 [3,H,W], or uint8 [H,W,3] (dequantized
-        on the device into the frame's buffer)."""
+        on the device into the frame's buffer).  antialiasing: the reference's pipe.antialiasing (each splat's opacity scaled
+        by the ratio of its 2D covariance determinants before and after the low-pass dilation, forward and backward)."""
         import ctypes as C
         from . import _lib
         if gt.dtype == torch.uint8:
@@ -199,8 +201,17 @@ class NativeFrame(_FrameSize):
             torch.cuda.current_stream(self.dev).wait_event(self._loss_read)     # done before this frame's loss kernels overwrite it
             self._loss_read = None
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
-        self._launch("gms_train_frame", a, cam, bg)
+        self._launch("gms_train_frame", a, cam, bg, antialiasing=antialiasing)
         return self.loss[0]
+
+
+def check_antialiasing(state: dict, antialiasing: bool, who: str) -> None:
+    """Refuse a trainer state written with the other antialiasing setting, so a resumed run renders as it was trained.  A
+    state without the entry was written before the setting was recorded, when every trainer ran without antialiasing."""
+    saved = bool(state.get("antialiasing", False))
+    if saved != antialiasing:
+        raise ValueError(f"{who}.load_state_dict: the state was trained with antialiasing={saved}, but this trainer runs "
+                         f"antialiasing={antialiasing}")
 
 
 def renderer_set(rs, cls, model, P: int):
@@ -227,12 +238,16 @@ class MeshTrainer:
     fast=False : the reference's op sequence (two-step expansion + getters, `loss_fn`, torch.optim.Adam) for A/B runs.
 
     Views may differ in size (one GPU): max_size (W, H), the largest view, sizes the one native frame (and the autograd
-    arm's ground-truth buffer) once; without it they are sized from the first view and grow when a larger one arrives."""
+    arm's ground-truth buffer) once; without it they are sized from the first view and grow when a larger one arrives.
+
+    antialiasing: the reference's pipe.antialiasing, a setting of the run: every training frame (native or autograd arm, one
+    GPU or data parallel) and evaluate() render with it, and state_dict() records it."""
 
     def __init__(self, model: MeshGaussianModel, bg: torch.Tensor, lambda_dssim: float = 0.2, world: int = 1,
                  rank: int = 0, optimizer_step: bool = True, fast: bool = True, native: bool = False, sync_free: bool = True,
-                 loss_fn=None, sh_factored: bool = True, max_size: Optional[Tuple[int, int]] = None):
+                 loss_fn=None, sh_factored: bool = True, max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False):
         self.model, self.bg, self.lambda_dssim = model, bg, lambda_dssim
+        self.antialiasing = bool(antialiasing)
         self.max_size = None if max_size is None else (int(max_size[0]), int(max_size[1]))
         self.world, self.rank = world, rank
         self.optimizer_step = optimizer_step
@@ -299,7 +314,7 @@ class MeshTrainer:
             # data parallel: the colour gradients are exchanged first and k_adam_sh consumes them
             fused = factored and self.world == 1 and before_update is None
             sh_adam = self.opt.begin_fused_sh_step() if fused else None
-            loss = self._frame.run(cam, gt, bg, factored=factored and not fused, sh_adam=sh_adam)
+            loss = self._frame.run(cam, gt, bg, factored=factored and not fused, sh_adam=sh_adam, antialiasing=self.antialiasing)
             if frame_end is not None:
                 frame_end.record(torch.cuda.current_stream(self._frame.dev))
             from . import rasterizer as _r
@@ -329,7 +344,7 @@ class MeshTrainer:
         prev = _r.DIRECT_SH_GRAD
         _r.DIRECT_SH_GRAD = self.fast      # FlatAdam keeps .grad preallocated and zeroed: write dL/dshs in place
         try:
-            image, radii, _ = render_frame(self.model, cam, bg, fused=self.fast)
+            image, radii, _ = render_frame(self.model, cam, bg, fused=self.fast, antialiasing=self.antialiasing)
             loss = fused_training_loss(image, gt, self.lambda_dssim) if self.fast else self.loss_fn(image, gt, self.lambda_dssim)
             loss.backward()
         finally:
@@ -365,18 +380,20 @@ class MeshTrainer:
         """L1 / SSIM / PSNR of the current model on held-out views with the trainer's background, the test half of
         training_report (train.py:183-218): NativeRenderer.evaluate, one host synchronisation per image size of the set."""
         self._renderer = renderer_set(self._renderer, NativeRenderer, self.model, self.model._scale.shape[0])
-        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol)
+        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol, antialiasing=self.antialiasing)
 
     def state_dict(self) -> dict:
-        """What resuming needs (single GPU, fast=True): FlatAdam's flat parameters, moments and step counts, and the active
-        SH degree.  Copies on the device."""
+        """What resuming needs (single GPU, fast=True): FlatAdam's flat parameters, moments and step counts, the active SH
+        degree and the antialiasing setting.  Copies on the device."""
         if not self.fast:
             raise ValueError("MeshTrainer.state_dict needs the FlatAdam trainer (fast=True)")
-        return {"adam": self.opt.state_dict(), "active_sh_degree": int(self.model.active_sh_degree)}
+        return {"adam": self.opt.state_dict(), "active_sh_degree": int(self.model.active_sh_degree), "antialiasing": self.antialiasing}
 
     def load_state_dict(self, state: dict) -> None:
+        """Restores state_dict(); refuses a state trained with the other antialiasing setting."""
         if not self.fast:
             raise ValueError("MeshTrainer.load_state_dict needs the FlatAdam trainer (fast=True)")
+        check_antialiasing(state, self.antialiasing, "MeshTrainer")
         self.opt.load_state_dict(state["adam"])
         self.model.active_sh_degree = int(state["active_sh_degree"])
 
@@ -458,10 +475,11 @@ class NativeFreeFrame(_FrameSize):
             raise RuntimeError("NativeFreeFrame: the model's Gaussian count changed; call resize()")
         self._check_view(cam, bg, "NativeFreeFrame.run", gt=gt, gt_fits=lambda W, H: tuple(gt.shape) == (3, H, W))
 
-    def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, stats: bool = True, sh_adam=None) -> torch.Tensor:
+    def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, stats: bool = True, sh_adam=None,
+            antialiasing: bool = False) -> torch.Tensor:
         """stats: add this frame's densification statistics to `accum` / `denom`.  sh_adam (FlatAdam.begin_fused_sh_step()):
         the frame also applies the SH parameters' Adam step and writes no SH gradient.  gt: float32 [3,H,W], or uint8 [H,W,3]
-        (dequantized on the device into the frame's buffer)."""
+        (dequantized on the device into the frame's buffer).  antialiasing: as NativeFrame.run."""
         import ctypes as C
         from . import _lib
         if gt.dtype == torch.uint8:
@@ -482,7 +500,7 @@ class NativeFreeFrame(_FrameSize):
         self.ev_loss = recorded_event(self.ev_loss, self.dev)
         a.event_loss_ready = self.ev_loss.cuda_event
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
-        self._launch("gms_free_train_frame", a, cam, bg)
+        self._launch("gms_free_train_frame", a, cam, bg, antialiasing=antialiasing)
         return self.loss[0]
 
 
@@ -537,11 +555,11 @@ class FreeTrainer:
         background at densify_from_iter) skips the opacity group only, whose bias correction lags by one from then on.
       - Appended rows start with zero Adam moments; reset_opacity zeroes the opacity moments.
     The split samples come from torch.randn on the device (`generator`).  Views may differ in size: max_size (W, H) as
-    MeshTrainer's; the frame keeps its size when densification changes P."""
+    MeshTrainer's; the frame keeps its size when densification changes P.  antialiasing: as MeshTrainer's."""
 
     def __init__(self, model, bg: torch.Tensor, extent: float, opt: FreeOptimizationParams = None, white_background: bool = None,
                  sync_free: bool = True, world: int = 1, generator: torch.Generator = None,
-                 max_size: Optional[Tuple[int, int]] = None):
+                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False):
         if world != 1:
             raise ValueError("FreeTrainer trains on one GPU: data-parallel densification (all-reduced statistics) is not implemented")
         from .optim import free_model_groups
@@ -550,6 +568,7 @@ class FreeTrainer:
         self.white_background = bool((bg == 1).all()) if white_background is None else bool(white_background)
         self.sync_free, self.generator = sync_free, generator
         self.max_size = None if max_size is None else (int(max_size[0]), int(max_size[1]))
+        self.antialiasing = bool(antialiasing)
         o = self.opt
         self.fused_sh = model._features.shape[1] == 16
         self.adam = FlatAdam(free_model_groups(model, self._xyz_lr(0), o.feature_lr, o.opacity_lr, o.scaling_lr, o.rotation_lr),
@@ -599,7 +618,7 @@ class FreeTrainer:
             self.frame.denom.copy_(self._loaded_stats[1])
             self._loaded_stats = None
         sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and not densify and before_update is None else None
-        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, stats=stats, sh_adam=sh_adam)
+        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, stats=stats, sh_adam=sh_adam, antialiasing=self.antialiasing)
         if frame_end is not None:
             frame_end.record(torch.cuda.current_stream(self.frame.dev))
         if before_update is not None:
@@ -621,7 +640,8 @@ class FreeTrainer:
 
     def state_dict(self) -> dict:
         """What resuming needs: FlatAdam's flat parameters, moments, group shapes and step counts, the active SH degree, the
-        iteration, P, the frame's densification statistics and the split generator's state.  Copies on the device."""
+        iteration, P, the frame's densification statistics, the split generator's state and the antialiasing setting.  Copies
+        on the device."""
         dev = self.model._xyz.device
         f = self.frame
         if f is not None:
@@ -633,11 +653,13 @@ class FreeTrainer:
             denom = torch.zeros(self.model.P, dtype=torch.float32, device=dev)
         gen = self.generator.get_state() if self.generator is not None else torch.cuda.get_rng_state(dev)
         return {"adam": self.adam.state_dict(), "active_sh_degree": int(self.model.active_sh_degree), "iteration": int(self.iteration),
-                "P": int(self.model.P), "accum": accum, "denom": denom, "generator": gen}
+                "P": int(self.model.P), "accum": accum, "denom": denom, "generator": gen, "antialiasing": self.antialiasing}
 
     def load_state_dict(self, state: dict) -> None:
-        """Restores state_dict(), also when the state's P differs from the model's (densified before it was captured)."""
+        """Restores state_dict(), also when the state's P differs from the model's (densified before it was captured); refuses
+        a state trained with the other antialiasing setting."""
         dev = self.model._xyz.device
+        check_antialiasing(state, self.antialiasing, "FreeTrainer")
         self.adam.load_state_dict(state["adam"])
         if self.model.P != int(state["P"]):
             raise ValueError(f"FreeTrainer.load_state_dict: the state holds P = {state['P']} but its parameters {self.model.P}")
@@ -695,7 +717,7 @@ class FreeTrainer:
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model on held-out views (NativeFreeRenderer.evaluate, MeshTrainer.evaluate)."""
         self._renderer = renderer_set(self._renderer, NativeFreeRenderer, self.model, self.model.P)
-        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol)
+        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol, antialiasing=self.antialiasing)
 
 
 # ---------------------------------------------------------------------------------------------- gs_flame
@@ -747,11 +769,12 @@ class FlameTrainer:
     No densification (train.py densifies gs / gs_flat only), a constant learning rate per group (update_learning_rate is a
     no-op, gaussian_flame_model.py:226-228), and no optimizer step at the last iteration.  After step(), model.vertices
     holds the pose the step rendered, not the updated parameters' (model.refresh_vertices() moves it; evaluate() does).
-    Views may differ in size: max_size (W, H) as MeshTrainer's."""
+    Views may differ in size: max_size (W, H) as MeshTrainer's.  antialiasing: as MeshTrainer's."""
 
     def __init__(self, model, bg: torch.Tensor, opt: FlameOptimizationParams = None, sync_free: bool = True,
-                 max_size: Optional[Tuple[int, int]] = None):
+                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False):
         self.model, self.bg = model, bg
+        self.antialiasing = bool(antialiasing)
         self.max_size = None if max_size is None else (int(max_size[0]), int(max_size[1]))
         self.opt = opt or FlameOptimizationParams()
         self.sync_free = sync_free
@@ -794,7 +817,7 @@ class FlameTrainer:
         take_step = it < self.opt.iterations         # train.py steps the optimizer on every iteration but the last
         fused = self.fused_sh and take_step and before_update is None
         sh_adam = self.adam.begin_fused_sh_step() if fused else None
-        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, sh_adam=sh_adam)
+        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, sh_adam=sh_adam, antialiasing=self.antialiasing)
         if native:
             self._lbs.backward()                 # writes the FLAME tensors' flat .grad views
         else:
@@ -816,10 +839,13 @@ class FlameTrainer:
 
     def state_dict(self) -> dict:
         """What resuming needs: FlatAdam's flat parameters (the FLAME tensors among them), moments and step counts, the active
-        SH degree and the iteration.  Copies on the device."""
-        return {"adam": self.adam.state_dict(), "active_sh_degree": int(self.model.active_sh_degree), "iteration": int(self.iteration)}
+        SH degree, the iteration and the antialiasing setting.  Copies on the device."""
+        return {"adam": self.adam.state_dict(), "active_sh_degree": int(self.model.active_sh_degree), "iteration": int(self.iteration),
+                "antialiasing": self.antialiasing}
 
     def load_state_dict(self, state: dict) -> None:
+        """Restores state_dict(); refuses a state trained with the other antialiasing setting."""
+        check_antialiasing(state, self.antialiasing, "FlameTrainer")
         self.adam.load_state_dict(state["adam"])
         self.model.active_sh_degree = int(state["active_sh_degree"])
         self.iteration = int(state["iteration"])
@@ -833,4 +859,4 @@ class FlameTrainer:
         """L1 / SSIM / PSNR of the current model (at its current pose) on held-out views (MeshTrainer.evaluate)."""
         self.model.refresh_vertices()
         self._renderer = renderer_set(self._renderer, NativeRenderer, self.model, self.model.P)
-        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol)
+        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol, antialiasing=self.antialiasing)
