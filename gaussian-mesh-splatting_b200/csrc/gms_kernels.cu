@@ -8,6 +8,7 @@
 #include <thrust/iterator/transform_iterator.h>
 #include <stdio.h>
 #include <string.h>
+#include <initializer_list>
 #include <utility>
 #include <vector>
 
@@ -29,6 +30,7 @@
 #include "gms_flame.cuh"
 #include "gms_lpips.cuh"
 #include "gms_alpha.cuh"
+#include "gms_anomaly.cuh"
 
 // ------------------------------------------------------------------------------------------ host state
 static thread_local char g_err[512] = "";
@@ -68,12 +70,12 @@ static int sm_count() {
 
 // Optional per-kernel timing with CUDA events recorded on the launching stream (bench.py's roofline numbers).
 enum { K_PRE_FWD = 0, K_SORT_P, K_SCAN, K_EMIT, K_SORT_N, K_RANGES, K_COMP_FWD, K_COMP_BWD, K_PRE_BWD, K_EXP_FWD, K_EXP_BWD, K_LOSS_STATS, K_LOSS_GRAD, K_ADAM, K_MISC,
-       K_METRICS, K_METRICS_FIN, K_LPIPS_CONV, K_LPIPS_POOL, K_LPIPS_HEAD, K_COUNT };
+       K_METRICS, K_METRICS_FIN, K_LPIPS_CONV, K_LPIPS_POOL, K_LPIPS_HEAD, K_NAN_SCAN, K_COUNT };
 static const char* const g_kernel_names[K_COUNT] = {"preprocess_fwd", "cub_sort_depth", "cub_scan_tiles", "emit_dups", "cub_sort_tiles",
                                                     "tile_ranges", "composite_fwd", "composite_bwd", "preprocess_bwd", "expand_fwd",
                                                     "expand_bwd", "ssim_stats", "ssim_grad", "adam", "misc",
                                                     "image_metrics", "metrics_finalize", "lpips_conv", "lpips_pool",
-                                                    "lpips_head"};
+                                                    "lpips_head", "nan_scan"};
 static int g_opt_time = 0;
 struct TimedSpan { int id; cudaEvent_t a, b; };
 static TimedSpan g_spans[1 << 15];
@@ -258,6 +260,36 @@ static BinLayout bin_layout(void* base, int64_t N) {
 }
 
 extern "C" int gms_loss_scratch_bytes(int32_t C, int32_t H, int32_t W, size_t* bytes);
+
+// One NaN scan of a stage's buffers into `record` (k_nan_scan): gms_nan_scan after its checks, and the training frames'
+// anomaly hooks.  Empty buffers are dropped; nothing is launched when every buffer is empty.  Each buffer gets as many blocks
+// as its float4 body needs at GMS_NAN_UNROLL loads per thread, at most 8 per SM (a full SM of 256-thread blocks).
+static int nan_scan_launch(int stage, const gms_nan_buffer* bufs, int nb, uint64_t* record, int dbg, cudaStream_t st) {
+    GmsNanTable t;
+    int m = 0;
+    int64_t most = 0;
+    for (int i = 0; i < nb; i++) {
+        if (bufs[i].n <= 0) continue;
+        const int64_t to16 = (int64_t)(((16 - (reinterpret_cast<size_t>(bufs[i].ptr) & 15)) & 15) >> 2);
+        GmsNanBuf& b = t.b[m++];
+        b.ptr = bufs[i].ptr; b.n = bufs[i].n; b.head = to16 < b.n ? to16 : b.n;
+        b.key = (uint64_t)stage << 56 | (uint64_t)bufs[i].tensor << 48;
+        const int64_t n4 = (b.n - b.head) >> 2;
+        most = n4 > most ? n4 : most;
+    }
+    if (m == 0) return GMS_OK;
+    const int64_t per_block = (int64_t)GMS_NAN_BLOCK * GMS_NAN_UNROLL, cap = 8 * (int64_t)sm_count();
+    int64_t gx = (most + per_block - 1) / per_block;
+    gx = gx < 1 ? 1 : gx > cap ? cap : gx;
+    return launch("nan_scan", K_NAN_SCAN, dbg, st, dim3((unsigned)gx, (unsigned)m), GMS_NAN_BLOCK, 0, k_nan_scan, t, record);
+}
+
+// A training frame's anomaly hook: scans the stage's buffers when the caller passed a record and selected the stage.
+static int anomaly_hook(uint64_t* record, uint32_t stages, int stage, std::initializer_list<gms_nan_buffer> bufs, int dbg,
+                        cudaStream_t st) {
+    if (!record || !((stages >> stage) & 1u)) return GMS_OK;
+    return nan_scan_launch(stage, bufs.begin(), (int)bufs.size(), record, dbg, st);
+}
 
 // ------------------------------------------------------------------------------------------ whole-frame orchestration
 
@@ -839,7 +871,8 @@ int gms_rasterize_forward_nosync(const gms_raster_settings* s, const gms_raster_
 
 static int raster_backward_impl(const gms_raster_settings* s, const gms_raster_inputs* in, const int32_t* radii,
                                 const gms_raster_saved* saved, const float* dL_dout_color, const float* dL_dout_invdepth,
-                                const gms_raster_grads* gr, void* cuda_stream, float* dopac_raw, const gms_sh_adam* sh_adam) {
+                                const gms_raster_grads* gr, void* cuda_stream, float* dopac_raw, const gms_sh_adam* sh_adam,
+                                uint64_t* anomaly, uint32_t anomaly_stages) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (!s || !saved || !gr || !dL_dout_color || !in) return set_err(GMS_E_ARG, "null argument%s%s");
     if (in->P == 0) return GMS_OK;
@@ -877,6 +910,8 @@ static int raster_backward_impl(const gms_raster_settings* s, const gms_raster_i
         };
         if ((rc = lists ? composite_bwd(bwd5[mb][depth], surv, IL.nsurv) : composite_bwd(bwd3[mb][depth]))) return rc;
     }
+    if ((rc = anomaly_hook(anomaly, anomaly_stages, GMS_ANOMALY_COMPOSITE_BWD,
+                           {{reinterpret_cast<const float*>(GL.dgeom), 12 * (int64_t)P, GMS_ANOMALY_DGEOM}}, dbg, st))) return rc;
     PreBwdArgs b;
     b.f = make_pre_args(s, in);
     b.radii = radii; b.cov3D = GL.cov3D; b.clamped = GL.clamped; b.dgeom = GL.dgeom;
@@ -905,13 +940,21 @@ static int raster_backward_impl(const gms_raster_settings* s, const gms_raster_i
         if (g_opt_sh_staged == 2) k = minb4 ? k_preprocess_bwd<2, 4> : k_preprocess_bwd<2, 1>;
         else k = minb4 ? k_preprocess_bwd<1, 4> : k_preprocess_bwd<1, 1>;
     }
-    return launch("preprocess_bwd", K_PRE_BWD, dbg, st, (P + 127) / 128, 128, 0, k, b);
+    if ((rc = launch("preprocess_bwd", K_PRE_BWD, dbg, st, (P + 127) / 128, 128, 0, k, b))) return rc;
+    // (a buffer the call did not write is NULL and counts 0 floats)
+    const int64_t Pn = P;
+    return anomaly_hook(anomaly, anomaly_stages, GMS_ANOMALY_PREPROCESS_BWD,
+                        {{b.dmeans3D, 3 * Pn, GMS_ANOMALY_DMEANS3D}, {b.dscales, b.dscales ? 3 * Pn : 0, GMS_ANOMALY_DSCALES},
+                         {b.drots, b.drots ? 4 * Pn : 0, GMS_ANOMALY_DROTATIONS},
+                         {dopac_raw ? dopac_raw : b.dopac, Pn, GMS_ANOMALY_DOPACITY_RAW},
+                         {b.dshs, b.dshs ? 3 * Pn * b.f.M : 0, GMS_ANOMALY_DSHS},
+                         {b.dcol_sh, b.dcol_sh ? 3 * Pn : 0, GMS_ANOMALY_DCOLOR_SH}}, dbg, st);
 }
 
 int gms_rasterize_backward(const gms_raster_settings* s, const gms_raster_inputs* in, const int32_t* radii,
                            const gms_raster_saved* saved, const float* dL_dout_color, const float* dL_dout_invdepth,
                            const gms_raster_grads* gr, void* cuda_stream) {
-    return raster_backward_impl(s, in, radii, saved, dL_dout_color, dL_dout_invdepth, gr, cuda_stream, nullptr, nullptr);
+    return raster_backward_impl(s, in, radii, saved, dL_dout_color, dL_dout_invdepth, gr, cuda_stream, nullptr, nullptr, nullptr, 0);
 }
 
 int gms_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present, void* cuda_stream) {
@@ -1163,6 +1206,8 @@ static int frame_loss_backward(const Args* a, const FrameLayout& FL, const gms_r
     int rc;
     if ((rc = gms_l1_ssim_loss(&la, cuda_stream))) return rc;
     if (a->event_loss_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_loss_ready), st));
+    if ((rc = anomaly_hook(a->anomaly, a->anomaly_stages, GMS_ANOMALY_LOSS, {{FL.dimage, 3 * (int64_t)la.H * la.W, GMS_ANOMALY_DIMAGE}}, 0,
+                           st))) return rc;
     gms_raster_grads gr;
     memset(&gr, 0, sizeof(gr));
     gr.dL_dmeans3D = d_xyz; gr.dL_dmeans2D = FL.d_m2d; gr.dL_dopacities = FL.d_opac;
@@ -1171,7 +1216,8 @@ static int frame_loss_backward(const Args* a, const FrameLayout& FL, const gms_r
         GMS_CUDA(cudaMemcpyAsync(d_color_sh + 3 * (size_t)in.P, a->settings.campos, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
     } else if (!a->sh_adam) gr.dL_dshs = a->d_features;
     gr.dL_dscales = FL.d_scales; gr.dL_drotations = FL.d_rots;
-    return raster_backward_impl(&a->settings, &in, FL.radii, &saved, FL.dimage, nullptr, &gr, cuda_stream, a->d_opacity_raw, a->sh_adam);
+    return raster_backward_impl(&a->settings, &in, FL.radii, &saved, FL.dimage, nullptr, &gr, cuda_stream, a->d_opacity_raw, a->sh_adam,
+                                a->anomaly, a->anomaly_stages);
 }
 
 }   // extern "C++"
@@ -1282,6 +1328,8 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
         return set_err(GMS_E_ARG, "gms_train_frame: gradient tensors required%s%s");
     if (a->sh_adam && (!a->sh_adam->m || !a->sh_adam->v || a->sh_adam->step < 1 || a->settings.sh_degree < 0 || a->settings.sh_degree > 3))
         return set_err(GMS_E_ARG, "gms_train_frame: bad sh_adam%s%s");
+    if (a->sh_adam && a->anomaly)
+        return set_err(GMS_E_ARG, "gms_train_frame: anomaly and sh_adam exclude each other (the fused step would update features before the scan)%s%s");
     const FrameModel m = {a->V, a->F, a->K, a->M, a->vertices, a->faces, a->alpha_raw, a->scale_raw, a->features, a->opacity_raw, a->eps,
                           a->segments, a->n_segments, a->alpha_activation};
     int P, rc;
@@ -1305,6 +1353,9 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     // expansion backward (vertex gradients are accumulated with atomics: the caller keeps d_vertices zeroed)
     if ((rc = mesh_expand_backward(ea, FL.d_xyz, FL.d_scales, FL.d_rots, a->d_vertices, a->d_alpha_raw, a->d_scale_raw, cuda_stream)))
         return rc;
+    if ((rc = anomaly_hook(a->anomaly, a->anomaly_stages, GMS_ANOMALY_EXPAND_BWD,
+                           {{a->d_vertices, 3 * (int64_t)a->V, GMS_ANOMALY_DVERTICES}, {a->d_alpha_raw, 3 * (int64_t)P, GMS_ANOMALY_DALPHA_RAW},
+                            {a->d_scale_raw, (int64_t)P, GMS_ANOMALY_DSCALE_RAW}}, 0, st))) return rc;
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;
     return GMS_OK;
 }
@@ -1339,6 +1390,8 @@ int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void*
     if (a->sh_adam && (!a->sh_adam->m || !a->sh_adam->v || a->sh_adam->step < 1 || a->M != 16 || a->settings.sh_degree < 0 ||
                        a->settings.sh_degree > 3))
         return set_err(GMS_E_ARG, "gms_free_train_frame: bad sh_adam%s%s");
+    if (a->sh_adam && a->anomaly)
+        return set_err(GMS_E_ARG, "gms_free_train_frame: anomaly and sh_adam exclude each other (the fused step would update features before the scan)%s%s");
     int rc;
     if ((rc = frame_sh_check("gms_free_train_frame", a->settings.sh_degree, a->M))) return rc;
     const int W = a->settings.image_width, H = a->settings.image_height;
@@ -1361,6 +1414,10 @@ int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void*
         b.counters = geom_layout(aligned_base(saved.geom), P).counters;
         if ((rc = launch("free_act_bwd", K_EXP_BWD, 0, st, (P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, k_free_act_bwd, b)))
             return rc;
+        if ((rc = anomaly_hook(a->anomaly, a->anomaly_stages, GMS_ANOMALY_ACTIVATION_BWD,
+                               {{a->d_scaling_raw, (int64_t)P * a->scale_cols, GMS_ANOMALY_DSCALING_RAW},
+                                {a->d_rotation_raw, 4 * (int64_t)P, GMS_ANOMALY_DROTATION_RAW},
+                                {a->accum, a->accum ? (int64_t)P : 0, GMS_ANOMALY_ACCUM}}, 0, st))) return rc;
     }
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;
     return GMS_OK;
@@ -1782,6 +1839,21 @@ int gms_flame_lbs_backward(const gms_flame_lbs_args* a, void* cuda_stream) {
                               a->J_regressor, w.dvp, w.dJ, a->d_shape, a->d_expression))) return rc;
     span_end(st);
     return GMS_OK;
+}
+
+int gms_nan_scan(const gms_nan_scan_args* a, void* cuda_stream) {
+    if (!a || !a->record) return set_err(GMS_E_ARG, "gms_nan_scan: null record%s%s");
+    if (a->n_buffers < 0 || a->n_buffers > GMS_NAN_SCAN_MAX_BUFFERS)
+        return set_err(GMS_E_ARG, "gms_nan_scan: n_buffers must be 0..GMS_NAN_SCAN_MAX_BUFFERS%s%s");
+    if (a->stage < 0 || a->stage >= GMS_ANOMALY_STAGES) return set_err(GMS_E_ARG, "gms_nan_scan: stage out of range%s%s");
+    for (int i = 0; i < a->n_buffers; i++) {
+        const gms_nan_buffer& b = a->buffers[i];
+        if (b.n < 0 || b.n >= ((int64_t)1 << 48)) return set_err(GMS_E_ARG, "gms_nan_scan: a buffer needs 0 <= n < 2^48%s%s");
+        if (b.tensor < 0 || b.tensor > 255) return set_err(GMS_E_ARG, "gms_nan_scan: tensor id out of range 0..255%s%s");
+        if (b.n > 0 && (!b.ptr || (reinterpret_cast<size_t>(b.ptr) & 3)))
+            return set_err(GMS_E_ARG, "gms_nan_scan: a non-empty buffer needs a 4-byte-aligned pointer%s%s");
+    }
+    return nan_scan_launch(a->stage, a->buffers, a->n_buffers, a->record, 0, reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
 }  // extern "C"

@@ -131,7 +131,8 @@ class FrameArgs(C.Structure):
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)),
                 ("binning_capacity", C.c_int64), ("n_host_mapped", C.c_void_p), ("d_color_sh", C.c_void_p),
                 ("event_sh_ready", C.c_void_p), ("event_loss_ready", C.c_void_p), ("sh_adam", C.POINTER(ShAdam)),
-                ("segments", C.POINTER(MeshSegment)), ("n_segments", C.c_int32), ("alpha_activation", C.c_int32)]
+                ("segments", C.POINTER(MeshSegment)), ("n_segments", C.c_int32), ("anomaly_stages", C.c_uint32),
+                ("anomaly", C.c_void_p), ("alpha_activation", C.c_int32)]
 
 
 class FrameView(C.Structure):
@@ -199,7 +200,8 @@ class FreeFrameArgs(C.Structure):
                 ("d_opacity_raw", C.c_void_p), ("accum", C.c_void_p), ("denom", C.c_void_p), ("settings", RasterSettings),
                 ("gt", C.c_void_p), ("lambda_dssim", C.c_float), ("loss", C.c_void_p), ("workspace", C.c_void_p),
                 ("workspace_bytes", C.c_size_t), ("num_rendered", C.POINTER(C.c_int64)), ("binning_capacity", C.c_int64),
-                ("n_host_mapped", C.c_void_p), ("event_loss_ready", C.c_void_p), ("sh_adam", C.POINTER(ShAdam))]
+                ("n_host_mapped", C.c_void_p), ("event_loss_ready", C.c_void_p), ("sh_adam", C.POINTER(ShAdam)),
+                ("anomaly", C.c_void_p), ("anomaly_stages", C.c_uint32)]
 
 
 class FreeRenderArgs(C.Structure):
@@ -303,6 +305,31 @@ class FlameLbsArgs(C.Structure):
                [("workspace_bytes", C.c_size_t)]
 
 
+ANOMALY_NONE = (1 << 64) - 1        # GMS_ANOMALY_NONE: the record of a scan that found no NaN
+# GMS_ANOMALY_*: the stages, in the order a frame runs them, and the tensors of each
+(ANOMALY_LOSS, ANOMALY_COMPOSITE_BWD, ANOMALY_PREPROCESS_BWD, ANOMALY_EXPAND_BWD, ANOMALY_ACTIVATION_BWD,
+ ANOMALY_FLAME_BWD) = range(6)
+ANOMALY_STAGES = 6
+ANOMALY_DIMAGE = 0
+ANOMALY_DGEOM = 0
+(ANOMALY_DMEANS3D, ANOMALY_DSCALES, ANOMALY_DROTATIONS, ANOMALY_DOPACITY_RAW, ANOMALY_DSHS, ANOMALY_DCOLOR_SH) = range(6)
+ANOMALY_DVERTICES, ANOMALY_DALPHA_RAW, ANOMALY_DSCALE_RAW = range(3)
+ANOMALY_DSCALING_RAW, ANOMALY_DROTATION_RAW, ANOMALY_ACCUM = range(3)
+(ANOMALY_DSHAPE, ANOMALY_DEXPRESSION, ANOMALY_DPOSE, ANOMALY_DNECK_POSE, ANOMALY_DTRANSL, ANOMALY_DENLARGEMENT) = range(6)
+NAN_SCAN_MAX_BUFFERS = 8            # GMS_NAN_SCAN_MAX_BUFFERS
+
+
+class NanBuffer(C.Structure):
+    """struct gms_nan_buffer"""
+    _fields_ = [("ptr", C.c_void_p), ("n", C.c_int64), ("tensor", C.c_int32)]
+
+
+class NanScanArgs(C.Structure):
+    """struct gms_nan_scan_args"""
+    _fields_ = [("buffers", NanBuffer * NAN_SCAN_MAX_BUFFERS), ("n_buffers", C.c_int32), ("stage", C.c_int32),
+                ("record", C.c_void_p)]
+
+
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_int, C.c_size_t)
 
 # every symbol include/gms_b200.h declares (tests/test_abi.py checks the library exports all of them)
@@ -319,7 +346,7 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_densify_plan", "gms_densify_apply", "gms_knn_scratch_bytes", "gms_knn_dist2",
                "gms_flame_render_workspace_bytes", "gms_flame_render_frame", "gms_image_composite_rgba", "gms_image_resize_u8",
                "gms_flame_lbs_workspace_bytes", "gms_flame_lbs_forward", "gms_flame_lbs_backward", "gms_lpips_scratch_bytes",
-               "gms_lpips_vgg", "gms_alpha_shape", "gms_normals_scratch_bytes", "gms_estimate_normals"]
+               "gms_lpips_vgg", "gms_alpha_shape", "gms_normals_scratch_bytes", "gms_estimate_normals", "gms_nan_scan"]
 
 _lib = None
 
@@ -411,6 +438,7 @@ def lib():
     L.gms_normals_scratch_bytes.restype = C.c_size_t
     L.gms_normals_scratch_bytes.argtypes = [C.c_int32]
     L.gms_estimate_normals.argtypes = [C.POINTER(NormalsArgs), C.c_void_p]
+    L.gms_nan_scan.argtypes = [C.POINTER(NanScanArgs), C.c_void_p]
     _lib = L
     # GMS_OPTIONS="key=value,key=value": tuning knobs applied at load (A/B runs of whole test suites / benches)
     for kv in filter(None, os.environ.get("GMS_OPTIONS", "").split(",")):

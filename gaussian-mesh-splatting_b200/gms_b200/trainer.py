@@ -11,6 +11,7 @@ All gradients live in ONE contiguous buffer (param.grad are views into it), so t
 """
 from __future__ import annotations
 
+import contextlib
 import math
 from dataclasses import dataclass
 from typing import List, Optional, Sequence, Tuple
@@ -21,6 +22,8 @@ import torch.distributed as dist
 
 import diff_gaussian_rasterization as dgr
 
+from . import _lib
+from .anomaly import FRAME_STAGES, AnomalyError, AnomalyRecord, layout_of
 from .capacity import SyncFreeCapacity, check_float32, grow_only_alloc, recorded_event
 from .flame import NativeFlame
 from .io_image import GroundTruthBuffer
@@ -161,11 +164,13 @@ class NativeFrame(_FrameSize):
         return dict(xyz=v.xyz, exchange=self.exchange, degree=self.model.active_sh_degree, event=self.ev_sh)
 
     def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, factored: bool = False, sh_adam=None,
-            antialiasing: bool = False) -> torch.Tensor:
+            antialiasing: bool = False, anomaly: Optional[AnomalyRecord] = None, anomaly_stages: int = FRAME_STAGES) -> torch.Tensor:
         """sh_adam (FlatAdam.begin_fused_sh_step()): the frame also applies the SH parameters' Adam step, and writes no SH
         gradient (unless `factored` asks for the colour gradient as well).  gt: float32 [3,H,W], or uint8 [H,W,3] (dequantized
         on the device into the frame's buffer).  antialiasing: the reference's pipe.antialiasing (each splat's opacity scaled
-        by the ratio of its 2D covariance determinants before and after the low-pass dilation, forward and backward)."""
+        by the ratio of its 2D covariance determinants before and after the low-pass dilation, forward and backward).
+        anomaly: the frame scans the outputs of each backward stage selected in anomaly_stages (bits 1 << _lib.ANOMALY_*) for
+        NaN into this record (not with sh_adam); the caller resets and reads it."""
         import ctypes as C
         from . import _lib
         if gt.dtype == torch.uint8:
@@ -201,6 +206,8 @@ class NativeFrame(_FrameSize):
             torch.cuda.current_stream(self.dev).wait_event(self._loss_read)     # done before this frame's loss kernels overwrite it
             self._loss_read = None
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
+        if anomaly is not None:
+            a.anomaly, a.anomaly_stages = anomaly.ptr, int(anomaly_stages)
         self._launch("gms_train_frame", a, cam, bg, antialiasing=antialiasing)
         return self.loss[0]
 
@@ -212,6 +219,29 @@ def check_antialiasing(state: dict, antialiasing: bool, who: str) -> None:
     if saved != antialiasing:
         raise ValueError(f"{who}.load_state_dict: the state was trained with antialiasing={saved}, but this trainer runs "
                          f"antialiasing={antialiasing}")
+
+
+def anomaly_record(record: Optional[AnomalyRecord], dev) -> AnomalyRecord:
+    """A trainer's anomaly record (`record`, or a new one on `dev`), reset for the next frame."""
+    return (record or AnomalyRecord(dev)).reset()
+
+
+def check_anomaly(record: AnomalyRecord, model, cam: Camera, opt, iteration: Optional[int] = None, restore=None) -> None:
+    """Reads the step's anomaly record (one host synchronisation).  On a NaN, the step is undone before AnomalyError is
+    raised: `restore()` (when given) puts back what the frame accumulated into, and the gradient buffer is zeroed (the vertex
+    gradient accumulates across frames), so the trainer can take its next step."""
+    try:
+        record.check(layout_of(model, cam), iteration)
+    except AnomalyError:
+        if restore is not None:
+            restore()
+        opt.zero_grad()
+        raise
+
+
+def refuse_data_parallel_anomaly(detect_anomaly: bool, world: int, who: str) -> None:
+    if detect_anomaly and world > 1:
+        raise ValueError(f"{who}: detect_anomaly needs one GPU (world {world}): data-parallel anomaly detection is not implemented")
 
 
 def renderer_set(rs, cls, model, P: int):
@@ -241,13 +271,22 @@ class MeshTrainer:
     arm's ground-truth buffer) once; without it they are sized from the first view and grow when a larger one arrives.
 
     antialiasing: the reference's pipe.antialiasing, a setting of the run: every training frame (native or autograd arm, one
-    GPU or data parallel) and evaluate() render with it, and state_dict() records it."""
+    GPU or data parallel) and evaluate() render with it, and state_dict() records it.
+
+    detect_anomaly: the reference's train.py --detect_anomaly (one GPU).  A native frame scans the outputs of each of its
+    backward stages for NaN on the device and step() raises anomaly.AnomalyError, naming the first stage, tensor and element
+    that held one, before before_update and before any parameter changes (the SH Adam step is not fused into the frame, one
+    host synchronisation per step).  The autograd arm runs its step under torch.autograd.detect_anomaly()."""
 
     def __init__(self, model: MeshGaussianModel, bg: torch.Tensor, lambda_dssim: float = 0.2, world: int = 1,
                  rank: int = 0, optimizer_step: bool = True, fast: bool = True, native: bool = False, sync_free: bool = True,
-                 loss_fn=None, sh_factored: bool = True, max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False):
+                 loss_fn=None, sh_factored: bool = True, max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False,
+                 detect_anomaly: bool = False):
+        refuse_data_parallel_anomaly(detect_anomaly, world, "MeshTrainer")
         self.model, self.bg, self.lambda_dssim = model, bg, lambda_dssim
         self.antialiasing = bool(antialiasing)
+        self.detect_anomaly = bool(detect_anomaly)
+        self._anomaly = None
         self.max_size = None if max_size is None else (int(max_size[0]), int(max_size[1]))
         self.world, self.rank = world, rank
         self.optimizer_step = optimizer_step
@@ -312,15 +351,20 @@ class MeshTrainer:
             factored = self.sh_factored and self.optimizer_step      # without an optimizer step the full gradient is materialised
             # one GPU: the frame applies the SH Adam step itself (no colour-gradient slot, no second read of the SH rows);
             # data parallel: the colour gradients are exchanged first and k_adam_sh consumes them
-            fused = factored and self.world == 1 and before_update is None
+            fused = factored and self.world == 1 and before_update is None and not self.detect_anomaly
             sh_adam = self.opt.begin_fused_sh_step() if fused else None
-            loss = self._frame.run(cam, gt, bg, factored=factored and not fused, sh_adam=sh_adam, antialiasing=self.antialiasing)
+            record = anomaly_record(self._anomaly, self._frame.dev) if self.detect_anomaly else None
+            self._anomaly = record
+            loss = self._frame.run(cam, gt, bg, factored=factored and not fused, sh_adam=sh_adam, antialiasing=self.antialiasing,
+                                   anomaly=record)
             if frame_end is not None:
                 frame_end.record(torch.cuda.current_stream(self._frame.dev))
             from . import rasterizer as _r
             _r.last_num_rendered = self._frame.last_num_rendered
             if loss_host is not None:
                 self._frame.read_loss_async(loss_host, loss_ready)
+            if record is not None:
+                check_anomaly(record, self.model, cam, self.opt)
             if before_update is not None:
                 before_update()
             self._all_reduce()
@@ -344,9 +388,10 @@ class MeshTrainer:
         prev = _r.DIRECT_SH_GRAD
         _r.DIRECT_SH_GRAD = self.fast      # FlatAdam keeps .grad preallocated and zeroed: write dL/dshs in place
         try:
-            image, radii, _ = render_frame(self.model, cam, bg, fused=self.fast, antialiasing=self.antialiasing)
-            loss = fused_training_loss(image, gt, self.lambda_dssim) if self.fast else self.loss_fn(image, gt, self.lambda_dssim)
-            loss.backward()
+            with torch.autograd.detect_anomaly() if self.detect_anomaly else contextlib.nullcontext():
+                image, radii, _ = render_frame(self.model, cam, bg, fused=self.fast, antialiasing=self.antialiasing)
+                loss = fused_training_loss(image, gt, self.lambda_dssim) if self.fast else self.loss_fn(image, gt, self.lambda_dssim)
+                loss.backward()
         finally:
             _r.DIRECT_SH_GRAD = prev       # never leak the in-place mode to other users of the rasterizer
         if frame_end is not None:
@@ -476,10 +521,10 @@ class NativeFreeFrame(_FrameSize):
         self._check_view(cam, bg, "NativeFreeFrame.run", gt=gt, gt_fits=lambda W, H: tuple(gt.shape) == (3, H, W))
 
     def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, stats: bool = True, sh_adam=None,
-            antialiasing: bool = False) -> torch.Tensor:
+            antialiasing: bool = False, anomaly: Optional[AnomalyRecord] = None, anomaly_stages: int = FRAME_STAGES) -> torch.Tensor:
         """stats: add this frame's densification statistics to `accum` / `denom`.  sh_adam (FlatAdam.begin_fused_sh_step()):
         the frame also applies the SH parameters' Adam step and writes no SH gradient.  gt: float32 [3,H,W], or uint8 [H,W,3]
-        (dequantized on the device into the frame's buffer).  antialiasing: as NativeFrame.run."""
+        (dequantized on the device into the frame's buffer).  antialiasing, anomaly, anomaly_stages: as NativeFrame.run."""
         import ctypes as C
         from . import _lib
         if gt.dtype == torch.uint8:
@@ -500,6 +545,8 @@ class NativeFreeFrame(_FrameSize):
         self.ev_loss = recorded_event(self.ev_loss, self.dev)
         a.event_loss_ready = self.ev_loss.cuda_event
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
+        if anomaly is not None:
+            a.anomaly, a.anomaly_stages = anomaly.ptr, int(anomaly_stages)
         self._launch("gms_free_train_frame", a, cam, bg, antialiasing=antialiasing)
         return self.loss[0]
 
@@ -555,11 +602,15 @@ class FreeTrainer:
         background at densify_from_iter) skips the opacity group only, whose bias correction lags by one from then on.
       - Appended rows start with zero Adam moments; reset_opacity zeroes the opacity moments.
     The split samples come from torch.randn on the device (`generator`).  Views may differ in size: max_size (W, H) as
-    MeshTrainer's; the frame keeps its size when densification changes P.  antialiasing: as MeshTrainer's."""
+    MeshTrainer's; the frame keeps its size when densification changes P.  antialiasing: as MeshTrainer's.  detect_anomaly: as
+    MeshTrainer's; step() raises before densification, the opacity reset and Adam, with the iteration counter and the
+    densification statistics as they were before the step (the learning rate and SH degree of the iteration stay applied, as
+    in the reference)."""
 
     def __init__(self, model, bg: torch.Tensor, extent: float, opt: FreeOptimizationParams = None, white_background: bool = None,
                  sync_free: bool = True, world: int = 1, generator: torch.Generator = None,
-                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False):
+                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False, detect_anomaly: bool = False):
+        refuse_data_parallel_anomaly(detect_anomaly, world, "FreeTrainer")
         if world != 1:
             raise ValueError("FreeTrainer trains on one GPU: data-parallel densification (all-reduced statistics) is not implemented")
         from .optim import free_model_groups
@@ -569,6 +620,8 @@ class FreeTrainer:
         self.sync_free, self.generator = sync_free, generator
         self.max_size = None if max_size is None else (int(max_size[0]), int(max_size[1]))
         self.antialiasing = bool(antialiasing)
+        self.detect_anomaly = bool(detect_anomaly)
+        self._anomaly = None
         o = self.opt
         self.fused_sh = model._features.shape[1] == 16
         self.adam = FlatAdam(free_model_groups(model, self._xyz_lr(0), o.feature_lr, o.opacity_lr, o.scaling_lr, o.rotation_lr),
@@ -617,10 +670,20 @@ class FreeTrainer:
             self.frame.accum.copy_(self._loaded_stats[0])
             self.frame.denom.copy_(self._loaded_stats[1])
             self._loaded_stats = None
-        sh_adam = self.adam.begin_fused_sh_step() if self.fused_sh and not densify and before_update is None else None
-        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, stats=stats, sh_adam=sh_adam, antialiasing=self.antialiasing)
+        fuse = self.fused_sh and not densify and before_update is None and not self.detect_anomaly
+        sh_adam = self.adam.begin_fused_sh_step() if fuse else None
+        record, restore = None, None
+        if self.detect_anomaly:
+            record = self._anomaly = anomaly_record(self._anomaly, self.frame.dev)
+            if stats:       # the frame adds this step's statistics in its last kernel
+                f, kept = self.frame, (self.frame.accum.clone(), self.frame.denom.clone())
+                restore = lambda: (f.accum.copy_(kept[0]), f.denom.copy_(kept[1]))
+        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, stats=stats, sh_adam=sh_adam, antialiasing=self.antialiasing,
+                              anomaly=record)
         if frame_end is not None:
             frame_end.record(torch.cuda.current_stream(self.frame.dev))
+        if record is not None:
+            check_anomaly(record, self.model, cam, self.adam, it, restore)
         if before_update is not None:
             before_update()
         if densify:
@@ -769,12 +832,17 @@ class FlameTrainer:
     No densification (train.py densifies gs / gs_flat only), a constant learning rate per group (update_learning_rate is a
     no-op, gaussian_flame_model.py:226-228), and no optimizer step at the last iteration.  After step(), model.vertices
     holds the pose the step rendered, not the updated parameters' (model.refresh_vertices() moves it; evaluate() does).
-    Views may differ in size: max_size (W, H) as MeshTrainer's.  antialiasing: as MeshTrainer's."""
+    Views may differ in size: max_size (W, H) as MeshTrainer's.  antialiasing: as MeshTrainer's.  detect_anomaly: as
+    MeshTrainer's, with the iteration counter unchanged when step() raises; a NativeFlame driver's parameter gradients are
+    scanned as one more stage (FLAME backward), and the ATen part of any other driver runs under
+    torch.autograd.detect_anomaly() after the frame's record was read."""
 
     def __init__(self, model, bg: torch.Tensor, opt: FlameOptimizationParams = None, sync_free: bool = True,
-                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False):
+                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False, detect_anomaly: bool = False):
         self.model, self.bg = model, bg
         self.antialiasing = bool(antialiasing)
+        self.detect_anomaly = bool(detect_anomaly)
+        self._anomaly = None
         self.max_size = None if max_size is None else (int(max_size[0]), int(max_size[1]))
         self.opt = opt or FlameOptimizationParams()
         self.sync_free = sync_free
@@ -803,25 +871,35 @@ class FlameTrainer:
         if it % 1000 == 0:
             m.oneupSHdegree()
         native = isinstance(m.driver, NativeFlame)
+        aten_anomaly = lambda: torch.autograd.detect_anomaly() if self.detect_anomaly else contextlib.nullcontext()
         if native:
             if self._lbs is None:
                 self._lbs = m.driver.bind(m)
             self._lbs.forward()                  # into model.vertices; zeroes model.vertices.grad
         else:
-            verts = m.driver_vertices()
+            with aten_anomaly():
+                verts = m.driver_vertices()
             with torch.no_grad():
                 m.vertices.copy_(verts)
             m.vertices.grad.zero_()
         self.frame = frame_for(self.frame, cam, self.max_size, lambda W, H: NativeFrame(
             m, W, H, self.opt.lambda_dssim, sync_free=self.sync_free, up_to=True))
         take_step = it < self.opt.iterations         # train.py steps the optimizer on every iteration but the last
-        fused = self.fused_sh and take_step and before_update is None
+        fused = self.fused_sh and take_step and before_update is None and not self.detect_anomaly
         sh_adam = self.adam.begin_fused_sh_step() if fused else None
-        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, sh_adam=sh_adam, antialiasing=self.antialiasing)
+        record = anomaly_record(self._anomaly, self.frame.dev) if self.detect_anomaly else None
+        self._anomaly = record
+        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, sh_adam=sh_adam, antialiasing=self.antialiasing, anomaly=record)
         if native:
             self._lbs.backward()                 # writes the FLAME tensors' flat .grad views
+            if record is not None:
+                record.scan(_lib.ANOMALY_FLAME_BWD, [(i, getattr(m, n).grad) for i, n in enumerate(m.FLAME_NAMES)])
+                check_anomaly(record, m, cam, self.adam, it)
         else:
-            torch.autograd.backward(verts, m.vertices.grad)      # accumulates into the FLAME tensors' flat .grad views
+            if record is not None:               # the frame's stages come first, as in one autograd backward
+                check_anomaly(record, m, cam, self.adam, it)
+            with aten_anomaly():
+                torch.autograd.backward(verts, m.vertices.grad)      # accumulates into the FLAME tensors' flat .grad views
         if frame_end is not None:
             frame_end.record(torch.cuda.current_stream(self.frame.dev))
         if before_update is not None:

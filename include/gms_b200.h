@@ -354,7 +354,12 @@ typedef struct gms_frame_args {
                                    this frame's SH gradient; then d_features and d_color_sh may be NULL */
     const gms_mesh_segment* segments;   /* HOST [n_segments] or NULL: gs_multi_mesh with a K per mesh (see gms_mesh_segment) */
     int32_t n_segments;                 /* 0: one mesh of F faces x K splats, P = F*K */
-    int32_t alpha_activation;           /* as gms_expand_args.alpha_activation (every segment): 0 gs_mesh, 1 gs_flame */
+    uint32_t anomaly_stages;            /* bit (1 << GMS_ANOMALY_*) per stage: LOSS, COMPOSITE_BWD, PREPROCESS_BWD, EXPAND_BWD */
+    uint64_t* anomaly;                  /* optional device record of gms_nan_scan: the outputs of every backward stage selected in
+                                           anomaly_stages are scanned for NaN right after that stage (see "anomaly detection");
+                                           NULL: no scan, the frame's launches are unchanged.  Not with sh_adam (GMS_E_ARG) */
+    int32_t alpha_activation;           /* as gms_expand_args.alpha_activation (every segment): 0 gs_mesh, 1 gs_flame; the trailing
+                                           field, as in gms_render_args and gms_expand_args */
 } gms_frame_args;
 size_t gms_frame_workspace_bytes(int32_t P, int32_t W, int32_t H);
 /* Device pointers into a frame workspace (valid after gms_train_frame): this step's expansion outputs and images. */
@@ -566,6 +571,8 @@ typedef struct gms_free_frame_args {
     uint32_t* n_host_mapped;
     void* event_loss_ready;
     const gms_sh_adam* sh_adam; /* optional: fused Adam step of `features` (M = 16); then d_features may be NULL */
+    uint64_t* anomaly;          /* as in gms_frame_args; the stages are LOSS, COMPOSITE_BWD, PREPROCESS_BWD, ACTIVATION_BWD */
+    uint32_t anomaly_stages;
 } gms_free_frame_args;
 int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void* alloc_user, void* cuda_stream);
 
@@ -853,6 +860,62 @@ typedef struct gms_resize_args {
     size_t scratch_bytes;
 } gms_resize_args;
 int gms_image_resize_u8(const gms_resize_args* a, void* cuda_stream);
+
+/* ---- anomaly detection (train.py --detect_anomaly) ------------------------------------------------ */
+
+/* torch.autograd.set_detect_anomaly(True) for the one-call frames, which run without an autograd graph: the outputs of a
+ * backward stage are scanned for NaN (only NaN, as torch's check: +-inf, denormals and -0 are not reported) and the first
+ * one is recorded in ONE device word
+ *   key = stage << 56 | tensor << 48 | element index (row-major, < 2^48),
+ * the smallest key over every scan since the caller last set the word to GMS_ANOMALY_NONE: the earliest stage, then the
+ * lowest tensor id, then the lowest index.  The scan reads each buffer once with 128-bit loads (scalar head and tail for any
+ * 4-byte-aligned pointer and any length) and makes at most one atomicMin per thread block, only when that block saw a NaN. */
+#define GMS_ANOMALY_NONE 0xFFFFFFFFFFFFFFFFull
+/* stages, in the order a frame runs them */
+#define GMS_ANOMALY_LOSS 0              /* the L1 + SSIM loss kernels */
+#define GMS_ANOMALY_COMPOSITE_BWD 1     /* the composite backward */
+#define GMS_ANOMALY_PREPROCESS_BWD 2    /* the preprocess backward */
+#define GMS_ANOMALY_EXPAND_BWD 3        /* the mesh expansion backward (gms_train_frame), after every segment */
+#define GMS_ANOMALY_ACTIVATION_BWD 4    /* the scale / rotation activation backward (gms_free_train_frame) */
+#define GMS_ANOMALY_FLAME_BWD 5         /* gms_flame_lbs_backward (scanned by the caller through gms_nan_scan) */
+#define GMS_ANOMALY_STAGES 6
+/* tensors of each stage */
+#define GMS_ANOMALY_DIMAGE 0            /* LOSS: dL/dimage [3,H,W] */
+#define GMS_ANOMALY_DGEOM 0             /* COMPOSITE_BWD: the per-Gaussian gradient records [P,12] (gms_debug_views.dgeom) */
+#define GMS_ANOMALY_DMEANS3D 0          /* PREPROCESS_BWD: [P,3] */
+#define GMS_ANOMALY_DSCALES 1           /*   [P,3] w.r.t. the activated scales */
+#define GMS_ANOMALY_DROTATIONS 2        /*   [P,4] w.r.t. the unit quaternions */
+#define GMS_ANOMALY_DOPACITY_RAW 3      /*   [P,1] w.r.t. the opacity logits */
+#define GMS_ANOMALY_DSHS 4              /*   [P,M,3] SH gradient rows (d_features) */
+#define GMS_ANOMALY_DCOLOR_SH 5         /*   [P,3] factored colour gradient (d_color_sh) */
+#define GMS_ANOMALY_DVERTICES 0         /* EXPAND_BWD: [V,3] (accumulated: includes whatever the caller left in it) */
+#define GMS_ANOMALY_DALPHA_RAW 1        /*   [P,3] */
+#define GMS_ANOMALY_DSCALE_RAW 2        /*   [P,1] */
+#define GMS_ANOMALY_DSCALING_RAW 0      /* ACTIVATION_BWD: [P,scale_cols] */
+#define GMS_ANOMALY_DROTATION_RAW 1     /*   [P,4] */
+#define GMS_ANOMALY_ACCUM 2             /*   [P] densification statistic (when gathered) */
+#define GMS_ANOMALY_DSHAPE 0            /* FLAME_BWD: [n_shape] */
+#define GMS_ANOMALY_DEXPRESSION 1       /*   [n_exp] */
+#define GMS_ANOMALY_DPOSE 2             /*   [6] */
+#define GMS_ANOMALY_DNECK_POSE 3        /*   [3] */
+#define GMS_ANOMALY_DTRANSL 4           /*   [3] */
+#define GMS_ANOMALY_DENLARGEMENT 5      /*   [V,3] */
+#define GMS_NAN_SCAN_MAX_BUFFERS 8
+typedef struct gms_nan_buffer {
+    const float* ptr;           /* device, 4-byte aligned; may be NULL when n == 0 */
+    int64_t n;                  /* floats, 0 <= n < 2^48 */
+    int32_t tensor;             /* 0..255 */
+} gms_nan_buffer;
+typedef struct gms_nan_scan_args {
+    gms_nan_buffer buffers[GMS_NAN_SCAN_MAX_BUFFERS];
+    int32_t n_buffers;          /* 0..GMS_NAN_SCAN_MAX_BUFFERS */
+    int32_t stage;              /* 0..GMS_ANOMALY_STAGES-1 */
+    uint64_t* record;           /* device word; left untouched when no buffer holds a NaN */
+} gms_nan_scan_args;
+/* One launch over every buffer of the table (none when they are all empty).  GMS_E_ARG before any launch: a null record,
+ * n < 0 or n >= 2^48, more than GMS_NAN_SCAN_MAX_BUFFERS buffers, a null or misaligned pointer with n > 0, a stage or a tensor
+ * id out of range.  Caller's stream, no host synchronisation. */
+int gms_nan_scan(const gms_nan_scan_args* a, void* cuda_stream);
 
 /* ---- misc ------------------------------------------------------------------------------------- */
 const char* gms_last_error(void);
