@@ -979,10 +979,16 @@ int gms_debug_get_views(const gms_raster_saved* saved, int32_t P, int32_t W, int
     }
     if (saved->binning && (saved->flags & 1)) {
         v->point_list = reinterpret_cast<const uint32_t*>(aligned_base(saved->binning)); v->tile_keys = nullptr;
+        if (saved->flags & 2)       // counting binning: the survivor lists follow the point list (raster_forward_impl)
+            v->surv = reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(v->point_list) +
+                                                        align_up((size_t)saved->binning_capacity * sizeof(uint32_t)));
     } else if (saved->binning && saved->binning_capacity > 0) {
         BinLayout BL = bin_layout(aligned_base(saved->binning), saved->binning_capacity);
         v->point_list = BL.vals_out; v->tile_keys = (saved->flags & 4) ? nullptr : BL.keys_out;     // (16-bit keys: callers derive them from the ranges)
+        if (saved->flags & 2) v->surv = BL.surv;
     }
+    if (v->surv && saved->image) v->nsurv = image_layout(aligned_base(saved->image), W, H).nsurv;
+    if (!v->nsurv) v->surv = nullptr;
     return GMS_OK;
 }
 

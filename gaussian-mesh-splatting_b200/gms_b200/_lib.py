@@ -58,7 +58,8 @@ class DebugViews(C.Structure):
     _fields_ = [("means2D", C.c_void_p), ("depths", C.c_void_p), ("cov3D", C.c_void_p),
                 ("conic_opacity", C.c_void_p), ("rgb", C.c_void_p), ("clamped", C.c_void_p),
                 ("tiles_touched", C.c_void_p), ("point_list", C.c_void_p), ("tile_keys", C.c_void_p),
-                ("ranges", C.c_void_p), ("final_T", C.c_void_p), ("n_contrib", C.c_void_p), ("dgeom", C.c_void_p)]
+                ("ranges", C.c_void_p), ("final_T", C.c_void_p), ("n_contrib", C.c_void_p), ("dgeom", C.c_void_p),
+                ("surv", C.c_void_p), ("nsurv", C.c_void_p)]
 
 
 class ExpandArgs(C.Structure):

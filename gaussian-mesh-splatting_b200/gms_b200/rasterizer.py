@@ -318,4 +318,7 @@ def forward_debug_state(ctx_scratch: _Scratch, num_rendered: int, P: int, W: int
         out["dgeom"] = view(v.dgeom, 12 * P, torch.float32).view(P, 12)     # meaningful after a backward call
     out["final_T"] = view(v.final_T, W * H, torch.float32).view(H, W)
     out["n_contrib"] = view(v.n_contrib, W * H, torch.int32).view(H, W)
+    if v.surv and v.nsurv:      # the forward wrote per-quad survivor lists (flags bit 1): quad q of tile t at 4 * start + q * len
+        out["surv"] = view(v.surv, 4 * int(num_rendered), torch.int32)
+        out["nsurv"] = view(v.nsurv, 4 * T, torch.int32).view(T, 4)
     return out

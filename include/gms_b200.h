@@ -176,6 +176,11 @@ typedef struct gms_debug_views {
     const float* dgeom;          /* [P,12] after a backward call: per-Gaussian sums the composite backward accumulated --
                                     dL/dmean2D.xy (NDC-scaled), dL/dconic.xyz (stock half convention for xy), dL/d(conic_opacity.w),
                                     dL/drgb.rgb, dL/dinvdepth, 2 unused -- i.e. the input of the preprocess backward */
+    const uint32_t* surv;        /* per-quad survivor lists, when the forward wrote them (saved->flags bit 1; else NULL): quad q
+                                    of tile t lists, ascending and relative to the tile's list, the positions whose splat blends
+                                    into at least one in-image pixel of that quad, at [4 * ranges[t].x + q * n_t, + nsurv[4t+q]),
+                                    n_t the length of the tile's list */
+    const uint32_t* nsurv;       /* [4T] the length of each of those lists (NULL when there are none) */
 } gms_debug_views;
 int gms_debug_get_views(const gms_raster_saved* saved, int32_t P, int32_t W, int32_t H, gms_debug_views* views);
 /* The per-Gaussian preprocess results live in packed 48-byte records; this unpacks them into the stock

@@ -880,6 +880,234 @@ int gmso_composite_backward64(const gmso_settings* s, const int32_t* ranges, con
 }
 
 /* =====================================================================
+ * A.2 in float64, with a per-pixel error budget.
+ *
+ * ref[5,H,W]: colour r, g, b, inverse depth and final T of every pixel, on the blend decisions of the fp32 forward above
+ * (gmso_composite_forward: which splats blend, where the pixel stops), every value in double: G = exp() in double of the
+ * canonical fp32 power (quad_power: bit-identical in the kernels, so power <= 0 is never in doubt and edge-on slivers stay
+ * defined), alpha = min(0.99f, op * G), the T product, w = alpha * T, the colour and inverse-depth sums and the T_final * bg
+ * term.  The inputs are the fp32 per-splat record: means2D, conic / opacity, rgb and the fp32 1 / depth the record holds.
+ *
+ * budget[5,H,W]: a first-order bound on |any correct fp32 implementation - ref|, from the operation sequence of the kernels
+ * (k_composite_fwd2: scalar FMAs; k_composite_fwd3: the same roundings on float2 pairs) and of the fp32 oracle (no
+ * contraction, expf).  u = 2^-24.  Per blended splat l, in list order:
+ *   G    = ex2.approx.ftz(power * log2e): 4 u (2^-22) for ex2, |power| * 1.23 u for the rounded argument and log2e, as in
+ *          gmso_composite_backward64 (the oracle's expf is within 1 ulp);
+ *   alpha = op * G: + u, so da_l = alpha_l * ea_l with ea_l = 4 u + 1.23 u |power| + u; the clamp min(0.99f, .) is 1-Lipschitz
+ *          and needs no allowance, and da_l = 0 where op * G * (1 - ea_l) >= 0.99f (both sides take the constant);
+ *   1 - alpha: da_l / (1 - alpha_l) relative (alpha's error amplified by alpha / (1 - alpha)) + u for the subtraction;
+ *   T_{l+1} = T_l * (1 - alpha_l): eT_{l+1} = eT_l + da_l / (1 - alpha_l) + 2 u (relative, eT_1 = 0);
+ *   w_l = alpha_l * T_l: da_l / alpha_l + eT_l + u;
+ *   colour: C_l = fma(c_l, w_l, C_{l-1}) (the oracle: a product and a sum, one more u): |c_l| w_l (da_l / alpha_l + eT_l + 2 u)
+ *          + min(u * sum_{k <= l} |c_k| w_k, |c_l| w_l), the rounding of the partial sum: at most half an ulp of it, and at most
+ *          the term itself, since the old sum is a representable candidate of the rounding (a faint splat that a long sum
+ *          absorbs costs no more than its own term); inverse depth alike;
+ *   final:  fma(T_final, bg, C) (the oracle: two roundings): |bg| T_final (eT_final + 2 u) + min(u (sum_l |c_l| w_l +
+ *          |bg| T_final), |bg| T_final);
+ *   final T: T_final * eT_final.
+ * rgb_tol > 0 adds rgb_tol * (|c_l| + 1) * w_l per blended splat: the colour record is then known to that relative and
+ * absolute tolerance only (a caller without the kernels' own record).
+ *
+ * Decision candidates, from the same bounds (nothing is a fixed band):
+ *   skip:  |alpha - 1/255| <= da: another exp() may blend a splat the fp32 forward skips, or skip one it blends;
+ *   stop:  |T (1 - alpha) - 1e-4| <= T (1 - alpha) (eT + da / (1 - alpha) + 2 u + Wf), Wf = the sum over the skip candidates
+ *          in front of r' = alpha / (1 - alpha) (blended) or alpha (skipped): a flipped skip in front scales this T by
+ *          (1 - alpha)^(-+1).  Tested at every splat the forward reaches with alpha >= 1/255 and, hypothetically, at the
+ *          skip candidates it passes.
+ * Each candidate f adds an ALLOWANCE, to first order what flipping it changes (T_f, the transmittance in front of f; S_f, the
+ * sum of |c_l| w_l over the blended splats behind f):
+ *   (A) f alone blends or not: alpha_f T_f |c_f| + r'_f (S_f + T_final |bg|); final T: r'_f T_final;
+ *   (B) the pixel stops at f (it went on in the forward): sum_{l >= f} |c_l| w_l + |bg| (T_f - T_final); final T: T_f - T_final;
+ *   (C) the pixel goes on past the splat it stopped at: at most all the remaining contributions, T_f (cmax + |bg|) with cmax
+ *       the largest |c| of the tile's list; final T: T_f.
+ * adm[H,W,8]: the admissible n_contrib values: the fp32 forward's, then those the candidates produce ((A): f's position or the
+ * blended one before it; (B): the blended one before f; (C): f's position and every later one the pixel may still blend, by
+ * walking the list with the upper bound of T).  -1 pads; -2 in the last slot: more than fit, any value >= adm[0] is admitted.
+ * cand[H,W] = 1 where the pixel has a candidate.
+ * qhit[N]: bit q of a list position set when its splat blends at some in-image pixel of 8x8 quad q of its tile (the fp32
+ * decisions); qcand[N]: bit q set when a candidate of a pixel of quad q may change whether that splat blends there.
+ * Like the functions above, it covers only the tiles gmso_set_tile_stride selects.
+ * ===================================================================== */
+#define GMSO_NADM 8
+
+typedef struct {
+    int pos, before, blend, stop, skipc, stopc;      /* before: the position of the blended splat in front (0: none) */
+    double a, da, T, eT, W, w, c[3], invd;
+} gmso_f64;
+
+static inline void gmso_adm_add(int32_t* adm, int v) {
+    for (int k = 0; k < GMSO_NADM; k++) {
+        if (adm[k] == v || adm[k] == -2) return;
+        if (adm[k] == -1) { adm[k] = v; return; }
+    }
+    adm[GMSO_NADM - 1] = -2;
+}
+
+int gmso_composite_forward64(const gmso_settings* s, const int32_t* ranges, const uint32_t* point_list,
+                             const float* means2D, const float* rgb, const float* conic_opacity, const float* depths,
+                             double rgb_tol, double* ref /*[5,H,W]*/, double* budget /*[5,H,W]*/, double* allowance /*[5,H,W]*/,
+                             int32_t* adm /*[H,W,8]*/, uint8_t* cand /*[H,W]*/, uint8_t* qhit /*[N]*/, uint8_t* qcand /*[N]*/) {
+    const int W = s->W, H = s->H;
+    const size_t HW = (size_t)W * H;
+    const int gx = (W + GMSO_BLOCK - 1) / GMSO_BLOCK, gy = (H + GMSO_BLOCK - 1) / GMSO_BLOCK;
+    const double u = GMSO_U, amax = (double)0.99f, thr = (double)(1.0f / 255.0f), tstop = (double)0.0001f;
+    const double bgc[3] = {s->bg[0], s->bg[1], s->bg[2]};
+    const double bga[3] = {fabs(bgc[0]), fabs(bgc[1]), fabs(bgc[2])};
+    int maxlen = 1;
+    for (int t = 0; t < gx * gy; t++) maxlen = imax(maxlen, ranges[2 * t + 1] - ranges[2 * t]);
+    memset(ref, 0, sizeof(double) * 5 * HW);
+    memset(budget, 0, sizeof(double) * 5 * HW);
+    memset(allowance, 0, sizeof(double) * 5 * HW);
+    memset(cand, 0, HW);
+    for (size_t k = 0; k < GMSO_NADM * HW; k++) adm[k] = -1;
+#pragma omp parallel
+    {
+        gmso_f64* e = (gmso_f64*)malloc(sizeof(gmso_f64) * (size_t)maxlen);
+#pragma omp for schedule(dynamic, 1)
+        for (int tile = 0; tile < gx * gy; tile++) {
+            if (tile % g_tile_stride) continue;
+            const int tx0 = (tile % gx) * GMSO_BLOCK, ty0 = (tile / gx) * GMSO_BLOCK;
+            const int r0 = ranges[2 * tile], r1 = ranges[2 * tile + 1];
+            double cmax[3] = {0.0, 0.0, 0.0}, dmax = 0.0;
+            for (int j = r0; j < r1; j++) {
+                const uint32_t g = point_list[j];
+                for (int ch = 0; ch < 3; ch++) cmax[ch] = fmax(cmax[ch], fabs((double)rgb[3 * g + ch]));
+                dmax = fmax(dmax, fabs((double)(1.f / depths[g])));
+            }
+            for (int j = r0; j < r1; j++) { qhit[j] = 0; qcand[j] = 0; }
+            for (int py = ty0; py < ty0 + GMSO_BLOCK && py < H; py++)
+                for (int px = tx0; px < tx0 + GMSO_BLOCK && px < W; px++) {
+                    const size_t pix = (size_t)py * W + px;
+                    const uint8_t qb = (uint8_t)(1u << (((py - ty0) >> 3) * 2 + ((px - tx0) >> 3)));
+                    const float pfx = (float)px, pfy = (float)py;
+                    int32_t* ad = adm + GMSO_NADM * pix;
+                    /* front to back: the fp32 forward's decisions (T32), the double values, the rounding bounds */
+                    float T32 = 1.0f;
+                    double T = 1.0, eT = 0.0, Wf = 0.0, C[3] = {0.0, 0.0, 0.0}, D = 0.0, Cabs[3] = {0.0, 0.0, 0.0}, Dabs = 0.0;
+                    double errC[3] = {0.0, 0.0, 0.0}, errD = 0.0;
+                    int n = 0, last = 0, stop_at = -1;
+                    for (int jj = 0; jj < r1 - r0; jj++) {
+                        const uint32_t g = point_list[r0 + jj];
+                        const float dx = means2D[2 * g] - pfx, dy = means2D[2 * g + 1] - pfy;
+                        const float* co = conic_opacity + 4 * g;
+                        const float power = quad_power(co, dx, dy);
+                        if (power > 0.0f) continue;
+                        const float a32 = fminf(0.99f, co[3] * expf(power));
+                        const double G = exp((double)power), opG = (double)co[3] * G, a = fmin(amax, opG);
+                        const double ea = 4.0 * u + 1.23 * u * fabs((double)power) + u;
+                        const double da = opG * (1.0 - ea) >= amax ? 0.0 : a * ea;
+                        const int skipc = fabs(a - thr) <= da;
+                        const int blendable = a32 >= 1.0f / 255.0f;
+                        if (!blendable && !skipc) continue;
+                        const float test32 = T32 * (1.f - a32);
+                        const int stop = blendable && test32 < 0.0001f;
+                        const int blend = blendable && !stop;
+                        gmso_f64* x = e + n++;
+                        x->pos = jj + 1; x->before = last; x->blend = blend; x->stop = stop; x->skipc = skipc;
+                        x->a = a; x->da = da; x->T = T; x->eT = eT; x->W = Wf; x->w = 0.0;
+                        for (int ch = 0; ch < 3; ch++) x->c[ch] = rgb[3 * g + ch];
+                        x->invd = (double)(1.f / depths[g]);
+                        const double tT = T * (1.0 - a);
+                        x->stopc = fabs(tT - tstop) <= tT * (eT + da / (1.0 - a) + 2.0 * u + Wf);
+                        if (skipc) Wf += blend ? a / (1.0 - a) : a;
+                        if (blend) {
+                            const double w = a * T, ew = da / a + eT + 2.0 * u;
+                            x->w = w;
+                            for (int ch = 0; ch < 3; ch++) {
+                                const double cw = fabs(x->c[ch]) * w;
+                                C[ch] += x->c[ch] * w;
+                                Cabs[ch] += cw;
+                                errC[ch] += cw * ew + fmin(u * Cabs[ch], cw) + rgb_tol * (fabs(x->c[ch]) + 1.0) * w;
+                            }
+                            D += x->invd * w;
+                            Dabs += fabs(x->invd) * w;
+                            errD += fabs(x->invd) * w * ew + fmin(u * Dabs, fabs(x->invd) * w);
+                            T = tT;
+                            eT += da / (1.0 - a) + 2.0 * u;
+                            T32 = test32;
+                            last = jj + 1;
+                            qhit[r0 + jj] |= qb;
+                        }
+                        if (stop) { stop_at = n - 1; break; }
+                    }
+                    const double Tfin = T;
+                    ad[0] = last;
+                    for (int ch = 0; ch < 3; ch++) {
+                        ref[ch * HW + pix] = C[ch] + Tfin * bgc[ch];
+                        budget[ch * HW + pix] = errC[ch] + bga[ch] * Tfin * (eT + 2.0 * u) + fmin(u * (Cabs[ch] + bga[ch] * Tfin), bga[ch] * Tfin);
+                    }
+                    ref[3 * HW + pix] = D;
+                    budget[3 * HW + pix] = errD;
+                    ref[4 * HW + pix] = Tfin;
+                    budget[4 * HW + pix] = Tfin * eT;
+                    /* allowances: S[k] = sum over the blended splats from entry k on of |c| w (and invd w) */
+                    double S[3] = {0.0, 0.0, 0.0}, Sd = 0.0, al[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+                    int any = 0;
+                    for (int k = n - 1; k >= 0; k--) {
+                        gmso_f64* f = e + k;
+                        const double Sb[3] = {S[0], S[1], S[2]}, Sdb = Sd;     /* behind f */
+                        for (int ch = 0; ch < 3; ch++) S[ch] += fabs(f->c[ch]) * f->w;
+                        Sd += fabs(f->invd) * f->w;
+                        const int before = f->before;
+                        if (f->skipc && !f->stop) {                             /* (A) */
+                            const double r = f->blend ? f->a / (1.0 - f->a) : f->a;
+                            for (int ch = 0; ch < 3; ch++) al[ch] += f->a * f->T * fabs(f->c[ch]) + r * (Sb[ch] + Tfin * bga[ch]);
+                            al[3] += f->a * f->T * fabs(f->invd) + r * Sdb;
+                            al[4] += r * Tfin;
+                            if (f->blend && f->pos == last) gmso_adm_add(ad, before);
+                            if (!f->blend && f->pos > last) gmso_adm_add(ad, f->pos);
+                            qcand[r0 + f->pos - 1] |= qb;
+                            any = 1;
+                        }
+                        if (f->stopc && (f->blend || (!f->stop && f->skipc))) {   /* (B) */
+                            for (int ch = 0; ch < 3; ch++) al[ch] += S[ch] + bga[ch] * (f->T - Tfin);
+                            al[3] += Sd;
+                            al[4] += f->T - Tfin;
+                            gmso_adm_add(ad, before);
+                            for (int m = k; m < n; m++) if (e[m].blend) qcand[r0 + e[m].pos - 1] |= qb;
+                            any = 1;
+                        }
+                        if (k == stop_at && (f->stopc || f->skipc)) {         /* (C) */
+                            for (int ch = 0; ch < 3; ch++) al[ch] += f->T * (cmax[ch] + bga[ch]);
+                            al[3] += f->T * dmax;
+                            al[4] += f->T;
+                            any = 1;
+                            /* the positions the pixel may still blend: walk on with the upper bound of T */
+                            const double rel = 1.0 + f->eT + f->W + 2.0 * u;
+                            double Thi = f->skipc ? f->T * rel : 0.0;
+                            if (f->stopc) {
+                                gmso_adm_add(ad, f->pos);
+                                qcand[r0 + f->pos - 1] |= qb;
+                                Thi = fmax(Thi, f->T * (1.0 - f->a + f->da) * rel);
+                            }
+                            for (int jj = f->pos; jj < r1 - r0; jj++) {
+                                const uint32_t g = point_list[r0 + jj];
+                                const float dx = means2D[2 * g] - pfx, dy = means2D[2 * g + 1] - pfy;
+                                const float* co = conic_opacity + 4 * g;
+                                const float power = quad_power(co, dx, dy);
+                                if (power > 0.0f) continue;
+                                const double G = exp((double)power), opG = (double)co[3] * G, a = fmin(amax, opG);
+                                const double ea = 4.0 * u + 1.23 * u * fabs((double)power) + u;
+                                const double da = opG * (1.0 - ea) >= amax ? 0.0 : a * ea;
+                                if (a + da < thr) continue;
+                                const int canskip = a - da < thr;
+                                const int canblend = Thi * (1.0 - a + da) >= tstop;
+                                if (canblend) { gmso_adm_add(ad, jj + 1); qcand[r0 + jj] |= qb; }
+                                if (!canskip && !canblend) break;
+                                if (!canskip) Thi *= 1.0 - a + da;
+                            }
+                        }
+                    }
+                    for (int c = 0; c < 5; c++) { allowance[c * HW + pix] = al[c]; budget[c * HW + pix] += al[c]; }
+                    cand[pix] = (uint8_t)any;
+                }
+        }
+        free(e);
+    }
+    return 0;
+}
+
+/* =====================================================================
  * A.4 preprocess backward (computeCov2D backward + projection + SH + cov3D).
  * Inputs are the per-Gaussian gradients from the composite backward (float).
  * ===================================================================== */

@@ -274,6 +274,33 @@ def composite_backward64(st: ForwardState, dL_dcolor, dL_dinvdepth=None) -> dict
     return out
 
 
+FWD64_OUTPUTS = ("r", "g", "b", "invdepth", "final_T")
+
+
+def composite_forward64(st: ForwardState, rgb=None, rgb_tol: float = 0.0) -> dict:
+    """The composite forward evaluated in float64 on the fp32 forward's blend decisions, with a per-pixel error budget
+    (gmso_composite_forward64 in gms_oracle.c derives it).  Returns ref [5,H,W] and budget [5,H,W] (colour r/g/b, inverse
+    depth, final T), allowance [5,H,W] (the share of the budget from flip candidates), adm [H,W,8] (admissible n_contrib;
+    -1 pads, -2 admits any value >= adm[..., 0]), cand [H,W] (pixels with a flip candidate), qhit [N] and qcand [N] (per list
+    position, bit q: the splat blends at / may flip at some pixel of quad q of its tile).  `rgb` [P,3] replaces the oracle's
+    colours (the kernels' own record); `rgb_tol` widens the budget for a colour record known only to that tolerance."""
+    H, W = st.settings.image_height, st.settings.image_width
+    rgb = st.rgb if rgb is None else np.ascontiguousarray(rgb, dtype=np.float32).reshape(st.rgb.shape)
+    n = max(st.N, 1)
+    out = dict(ref=np.zeros((5, H, W)), budget=np.zeros((5, H, W)), allowance=np.zeros((5, H, W)),
+               adm=np.zeros((H, W, 8), np.int32), cand=np.zeros((H, W), np.uint8), qhit=np.zeros(n, np.uint8),
+               qcand=np.zeros(n, np.uint8))
+    pl = st.point_list if st.N > 0 else np.zeros(1, np.uint32)
+    rc = lib().gmso_composite_forward64(ctypes.byref(st.cs), _p(st.ranges), _p(pl), _p(st.means2D), _p(rgb),
+                                        _p(st.conic_opacity), _p(st.depths), ctypes.c_double(rgb_tol), _p(out["ref"]),
+                                        _p(out["budget"]), _p(out["allowance"]), _p(out["adm"]), _p(out["cand"]),
+                                        _p(out["qhit"]), _p(out["qcand"]))
+    if rc != 0:
+        raise RuntimeError(f"gmso_composite_forward64 failed rc={rc}")
+    out["qhit"], out["qcand"] = out["qhit"][:st.N], out["qcand"][:st.N]
+    return out
+
+
 def preprocess_backward(st: ForwardState, g: dict) -> dict:
     P = st.radii.shape[0]
     inp = st.inputs

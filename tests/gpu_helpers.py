@@ -92,10 +92,11 @@ def oracle_chain(p, S, dC, gpu, triangles=None):
 
 
 def assert_forward_parity(st, color, radii, invd, state, tol=1e-5, max_ambiguous=5e-4):
-    """Bit-exact indices, <= tol per pixel (threshold-ambiguous pixels get a bounded looser check; at most `max_ambiguous` of
-    the image may be threshold-ambiguous)."""
+    """Bit-exact indices, <= tol per pixel outside the threshold-ambiguous pixels (at most `max_ambiguous` of the image), and
+    every pixel within its per-pixel budget (assert_composite_forward_per_pixel).  Returns the worst err / budget per output."""
     np.testing.assert_array_equal(radii, st.radii)
     assert state["num_rendered"] == st.N
+    rgb = None
     if st.radii.shape[0]:
         np.testing.assert_array_equal(state["tiles_touched"].astype(np.uint32), st.tiles_touched)
         vis = st.radii > 0
@@ -105,33 +106,130 @@ def assert_forward_parity(st, color, radii, invd, state, tol=1e-5, max_ambiguous
         np.testing.assert_array_equal(state["cov3D"].view(np.uint32)[vis], st.cov3Ds.view(np.uint32)[vis])
         np.testing.assert_array_equal(state["clamped"][vis], st.clamped[vis])
         np.testing.assert_allclose(state["rgb"][vis], st.rgb[vis], rtol=1e-6, atol=1e-6)
+        rgb = np.where(vis[:, None], state["rgb"], st.rgb)       # the colour record the kernels composite
     np.testing.assert_array_equal(state["point_list"].astype(np.uint32), st.point_list)
     np.testing.assert_array_equal(state["tile_keys"].astype(np.uint64), st.keys_sorted >> np.uint64(32))
     np.testing.assert_array_equal(state["ranges"], st.ranges)
-    ok = assert_image_parity(st, color, tol, max_ambiguous)
+    ok = assert_image_parity(st, color, tol, max_ambiguous, per_pixel=False)
     np.testing.assert_array_equal(state["n_contrib"][ok], st.n_contrib[ok])
     assert np.abs(invd - st.invdepth)[:, ok].max() <= tol
     assert np.abs(state["final_T"] - st.final_T)[ok].max() <= tol
+    return assert_composite_forward_per_pixel(st, color, invd, state["final_T"], state["n_contrib"], state.get("surv"),
+                                              state.get("nsurv"), rgb=rgb)
 
 
-def assert_image_parity(st, color, tol=1e-5, max_ambiguous=5e-4):
+# The per-splat colour record the kernels composite is held to the oracle's to 1e-6 relative and absolute
+# (assert_forward_parity); a caller that has only the image composites the oracle's record within that tolerance.
+RGB_RECORD_TOL = 1e-6
+
+
+def assert_image_parity(st, color, tol=1e-5, max_ambiguous=5e-4, per_pixel=True):
     """<= tol per pixel outside the threshold-ambiguous pixels; returns the mask of those other pixels.
     Threshold-ambiguous pixels: the oracle flags a pixel when one of its skip / stop decisions (alpha < 1/255,
     T(1-alpha) < 1e-4) lies within the +-1e-6 relative band in which exp() (GPU: ex2.approx.ftz) may fall on the other side.
-    They are REPORTED (count, worst error) and bounded by the largest change one flipped decision can cause: a splat
-    blended at alpha = 1/255 with unit transmittance moves a channel by <= |c - behind| / 255 <= max colour / 255."""
+    They are REPORTED (count, worst error) and, with `per_pixel`, every pixel is held to its per-pixel budget, whose
+    allowance covers the decisions an exp() may flip (assert_composite_forward_per_pixel; assert_forward_parity runs that
+    check on every output itself)."""
     ok = st.ambiguous == 0
     n_amb = int((~ok).sum())
     err = np.abs(color - st.color)
     err_ok = float(err[:, ok].max()) if ok.any() else 0.0
     err_amb = float(err[:, ~ok].max()) if n_amb else 0.0
-    cmax = float(max(1.0, np.abs(st.rgb).max())) if st.radii.shape[0] else 1.0
     print(f"[parity] {st.settings.image_width}x{st.settings.image_height} P={st.radii.shape[0]} N={st.N}: max|image-oracle| = {err_ok:.2e}; "
-          f"threshold-ambiguous pixels = {n_amb} ({n_amb / ok.size:.1e} of the image), worst there = {err_amb:.2e} (bound {cmax / 255:.1e})")
+          f"threshold-ambiguous pixels = {n_amb} ({n_amb / ok.size:.1e} of the image), worst there = {err_amb:.2e}")
     assert n_amb <= max(4, max_ambiguous * ok.size), f"too many threshold-ambiguous pixels: {n_amb}"
     assert err_ok <= tol, err_ok
-    assert err_amb <= 2.0 * cmax / 255.0, err_amb
+    if per_pixel:
+        assert_composite_forward_per_pixel(st, color, rgb_tol=RGB_RECORD_TOL)
     return ok
+
+
+def forward_budget_ratios(got, ref, budget):
+    """|got - ref| / budget (0 where both are exactly equal, inf where the budget is 0 and the value is not, NaN where the
+    value is NaN)."""
+    err = np.abs(np.asarray(got, np.float64) - ref)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.where(err == 0, 0.0, err / budget)
+
+
+def n_contrib_admissible(n_contrib, adm):
+    """Per pixel: n_contrib is one of the admissible values of oracle.raster.composite_forward64 (-2: any value >= the first)."""
+    n = np.asarray(n_contrib).astype(np.int64)
+    return (adm == n[..., None]).any(-1) | ((adm[..., -1] == -2) & (n >= adm[..., 0]))
+
+
+def survivor_mismatch(st, surv, nsurv, qhit, qcand):
+    """Positions of the tile lists at which the per-quad survivor lists differ from the oracle's quad-hit mask outside the
+    flip candidates of that quad, and the tiles whose lists are not strictly ascending or run past the tile's list."""
+    got = np.zeros(st.N, np.uint8)
+    bad_tiles = []
+    surv = np.asarray(surv).astype(np.int64)
+    for t, (r0, r1) in enumerate(st.ranges):
+        n = int(r1 - r0)
+        for q in range(4):
+            c = int(nsurv[t, q])
+            lst = surv[4 * r0 + q * n: 4 * r0 + q * n + c] if c else surv[:0]
+            if c > n or lst.size != c or (c and (lst.min() < 0 or lst.max() >= n or (np.diff(lst) <= 0).any())):
+                bad_tiles.append(t)
+                continue
+            got[r0 + lst] |= np.uint8(1 << q)
+    return np.flatnonzero((got ^ qhit) & ~qcand), bad_tiles
+
+
+FWD_OUTPUTS = ("r", "g", "b", "invdepth", "final_T")
+
+
+def assert_composite_forward_per_pixel(st, color, invd=None, final_T=None, n_contrib=None, surv=None, nsurv=None, rgb=None,
+                                       rgb_tol=0.0, r=None, label=""):
+    """Every pixel of the composite forward against the float64 reference of oracle.raster.composite_forward64, within its
+    a-priori budget (the derivation is next to gmso_composite_forward64): colour, and when given inverse depth and final T,
+    each within budget; n_contrib admissible; no NaN or Inf anywhere; survivor lists equal to the oracle's quad-hit mask
+    bit for bit, except at the flip candidates of a quad.  Prints the worst err / budget per output; returns them."""
+    if r is None:
+        r = raster.composite_forward64(st, rgb=rgb, rgb_tol=rgb_tol)
+    ref, bud = r["ref"], r["budget"]
+    assert np.isfinite(ref).all() and np.isfinite(bud).all(), "non-finite float64 reference or budget"
+    H, W = st.final_T.shape
+    got = [np.asarray(color, np.float64).reshape(3, H, W)]
+    outs = [0, 1, 2]
+    if invd is not None:
+        got.append(np.asarray(invd, np.float64).reshape(1, H, W)); outs.append(3)
+    if final_T is not None:
+        got.append(np.asarray(final_T, np.float64).reshape(1, H, W)); outs.append(4)
+    got = np.concatenate(got)
+    finite = np.isfinite(got)
+    assert finite.all(), (f"non-finite composite forward at {int((~finite).sum())} values, e.g. "
+                          f"{FWD_OUTPUTS[outs[np.argwhere(~finite)[0][0]]]} pixel {np.argwhere(~finite)[0][1:].tolist()}")
+    ratio = forward_budget_ratios(got, ref[outs], bud[outs])
+    worst = {FWD_OUTPUTS[o]: float(ratio[k].max()) for k, o in enumerate(outs)}
+    cand = r["cand"].astype(bool)
+    amb = st.ambiguous.astype(bool)
+    adm_ok = n_contrib_admissible(n_contrib, r["adm"]) if n_contrib is not None else None
+    flips = int((np.asarray(n_contrib) != st.n_contrib).sum()) if n_contrib is not None else 0
+    mism, bad_tiles = (survivor_mismatch(st, surv, nsurv, r["qhit"], r["qcand"]) if surv is not None and nsurv is not None
+                       else (np.zeros(0, np.int64), []))
+    print(f"[per-pixel{(' ' + label) if label else ''}] worst |gpu - ref| / budget: "
+          + ", ".join(f"{k} {v:.3g}" for k, v in worst.items())
+          + f"; flip-candidate pixels {int(cand.sum())}, old ambiguous {int(amb.sum())}, both {int((cand & amb).sum())}"
+          + (f"; n_contrib off the fp32 oracle's at {flips}" if n_contrib is not None else "")
+          + (f"; survivor lists checked ({st.N} positions)" if surv is not None and nsurv is not None else ""))
+    bad = np.argwhere(~(ratio <= 1))
+    if bad.shape[0]:
+        k, y, x = bad[0]
+        o = outs[k]
+        raise AssertionError(
+            f"composite forward outside its budget at {bad.shape[0]} values, e.g. {FWD_OUTPUTS[o]} pixel (x={x}, y={y}): "
+            f"gpu {got[k, y, x]:.9g} ref {ref[o, y, x]:.9g} |err| {abs(got[k, y, x] - ref[o, y, x]):.3g} budget "
+            f"{bud[o, y, x]:.3g} (allowance {r['allowance'][o, y, x]:.3g}); flip candidate {bool(cand[y, x])}, n_contrib "
+            f"{int(np.asarray(n_contrib)[y, x]) if n_contrib is not None else '-'} (oracle {int(st.n_contrib[y, x])})")
+    if adm_ok is not None:
+        nb = np.argwhere(~adm_ok)
+        assert nb.shape[0] == 0, (f"n_contrib not admissible at {nb.shape[0]} pixels, e.g. (x={nb[0][1]}, y={nb[0][0]}): "
+                                  f"{int(np.asarray(n_contrib)[tuple(nb[0])])}, admissible {r['adm'][tuple(nb[0])].tolist()}")
+    assert not bad_tiles, f"survivor lists malformed (not ascending, or past the list) in tiles {bad_tiles[:8]}"
+    assert mism.size == 0, (f"survivor lists differ from the quad-hit mask at {mism.size} list positions outside the flip "
+                            f"candidates, e.g. position {int(mism[0])}")
+    return worst
 
 
 # Gradients w.r.t. scales / rotations / cov3D go through the inverse of a nearly singular 2D covariance (flat mesh
