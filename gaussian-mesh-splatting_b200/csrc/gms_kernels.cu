@@ -31,6 +31,7 @@
 #include "gms_lpips.cuh"
 #include "gms_alpha.cuh"
 #include "gms_anomaly.cuh"
+#include "gms_debug.cuh"
 
 // ------------------------------------------------------------------------------------------ host state
 static thread_local char g_err[512] = "";
@@ -70,12 +71,12 @@ static int sm_count() {
 
 // Optional per-kernel timing with CUDA events recorded on the launching stream (bench.py's roofline numbers).
 enum { K_PRE_FWD = 0, K_SORT_P, K_SCAN, K_EMIT, K_SORT_N, K_RANGES, K_COMP_FWD, K_COMP_BWD, K_PRE_BWD, K_EXP_FWD, K_EXP_BWD, K_LOSS_STATS, K_LOSS_GRAD, K_ADAM, K_MISC,
-       K_METRICS, K_METRICS_FIN, K_LPIPS_CONV, K_LPIPS_POOL, K_LPIPS_HEAD, K_NAN_SCAN, K_COUNT };
+       K_METRICS, K_METRICS_FIN, K_LPIPS_CONV, K_LPIPS_POOL, K_LPIPS_HEAD, K_NAN_SCAN, K_DEBUG, K_COUNT };
 static const char* const g_kernel_names[K_COUNT] = {"preprocess_fwd", "cub_sort_depth", "cub_scan_tiles", "emit_dups", "cub_sort_tiles",
                                                     "tile_ranges", "composite_fwd", "composite_bwd", "preprocess_bwd", "expand_fwd",
                                                     "expand_bwd", "ssim_stats", "ssim_grad", "adam", "misc",
                                                     "image_metrics", "metrics_finalize", "lpips_conv", "lpips_pool",
-                                                    "lpips_head", "nan_scan"};
+                                                    "lpips_head", "nan_scan", "debug_check"};
 static int g_opt_time = 0;
 struct TimedSpan { int id; cudaEvent_t a, b; };
 static TimedSpan g_spans[1 << 15];
@@ -291,6 +292,65 @@ static int anomaly_hook(uint64_t* record, uint32_t stages, int stage, std::initi
     return nan_scan_launch(stage, bufs.begin(), (int)bufs.size(), record, dbg, st);
 }
 
+// Debug mode: wait for work queued outside launch() (the cub sorts and scan, the hand-written sort) and name it on a fault.
+static int debug_sync(const char* what, cudaStream_t st) {
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return set_err(GMS_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
+    return GMS_OK;
+}
+
+// The binning check's record lives in the library, not in a caller's workspace: one per device and host thread, so checks on
+// different devices, or from different threads, never share one (a record is allocated on first use and kept).
+#define GMS_DBG_MAX_DEVICES 64
+static thread_local GmsBinRecord* t_bin_rec[GMS_DBG_MAX_DEVICES];
+
+// The binning check (gms_debug.cuh) of `c`: the list and its ranges (k_debug_ranges, k_debug_list), or with `surv` the
+// per-quad survivor lists (k_debug_surv).  Synchronises the stream and reads the record (into *out when given): GMS_E_DEBUG
+// on a violation.
+static int bins_check(GmsBinCheck c, bool surv, cudaStream_t st, GmsBinRecord* out = nullptr) {
+    int dev = 0;
+    GMS_CUDA(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= GMS_DBG_MAX_DEVICES) return set_err(GMS_E_UNSUPPORTED, "binning check: device ordinal %s%s", "out of range");
+    GmsBinRecord*& rec = t_bin_rec[dev];
+    if (!rec) GMS_CUDA(cudaMalloc(reinterpret_cast<void**>(&rec), sizeof(GmsBinRecord)));
+    c.rec = rec;
+    GMS_CUDA(cudaMemsetAsync(c.rec, 0xFF, sizeof(GmsBinRecord), st));
+    GMS_CUDA(cudaMemsetAsync(&c.rec->area, 0, sizeof(c.rec->area), st));
+    int rc;
+    if (surv) {
+        if ((rc = launch("debug_surv", K_DEBUG, 1, st, (unsigned)((4 * (int64_t)c.T + GMS_DBG_BLOCK / 32 - 1) / (GMS_DBG_BLOCK / 32)),
+                         GMS_DBG_BLOCK, 0, k_debug_surv, c))) return rc;
+    } else {
+        if ((rc = launch("debug_ranges", K_DEBUG, 1, st, 1, GMS_DBG_RANGES_BLOCK, 0, k_debug_ranges, c))) return rc;
+        if ((rc = launch("debug_list", K_DEBUG, 1, st, (unsigned)(((int64_t)c.T + GMS_DBG_BLOCK / 32 - 1) / (GMS_DBG_BLOCK / 32)),
+                         GMS_DBG_BLOCK, 0, k_debug_list, c))) return rc;
+    }
+    GmsBinRecord h;
+    GMS_CUDA(cudaMemcpyAsync(&h, c.rec, sizeof(h), cudaMemcpyDeviceToHost, st));
+    GMS_CUDA(cudaStreamSynchronize(st));
+    if (out) *out = h;
+    static const char* const what[5] = {"", "point list order", "tile ranges", "entry Gaussian", "survivor list"};
+    char msg[400];
+    if (h.key != GMS_DEBUG_NONE) {
+        const int check = (int)(h.key >> 56);
+        const unsigned long long index = h.key & ((1ull << 56) - 1);
+        const uint32_t gid = (uint32_t)h.gid[check], tile = (uint32_t)h.tile[check];
+        char g[32] = "none", t[32] = "none";
+        if (gid != GMS_DBG_NONE) snprintf(g, sizeof(g), "%u", gid);
+        if (tile != GMS_DBG_NONE) snprintf(t, sizeof(t), "%u", tile);
+        snprintf(msg, sizeof(msg), "binning check %d (%s) failed at %s %llu, tile %s, Gaussian %s", check, what[check],
+                 check == GMS_DEBUG_SURVIVOR ? "survivor slot" : "list index", index, t, g);
+        return set_err(GMS_E_DEBUG, "%s%s", msg);
+    }
+    if (!surv && h.n != ~0ull && h.area != h.n) {
+        snprintf(msg, sizeof(msg), "binning check 2 (tile ranges) failed at list index %llu, tile none, Gaussian none: the "
+                 "ranges hold %llu entries but the Gaussians' tile rectangles cover %llu tiles", h.n, h.n, h.area);
+        return set_err(GMS_E_DEBUG, "%s%s", msg);
+    }
+    return GMS_OK;
+}
+
 // ------------------------------------------------------------------------------------------ whole-frame orchestration
 
 // The workspace of a forward-only frame: the activated Gaussians an expansion step writes, and sigmoid(opacity).
@@ -345,8 +405,8 @@ static GmsGaussWin ssim_window() {
     return win;
 }
 
-int gms_l1_ssim_loss(const gms_loss_args* a, void* cuda_stream) {
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+// gms_l1_ssim_loss, with every launch waited for under `dbg` (the training frames' debug mode)
+static int l1_ssim_loss(const gms_loss_args* a, int dbg, cudaStream_t st) {
     if (!a || !a->img || !a->gt || !a->loss || !a->scratch) return set_err(GMS_E_ARG, "gms_l1_ssim_loss: null argument%s%s");
     const int C = a->C, H = a->H, W = a->W;
     size_t need = 0;
@@ -359,13 +419,17 @@ int gms_l1_ssim_loss(const gms_loss_args* a, void* cuda_stream) {
     GMS_CUDA(cudaMemsetAsync(acc, 0, 2 * sizeof(float), st));
     dim3 grid((W + GMS_SSIM_T - 1) / GMS_SSIM_T, (H + GMS_SSIM_T - 1) / GMS_SSIM_T, C);
     int rc;
-    if ((rc = launch("ssim_stats", K_LOSS_STATS, 0, st, grid, 256, 0, k_ssim_stats, C, H, W, a->img, a->gt, win,
+    if ((rc = launch("ssim_stats", K_LOSS_STATS, dbg, st, grid, 256, 0, k_ssim_stats, C, H, W, a->img, a->gt, win,
                      a->dL_dimg ? dmap : nullptr, acc))) return rc;
     const float inv_n = 1.0f / ((float)C * (float)H * (float)W);
-    if ((rc = launch("loss_finalize", -1, 0, st, 1, 1, 0, k_loss_finalize, acc, inv_n, a->lambda_dssim, a->loss))) return rc;
+    if ((rc = launch("loss_finalize", -1, dbg, st, 1, 1, 0, k_loss_finalize, acc, inv_n, a->lambda_dssim, a->loss))) return rc;
     if (!a->dL_dimg) return GMS_OK;
-    return launch("ssim_grad", K_LOSS_GRAD, 0, st, grid, 256, 0, k_ssim_grad, C, H, W, a->img, a->gt, win, dmap,
+    return launch("ssim_grad", K_LOSS_GRAD, dbg, st, grid, 256, 0, k_ssim_grad, C, H, W, a->img, a->gt, win, dmap,
                   -a->lambda_dssim * inv_n, (1.f - a->lambda_dssim) * inv_n, a->dL_dloss, a->dL_dimg);
+}
+
+int gms_l1_ssim_loss(const gms_loss_args* a, void* cuda_stream) {
+    return l1_ssim_loss(a, 0, reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
 static int metric_tiles(int32_t H, int32_t W) { return ((W + GMS_SSIM_T - 1) / GMS_SSIM_T) * ((H + GMS_SSIM_T - 1) / GMS_SSIM_T); }
@@ -637,27 +701,37 @@ static PreArgs make_pre_args(const gms_raster_settings* s, const gms_raster_inpu
 }
 
 // The end of a forward with a binned point list: tiles in launch order, then the composite forward, which writes the
-// per-quad survivor lists to `surv` when `emit`.
+// per-quad survivor lists to `surv` when `emit`.  With `chk` (a one-call frame under debug) the binning check runs on the list
+// and its ranges before the composite, and on the survivor lists after it.
 static int composite_forward(const gms_raster_settings* s, const gms_raster_outputs* out, const ImageLayout& IL, const float4* rec,
-                             const uint32_t* point_list, bool emit, uint32_t* surv, int T, cudaStream_t st) {
+                             const uint32_t* point_list, bool emit, uint32_t* surv, int T, cudaStream_t st,
+                             const GmsBinCheck* chk) {
     const int W = s->image_width, H = s->image_height, gx = (W + GMS_TILE - 1) / GMS_TILE;
     const int dbg = s->debug;
     int rc;
+    if (chk && (rc = bins_check(*chk, false, st))) return rc;
     if (g_opt_tile_order && (rc = launch("tile_order", -1, dbg, st, 1, 1024, 0, k_tile_order, T, IL.ranges, IL.tile_order))) return rc;
     const int* to = g_opt_tile_order ? IL.tile_order : nullptr;
     if (g_opt_fwd == 3)
-        return launch("composite_fwd", K_COMP_FWD, dbg, st, T, GMS_CB, 0, k_composite_fwd3, IL.ranges, to, point_list, rec, W, H, gx, s->bg,
-                      out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth);
-    return launch("composite_fwd", K_COMP_FWD, dbg, st, T, GMS_CB, 0, emit ? k_composite_fwd2<true> : k_composite_fwd2<false>, IL.ranges,
-                  to, point_list, rec, W, H, gx, s->bg, out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth,
-                  emit ? surv : nullptr, emit ? IL.nsurv : nullptr);
+        rc = launch("composite_fwd", K_COMP_FWD, dbg, st, T, GMS_CB, 0, k_composite_fwd3, IL.ranges, to, point_list, rec, W, H, gx, s->bg,
+                    out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth);
+    else
+        rc = launch("composite_fwd", K_COMP_FWD, dbg, st, T, GMS_CB, 0, emit ? k_composite_fwd2<true> : k_composite_fwd2<false>, IL.ranges,
+                    to, point_list, rec, W, H, gx, s->bg, out->out_color, IL.final_T, IL.n_contrib, out->out_invdepth,
+                    emit ? surv : nullptr, emit ? IL.nsurv : nullptr);
+    if (rc || !chk || !emit) return rc;
+    GmsBinCheck c = *chk;
+    c.surv = surv; c.nsurv = IL.nsurv;
+    return bins_check(c, true, st);
 }
 
 // nosync_capacity > 0: never synchronise with the host -- the binning region is requested for that many duplicates, N stays
 // on the device (and, when n_host is given, is mirrored into mapped pinned host memory by the kernel that computes it).
+// frame: called by a one-call frame, whose debug mode also waits for the sorts and the scan and runs the binning check (the
+// rasterizer ABI's debug path stays the stock one).
 static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_inputs* in, const gms_raster_outputs* out,
                                gms_alloc_fn alloc, void* user, gms_raster_saved* saved, void* cuda_stream,
-                               int64_t nosync_capacity, uint32_t* n_host, const float* opac_raw = nullptr) {
+                               int64_t nosync_capacity, uint32_t* n_host, const float* opac_raw = nullptr, bool frame = false) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
     if (!s || !out || !alloc || !saved || !in) return set_err(GMS_E_ARG, "null argument%s%s");
     int rc = in->P == 0 ? GMS_OK : check_inputs(in);   // P = 0: nothing to check, background-only images (stock behaviour)
@@ -667,6 +741,7 @@ static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_in
     const int P = in->P, W = s->image_width, H = s->image_height;
     const int gx = (W + GMS_TILE - 1) / GMS_TILE, gy = (H + GMS_TILE - 1) / GMS_TILE, T = gx * gy;
     const int dbg = s->debug;
+    const bool fdbg = frame && dbg;
     saved->geom = saved->binning = saved->image = nullptr; saved->num_rendered = 0; saved->num_visible = -1;
     saved->binning_capacity = 0; saved->flags = 0;
     if (g_opt_fwd != 2 && g_opt_fwd != 3) return set_err(GMS_E_ARG, "option composite_fwd must be 2 or 3%s%s");
@@ -740,6 +815,12 @@ static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_in
         GMS_CUDA(cub::DeviceRadixSort::SortPairs(GL.cub_temp, tb, GL.dkey, GL.dkey_s, GL.idx, GL.order, P, 0, 32, st));
     }
     span_end(st);
+    if (fdbg && (rc = debug_sync(g_opt_sort ? "radix_sort_depth" : "cub_sort_depth", st))) return rc;
+    // the binning check's view of this frame (list, keys and range fields are filled where the list is binned)
+    GmsBinCheck chk;
+    memset(&chk, 0, sizeof(chk));
+    chk.P = P; chk.T = T; chk.gx = gx; chk.d_n = GL.counters; chk.ranges = IL.ranges; chk.radii = out->radii; chk.rect = GL.rect;
+    chk.dkey = GL.dkey;
     if (counting) {
         int64_t N = -1, cap = nosync_capacity;
         if (n_ready) {
@@ -771,7 +852,8 @@ static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_in
             GMS_CUDA(cudaLaunchCooperativeKernel((void*)k_bin_tiles, dim3(G), dim3(GMS_BIN_THREADS), kargs, bin_smem, st));
             GMS_AFTER_LAUNCH("bin_tiles", dbg, st);
             span_end(st);
-            return composite_forward(s, out, IL, GL.rec, point_list, emit, surv, T, st);
+            chk.cap = cap; chk.point_list = point_list;
+            return composite_forward(s, out, IL, GL.rec, point_list, emit, surv, T, st, fdbg ? &chk : nullptr);
         } else {
             if ((rc = fill_background())) return rc;
             GMS_CUDA(cudaMemsetAsync(IL.n_contrib, 0, sizeof(int) * HW, st));
@@ -784,6 +866,7 @@ static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_in
         span_begin(K_SCAN, st);
         GMS_CUDA(cub::DeviceScan::InclusiveSum(GL.cub_temp, tb, it, GL.offs, P, st));
         span_end(st);
+        if (fdbg && (rc = debug_sync("cub_scan_tiles", st))) return rc;
     }
     // N = offs[P-1] stays on the device.  Stock-style call: one 4-byte read-back sizes the binning region exactly (cap = N).
     // Sync-free call: the region is sized for `nosync_capacity` entries, the tail beyond N is filled with sentinel keys that
@@ -842,13 +925,15 @@ static int raster_forward_impl(const gms_raster_settings* s, const gms_raster_in
             GMS_CUDA(cub::DeviceRadixSort::SortPairs(BL.cub_temp, sb, BL.keys_in, BL.keys_out, BL.vals_in, BL.vals_out, (int)cap, 0, tbits, st));
         }
         span_end(st);
+        if (fdbg && (rc = debug_sync(g_opt_sort ? "radix_sort_tiles" : "cub_sort_tiles", st))) return rc;
         auto tile_ranges = [&](auto k, const auto* keys) {
             return launch("tile_ranges", K_RANGES, dbg, st, (unsigned)((cap + 255) / 256), 256, 0, k, cap, keys, IL.ranges, (uint32_t)T,
                           GL.offs + (P - 1), GL.counters, n_host);
         };
         if ((rc = k16 ? tile_ranges(k_tile_ranges<uint16_t>, reinterpret_cast<const uint16_t*>(BL.keys_out))
                       : tile_ranges(k_tile_ranges<uint32_t>, BL.keys_out))) return rc;
-        return composite_forward(s, out, IL, GL.rec, BL.vals_out, emit, BL.surv, T, st);
+        chk.cap = cap; chk.point_list = BL.vals_out; chk.keys = BL.keys_out; chk.key16 = k16;
+        return composite_forward(s, out, IL, GL.rec, BL.vals_out, emit, BL.surv, T, st, fdbg ? &chk : nullptr);
     } else {
         if ((rc = fill_background())) return rc;
         GMS_CUDA(cudaMemsetAsync(IL.tile_last, 0, sizeof(int) * (size_t)T, st));
@@ -1012,8 +1097,8 @@ static bool expand_wide(const gms_expand_args& a) {
     return a.alpha_activation == GMS_ALPHA_SOFTMAX && a.K >= GMS_EXP_WIDE_MIN_K;
 }
 
-int gms_expand_forward(const gms_expand_args* a, void* cuda_stream) {
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+// gms_expand_forward, with the launch waited for under `dbg` (the frames' debug mode)
+static int expand_forward(const gms_expand_args* a, int dbg, cudaStream_t st) {
     if (!a || a->F < 0 || a->K <= 0) return set_err(GMS_E_ARG, "bad expansion sizes%s%s");
     if (!a->triangles_in && (!a->vertices || !a->faces)) return set_err(GMS_E_ARG, "vertices/faces or triangles_in required%s%s");
     if (!a->alpha_raw || !a->scale_raw) return set_err(GMS_E_ARG, "_alpha and _scale required%s%s");
@@ -1021,21 +1106,28 @@ int gms_expand_forward(const gms_expand_args* a, void* cuda_stream) {
         return set_err(GMS_E_ARG, "alpha_activation must be 0 (relu) or 1 (softmax)%s%s");
     if (a->F == 0) return GMS_OK;
     if (expand_wide(*a))
-        return launch("expand_fwd", K_EXP_FWD, 0, st, (a->F + GMS_EXP_WIDE_BLOCK / 32 - 1) / (GMS_EXP_WIDE_BLOCK / 32), GMS_EXP_WIDE_BLOCK, 0,
+        return launch("expand_fwd", K_EXP_FWD, dbg, st, (a->F + GMS_EXP_WIDE_BLOCK / 32 - 1) / (GMS_EXP_WIDE_BLOCK / 32), GMS_EXP_WIDE_BLOCK, 0,
                       k_expand_wide_fwd, *a);
     const bool softmax = a->alpha_activation == GMS_ALPHA_SOFTMAX;
     const size_t smem = (size_t)GMS_EXP_BLOCK * a->K * exp_fwd_stage_width(*a) * sizeof(float);
     const bool staged = smem <= 48 * 1024;
     void (*k)(gms_expand_args) = softmax ? (staged ? k_expand_fwd<true, GMS_ALPHA_SOFTMAX> : k_expand_fwd<false, GMS_ALPHA_SOFTMAX>)
                                          : (staged ? k_expand_fwd<true, GMS_ALPHA_RELU> : k_expand_fwd<false, GMS_ALPHA_RELU>);
-    return launch("expand_fwd", K_EXP_FWD, 0, st, (a->F + GMS_EXP_BLOCK - 1) / GMS_EXP_BLOCK, GMS_EXP_BLOCK, staged ? smem : 0, k, *a);
+    return launch("expand_fwd", K_EXP_FWD, dbg, st, (a->F + GMS_EXP_BLOCK - 1) / GMS_EXP_BLOCK, GMS_EXP_BLOCK, staged ? smem : 0, k, *a);
+}
+
+int gms_expand_forward(const gms_expand_args* a, void* cuda_stream) {
+    return expand_forward(a, 0, reinterpret_cast<cudaStream_t>(cuda_stream));
+}
+
+static int points_expand_forward(const gms_points_args* a, int dbg, cudaStream_t st) {
+    if (!a || a->P < 0 || !a->triangles) return set_err(GMS_E_ARG, "gms_points_expand_forward: bad arguments%s%s");
+    if (a->P == 0) return GMS_OK;
+    return launch("points_expand_fwd", K_EXP_FWD, dbg, st, (a->P + 127) / 128, 128, 0, k_points_expand_fwd, *a);
 }
 
 int gms_points_expand_forward(const gms_points_args* a, void* cuda_stream) {
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-    if (!a || a->P < 0 || !a->triangles) return set_err(GMS_E_ARG, "gms_points_expand_forward: bad arguments%s%s");
-    if (a->P == 0) return GMS_OK;
-    return launch("points_expand_fwd", K_EXP_FWD, 0, st, (a->P + 127) / 128, 128, 0, k_points_expand_fwd, *a);
+    return points_expand_forward(a, 0, reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
 int gms_points_prepare_vertices(const gms_points_vertices_args* a, void* cuda_stream) {
@@ -1048,8 +1140,7 @@ int gms_points_prepare_vertices(const gms_points_vertices_args* a, void* cuda_st
     return launch("points_vertices", K_EXP_FWD, 0, st, (a->P + 127) / 128, 128, 0, k_points_vertices, *a);
 }
 
-int gms_expand_backward(const gms_expand_args* a, const gms_expand_grads* g, void* cuda_stream) {
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+static int expand_backward(const gms_expand_args* a, const gms_expand_grads* g, int dbg, cudaStream_t st) {
     if (!a || !g || a->F < 0 || a->K <= 0) return set_err(GMS_E_ARG, "bad expansion sizes%s%s");
     if (!a->triangles_in && (!a->vertices || !a->faces)) return set_err(GMS_E_ARG, "vertices/faces or triangles_in required%s%s");
     if (!a->alpha_raw || !a->scale_raw) return set_err(GMS_E_ARG, "_alpha and _scale required%s%s");
@@ -1057,10 +1148,14 @@ int gms_expand_backward(const gms_expand_args* a, const gms_expand_grads* g, voi
         return set_err(GMS_E_ARG, "alpha_activation must be 0 (relu) or 1 (softmax)%s%s");
     if (a->F == 0) return GMS_OK;
     if (expand_wide(*a))
-        return launch("expand_bwd", K_EXP_BWD, 0, st, (a->F + GMS_EXP_WIDE_BLOCK / 32 - 1) / (GMS_EXP_WIDE_BLOCK / 32), GMS_EXP_WIDE_BLOCK, 0,
+        return launch("expand_bwd", K_EXP_BWD, dbg, st, (a->F + GMS_EXP_WIDE_BLOCK / 32 - 1) / (GMS_EXP_WIDE_BLOCK / 32), GMS_EXP_WIDE_BLOCK, 0,
                       k_expand_wide_bwd, *a, *g);
-    return launch("expand_bwd", K_EXP_BWD, 0, st, (a->F + GMS_EXP_BLOCK - 1) / GMS_EXP_BLOCK, GMS_EXP_BLOCK, 0,
+    return launch("expand_bwd", K_EXP_BWD, dbg, st, (a->F + GMS_EXP_BLOCK - 1) / GMS_EXP_BLOCK, GMS_EXP_BLOCK, 0,
                   a->alpha_activation == GMS_ALPHA_SOFTMAX ? k_expand_bwd<GMS_ALPHA_SOFTMAX> : k_expand_bwd<GMS_ALPHA_RELU>, *a, *g);
+}
+
+int gms_expand_backward(const gms_expand_args* a, const gms_expand_grads* g, void* cuda_stream) {
+    return expand_backward(a, g, 0, reinterpret_cast<cudaStream_t>(cuda_stream));
 }
 
 size_t gms_frame_workspace_bytes(int32_t P, int32_t W, int32_t H) { return frame_layout(nullptr, P, W, H).total + 512; }
@@ -1101,7 +1196,7 @@ static int frame_gaussian_count(const char* fn, const FrameModel& m, int* P) {
 
 // gs_mesh: E1-E4 mesh -> Gaussians (activated scales / rotations) into xyz / scales / rots, one launch per mesh segment
 // (one in all without segments).  `ea` receives each launch's arguments for the training frame's expansion backward.
-static int mesh_expand_forward(const FrameModel& m, float* xyz, float* scales, float* rots, void* cuda_stream,
+static int mesh_expand_forward(const FrameModel& m, float* xyz, float* scales, float* rots, int dbg, void* cuda_stream,
                                std::vector<gms_expand_args>* ea) {
     const gms_mesh_segment whole = {m.F, m.K};
     const gms_mesh_segment* seg = m.n_segments ? m.segments : &whole;
@@ -1116,7 +1211,7 @@ static int mesh_expand_forward(const FrameModel& m, float* xyz, float* scales, f
         e.xyz = xyz + 3 * g0; e.scaling_act = scales + 3 * g0; e.rotation_act = rots + 4 * g0;
         e.alpha_activation = m.alpha_activation;
         int rc;
-        if ((rc = gms_expand_forward(&e, cuda_stream))) return rc;
+        if ((rc = expand_forward(&e, dbg, reinterpret_cast<cudaStream_t>(cuda_stream)))) return rc;
         f0 += (size_t)seg[i].F;
         g0 += (size_t)seg[i].F * seg[i].K;
     }
@@ -1126,7 +1221,7 @@ static int mesh_expand_forward(const FrameModel& m, float* xyz, float* scales, f
 // The expansion backward of mesh_expand_forward's launches: per segment, the incoming gradients and the raw-parameter
 // gradients are offset like the forward's outputs and inputs; the vertex gradient is shared (accumulated with atomics).
 static int mesh_expand_backward(const std::vector<gms_expand_args>& ea, const float* d_xyz, const float* d_scales, const float* d_rots,
-                                float* d_vertices, float* d_alpha_raw, float* d_scale_raw, void* cuda_stream) {
+                                float* d_vertices, float* d_alpha_raw, float* d_scale_raw, int dbg, void* cuda_stream) {
     size_t g0 = 0;
     for (const gms_expand_args& e : ea) {
         gms_expand_grads g;
@@ -1134,7 +1229,7 @@ static int mesh_expand_backward(const std::vector<gms_expand_args>& ea, const fl
         g.dL_dxyz = d_xyz + 3 * g0; g.dL_dscaling_act = d_scales + 3 * g0; g.dL_drotation_act = d_rots + 4 * g0;
         g.dL_dvertices = d_vertices; g.dL_dalpha_raw = d_alpha_raw + 3 * g0; g.dL_dscale_raw = d_scale_raw + g0;
         int rc;
-        if ((rc = gms_expand_backward(&e, &g, cuda_stream))) return rc;
+        if ((rc = expand_backward(&e, &g, dbg, reinterpret_cast<cudaStream_t>(cuda_stream)))) return rc;
         g0 += (size_t)e.F * e.K;
     }
     return GMS_OK;
@@ -1155,7 +1250,7 @@ static int frame_raster_forward(const FrameGaussians& g, const gms_raster_settin
     memset(in, 0, sizeof(*in));
     in->P = g.P; in->M = g.M; in->means3D = g.xyz; in->opacities = g.opac; in->shs = g.features; in->scales = g.scales;
     in->rotations = g.rots;
-    return raster_forward_impl(s, in, out, alloc, user, saved, cuda_stream, binning_capacity, n_host, g.opacity_raw);
+    return raster_forward_impl(s, in, out, alloc, user, saved, cuda_stream, binning_capacity, n_host, g.opacity_raw, true);
 }
 
 size_t gms_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { (void)W; (void)H; return render_layout(nullptr, P).total + 512; }
@@ -1210,9 +1305,10 @@ static int frame_loss_backward(const Args* a, const FrameLayout& FL, const gms_r
     la.lambda_dssim = a->lambda_dssim; la.loss = a->loss;
     la.dL_dimg = FL.dimage; la.scratch = FL.loss_scratch; la.scratch_bytes = FL.loss_bytes;
     int rc;
-    if ((rc = gms_l1_ssim_loss(&la, cuda_stream))) return rc;
+    const int dbg = a->settings.debug;
+    if ((rc = l1_ssim_loss(&la, dbg, st))) return rc;
     if (a->event_loss_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_loss_ready), st));
-    if ((rc = anomaly_hook(a->anomaly, a->anomaly_stages, GMS_ANOMALY_LOSS, {{FL.dimage, 3 * (int64_t)la.H * la.W, GMS_ANOMALY_DIMAGE}}, 0,
+    if ((rc = anomaly_hook(a->anomaly, a->anomaly_stages, GMS_ANOMALY_LOSS, {{FL.dimage, 3 * (int64_t)la.H * la.W, GMS_ANOMALY_DIMAGE}}, dbg,
                            st))) return rc;
     gms_raster_grads gr;
     memset(&gr, 0, sizeof(gr));
@@ -1239,7 +1335,9 @@ int gms_render_frame(const gms_render_args* a, gms_alloc_fn alloc, void* alloc_u
                  a->segments, a->n_segments, a->alpha_activation};
             return frame_gaussian_count("gms_render_frame", m, P);
         },
-        [&](int, const RenderLayout& RL, const float**) { return mesh_expand_forward(m, RL.xyz, RL.scales, RL.rots, cuda_stream, &ea); });
+        [&](int, const RenderLayout& RL, const float**) {
+            return mesh_expand_forward(m, RL.xyz, RL.scales, RL.rots, a->settings.debug, cuda_stream, &ea);
+        });
 }
 
 size_t gms_points_render_workspace_bytes(int32_t P, int32_t W, int32_t H) { return gms_render_workspace_bytes(P, W, H); }
@@ -1257,7 +1355,7 @@ int gms_points_render_frame(const gms_points_render_args* a, gms_alloc_fn alloc,
             gms_points_args pa;
             memset(&pa, 0, sizeof(pa));
             pa.P = P; pa.triangles = a->triangles; pa.eps = a->eps; pa.xyz = RL.xyz; pa.scaling_act = RL.scales; pa.rotation_act = RL.rots;
-            return gms_points_expand_forward(&pa, cuda_stream);
+            return points_expand_forward(&pa, a->settings.debug, reinterpret_cast<cudaStream_t>(cuda_stream));
         });
 }
 
@@ -1320,7 +1418,7 @@ int gms_bound_points_render_frame(const gms_bound_points_render_args* a, gms_all
             gms_points_args pa;
             memset(&pa, 0, sizeof(pa));
             pa.P = P; pa.eps = a->eps; pa.xyz = RL.xyz; pa.scaling_act = RL.scales; pa.rotation_act = RL.rots;
-            return launch("points_bound_expand_fwd", K_EXP_FWD, 0, st, (P + GMS_PM_BLOCK - 1) / GMS_PM_BLOCK, GMS_PM_BLOCK, 0,
+            return launch("points_bound_expand_fwd", K_EXP_FWD, a->settings.debug, st, (P + GMS_PM_BLOCK - 1) / GMS_PM_BLOCK, GMS_PM_BLOCK, 0,
                           k_points_bound_expand_fwd, r, pa, a->settings.viewmatrix);
         });
 }
@@ -1348,7 +1446,8 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     std::vector<gms_expand_args> ea;
     gms_raster_inputs in;
     gms_raster_saved saved;
-    if ((rc = mesh_expand_forward(m, FL.g.xyz, FL.g.scales, FL.g.rots, cuda_stream, &ea))) return rc;
+    const int dbg = a->settings.debug;
+    if ((rc = mesh_expand_forward(m, FL.g.xyz, FL.g.scales, FL.g.rots, dbg, cuda_stream, &ea))) return rc;
     const FrameGaussians g = {P, a->M, FL.g.xyz, FL.g.scales, FL.g.rots, a->features, a->opacity_raw, FL.g.opac};
     if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
                                    &saved))) return rc;
@@ -1357,11 +1456,11 @@ int gms_train_frame(const gms_frame_args* a, gms_alloc_fn alloc, void* alloc_use
     if ((rc = frame_loss_backward(a, FL, in, saved, FL.d_xyz, a->d_color_sh, cuda_stream))) return rc;
     if (a->event_sh_ready) GMS_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(a->event_sh_ready), st));
     // expansion backward (vertex gradients are accumulated with atomics: the caller keeps d_vertices zeroed)
-    if ((rc = mesh_expand_backward(ea, FL.d_xyz, FL.d_scales, FL.d_rots, a->d_vertices, a->d_alpha_raw, a->d_scale_raw, cuda_stream)))
+    if ((rc = mesh_expand_backward(ea, FL.d_xyz, FL.d_scales, FL.d_rots, a->d_vertices, a->d_alpha_raw, a->d_scale_raw, dbg, cuda_stream)))
         return rc;
     if ((rc = anomaly_hook(a->anomaly, a->anomaly_stages, GMS_ANOMALY_EXPAND_BWD,
                            {{a->d_vertices, 3 * (int64_t)a->V, GMS_ANOMALY_DVERTICES}, {a->d_alpha_raw, 3 * (int64_t)P, GMS_ANOMALY_DALPHA_RAW},
-                            {a->d_scale_raw, (int64_t)P, GMS_ANOMALY_DSCALE_RAW}}, 0, st))) return rc;
+                            {a->d_scale_raw, (int64_t)P, GMS_ANOMALY_DSCALE_RAW}}, dbg, st))) return rc;
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;
     return GMS_OK;
 }
@@ -1376,9 +1475,9 @@ static bool free_model_ok(int P, int M, int cols, const float* xyz, const float*
 static bool aligned16(const void* p) { return (reinterpret_cast<size_t>(p) & 15) == 0; }
 
 static int free_act_fwd(int P, int cols, const float* scaling_raw, const float* rotation_raw, float eps, float* scales, float* rots,
-                        cudaStream_t st) {
+                        int dbg, cudaStream_t st) {
     if (P == 0) return GMS_OK;
-    return launch("free_act_fwd", K_EXP_FWD, 0, st, (P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, k_free_act_fwd, P, cols,
+    return launch("free_act_fwd", K_EXP_FWD, dbg, st, (P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, k_free_act_fwd, P, cols,
                   scaling_raw, rotation_raw, eps, scales, rots);
 }
 
@@ -1407,7 +1506,8 @@ int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void*
     gms_raster_outputs out = {FL.image, FL.radii, FL.invdepth, 0};
     gms_raster_inputs in;
     gms_raster_saved saved;
-    if ((rc = free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, FL.g.scales, FL.g.rots, st))) return rc;
+    const int dbg = a->settings.debug;
+    if ((rc = free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, FL.g.scales, FL.g.rots, dbg, st))) return rc;
     const FrameGaussians g = {P, a->M, a->xyz, FL.g.scales, FL.g.rots, a->features, a->opacity_raw, FL.g.opac};
     if ((rc = frame_raster_forward(g, &a->settings, &out, alloc, alloc_user, a->binning_capacity, a->n_host_mapped, cuda_stream, &in,
                                    &saved))) return rc;
@@ -1418,12 +1518,12 @@ int gms_free_train_frame(const gms_free_frame_args* a, gms_alloc_fn alloc, void*
         b.d_scales = FL.d_scales; b.d_rots = FL.d_rots; b.d_m2d = FL.d_m2d; b.radii = FL.radii;
         b.d_scaling_raw = a->d_scaling_raw; b.d_rotation_raw = a->d_rotation_raw; b.accum = a->accum; b.denom = a->denom;
         b.counters = geom_layout(aligned_base(saved.geom), P).counters;
-        if ((rc = launch("free_act_bwd", K_EXP_BWD, 0, st, (P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, k_free_act_bwd, b)))
+        if ((rc = launch("free_act_bwd", K_EXP_BWD, dbg, st, (P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, k_free_act_bwd, b)))
             return rc;
         if ((rc = anomaly_hook(a->anomaly, a->anomaly_stages, GMS_ANOMALY_ACTIVATION_BWD,
                                {{a->d_scaling_raw, (int64_t)P * a->scale_cols, GMS_ANOMALY_DSCALING_RAW},
                                 {a->d_rotation_raw, 4 * (int64_t)P, GMS_ANOMALY_DROTATION_RAW},
-                                {a->accum, a->accum ? (int64_t)P : 0, GMS_ANOMALY_ACCUM}}, 0, st))) return rc;
+                                {a->accum, a->accum ? (int64_t)P : 0, GMS_ANOMALY_ACCUM}}, dbg, st))) return rc;
     }
     if (a->num_rendered) *a->num_rendered = saved.num_rendered;
     return GMS_OK;
@@ -1441,7 +1541,7 @@ int gms_free_render_frame(const gms_free_render_args* a, gms_alloc_fn alloc, voi
         },
         [&](int P, const RenderLayout& RL, const float** xyz) {
             *xyz = a->xyz;
-            return free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, RL.scales, RL.rots, st);
+            return free_act_fwd(P, a->scale_cols, a->scaling_raw, a->rotation_raw, a->eps, RL.scales, RL.rots, a->settings.debug, st);
         });
 }
 
@@ -1463,7 +1563,7 @@ int gms_flame_render_frame(const gms_flame_render_args* a, gms_alloc_fn alloc, v
         },
         [&](int P, const RenderLayout& RL, const float**) {
             if (P == 0) return GMS_OK;
-            return launch("flame_act", K_EXP_FWD, 0, st, (P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, k_flame_act, P, a->K,
+            return launch("flame_act", K_EXP_FWD, a->settings.debug, st, (P + GMS_FREE_BLOCK - 1) / GMS_FREE_BLOCK, GMS_FREE_BLOCK, 0, k_flame_act, P, a->K,
                           a->alpha, a->faces, a->vertices, a->scaling_log, a->rotation_raw, RL.xyz, RL.scales, RL.rots);
         });
 }
@@ -1860,6 +1960,32 @@ int gms_nan_scan(const gms_nan_scan_args* a, void* cuda_stream) {
             return set_err(GMS_E_ARG, "gms_nan_scan: a non-empty buffer needs a 4-byte-aligned pointer%s%s");
     }
     return nan_scan_launch(a->stage, a->buffers, a->n_buffers, a->record, 0, reinterpret_cast<cudaStream_t>(cuda_stream));
+}
+
+int gms_debug_check_bins(const gms_debug_bins_args* a, void* cuda_stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+    if (!a || !a->point_list || !a->ranges || !a->radii || !a->rect || !a->depth_keys)
+        return set_err(GMS_E_ARG, "gms_debug_check_bins: null argument%s%s");
+    if (a->P < 0 || a->tiles_x < 1 || a->tiles_x > 65535 || a->tiles_y < 1 || a->tiles_y > 65535 ||
+        (int64_t)a->tiles_x * a->tiles_y > ((int64_t)1 << 26) || a->n < 0 || a->n > INT32_MAX)
+        return set_err(GMS_E_ARG, "gms_debug_check_bins: need P >= 0, 1 <= tiles_x, tiles_y <= 65535, at most 2^26 tiles and 0 <= n < 2^31%s%s");
+    if (a->tile_keys && a->key_bits != 16 && a->key_bits != 32) return set_err(GMS_E_ARG, "gms_debug_check_bins: key_bits must be 16 or 32%s%s");
+    if (!a->surv != !a->nsurv) return set_err(GMS_E_ARG, "gms_debug_check_bins: surv and nsurv go together%s%s");
+    GmsBinCheck c;
+    memset(&c, 0, sizeof(c));
+    c.P = a->P; c.T = a->tiles_x * a->tiles_y; c.gx = a->tiles_x; c.n = a->n; c.cap = a->n;
+    c.point_list = a->point_list; c.keys = a->tile_keys; c.key16 = a->key_bits == 16;
+    c.ranges = reinterpret_cast<const int2*>(a->ranges); c.radii = a->radii; c.rect = reinterpret_cast<const uint2*>(a->rect);
+    c.dkey = a->depth_keys;
+    if (a->key) *a->key = GMS_DEBUG_NONE;
+    GmsBinRecord h;
+    int rc = bins_check(c, false, st, &h);
+    if (rc == GMS_OK && a->surv) {
+        c.surv = a->surv; c.nsurv = a->nsurv;
+        rc = bins_check(c, true, st, &h);
+    }
+    if (rc == GMS_E_DEBUG && a->key) *a->key = h.key != GMS_DEBUG_NONE ? h.key : (unsigned long long)GMS_DEBUG_RANGES << 56 | h.n;
+    return rc;
 }
 
 }  // extern "C"

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libgms_b200.so")
 
 ALPHA_RELU, ALPHA_SOFTMAX = 0, 1   # gms_*_args.alpha_activation: relu + 1e-8, normalised (gs_mesh); softmax (gs_flame)
 FORWARD_ONLY = 1        # gms_raster_outputs.flags: no backward will follow (skip the survivor lists)
-GMS_OK, GMS_E_ARG, GMS_E_CUDA, GMS_E_ALLOC, GMS_E_UNSUPPORTED = 0, -1, -2, -3, -4
+GMS_OK, GMS_E_ARG, GMS_E_CUDA, GMS_E_ALLOC, GMS_E_UNSUPPORTED, GMS_E_DEBUG = 0, -1, -2, -3, -4, -5
 BUF_GEOM, BUF_BINNING, BUF_IMAGE = 0, 1, 2
 
 c_float_p = C.c_void_p   # raw device pointers travel as integers
@@ -331,6 +331,18 @@ class NanScanArgs(C.Structure):
                 ("record", C.c_void_p)]
 
 
+DEBUG_NONE = (1 << 64) - 1        # GMS_DEBUG_NONE: the key of a binning check that found no violation
+DEBUG_ORDER, DEBUG_RANGES, DEBUG_GAUSSIAN, DEBUG_SURVIVOR = 1, 2, 3, 4     # GMS_DEBUG_*: the checks (key >> 56)
+
+
+class DebugBinsArgs(C.Structure):
+    """struct gms_debug_bins_args"""
+    _fields_ = [("P", C.c_int32), ("tiles_x", C.c_int32), ("tiles_y", C.c_int32), ("n", C.c_int64), ("point_list", C.c_void_p),
+                ("tile_keys", C.c_void_p), ("key_bits", C.c_int32), ("ranges", C.c_void_p), ("radii", C.c_void_p),
+                ("rect", C.c_void_p), ("depth_keys", C.c_void_p), ("surv", C.c_void_p), ("nsurv", C.c_void_p),
+                ("key", C.POINTER(C.c_uint64))]
+
+
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_int, C.c_size_t)
 
 # every symbol include/gms_b200.h declares (tests/test_abi.py checks the library exports all of them)
@@ -347,7 +359,8 @@ ABI_SYMBOLS = ["gms_scratch_bytes", "gms_binning_bytes", "gms_rasterize_forward"
                "gms_densify_plan", "gms_densify_apply", "gms_knn_scratch_bytes", "gms_knn_dist2",
                "gms_flame_render_workspace_bytes", "gms_flame_render_frame", "gms_image_composite_rgba", "gms_image_resize_u8",
                "gms_flame_lbs_workspace_bytes", "gms_flame_lbs_forward", "gms_flame_lbs_backward", "gms_lpips_scratch_bytes",
-               "gms_lpips_vgg", "gms_alpha_shape", "gms_normals_scratch_bytes", "gms_estimate_normals", "gms_nan_scan"]
+               "gms_lpips_vgg", "gms_alpha_shape", "gms_normals_scratch_bytes", "gms_estimate_normals", "gms_nan_scan",
+               "gms_debug_check_bins"]
 
 _lib = None
 
@@ -440,6 +453,7 @@ def lib():
     L.gms_normals_scratch_bytes.argtypes = [C.c_int32]
     L.gms_estimate_normals.argtypes = [C.POINTER(NormalsArgs), C.c_void_p]
     L.gms_nan_scan.argtypes = [C.POINTER(NanScanArgs), C.c_void_p]
+    L.gms_debug_check_bins.argtypes = [C.POINTER(DebugBinsArgs), C.c_void_p]
     _lib = L
     # GMS_OPTIONS="key=value,key=value": tuning knobs applied at load (A/B runs of whole test suites / benches)
     for kv in filter(None, os.environ.get("GMS_OPTIONS", "").split(",")):

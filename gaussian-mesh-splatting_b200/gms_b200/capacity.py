@@ -153,18 +153,20 @@ class SyncFreeCapacity:
             raise ValueError(f"{owner} was sized {sized}; got a {cam.image_width}x{cam.image_height} camera")
 
     def _launch(self, fn: str, a, cam, bg, scale_modifier: float = 1.0, antialiasing: bool = False, capacity: int = None,
-                n_host: int = None) -> bool:
+                n_host: int = None, debug: bool = False) -> bool:
         """Fills the settings, workspace, num_rendered and capacity fields every one-call frame's args struct shares and
         calls `fn` on the current stream.  With `capacity` (and the mapped (N, flag) address `n_host`) the frame is sync-free
         at that capacity.  Otherwise the frame is synchronising when it has to learn N (the first frame, or the view's first
         frame since _forget_views) or the frames are not sync-free, and sync-free on the next ring slot at the view's
-        predicted capacity else.  The image size is the camera's.  Returns whether the frame learned N."""
+        predicted capacity else.  The image size is the camera's.  debug: the reference's pipe.debug (settings.debug: every
+        launch waited for and checked by name, the binning check on the frame's own buffers).  Returns whether the frame
+        learned N."""
         from . import _lib
         s = a.settings
         s.image_height, s.image_width, s.tanfovx, s.tanfovy = int(cam.image_height), int(cam.image_width), cam.tanfovx, cam.tanfovy
         s.bg, s.scale_modifier = bg.data_ptr(), float(scale_modifier)
         s.viewmatrix, s.projmatrix, s.campos = cam.world_view_transform.data_ptr(), cam.full_proj_transform.data_ptr(), cam.camera_center.data_ptr()
-        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = self.model.active_sh_degree, 0, 0, int(bool(antialiasing))
+        s.sh_degree, s.prefiltered, s.debug, s.antialiasing = self.model.active_sh_degree, 0, int(bool(debug)), int(bool(antialiasing))
         a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
         a.num_rendered = C.pointer(self.n_rendered)
         learn = False

@@ -19,6 +19,7 @@ per view (SyncFreeCapacity).  An overflowed render (N above its capacity) gives 
 re-renders those views before it reads its results."""
 from __future__ import annotations
 
+import contextlib
 from dataclasses import dataclass
 from typing import List, Optional, Sequence
 
@@ -113,17 +114,29 @@ class NativeRenderer(SyncFreeCapacity):
     def _call(self, fn: str, a, cam, bg, scale_modifier: float, antialiasing: bool, capacity: int, n_host: int) -> None:
         """Points `a`'s outputs at the renderer's buffers and issues `fn`."""
         a.image, a.invdepth, a.radii = self.image.data_ptr(), self.invdepth.data_ptr(), self.radii.data_ptr()
-        self._launch(fn, a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
+        self._launch(fn, a, cam, bg, scale_modifier, antialiasing, capacity, n_host, debug=self._debug)
+
+    _debug = False      # set by render(debug=...) / evaluate(debug=...) for that call
+
+    @contextlib.contextmanager
+    def _debug_mode(self, debug: bool):
+        self._debug = bool(debug)
+        try:
+            yield
+        finally:
+            self._debug = False
 
     def render(self, cam, bg: torch.Tensor, scale_modifier: float = 1.0, antialiasing: bool = False,
-               vertices: torch.Tensor = None):
+               vertices: torch.Tensor = None, debug: bool = False):
         """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view, the reference's render(...)["render"], ["radii"],
         ["depth"].  `vertices` (float32, model.vertices' shape), when given, is this frame's mesh in place of the model's
         (one frame of an animated sweep, renderer/gaussian_animated_renderer's `triangles` as vertices[faces]); the model
-        is never modified."""
+        is never modified.  debug: the reference's pipe.debug (every launch of the frame waited for and named on a fault,
+        the binning check on the frame's buffers)."""
         self._sweep_vertices = None if vertices is None else vertices.detach()
         try:
-            self._render(cam, bg, scale_modifier, antialiasing)
+            with self._debug_mode(debug):
+                self._render(cam, bg, scale_modifier, antialiasing)
         finally:
             self._sweep_vertices = None
         return self.image, self.radii, self.invdepth
@@ -137,12 +150,17 @@ class NativeRenderer(SyncFreeCapacity):
         return gt.to(self.dev, non_blocking=True)
 
     def evaluate(self, cams: Sequence, gts: Sequence[torch.Tensor], bg: torch.Tensor, protocol: str = "training_report",
-                 scale_modifier: float = 1.0, antialiasing: bool = False, lpips=None) -> Evaluation:
+                 scale_modifier: float = 1.0, antialiasing: bool = False, lpips=None, debug: bool = False) -> Evaluation:
         """Renders every view and scores it against its ground truth (metrics.METRIC_NAMES under `protocol`, "training_report"
         or "metrics"), all on the current stream into one device array; the host synchronises once, at the end.  Views whose
         render overflowed its predicted capacity are then re-rendered, sized from their true N, and re-scored before the
         array is read.  Given an lpips.Lpips (protocol "metrics" only, as metrics.py alone reports LPIPS), each view's LPIPS
-        is scored in the same pass on the 8-bit round trip of the render and of the ground truth, into Evaluation.lpips."""
+        is scored in the same pass on the 8-bit round trip of the render and of the ground truth, into Evaluation.lpips.
+        debug: every view renders in the reference's debug mode (render)."""
+        with self._debug_mode(debug):
+            return self._evaluate(cams, gts, bg, protocol, scale_modifier, antialiasing, lpips)
+
+    def _evaluate(self, cams, gts, bg, protocol, scale_modifier, antialiasing, lpips) -> Evaluation:
         if len(cams) != len(gts):
             raise ValueError(f"evaluate: {len(cams)} cameras but {len(gts)} ground-truth images")
         if lpips is not None and protocol != "metrics":
@@ -231,14 +249,15 @@ class PointsRenderer(NativeRenderer):
     def _triangles(self) -> torch.Tensor:
         return self.model.triangles if self._frame_triangles is None else self._frame_triangles
 
-    def render(self, cam, bg: torch.Tensor, triangles: torch.Tensor = None, scale_modifier: float = 1.0, antialiasing: bool = False):
+    def render(self, cam, bg: torch.Tensor, triangles: torch.Tensor = None, scale_modifier: float = 1.0, antialiasing: bool = False,
+               debug: bool = False):
         """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view.  `triangles` [P,3,3], when given, are this frame's
         pseudo-mesh in place of the model's (the `triangles` argument of renderer/gaussian_points_animated_renderer's
         render); the model is never modified.  (The reference's render calls pc.prepare_scaling_rot(triangles), which
         overwrites pc._scaling and pc._rotation with those of the frame's triangles.)"""
         self._frame_triangles = None if triangles is None else triangles.detach()
         try:
-            return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing)
+            return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing, debug=debug)
         finally:
             self._frame_triangles = None
 
@@ -285,13 +304,14 @@ class MeshBoundPointsRenderer(NativeRenderer):
         a.features, a.opacity_raw, a.eps = m._features.data_ptr(), m._opacity.data_ptr(), m.eps_s0
         self._call("gms_bound_points_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
 
-    def render(self, cam, bg: torch.Tensor, vertices: torch.Tensor = None, scale_modifier: float = 1.0, antialiasing: bool = False):
+    def render(self, cam, bg: torch.Tensor, vertices: torch.Tensor = None, scale_modifier: float = 1.0, antialiasing: bool = False,
+               debug: bool = False):
         """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view.  `vertices` [V,3], when given, is this frame's pose of
         the driving mesh in place of the model's (an edited mesh, or one frame of an animation); the model is never
         modified."""
         self._frame_vertices = None if vertices is None else self.model.binding.check_vertices(vertices)
         try:
-            return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing)
+            return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing, debug=debug)
         finally:
             self._frame_vertices = None
 
@@ -418,11 +438,12 @@ class FlameRenderer(NativeRenderer):
         a.features, a.opacity_raw = m._features.data_ptr(), m._opacity.data_ptr()
         self._call("gms_flame_render_frame", a, cam, bg, scale_modifier, antialiasing, capacity, n_host)
 
-    def render(self, cam, bg: torch.Tensor, vertices: torch.Tensor = None, scale_modifier: float = 1.0, antialiasing: bool = False):
+    def render(self, cam, bg: torch.Tensor, vertices: torch.Tensor = None, scale_modifier: float = 1.0, antialiasing: bool = False,
+               debug: bool = False):
         """(image [3,H,W], radii [P], invdepth [1,H,W]) of one view at the pose `vertices` [V,3] (default: the checkpoint's
         `vertices`); the checkpoint is never modified."""
         self._frame_vertices = None if vertices is None else vertices.detach().float().contiguous()
         try:
-            return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing)
+            return super().render(cam, bg, scale_modifier=scale_modifier, antialiasing=antialiasing, debug=debug)
         finally:
             self._frame_vertices = None

@@ -22,7 +22,7 @@ import torch.distributed as dist
 
 import diff_gaussian_rasterization as dgr
 
-from . import _lib
+from . import _lib, debug as _debug
 from .anomaly import FRAME_STAGES, AnomalyError, AnomalyRecord, layout_of
 from .capacity import SyncFreeCapacity, check_float32, grow_only_alloc, recorded_event
 from .flame import NativeFlame
@@ -164,17 +164,21 @@ class NativeFrame(_FrameSize):
         return dict(xyz=v.xyz, exchange=self.exchange, degree=self.model.active_sh_degree, event=self.ev_sh)
 
     def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, factored: bool = False, sh_adam=None,
-            antialiasing: bool = False, anomaly: Optional[AnomalyRecord] = None, anomaly_stages: int = FRAME_STAGES) -> torch.Tensor:
+            antialiasing: bool = False, anomaly: Optional[AnomalyRecord] = None, anomaly_stages: int = FRAME_STAGES,
+            debug: bool = False) -> torch.Tensor:
         """sh_adam (FlatAdam.begin_fused_sh_step()): the frame also applies the SH parameters' Adam step, and writes no SH
         gradient (unless `factored` asks for the colour gradient as well).  gt: float32 [3,H,W], or uint8 [H,W,3] (dequantized
         on the device into the frame's buffer).  antialiasing: the reference's pipe.antialiasing (each splat's opacity scaled
         by the ratio of its 2D covariance determinants before and after the low-pass dilation, forward and backward).
         anomaly: the frame scans the outputs of each backward stage selected in anomaly_stages (bits 1 << _lib.ANOMALY_*) for
-        NaN into this record (not with sh_adam); the caller resets and reads it."""
+        NaN into this record (not with sh_adam); the caller resets and reads it.  debug: the reference's pipe.debug (every
+        launch waited for and named on a fault, the binning check on the frame's buffers, a violation raises)."""
         import ctypes as C
         from . import _lib
         if gt.dtype == torch.uint8:
             gt = self._gt_u8(gt, "NativeFrame.run")
+            if debug:
+                _debug.sync("gms_image_dequantize", self.dev)
         self._check_view(cam, bg, "NativeFrame.run", gt=gt, gt_fits=lambda W, H: tuple(gt.shape[-2:]) == (H, W))
         self.view_size = (int(cam.image_width), int(cam.image_height))
         if not gt.is_contiguous() or gt.dtype != torch.float32:
@@ -208,7 +212,7 @@ class NativeFrame(_FrameSize):
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
         if anomaly is not None:
             a.anomaly, a.anomaly_stages = anomaly.ptr, int(anomaly_stages)
-        self._launch("gms_train_frame", a, cam, bg, antialiasing=antialiasing)
+        self._launch("gms_train_frame", a, cam, bg, antialiasing=antialiasing, **({"debug": True} if debug else {}))
         return self.loss[0]
 
 
@@ -244,6 +248,11 @@ def refuse_data_parallel_anomaly(detect_anomaly: bool, world: int, who: str) -> 
         raise ValueError(f"{who}: detect_anomaly needs one GPU (world {world}): data-parallel anomaly detection is not implemented")
 
 
+def refuse_data_parallel_debug(debug: bool, debug_from: int, world: int, who: str) -> None:
+    if (debug or debug_from >= 0) and world > 1:
+        raise ValueError(f"{who}: debug needs one GPU (world {world}): data-parallel debug mode is not implemented")
+
+
 def renderer_set(rs, cls, model, P: int):
     """A trainer's evaluate() renderers: `rs` while it was made for the model's Gaussian count P, else a new set."""
     return rs if rs is not None and rs.P == P else RendererSet(cls, model, P)
@@ -276,13 +285,25 @@ class MeshTrainer:
     detect_anomaly: the reference's train.py --detect_anomaly (one GPU).  A native frame scans the outputs of each of its
     backward stages for NaN on the device and step() raises anomaly.AnomalyError, naming the first stage, tensor and element
     that held one, before before_update and before any parameter changes (the SH Adam step is not fused into the frame, one
-    host synchronisation per step).  The autograd arm runs its step under torch.autograd.detect_anomaly()."""
+    host synchronisation per step).  The autograd arm runs its step under torch.autograd.detect_anomaly().
+
+    debug, debug_from: the reference's pipe.debug, train.py --debug and --debug_from (one GPU): debug mode from the first
+    step, or from the step whose iteration - 1 == debug_from on.  A debug step copies what repeating it needs to the host
+    (debug.DebugMode.snapshot), runs its frame with settings.debug and synchronises after every other library call; when it
+    fails, the copy is written to `debug_snapshot`, the reference's message is printed, the trainer's state is put back and
+    the error re-raised (debug.replay repeats the step)."""
 
     def __init__(self, model: MeshGaussianModel, bg: torch.Tensor, lambda_dssim: float = 0.2, world: int = 1,
                  rank: int = 0, optimizer_step: bool = True, fast: bool = True, native: bool = False, sync_free: bool = True,
                  loss_fn=None, sh_factored: bool = True, max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False,
-                 detect_anomaly: bool = False):
+                 detect_anomaly: bool = False, debug: bool = False, debug_from: int = -1, debug_snapshot: str = _debug.SNAPSHOT):
         refuse_data_parallel_anomaly(detect_anomaly, world, "MeshTrainer")
+        refuse_data_parallel_debug(debug, debug_from, world, "MeshTrainer")
+        if (debug or debug_from >= 0) and not (native and fast):
+            raise ValueError("MeshTrainer: debug runs the native frame (native=True, fast=True); the autograd arms have no debug mode")
+        self._debug = _debug.DebugMode(debug, debug_from, debug_snapshot)
+        self.iteration = 0          # steps taken (debug_from counts them)
+        self._sh_factored_arg = bool(sh_factored)
         self.model, self.bg, self.lambda_dssim = model, bg, lambda_dssim
         self.antialiasing = bool(antialiasing)
         self.detect_anomaly = bool(detect_anomaly)
@@ -322,6 +343,27 @@ class MeshTrainer:
                     dist.all_reduce(p.grad, op=dist.ReduceOp.SUM)
                     p.grad.mul_(1.0 / self.world)
 
+    def _debug_config(self) -> dict:
+        """The constructor arguments a replay (debug.replay) rebuilds this trainer with."""
+        return dict(lambda_dssim=self.lambda_dssim, fast=self.fast, native=self.native, sync_free=self.sync_free,
+                    sh_factored=self._sh_factored_arg, max_size=self.max_size, antialiasing=self.antialiasing)
+
+    def _debug_flat(self) -> torch.Tensor:
+        """The optimizer's flat parameter buffer (a debug snapshot takes the parameters from state_dict())."""
+        return self.opt.p
+
+    def _debug_restore(self, snap: dict) -> None:
+        """The state a debug snapshot recorded before its step: parameters, moments, step counts, SH degree, iteration."""
+        self.load_state_dict(_debug.to_device(snap["state_dict"], self.model.vertices.device))
+        self.model.active_sh_degree = int(snap["active_sh_degree"])
+        self.iteration = int(snap["iteration"]) - 1
+        self.opt.zero_grad()
+
+    @property
+    def native_frame(self):
+        """The native frame of the last step (None before the first)."""
+        return self._frame
+
     def step(self, cam: Camera, gt: torch.Tensor, loss_host: Optional[torch.Tensor] = None,
              loss_ready: Optional[torch.cuda.Event] = None, bg: Optional[torch.Tensor] = None, before_update=None,
              frame_end: Optional[torch.cuda.Event] = None) -> torch.Tensor:
@@ -334,8 +376,16 @@ class MeshTrainer:
         iteration's Adam step); the step then does not fuse the SH Adam update into the frame.  frame_end: recorded on the
         current stream right after the frame's launches (render, loss and backward, and on one GPU the SH Adam step the
         frame fuses in), before before_update and any other optimizer work: with an event recorded just before step(), it
-        brackets train.py's iter_start / iter_end window."""
+        brackets train.py's iter_start / iter_end window.  In debug mode (debug, debug_from) the step runs as the class
+        describes."""
         bg = self.bg if bg is None else bg
+        it = self.iteration + 1
+        loss = _debug.run_step(self, lambda debug: self._step(cam, gt, loss_host, loss_ready, bg, before_update, frame_end, debug),
+                               cam, gt, bg, it)
+        self.iteration = it
+        return loss
+
+    def _step(self, cam, gt, loss_host, loss_ready, bg, before_update, frame_end, debug: bool) -> torch.Tensor:
         if self.native:
             if self.world > 1:
                 if self._frame is None:
@@ -356,7 +406,7 @@ class MeshTrainer:
             record = anomaly_record(self._anomaly, self._frame.dev) if self.detect_anomaly else None
             self._anomaly = record
             loss = self._frame.run(cam, gt, bg, factored=factored and not fused, sh_adam=sh_adam, antialiasing=self.antialiasing,
-                                   anomaly=record)
+                                   anomaly=record, debug=debug)
             if frame_end is not None:
                 frame_end.record(torch.cuda.current_stream(self._frame.dev))
             from . import rasterizer as _r
@@ -375,6 +425,8 @@ class MeshTrainer:
                 self.opt.step(zero_end=self.opt.ends[0], sh=self._frame.sh_factors() if factored else None)
             else:
                 self.opt.zero_grad_partial(self.opt.ends[0])
+            if debug:
+                _debug.sync("FlatAdam step (gms_adam_step, gms_adam_sh_factored)", self._frame.dev)
             return loss
         if gt.dtype == torch.uint8:
             H, W = int(gt.shape[0]), int(gt.shape[1])
@@ -425,7 +477,7 @@ class MeshTrainer:
         """L1 / SSIM / PSNR of the current model on held-out views with the trainer's background, the test half of
         training_report (train.py:183-218): NativeRenderer.evaluate, one host synchronisation per image size of the set."""
         self._renderer = renderer_set(self._renderer, NativeRenderer, self.model, self.model._scale.shape[0])
-        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol, antialiasing=self.antialiasing)
+        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol, antialiasing=self.antialiasing, debug=self._debug.on)
 
     def state_dict(self) -> dict:
         """What resuming needs (single GPU, fast=True): FlatAdam's flat parameters, moments and step counts, the active SH
@@ -441,6 +493,7 @@ class MeshTrainer:
         check_antialiasing(state, self.antialiasing, "MeshTrainer")
         self.opt.load_state_dict(state["adam"])
         self.model.active_sh_degree = int(state["active_sh_degree"])
+        self.iteration = self.opt.t
 
 
 # ---------------------------------------------------------------------------------------------- free Gaussians (gs, gs_flat)
@@ -521,14 +574,17 @@ class NativeFreeFrame(_FrameSize):
         self._check_view(cam, bg, "NativeFreeFrame.run", gt=gt, gt_fits=lambda W, H: tuple(gt.shape) == (3, H, W))
 
     def run(self, cam: Camera, gt: torch.Tensor, bg: torch.Tensor, stats: bool = True, sh_adam=None,
-            antialiasing: bool = False, anomaly: Optional[AnomalyRecord] = None, anomaly_stages: int = FRAME_STAGES) -> torch.Tensor:
+            antialiasing: bool = False, anomaly: Optional[AnomalyRecord] = None, anomaly_stages: int = FRAME_STAGES,
+            debug: bool = False) -> torch.Tensor:
         """stats: add this frame's densification statistics to `accum` / `denom`.  sh_adam (FlatAdam.begin_fused_sh_step()):
         the frame also applies the SH parameters' Adam step and writes no SH gradient.  gt: float32 [3,H,W], or uint8 [H,W,3]
-        (dequantized on the device into the frame's buffer).  antialiasing, anomaly, anomaly_stages: as NativeFrame.run."""
+        (dequantized on the device into the frame's buffer).  antialiasing, anomaly, anomaly_stages, debug: as NativeFrame.run."""
         import ctypes as C
         from . import _lib
         if gt.dtype == torch.uint8:
             gt = self._gt_u8(gt, "NativeFreeFrame.run")
+            if debug:
+                _debug.sync("gms_image_dequantize", self.dev)
         gt = gt.contiguous()
         self._check(gt, bg, cam)
         m = self.model
@@ -547,7 +603,7 @@ class NativeFreeFrame(_FrameSize):
         a.gt, a.lambda_dssim, a.loss = gt.data_ptr(), self.lam, self.loss.data_ptr()
         if anomaly is not None:
             a.anomaly, a.anomaly_stages = anomaly.ptr, int(anomaly_stages)
-        self._launch("gms_free_train_frame", a, cam, bg, antialiasing=antialiasing)
+        self._launch("gms_free_train_frame", a, cam, bg, antialiasing=antialiasing, **({"debug": True} if debug else {}))
         return self.loss[0]
 
 
@@ -605,12 +661,16 @@ class FreeTrainer:
     MeshTrainer's; the frame keeps its size when densification changes P.  antialiasing: as MeshTrainer's.  detect_anomaly: as
     MeshTrainer's; step() raises before densification, the opacity reset and Adam, with the iteration counter and the
     densification statistics as they were before the step (the learning rate and SH degree of the iteration stay applied, as
-    in the reference)."""
+    in the reference).  debug, debug_from, debug_snapshot: as MeshTrainer's; a failed debug step leaves the iteration
+    counter, the densification statistics and the split generator as they were before it."""
 
     def __init__(self, model, bg: torch.Tensor, extent: float, opt: FreeOptimizationParams = None, white_background: bool = None,
                  sync_free: bool = True, world: int = 1, generator: torch.Generator = None,
-                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False, detect_anomaly: bool = False):
+                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False, detect_anomaly: bool = False,
+                 debug: bool = False, debug_from: int = -1, debug_snapshot: str = _debug.SNAPSHOT):
         refuse_data_parallel_anomaly(detect_anomaly, world, "FreeTrainer")
+        refuse_data_parallel_debug(debug, debug_from, world, "FreeTrainer")
+        self._debug = _debug.DebugMode(debug, debug_from, debug_snapshot)
         if world != 1:
             raise ValueError("FreeTrainer trains on one GPU: data-parallel densification (all-reduced statistics) is not implemented")
         from .optim import free_model_groups
@@ -660,6 +720,31 @@ class FreeTrainer:
         the frame.  frame_end: recorded on the current stream right after the frame's launches, before before_update,
         densification and any Adam step outside the frame (MeshTrainer.step)."""
         it = self.iteration + 1
+        bg = self.bg if bg is None else bg
+        return _debug.run_step(self, lambda debug: self._step(cam, gt, bg, before_update, frame_end, debug), cam, gt, bg, it)
+
+    def _debug_config(self) -> dict:
+        """The constructor arguments a replay (debug.replay) rebuilds this trainer with."""
+        return dict(extent=self.extent, opt=self.opt, white_background=self.white_background, sync_free=self.sync_free,
+                    max_size=self.max_size, antialiasing=self.antialiasing)
+
+    def _debug_flat(self) -> torch.Tensor:
+        return self.adam.p
+
+    def _debug_restore(self, snap: dict) -> None:
+        """The state a debug snapshot recorded before its step (MeshTrainer._debug_restore), statistics and generator too."""
+        self.load_state_dict(_debug.to_device(snap["state_dict"], self.model._xyz.device))
+        self.model.active_sh_degree = int(snap["active_sh_degree"])
+        self.iteration = int(snap["iteration"]) - 1
+        self.adam.zero_grad()
+
+    @property
+    def native_frame(self):
+        """The native frame of the last step (None before the first)."""
+        return self.frame
+
+    def _step(self, cam, gt, bg, before_update, frame_end, debug: bool) -> torch.Tensor:
+        it = self.iteration + 1
         self.adam.groups[0]["lr"] = self._xyz_lr(it)
         if it % 1000 == 0:
             self.model.oneupSHdegree()
@@ -678,8 +763,7 @@ class FreeTrainer:
             if stats:       # the frame adds this step's statistics in its last kernel
                 f, kept = self.frame, (self.frame.accum.clone(), self.frame.denom.clone())
                 restore = lambda: (f.accum.copy_(kept[0]), f.denom.copy_(kept[1]))
-        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, stats=stats, sh_adam=sh_adam, antialiasing=self.antialiasing,
-                              anomaly=record)
+        loss = self.frame.run(cam, gt, bg, stats=stats, sh_adam=sh_adam, antialiasing=self.antialiasing, anomaly=record, debug=debug)
         if frame_end is not None:
             frame_end.record(torch.cuda.current_stream(self.frame.dev))
         if record is not None:
@@ -688,6 +772,8 @@ class FreeTrainer:
             before_update()
         if densify:
             self.densify(size_prune=it > self.opt.opacity_reset_interval)
+            if debug:
+                _debug.sync("densification (gms_densify_plan, gms_densify_apply)", self.frame.dev)
         if reset:
             self.reset_opacity()
         if not densify and it < self.opt.iterations:     # train.py steps the optimizer on every iteration but the last
@@ -698,6 +784,8 @@ class FreeTrainer:
                 self.adam.step_dense(zero_end=0, skip=skip)
             else:
                 self.adam.step(zero_end=0, skip=skip)
+            if debug:
+                _debug.sync("FlatAdam step (gms_adam_step)", self.frame.dev)
         self.iteration = it
         return loss
 
@@ -780,7 +868,7 @@ class FreeTrainer:
     def evaluate(self, cams: Sequence[Camera], gts: Sequence[torch.Tensor], protocol: str = "training_report"):
         """L1 / SSIM / PSNR of the current model on held-out views (NativeFreeRenderer.evaluate, MeshTrainer.evaluate)."""
         self._renderer = renderer_set(self._renderer, NativeFreeRenderer, self.model, self.model.P)
-        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol, antialiasing=self.antialiasing)
+        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol, antialiasing=self.antialiasing, debug=self._debug.on)
 
 
 # ---------------------------------------------------------------------------------------------- gs_flame
@@ -835,10 +923,13 @@ class FlameTrainer:
     Views may differ in size: max_size (W, H) as MeshTrainer's.  antialiasing: as MeshTrainer's.  detect_anomaly: as
     MeshTrainer's, with the iteration counter unchanged when step() raises; a NativeFlame driver's parameter gradients are
     scanned as one more stage (FLAME backward), and the ATen part of any other driver runs under
-    torch.autograd.detect_anomaly() after the frame's record was read."""
+    torch.autograd.detect_anomaly() after the frame's record was read.  debug, debug_from, debug_snapshot: as MeshTrainer's;
+    a debug step also synchronises after the NativeFlame LBS forward and backward."""
 
     def __init__(self, model, bg: torch.Tensor, opt: FlameOptimizationParams = None, sync_free: bool = True,
-                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False, detect_anomaly: bool = False):
+                 max_size: Optional[Tuple[int, int]] = None, antialiasing: bool = False, detect_anomaly: bool = False,
+                 debug: bool = False, debug_from: int = -1, debug_snapshot: str = _debug.SNAPSHOT):
+        self._debug = _debug.DebugMode(debug, debug_from, debug_snapshot)
         self.model, self.bg = model, bg
         self.antialiasing = bool(antialiasing)
         self.detect_anomaly = bool(detect_anomaly)
@@ -867,6 +958,30 @@ class FlameTrainer:
         SH Adam update into the frame.  frame_end: recorded on the current stream right after the frame's launches and the
         driver's backward, before before_update and any Adam step outside the frame (MeshTrainer.step)."""
         it = self.iteration + 1
+        bg = self.bg if bg is None else bg
+        return _debug.run_step(self, lambda debug: self._step(cam, gt, bg, before_update, frame_end, debug), cam, gt, bg, it)
+
+    def _debug_config(self) -> dict:
+        """The constructor arguments a replay (debug.replay) rebuilds this trainer with."""
+        return dict(opt=self.opt, sync_free=self.sync_free, max_size=self.max_size, antialiasing=self.antialiasing)
+
+    def _debug_flat(self) -> torch.Tensor:
+        return self.adam.p
+
+    def _debug_restore(self, snap: dict) -> None:
+        """The state a debug snapshot recorded before its step (MeshTrainer._debug_restore)."""
+        self.load_state_dict(_debug.to_device(snap["state_dict"], self.model.vertices.device))
+        self.model.active_sh_degree = int(snap["active_sh_degree"])
+        self.iteration = int(snap["iteration"]) - 1
+        self.adam.zero_grad()
+
+    @property
+    def native_frame(self):
+        """The native frame of the last step (None before the first)."""
+        return self.frame
+
+    def _step(self, cam, gt, bg, before_update, frame_end, debug: bool) -> torch.Tensor:
+        it = self.iteration + 1
         m = self.model
         if it % 1000 == 0:
             m.oneupSHdegree()
@@ -876,6 +991,8 @@ class FlameTrainer:
             if self._lbs is None:
                 self._lbs = m.driver.bind(m)
             self._lbs.forward()                  # into model.vertices; zeroes model.vertices.grad
+            if debug:
+                _debug.sync("gms_flame_lbs_forward", self.model.vertices.device)
         else:
             with aten_anomaly():
                 verts = m.driver_vertices()
@@ -889,9 +1006,11 @@ class FlameTrainer:
         sh_adam = self.adam.begin_fused_sh_step() if fused else None
         record = anomaly_record(self._anomaly, self.frame.dev) if self.detect_anomaly else None
         self._anomaly = record
-        loss = self.frame.run(cam, gt, self.bg if bg is None else bg, sh_adam=sh_adam, antialiasing=self.antialiasing, anomaly=record)
+        loss = self.frame.run(cam, gt, bg, sh_adam=sh_adam, antialiasing=self.antialiasing, anomaly=record, debug=debug)
         if native:
             self._lbs.backward()                 # writes the FLAME tensors' flat .grad views
+            if debug:
+                _debug.sync("gms_flame_lbs_backward", self.frame.dev)
             if record is not None:
                 record.scan(_lib.ANOMALY_FLAME_BWD, [(i, getattr(m, n).grad) for i, n in enumerate(m.FLAME_NAMES)])
                 check_anomaly(record, m, cam, self.adam, it)
@@ -912,6 +1031,8 @@ class FlameTrainer:
             self.adam.step_dense()
         else:
             self.adam.step()
+        if debug:
+            _debug.sync("FlatAdam step (gms_adam_step)", self.frame.dev)
         self.iteration = it
         return loss
 
@@ -937,4 +1058,4 @@ class FlameTrainer:
         """L1 / SSIM / PSNR of the current model (at its current pose) on held-out views (MeshTrainer.evaluate)."""
         self.model.refresh_vertices()
         self._renderer = renderer_set(self._renderer, NativeRenderer, self.model, self.model.P)
-        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol, antialiasing=self.antialiasing)
+        return self._renderer.evaluate(cams, gts, self.bg, protocol=protocol, antialiasing=self.antialiasing, debug=self._debug.on)

@@ -50,6 +50,7 @@ extern "C" {
 #define GMS_E_CUDA (-2)       /* a CUDA call or launch failed; see gms_last_error() */
 #define GMS_E_ALLOC (-3)      /* the allocation callback returned NULL */
 #define GMS_E_UNSUPPORTED (-4)
+#define GMS_E_DEBUG (-5)      /* debug mode: the binning check found a violated invariant; gms_last_error() names it */
 
 #define GMS_BUF_GEOM 0
 #define GMS_BUF_BINNING 1
@@ -73,7 +74,9 @@ typedef struct gms_raster_settings {
     int32_t sh_degree;        /* active degree 0..3 */
     const float* campos;      /* device [3] */
     int32_t prefiltered;
-    int32_t debug;            /* 1: synchronise + check after every launch (stock --debug behaviour) */
+    int32_t debug;            /* 1: synchronise + check after every launch (stock --debug behaviour).  The one-call frames
+                                 also synchronise after the sorts and the scan and run the binning check (gms_debug_check_bins)
+                                 on their own buffers; a violation is GMS_E_DEBUG */
     int32_t antialiasing;
 } gms_raster_settings;
 
@@ -921,6 +924,39 @@ typedef struct gms_nan_scan_args {
  * n < 0 or n >= 2^48, more than GMS_NAN_SCAN_MAX_BUFFERS buffers, a null or misaligned pointer with n > 0, a stage or a tensor
  * id out of range.  Caller's stream, no host synchronisation. */
 int gms_nan_scan(const gms_nan_scan_args* a, void* cuda_stream);
+
+/* ---- debug mode: the binning check ------------------------------------------------------------ */
+/* The invariants the composite kernels rely on, checked on a binned point list.  The first violation is keyed
+ *   key = check << 56 | index,
+ * the smallest key over the whole check: */
+#define GMS_DEBUG_NONE 0xFFFFFFFFFFFFFFFFull
+#define GMS_DEBUG_ORDER 1       /* index = list position whose (depth key, Gaussian) does not exceed its predecessor's in the tile */
+#define GMS_DEBUG_RANGES 2      /* index = start of a range that is out of [0, n) or not where the previous non-empty range ended,
+                                   the list position of an entry whose tile key is not its range's tile, or the end of the last
+                                   range when it is not n.  Also: the rectangles of the Gaussians with radii > 0 cover a different
+                                   number of tiles than n (index n) */
+#define GMS_DEBUG_GAUSSIAN 3    /* index = list position whose Gaussian is >= P, has radii <= 0, or whose rectangle misses the tile */
+#define GMS_DEBUG_SURVIVOR 4    /* index = slot in surv of a survivor outside its tile's range or not above its predecessor */
+typedef struct gms_debug_bins_args {
+    int32_t P;                  /* Gaussians */
+    int32_t tiles_x, tiles_y;   /* tile grid (16x16 px tiles) */
+    int64_t n;                  /* list entries */
+    const uint32_t* point_list; /* device [n] Gaussian indices */
+    const void* tile_keys;      /* device [n] tile ids (uint16 when key_bits == 16, else uint32), or NULL */
+    int32_t key_bits;           /* 16 or 32 (ignored without tile_keys) */
+    const int32_t* ranges;      /* device [T,2] (start, end) per tile */
+    const int32_t* radii;       /* device [P] */
+    const uint32_t* rect;       /* device [P,2] tile rectangle: x0 | y0 << 16, x1 | y1 << 16 (end exclusive) */
+    const uint32_t* depth_keys; /* device [P] the depth sort's keys */
+    const uint32_t* surv;       /* device [4n] per-quad survivor lists (gms_debug_views.surv), or NULL */
+    const uint32_t* nsurv;      /* device [4T] survivors per (tile, quad); with surv */
+    uint64_t* key;              /* host, optional: the key of the first violation, GMS_DEBUG_NONE when clean */
+} gms_debug_bins_args;
+/* Runs the check the frames run under debug on caller-given buffers and synchronises the stream: GMS_OK when every invariant
+ * holds, GMS_E_DEBUG naming the check, the index, the tile and the Gaussian otherwise.  Every read is bounds-checked, so any
+ * in-bounds buffers are safe to check.  GMS_E_ARG before any launch: a null pointer, P < 0, a tile grid outside 1..65535
+ * or of more than 2^26 tiles, n < 0 or n >= 2^31, key_bits other than 16 or 32 with tile_keys, or exactly one of surv / nsurv. */
+int gms_debug_check_bins(const gms_debug_bins_args* a, void* cuda_stream);
 
 /* ---- misc ------------------------------------------------------------------------------------- */
 const char* gms_last_error(void);
